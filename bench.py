@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- CTC-CRF loss+grad frames/sec on synthetic (N,T,V) log-probs (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path (numerator + denominator forward-backward, loss and (N,T,V) gradient)
@@ -54,7 +54,13 @@ def parse():
     ap.add_argument("--cpu-sample", default="auto", help="N,T of the CPU sample (default sized for ~15 s)")
     ap.add_argument("--no-strong", action="store_true", help="skip the strong-scaling block (global batches sharded over the ranks)")
     ap.add_argument("--strong-configs", default="5,4", help="which SURVEY configs the strong block runs (5: N=256 var-len; 4: N=128, 5M-arc graph)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path returned in its last step (loss, gradient) to DIR/<name>.npy; "
+                         "with --gpus > 1, rank 0's shard of the batch (its local loss and gradient)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 def peaks():
@@ -62,7 +68,7 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, sustained copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM, HBM3)"
 
 
 def den_graph_file(H, d, V):
@@ -73,6 +79,25 @@ def den_graph_file(H, d, V):
         fst.write_fst(path + ".tmp", g)
         os.replace(path + ".tmp", path)
     return path, g
+
+
+DUMP_GRAD_BYTES = 48 << 20   # the gradient share of --dump-outputs (64 MB in all)
+
+
+def dump_outputs(d, loss, grad):
+    """loss.npy, and the (N,T,V) gradient as grad.npy -- or, above DUMP_GRAD_BYTES, the rows of a fixed seeded sample
+    of its (utterance, frame) pairs as grad_sample.npy, with their flat row indices in grad_sample_rows.npy."""
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "loss.npy"), loss.detach().float().cpu().numpy())
+    g = grad.detach().float()
+    if g.numel() * 4 <= DUMP_GRAD_BYTES:
+        np.save(os.path.join(d, "grad.npy"), g.cpu().numpy())
+        return
+    g = g.reshape(-1, g.shape[-1])
+    k = DUMP_GRAD_BYTES // (4 * g.shape[1])
+    rows = np.sort(np.random.default_rng(0).choice(g.shape[0], size=k, replace=False))
+    np.save(os.path.join(d, "grad_sample_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(d, "grad_sample.npy"), g[torch.from_numpy(rows).to(g.device)].cpu().numpy())
 
 
 def synth_labels(N, T, V, seed, varlen=False):
@@ -86,7 +111,7 @@ def synth_labels(N, T, V, seed, varlen=False):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -235,12 +260,15 @@ def main():
     crit = ctc_crf.CTC_CRF_LOSS(lamb=args.lamb, size_average=True)
 
     host_s = [0.0, 0]   # host-side enqueue time of the resident steps (diagnostic: the GPU must never wait for it)
+    last = {}           # --dump-outputs: what the last timed step returned
 
     def step_resident():
         t0 = time.perf_counter()
         loss, grad, _ = _C.ctc_crf_loss_fwd(y, labels, lx, ly, args.lamb, True)
         host_s[0] += time.perf_counter() - t0
         host_s[1] += 1
+        if args.dump_outputs:
+            last["loss"], last["grad"] = loss, grad
         if world > 1:
             v = torch.stack([loss.reshape(()) * N, torch.tensor(float(N), device=dev)])
             dist.all_reduce(v)
@@ -276,6 +304,9 @@ def main():
     launches = _C.launch_count() - timed.launches_before
     clocks = sampler.stop() if rank == 0 else None
     ms_per_step = ms_total / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], last["grad"])
+    last.clear()
     value = world * frames_per_step / (ms_per_step * 1e-3)
 
     # ---- e2e: public API, host buffers, H2D of the step's logits + D2H of the loss inside the timed region ----
@@ -329,7 +360,7 @@ def main():
     bytes_bwd = frames_per_step * (V * b_in + 4 * V + 4 * S_plan) + graph_bytes // 2
     bytes_den = frames_per_step * (2 * V * b_in + 4 * V + 8 * S_plan) + graph_bytes
     ach = bytes_den / (ms_fb * 1e-3) / 1e9
-    # measured DRAM traffic per launch: per-frame bytes from the committed ncu --set full capture (profiles/traffic.json,
+    # measured DRAM traffic per launch: per-frame bytes from an ncu --set full capture (profiles/traffic.json, when present,
     # taken at the same N/V/graph) x the frames of this launch; null for other workloads
     traffic = None
     pipes = None
@@ -461,7 +492,7 @@ def main():
                         rctx.close()
                         dt = sorted(times)[1]
                         ref_cuda_res = {"value": rN * rT / dt, "unit": UNIT, "reps_s": times,
-                                        "sample": f"reference CUDA sources (oracle/_ref, sm_100a build with the two sm_100 fixes of oracle/Makefile) on this GPU, "
+                                        "sample": f"reference CUDA sources (oracle/_ref, sm_90a build with the two fixes of oracle/Makefile) on this GPU, "
                                                   f"N={rN},T={rT} slice of the headline batch, same graph; CUDA events, 1 warm-up + 3 reps, median"}
                 except Exception as e:  # the reference arm must never take the bench down
                     ref_cuda_res = {"error": repr(e)}
@@ -485,7 +516,7 @@ def main():
                        "den_graph": f"synthetic T-compose-LM H={args.H},d={args.d}: file S={graph.num_states} A={graph.num_arcs}; plan S={info['states']} pairs={info['pairs']} gathered arcs fwd/bwd={info['fwd_arcs']}/{info['bwd_arcs']}",
                        "global_batch": N * world, "parallelism": f"minibatch sharded x{world}, den graph replicated, 1 all-reduce of [cost,count]",
                        "lamb": args.lamb,
-                       "l2": "no explicit flush: each step streams a 15.4 GB alpha spill (>> 126 MB L2)" if N * T >= 20000 else "small dev workload"},
+                       "l2": "no explicit flush: each step streams a 15.4 GB alpha spill (>> 50 MB L2)" if N * T >= 20000 else "small dev workload"},
             "e2e": {"value": e2e_value, "unit": UNIT, "ms_per_step": ms_e2e, "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": 4,
                     "h2d_ms_median": h2d_ms[len(h2d_ms) // 2], "h2d_ms_max": h2d_ms[-1],
                     "api": "ctc_crf.CTC_CRF_LOSS.forward on pinned-host logits copied H2D inside the step, loss.item() back"},

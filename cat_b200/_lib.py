@@ -34,7 +34,7 @@ def lib() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB):
         raise ImportError(
-            f"{LIB} is missing: build it with `python -m cat_b200.build` (nvcc, sm_100a). "
+            f"{LIB} is missing: build it with `python -m cat_b200.build` (nvcc, sm_90a). "
             "cat_b200 has no CPU or PyTorch fallback.")
     L = C.CDLL(LIB)
     vp, ip, fp = C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_float)

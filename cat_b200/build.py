@@ -1,4 +1,4 @@
-"""In-tree build of the native library (nvcc, sm_100a only).
+"""In-tree build of the native library (nvcc, sm_90a only).
 
 The product has exactly one native artefact, ``cat_b200/libctc_crf_b200.so`` (CUDA kernels + C ABI,
 no torch dependency).  It is built in-tree so the file travels to the GPU box with the repository
@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, os.environ.get("CCB_LIB_NAME", "libctc_crf_b200.so"))   # (name/defines: tuning builds only)
 SOURCES = ["api.cu", "den_kernels.cu", "ctc_kernels.cu", "den_graph.cc"]
 HEADERS = ["common.cuh", "den_graph.h", os.path.join("..", "..", "include", "ctc_crf_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

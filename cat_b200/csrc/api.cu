@@ -42,11 +42,10 @@ struct LegacyScratch {
 };
 LegacyScratch g_legacy[kMaxDevices];
 
-// Side stream of the fused loss (OPT-IN, CCB_OVERLAP=1 at Init; measured and left off, profiles/r02_experiments.md section 14):
+// Side stream of the fused loss (OPT-IN, CCB_OVERLAP=1 at Init; off by default):
 // the numerator's alpha || beta chains (a latency-bound ~1 ms on 2N small CTAs) run here next to the den forward pass, whose
-// persistent CTAs leave room for one of them per SM (78 x 512 + 39 x 256 registers, 167 + 11 KB of shared memory).  On the
-// B200 the two grids do become co-resident, but not profitably: either the cooperative den grid is admitted only after ~1 ms
-// (step -0.4 ms), or both run at once and BOTH crawl until the numerator is through (numerator 1.5 -> 5.4 ms, den forward + 5 ms).
+// persistent CTAs leave room for one of them per SM.  Co-residence is not profitable: either the cooperative den grid is
+// admitted only after the numerator, or both run at once and both slow down until the numerator is through.
 // Created at Init, destroyed by Release.
 struct SideStream {
     cudaStream_t s = nullptr;
@@ -205,8 +204,7 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
         d.own_rows = g_plan.own_rows;
         { const char *e = getenv("CCB_ARCS_IN_GLOBAL"); d.tune_arcs_in_global = e && e[0] == '1'; }
         { const char *e = getenv("CCB_W1_IN_GLOBAL"); d.tune_w1_in_global = e && e[0] == '1'; }
-        { const char *e = getenv("CCB_NO_TMA"); d.tune_no_tma = e && e[0] == '1'; }   // A/B: register gathers instead of TMA gather4
-        { const char *e = getenv("CCB_RING_ROWS"); d.tune_ring_rows = e ? atoi(e) : 0; }   // A/B: rows per TMA ring stage (16 / 8)
+        { const char *e = getenv("CCB_NO_TMA"); d.tune_no_tma = e && e[0] == '1'; }   // A/B: register gathers instead of TMA row staging
         // streamed-arc tier: only graphs whose arc stream may not fit shared memory next to the TMA rings carry the copy
         if (rc == 0 && g_plan.hub_states.empty() && !d.tune_no_tma &&
             (d.tune_arcs_in_global || (size_t)d.bwd.max_tile_arcs * 12 > kStreamTierArcBytes))

@@ -55,7 +55,6 @@ struct DeviceGraph {
     int max_smem_optin = 0;
     // test hooks, read ONCE at Init (never on the per-call path): force the large-graph tiers on a small graph
     bool tune_arcs_in_global = false, tune_w1_in_global = false, tune_no_tma = false;
-    int tune_ring_rows = 0;    // > 0: force this many rows per TMA ring stage (A/B runs)
     // batches of <= 16 utterances run the small-batch TMA kernels (rows of 8 / 16 floats): needs both arc streams in
     // shared memory next to the rings, no hub rows, and a usable TMA descriptor -- decided once at Init
     bool small_ok = false;
@@ -66,9 +65,9 @@ struct DeviceGraph {
 // descriptor inside it is read by the hardware straight from parameter memory and must sit on a 64-byte boundary).
 struct alignas(64) DenParams {
     // TMA view of the pass's gather table (forward: the alpha spill, backward: the beta ping-pong) as a 2-D tensor
-    // [rows][Npad] of fp32 with a box of one row x (32 * utterances per lane) columns; used by the gather4 kernels only
+    // [rows][Npad] of fp32 with a box of one row x (32 * utterances per lane) columns; used by the full-width TMA kernels only
     CUtensorMap tmap;
-    int use_tma;          // 1: rows are staged in shared memory by TMA gather4 (den_kernels.cu), 0: register gathers
+    int use_tma;          // 1: rows are staged in shared memory by TMA / bulk copies (den_kernels.cu), 0: register gathers
     int ring_off;         // byte offset of the per-warp row rings in dynamic shared memory (128-byte aligned)
     int bar_off;          // byte offset of the rings' mbarriers
     // graph
@@ -131,8 +130,7 @@ struct DenAuxLayout {
 // on a graph that supports the small-batch kernels (DeviceGraph::small_ok) use 8- or 16-float rows instead, with the
 // lanes of a warp spread over (arc of the quad) x (utterance)  (den_kernels.cu, LPR template parameter).
 inline int PadLanes(int N, bool small_ok) {
-    // (8-float rows were measured slower than 16-float rows with half the lanes idle -- N=8, T=600: 11.1 + 14.2 ms against
-    // 8.1 + 8.7 ms -- because the gather4 copies are bound by their count, not by their bytes: profiles/r02_experiments.md)
+    // (16-float rows even for N <= 8: the row copies are bound by their count, not by their bytes)
     if (small_ok && N <= 16) return 16;
     int g = (N + 31) / 32;
     if (g >= 3) g = (g + 3) / 4 * 4;   // lanes carry 1, 2 or 4 utterances each

@@ -611,7 +611,7 @@ static bool BuildDenPlanImpl(const HostFst &fst, int n_ctas, int n_warps, bool a
     build(gk);
     const int G = (int)gk.size();
     auto seg_quads = [](const Segment &sg) { return std::max<int64_t>(1, ((int64_t)sg.arcs.size() + kQuad - 1) / kQuad); };
-    // per-row costs in arc units, fitted to per-warp timelines on B200 (tools/timeline.py)
+    // per-row costs in arc units, fitted to per-warp timelines (tools/timeline.py)
     constexpr int64_t kRowCostFwd = 5, kRowCostBwd = 8;
     std::vector<int64_t> cost((size_t)G, 0), cost_f((size_t)G, 0), cost_b((size_t)G, 0);
     for (int g = 0; g < G; ++g) {

@@ -94,8 +94,7 @@ struct DenPlan {
     //     own[2q] * X(first row of its group) + own[2q+1] * X(second row of its group, or the row itself if unpaired)
     // on top of its gathered sum, X = the previous frame's alpha rows (forward) / the next frame's beta-hat rows (backward),
     // which the kernels fetch with two plain row loads per group, one group ahead of use.  Frame time follows the number of
-    // slots a warp walks through its TMA ring (profiles/r02_experiments.md section 15), so this is worth 554 k -> 514 k forward
-    // and 564 k -> 488 k backward slots per frame.  All or nothing: only plans without hub rows in which every pair's first
+    // slots a warp walks through its TMA ring, so this removes gathered slots from both passes.  All or nothing: only plans without hub rows in which every pair's first
     // member is left with NO gathered in-arc (then every pair is one merged forward segment without a tail slot).
     bool own_rows = false;
     std::vector<float> own_fwd, own_bwd;   // [2S + 4] (zero when !own_rows; padded so that a 4-float read at 2q stays inside)

@@ -1,4 +1,4 @@
-// Denominator forward-backward over the shared phone-LM WFST: persistent sm_100a kernels.
+// Denominator forward-backward over the shared phone-LM WFST: persistent sm_90a kernels.
 //
 // What the reference does (src/ctc_crf/gpu_den/den_calculate.cu): 3T+6 launches of <<<N,1024>>> kernels,
 // one CTA per utterance, thread per state, log-domain log1p(exp()) per arc, per-arc atomicCAS gradient.
@@ -43,7 +43,7 @@ constexpr unsigned kFull = 0xffffffffu;
 // frame ends in the grid barrier's gpu-scope acquire fence + bar.sync, after which ordinary loads must observe the other
 // CTAs' released writes (the same contract cooperative-groups grid.sync() gives), and no row is re-read within a frame
 // after being rewritten.  Against ld.global.cg this makes the zero-weight padding slots (which repeat the address of
-// the preceding arc) L1 hits: forward pass -5.6 % on B200 (profiles/r01_experiments.md).  -DCCB_GATHER_CG restores
+// the preceding arc) L1 hits.  -DCCB_GATHER_CG restores
 // the L2-only loads for A/B runs.
 #ifdef CCB_GATHER_CG
 #define CCB_GATHER_LOAD(p) __ldcg(p)
@@ -118,9 +118,8 @@ template <int U>
 __device__ __forceinline__ Vec<U> gather_row(const char *lane_base, uint32_t byte_off) {
     return Vec<U>::ld_row(reinterpret_cast<const float *>(lane_base + byte_off));
 }
-// The gathers of one quad.  (Skipping the zero-weight padding slots -- ~17 % of the forward stream -- was tried with a
-// per-quad count in the last offset: the extra branches cost 10 % of the forward pass and the saved gathers returned
-// 1.6 %; measured on B200, profiles/r01_experiments.md.)
+// The gathers of one quad.  (Skipping the zero-weight padding slots -- ~17 % of the forward stream -- with a per-quad
+// count in the last offset costs more in branches than the saved gathers return.)
 template <int U>
 __device__ __forceinline__ void gather_quad(const char *lane_base, const uint4 pr, Vec<U> *v) {
     v[0] = gather_row<U>(lane_base, pr.x);
@@ -366,13 +365,10 @@ __device__ __forceinline__ void walk_arcs_dual(const uint4 *arcs, const float4 *
 }
 
 // ------------------------------------------------------------------------------------------------
-// TMA row gathers (sm_100a): `cp.async.bulk.tensor.2d ... tile::gather4` (SASS UTMALDG.2D.GATHER4) copies FOUR rows of
-// the gather table, named by four row coordinates, into shared memory with one instruction issued by one lane -- exactly
-// one arc quad.  The rows of a batch land in a per-warp ring (STAGES stages of R rows) and complete an mbarrier; the warp
-// then reads them with LDS.  Measured on this B200 (tools/l2_gather4_bench.cu, profiles/r02_l2_gather4_microbench.txt):
-// random 256-byte rows from an L2-resident table at 62 G rows/s = 15.9 TB/s with 512 threads (1-D bulk copies, one
-// instruction per row: 43 G rows/s; the register path of round 1: 42 G rows/s inside the kernels), and the rows in flight
-// cost no registers and 5 instructions per arc slot instead of 13.
+// TMA row gathers (sm_90a): one tile-mode `cp.async.bulk.tensor.2d` (a box of one row of the gather table) per arc slot,
+// issued by the lanes of the warp, one row each.  The rows of a batch land in a per-warp ring (STAGES stages of R rows)
+// and complete an mbarrier; the warp then reads them with LDS.  A row coordinate beyond the tensor (kOobRow) is
+// zero-filled by the TMA unit without touching L2.  The rows in flight cost no registers.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, unsigned count) {
@@ -388,10 +384,13 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, unsigned parity) {
                      : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
     } while (!ok);
 }
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const CUtensorMap *tm, int col, int r0, int r1, int r2, int r3, uint32_t bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5, %6}], [%7];"
-                 ::"r"(dst), "l"(tm), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(bar) : "memory");
+// one row (the tensor map's box: 1 row x box_cols columns) into shared memory; `dst` must be 128-byte aligned
+__device__ __forceinline__ void tma_row(uint32_t dst, const CUtensorMap *tm, int col, int row, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(dst), "l"(tm), "r"(col), "r"(row), "r"(bar) : "memory");
 }
+// the arc slot j (0..3) of a quad's row word
+__device__ __forceinline__ int quad_row(const uint4 &pr, int j) { return (int)(j == 0 ? pr.x : j == 1 ? pr.y : j == 2 ? pr.z : pr.w); }
 // 1-D bulk copy global -> shared (SASS UBLKCP): sequential arc words of a batch, completing on the batch's mbarrier
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, unsigned bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cta.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -405,11 +404,11 @@ __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence
 struct TmaRing {
     uint32_t buf, bar, phase;
 };
-// rows per ring stage (two stages per warp): the default, and a shallower ring (A/B hook CCB_RING_ROWS)
+// rows per ring stage (two stages per warp) of the streamed-arc backward tier
 template <int U> struct TmaShape;
-template <> struct TmaShape<1> { static constexpr int R = 16, R_SMALL = 16; };
-template <> struct TmaShape<2> { static constexpr int R = 16, R_SMALL = 8; };
-template <> struct TmaShape<4> { static constexpr int R = 8, R_SMALL = 8; };
+template <> struct TmaShape<1> { static constexpr int R = 16; };
+template <> struct TmaShape<2> { static constexpr int R = 16; };
+template <> struct TmaShape<4> { static constexpr int R = 8; };
 
 template <int U> __device__ __forceinline__ Vec<U> lds_row(uint32_t addr);
 template <> __device__ __forceinline__ Vec<1> lds_row<1>(uint32_t addr) {
@@ -429,22 +428,21 @@ template <> __device__ __forceinline__ Vec<4> lds_row<4>(uint32_t addr) {
 }
 
 // The arc walk with TMA-staged rows.  `arcs`: the chunk's quads in shared memory, WPQ 16-byte words per quad
-// {row index 0..3}{w0..3}[{w1 0..3}]; n_batches = chunk arcs / R.  One batch = R/4 quads, issued by lanes 0..R/4-1 (one
-// gather4 each).  `consume_quad(words of the quad, rows v[4])` does the FMAs and the segment-end work.
+// {row index 0..3}{w0..3}[{w1 0..3}]; n_batches = chunk arcs / R.  One batch = R/4 quads, issued by lanes 0..R-1 (one
+// row each).  `consume_quad(words of the quad, rows v[4])` does the FMAs and the segment-end work.
 template <int U, int R, int WPQ, typename Prologue, typename ConsumeQuad>
 __device__ __forceinline__ void walk_arcs_tma(const uint4 *arcs, int n_batches, const CUtensorMap *tm, int col, int row_base,
                                               TmaRing &ring, int lane, Prologue &&prologue, ConsumeQuad &&consume_quad) {
     constexpr int QB = R / kQuad;   // (two stages)
     constexpr uint32_t ROWB = 32u * U * 4u;
-    static_assert(R % kQuad == 0 && kChunkArcPad % R == 0, "a batch is whole quads and divides the chunk padding");
+    static_assert(R % kQuad == 0 && kChunkArcPad % R == 0 && R <= 32, "a batch is whole quads, divides the chunk padding, one row per lane");
     auto issue = [&](int k, int s) {
         const uint32_t bar = ring.bar + 8u * s;
         if (lane == 0) mbar_expect_tx(bar, R * ROWB);
         __syncwarp();
-        if (lane < QB) {
-            const uint4 pr = arcs[(size_t)WPQ * (k * QB + lane)];
-            tma_gather4(ring.buf + (uint32_t)(s * R + kQuad * lane) * ROWB, tm, col, row_base + (int)pr.x, row_base + (int)pr.y,
-                        row_base + (int)pr.z, row_base + (int)pr.w, bar);
+        if (lane < R) {
+            const uint4 pr = arcs[(size_t)WPQ * (k * QB + lane / kQuad)];
+            tma_row(ring.buf + (uint32_t)(s * R + lane) * ROWB, tm, col, row_base + quad_row(pr, lane % kQuad), bar);
         }
     };
     auto consume = [&](int k, int s) {
@@ -520,10 +518,9 @@ __device__ __forceinline__ void walk_arcs_tma_stream(ArcRing &ar, int n_batches,
         const uint32_t bar = ring.bar + 8u * s;
         if (lane == 0) mbar_expect_tx(bar, R * ROWB);
         __syncwarp();
-        if (lane < QB) {
-            const uint4 pr = ar.buf[st * AW + WPQ * lane];
-            tma_gather4(ring.buf + (uint32_t)(s * R + kQuad * lane) * ROWB, tm, col, row_base + (int)pr.x, row_base + (int)pr.y,
-                        row_base + (int)pr.z, row_base + (int)pr.w, bar);
+        if (lane < R) {
+            const uint4 pr = ar.buf[st * AW + WPQ * (lane / kQuad)];
+            tma_row(ring.buf + (uint32_t)(s * R + lane) * ROWB, tm, col, row_base + quad_row(pr, lane % kQuad), bar);
         }
     };
     auto consume = [&](int k, int s) {
@@ -562,7 +559,9 @@ __device__ __forceinline__ void walk_arcs_tma_stream(ArcRing &ar, int n_batches,
 // instructions), each lane multiplies by the weight of ITS arc, and the partial sums of the 32 / LPR lane groups are
 // combined with one or two shuffles when a segment ends.  A warp thus spends 4x (2x) fewer instructions and rows of L2
 // traffic per utterance than with 24 (16) of 32 lanes idle -- the per-GPU share of a batch sharded over 8 GPUs is 8-32
-// utterances (SURVEY.md 8e).  Rings: kSmallStages stages of 16 rows per warp.
+// utterances (SURVEY.md 8e).  Rings: kSmallStages stages of 16 rows per warp.  Rows this short sit below the 128-byte
+// alignment a tensor copy's destination needs, so each row is a 1-D bulk copy from `table` (16-byte alignment), one per
+// lane, and the lane of a padding slot (kOobRow) zero-fills its row with shared stores instead.
 constexpr int kSmallStages = 4;
 __device__ __forceinline__ float lds_f32(uint32_t addr) {
     float r;
@@ -573,23 +572,27 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
 // consecutive floats of DenPlan::bwd.w1 -- are not resident; they ride along with the batch's rows as one 64-byte bulk copy
 // into `w1buf` (one 64-byte slot per stage) on the same mbarrier, and `consume_quad` receives their shared-memory address.
 template <int LPR, int WPQ, bool W1_STREAM = false, typename Prologue, typename ConsumeQuad>
-__device__ __forceinline__ void walk_arcs_tma_small(const uint4 *arcs, int n_batches, const CUtensorMap *tm, int row_base,
+__device__ __forceinline__ void walk_arcs_tma_small(const uint4 *arcs, int n_batches, const float *table, int row_base,
                                                     TmaRing &ring, int lane, Prologue &&prologue, ConsumeQuad &&consume_quad,
                                                     const float *w1g = nullptr, uint32_t w1buf = 0u) {
     constexpr int R = 16, QB = R / kQuad, STEPS = LPR / 8;      // LDS steps per quad: 1 (LPR = 8) or 2 (LPR = 16)
     constexpr uint32_t ROWB = LPR * 4u;
     auto issue = [&](int k, int s) {
-        const uint32_t bar = ring.bar + 8u * s;
+        const uint32_t bar = ring.bar + 8u * s, dst = ring.buf + (uint32_t)(s * R + lane) * ROWB;
+        const uint32_t row = lane < R ? (uint32_t)quad_row(arcs[(size_t)WPQ * (k * QB + lane / kQuad)], lane % kQuad) : kOobRow;
+        const unsigned live = __ballot_sync(0xffffffffu, row != kOobRow);
+        if (lane < R && row == kOobRow) {
+#pragma unroll
+            for (uint32_t b = 0; b < ROWB; b += 16u)
+                asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(dst + b), "r"(0u) : "memory");
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // before a later bulk copy refills the slot
+        }
         if (lane == 0) {
-            mbar_expect_tx(bar, R * ROWB + (W1_STREAM ? R * 4u : 0u));
+            mbar_expect_tx(bar, (unsigned)__popc(live) * ROWB + (W1_STREAM ? R * 4u : 0u));
             if (W1_STREAM) bulk_g2s(w1buf + 64u * s, w1g + (size_t)k * R, R * 4u, bar);
         }
-        __syncwarp();
-        if (lane < QB) {
-            const uint4 pr = arcs[(size_t)WPQ * (k * QB + lane)];
-            tma_gather4(ring.buf + (uint32_t)(s * R + kQuad * lane) * ROWB, tm, 0, row_base + (int)pr.x, row_base + (int)pr.y,
-                        row_base + (int)pr.z, row_base + (int)pr.w, bar);
-        }
+        __syncwarp();   // (also orders the zero stores before every lane's reads of the stage)
+        if (row != kOobRow) bulk_g2s(dst, table + (size_t)(row_base + (int)row) * LPR, ROWB, bar);
     };
     if (n_batches <= 0) { prologue(); return; }
     for (int k = 0; k < kSmallStages && k < n_batches; ++k) issue(k, k);
@@ -658,7 +661,7 @@ __device__ __noinline__ void forward_partial_row(const int *state_label, const i
 // ------------------------------------------------------------------------------------------------
 // HUBS: the plan contains high in-degree rows split into parts (kEvPartial segments); the common case compiles the
 // partial-row path out entirely so that it costs the hot row-end code nothing.
-// TMA: the gathered rows are staged in shared memory by gather4 copies (walk_arcs_tma) instead of register gathers; needs
+// TMA: the gathered rows are staged in shared memory by TMA row copies (walk_arcs_tma) instead of register gathers; needs
 // the arc tile in shared memory (SMEM_ARCS) and DenParams::tmap.
 // LPR < 32 (8 or 16 lanes per row): the small-batch variant, see walk_arcs_tma_small (TMA, U = 1, no hub rows).
 template <int NT, int U, int BATCH, bool SMEM_ARCS, bool HUBS, bool TMA = false, int LPR = 32>
@@ -911,7 +914,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
             };
             if (TMA && LPR < 32) {
                 float acc[1] = {0.f};
-                walk_arcs_tma_small<LPR, 2>(arc4, n_batches, &P.tmap, (t - 1) * S, ring, lane, frame_scalars,
+                walk_arcs_tma_small<LPR, 2>(arc4, n_batches, P.alpha, (t - 1) * S, ring, lane, frame_scalars,
                                             [&](const uint4 *quad, const float *v, uint32_t) {
                     const uint4 wq = quad[1];
                     constexpr int STEPS = LPR / 8, SUBS = 32 / LPR;
@@ -1250,7 +1253,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
             if (TMA && LPR < 32) {
                 float acc0[1] = {0.f}, acc1[1] = {0.f};
                 const uint32_t w1buf = smem_u32(smem_raw + P.bar_off) + (uint32_t)P.n_warps * 8u * kSmallStages + (uint32_t)warp * 64u * kSmallStages;
-                walk_arcs_tma_small<LPR, W1_SMEM ? 3 : 2, !W1_SMEM>(arc4, n_batches, &P.tmap, ((tau + 1) & 1) * S, ring, lane, frame_scalars,
+                walk_arcs_tma_small<LPR, W1_SMEM ? 3 : 2, !W1_SMEM>(arc4, n_batches, P.bh, ((tau + 1) & 1) * S, ring, lane, frame_scalars,
                                             [&](const uint4 *quad, const float *v, uint32_t w1s) {
                     const uint4 wq = quad[1];
                     uint4 t1;
@@ -1418,14 +1421,6 @@ int LaunchBwd(bool w1_smem, const DenParams &p, int n_ctas, size_t smem, cudaStr
     return LaunchCoop(fn, NT, p, n_ctas, smem, stream, err);
 }
 
-// TMA gather4 variants (arc tile and, backward, both weights in shared memory); R = rows per ring stage
-template <int NT, int U, int R>
-int LaunchTma(bool backward, const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    const void *fn = backward ? (const void *)den_backward_kernel<NT, U, R, true, true, true>
-                     : p.n_hubs > 0 ? (const void *)den_forward_kernel<NT, U, R, true, true, true>
-                                    : (const void *)den_forward_kernel<NT, U, R, true, false, true>;
-    return LaunchCoop(fn, NT, p, n_ctas, smem, stream, err);
-}
 // backward pass with the arc stream flowing through per-warp rings instead of being resident (walk_arcs_tma_stream)
 template <int NT, int U, int R>
 int LaunchTmaStreamBwd(const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
@@ -1441,19 +1436,17 @@ int LaunchTmaSmall(bool backward, bool w1_smem, const DenParams &p, int n_ctas, 
     return LaunchCoop(fn, NT, p, n_ctas, smem, stream, err);
 }
 
-constexpr int kBwdMaxLaneWidth = 2;   // N=256: bwd 163 ms at 2 vs 248 ms at 4 (profiles/r01_experiments.md)
+constexpr int kBwdMaxLaneWidth = 2;   // four utterances per lane spill the backward pass's two accumulators
 
-// Gathers per batch (two batches are in flight per warp), fixed per variant by the register budget at 512 threads
-// (profiles/r01_experiments.md #4/#5): forward 2x16 rows (2x8 at four utterances per lane), backward 2x8.
+// Gathers per batch (two batches are in flight per warp), fixed per variant by the register budget at 512 threads:
+// forward 2x16 rows (2x8 at four utterances per lane), backward 2x8.
 template <int U> struct FwdBatch { static constexpr int value = U == 4 ? 8 : 16; };
 constexpr int kBwdBatch = 8;
 
 template <int NT, int U>
-int DispatchU(bool backward, bool tma, int ring_rows, bool smem_arcs, bool w1_smem, const DenParams &p, int n_ctas, size_t smem,
+int DispatchU(bool backward, bool tma, bool smem_arcs, bool w1_smem, const DenParams &p, int n_ctas, size_t smem,
               cudaStream_t stream, std::string *err) {
-    if (tma && !smem_arcs) return LaunchTmaStreamBwd<NT, U, TmaShape<U>::R>(p, n_ctas, smem, stream, err);
-    if (tma) return ring_rows == TmaShape<U>::R ? LaunchTma<NT, U, TmaShape<U>::R>(backward, p, n_ctas, smem, stream, err)
-                                                : LaunchTma<NT, U, TmaShape<U>::R_SMALL>(backward, p, n_ctas, smem, stream, err);
+    if (tma) return LaunchTmaStreamBwd<NT, U, TmaShape<U>::R>(p, n_ctas, smem, stream, err);
     if (backward)
         return smem_arcs ? LaunchBwd<NT, U, kBwdBatch, true>(w1_smem, p, n_ctas, smem, stream, err)
                          : LaunchBwd<NT, U, kBwdBatch, false>(w1_smem, p, n_ctas, smem, stream, err);
@@ -1465,9 +1458,11 @@ template <int NT>
 int Dispatch(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_smem, cudaStream_t stream,
              std::string *err) {
     const DevicePass &pass = backward ? g.bwd : g.fwd;
-    // Tiers by graph size.  (1) TMA: the whole arc stream in shared memory (8 bytes per forward slot, 12 per backward slot)
-    // next to the per-warp row rings the gather4 copies fill; (2) the same stream with register gathers (no ring);
-    // (3) backward only: offsets + first weights in shared memory, second weights streamed from L2; (4) everything from L2.
+    // Tiers by graph size, for batches of more than 16 utterances.  (1) The whole arc stream in shared memory (8 bytes per
+    // forward slot, 12 per backward slot), rows gathered into registers: on an H100 this beats staging the rows by one TMA
+    // copy each at every batch width (N = 32 / 64 / 128, T = 1500, 1.02 M arcs: 46.7 / 79.9 / 160.1 ms per step against
+    // 56.0 / 87.5 / 175.1 ms, 700 W, 1980 MHz); (2) backward only: offsets + first weights in shared memory, second weights
+    // streamed from L2, or the streamed-arc TMA tier below; (3) everything from L2.
     const size_t budget = (size_t)g.max_smem_optin > 2048 ? (size_t)g.max_smem_optin - 1024 : 0;
     const bool no_smem = g.tune_arcs_in_global;   // test hooks (read once at Init): exercise the large-graph tiers
     bool w1_smem = backward && !g.tune_w1_in_global;
@@ -1503,30 +1498,13 @@ int Dispatch(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_sme
         return LPR == 8 ? LaunchTmaSmall<NT, 8>(backward, w1_smem, p, g.n_ctas, total, stream, err)
                         : LaunchTmaSmall<NT, 16>(backward, w1_smem, p, g.n_ctas, total, stream, err);
     }
-    // TMA tier: needs the full shared-memory stream, room for the rings (two stages of R rows per warp), and a descriptor the
-    // driver accepts.
     bool tma = false;
-    int ring_rows = 0;
     p.use_tma = 0;
-    if (smem_arcs && (!backward || w1_smem) && !g.tune_no_tma && rows < ((size_t)1 << 30) &&
-        EncodeRowTensorMap(&p.tmap, table, rows, p.Npad, 32 * U)) {
-        const int r_def = U == 4 ? TmaShape<4>::R : 16, r_small = U == 2 ? TmaShape<2>::R_SMALL : r_def;
-        const int R = g.tune_ring_rows == r_small ? r_small : r_def;   // (A/B hook: the shallow ring)
-        const size_t ring_off = (smem + 127) & ~(size_t)127;
-        const size_t bar_off = ring_off + (size_t)g.n_warps * 2 * R * 32 * U * 4;
-        const size_t total = bar_off + (size_t)g.n_warps * 2 * 8;
-        if (total <= budget) {
-            tma = true; ring_rows = R;
-            p.use_tma = 1; p.ring_off = (int)ring_off; p.bar_off = (int)bar_off;
-            smem = total;
-        }
-    }
     // Streamed-arc TMA tier, BACKWARD pass only: the stream does not fit (or the test hook says so) but the graph carries the
-    // transposed copy.  The forward pass of such graphs keeps the register gathers with the arcs read from L2: measured
-    // on the 5.1 M-arc graph (N=16, T=2000) forward 97.9 ms against 138.8 ms streamed -- its 8-byte slots make 128-byte
-    // bulk copies, one per 16 rows -- while the backward pass gains (151.4 against 156.4 ms; profiles/r02_experiments.md).
+    // transposed copy.  The forward pass of such graphs keeps the register gathers with the arcs read from L2: its 8-byte
+    // slots would make 128-byte bulk copies, one per 16 rows.
     bool smem_arcs_eff = smem_arcs;
-    if (!tma && backward && pass.tq != nullptr && p.n_hubs == 0 && !g.tune_no_tma && rows < ((size_t)1 << 30) && p.Npad >= 32 &&
+    if (backward && !(smem_arcs && w1_smem) && pass.tq != nullptr && p.n_hubs == 0 && !g.tune_no_tma && rows < ((size_t)1 << 30) &&
         EncodeRowTensorMap(&p.tmap, table, rows, p.Npad, 32 * U)) {
         const int R = U == 4 ? TmaShape<4>::R : 16;
         const size_t ring_off = (fixed_smem + 127) & ~(size_t)127;
@@ -1536,15 +1514,15 @@ int Dispatch(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_sme
         const size_t arc_ring = (size_t)g.n_warps * kArcStages * (R / kQuad) * 3 * 16;
         const size_t total = aring_off + arc_ring;
         if (total <= budget) {
-            tma = true; ring_rows = R; smem_arcs_eff = false;
+            tma = true; smem_arcs_eff = false;
             p.use_tma = 1; p.ring_off = (int)ring_off; p.bar_off = (int)bar_off;
             p.abar_off = (int)abar_off; p.aring_off = (int)aring_off; p.tq = pass.tq;
             smem = total;
         }
     }
-    if (U == 1) return DispatchU<NT, 1>(backward, tma, ring_rows, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
-    if (U == 2) return DispatchU<NT, 2>(backward, tma, ring_rows, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
-    return DispatchU<NT, 4>(backward, tma, ring_rows, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
+    if (U == 1) return DispatchU<NT, 1>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
+    if (U == 2) return DispatchU<NT, 2>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
+    return DispatchU<NT, 4>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
 }
 
 int DispatchThreads(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_smem, cudaStream_t stream,

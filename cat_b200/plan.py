@@ -89,7 +89,7 @@ class PlanView:
         return bool((sign[:, 3] & sign[:, 2] & sign[:, 1]).any())
 
 
-def load_plan(path: str, n_ctas: int = 148, n_warps: int = 16) -> PlanView:
+def load_plan(path: str, n_ctas: int = 132, n_warps: int = 16) -> PlanView:
     L = _lib.lib()
     h = L.ccb_plan_create(path.encode(), n_ctas, n_warps)
     if not h:

@@ -1,5 +1,5 @@
 /*
- * ctc_crf_b200 -- C ABI of the B200-native CTC-CRF loss hot path (drop-in for thu-spmi/CAT src/ctc_crf).
+ * ctc_crf_b200 -- C ABI of the H100-native CTC-CRF loss hot path (drop-in for thu-spmi/CAT src/ctc_crf).
  *
  * Plain C, no torch types: pointers, sizes, a cudaStream_t passed as void*.  All device pointers must
  * belong to the CUDA device that is current when the call is made (the reference has the same contract,

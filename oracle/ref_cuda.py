@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE -- NOT PRODUCT CODE.
 
 Drives ``oracle/_ref/libctc_crf_ref.so`` -- the reference's own den_calculate.cu + ctc_entrypoint.cu compiled
-UNMODIFIED for sm_100a (oracle/Makefile) -- exactly the way the reference's binding.cpp:65-117 and
+UNMODIFIED for sm_90a (oracle/Makefile) -- exactly the way the reference's binding.cpp:65-117 and
 ctc_crf/__init__.py:58-90 drive it (same allocations, same call order, same post-processing), with torch
 tensors for memory.  This is the parity target named in BASELINE.json ("the reference's own CUDA ctc_crf").
 Needs a GPU; never imported by the product.
@@ -14,12 +14,11 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# "sm100fix": the reference sources with the two sm_70+ defects patched at build time (oracle/Makefile): the
-#             shfl.sync membermask in moderngpu's intrinsics and the non-volatile warp-synchronous reduction in
-#             alpha_lld_kernal.  "unmodified": the sources exactly as they are -- on B200 its CTC kernel traps
-#             (Illegal instruction) and its logZ/gradients are wrong (profiles/ref_unmodified_on_b200.txt).
-VARIANT = os.environ.get("CCB_REF_VARIANT", "sm100fix")
-_SO = os.path.join(_HERE, "_ref", "libctc_crf_ref.so" if VARIANT == "unmodified" else "libctc_crf_ref_sm100fix.so")
+# "patched": the reference sources with the two sm_70+ defects patched at build time (oracle/Makefile): the
+#            shfl.sync membermask in moderngpu's intrinsics and the non-volatile warp-synchronous reduction in
+#            alpha_lld_kernal.  "unmodified": the sources exactly as they are (see oracle/Makefile for what goes wrong).
+VARIANT = os.environ.get("CCB_REF_VARIANT", "patched")
+_SO = os.path.join(_HERE, "_ref", "libctc_crf_ref.so" if VARIANT == "unmodified" else "libctc_crf_ref_patched.so")
 _lib = None
 ATOMIC_CONST = 32   # binding.cpp:17-18
 
@@ -36,7 +35,7 @@ def lib():
     global _lib
     if _lib is None:
         if not available():
-            raise RuntimeError(f"{_SO} missing: run `make -C oracle ref` where /root/reference exists")
+            raise RuntimeError(f"{_SO} missing: run `make -C oracle ref` where the reference sources are present (oracle/Makefile REF)")
         L = C.CDLL(_SO)
         vp, ip = C.c_void_p, C.POINTER(C.c_int)
         L.Init.argtypes = [C.c_char_p, C.c_int, ip]; L.Init.restype = None

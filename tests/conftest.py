@@ -14,7 +14,7 @@ FIXTURE_FST = os.path.join(GOLDEN, "den_lm_fixture.fst")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100)")
 
 
 def pytest_collection_modifyitems(config, items):

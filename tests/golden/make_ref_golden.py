@@ -1,5 +1,5 @@
 """Records golden vectors from the REFERENCE'S OWN CUDA CODE (oracle/_ref: den_calculate.cu + ctc_entrypoint.cu
-compiled unmodified for sm_100a) on seeded inputs.  Needs a GPU:
+compiled unmodified for sm_90a) on seeded inputs.  Needs a GPU:
 
     gpurun -- 'python tests/golden/make_ref_golden.py'     # writes gpurun_out/ref_cuda_golden.npz
     cp gpurun_out/ref_cuda_golden.npz tests/golden/        # commit

@@ -60,7 +60,7 @@ def test_bad_files_raise_not_exit(tmp_path, fixture_fst, bad):
             fst.read_fst(str(p))
 
 
-@pytest.mark.parametrize("n_ctas,n_warps", [(1, 1), (4, 2), (148, 16), (148, 32)])
+@pytest.mark.parametrize("n_ctas,n_warps", [(1, 1), (4, 2), (132, 16), (132, 32), (148, 16), (148, 32)])
 def test_plan_invariants(tmp_graphs, n_ctas, n_warps):
     for name in ("tlm_small", "random_split", "tlm_mid"):
         path, g, V = tmp_graphs[name]
@@ -249,11 +249,11 @@ def test_plan_balance(tmp_path):
     g = fst.make_synthetic_den(4000, 24, 60, seed=7)
     p = str(tmp_path / "g.fst")
     fst.write_fst(p, g)
-    P = plan.load_plan(p, 148, 16)
+    P = plan.load_plan(p, 132, 16)
     for pv in (P.fwd, P.bwd):
         per_cta = np.diff(pv.chunk_arc[::16])
         assert per_cta.max() <= 1.3 * per_cta.mean() + 64
-        per_warp = np.diff(pv.chunk_arc).reshape(148, 16)
+        per_warp = np.diff(pv.chunk_arc).reshape(132, 16)
         assert (per_warp.max(1) - per_warp.min(1)).max() <= 48          # LPT: warps of a CTA within a few quads
     assert P.max_tile_arcs * 8 < 200 * 1024
 
@@ -263,7 +263,7 @@ def test_kernel_arithmetic_emulation_matches_oracle(tmp_graphs, name, lens):
     """The scaled-linear / hoisted-emission / state-product algorithm the kernels implement, emulated in numpy on
     the product's own plan arrays, equals the arc-based log-domain reference semantics."""
     path, g, V = tmp_graphs[name]
-    P = plan.load_plan(path, 148, 16)
+    P = plan.load_plan(path, 132, 16)
     y, _, lens, _ = oracle.synth_batch(len(lens), max(lens), V, seed=6, lens=lens)
     la, lb, gd = oracle.den(g, y, lens)
     ea, eb, eg = emulate.den_emulate(P, y, lens)
@@ -279,7 +279,7 @@ def test_hub_rows_split_into_parts(tmp_graphs, monkeypatch):
     monkeypatch.setenv("CCB_PART_ARCS", "7")
     for name in ("tlm_small", "random_split"):
         path, g, V = tmp_graphs[name]
-        P = plan.load_plan(path, 148, 16)
+        P = plan.load_plan(path, 132, 16)
         assert len(P.hub_states) > 0
         parts = [x for x in P.fwd.segments() if x[2] == plan.EV_PARTIAL]
         assert len(parts) > len(P.hub_states)                      # some rows have several parts
@@ -293,7 +293,7 @@ def test_hub_rows_split_into_parts(tmp_graphs, monkeypatch):
 
 
 def test_fixture_emulation(fixture_fst, fixture_inputs):
-    P = plan.load_plan(fixture_fst, 148, 16)
+    P = plan.load_plan(fixture_fst, 132, 16)
     ea, eb, eg = emulate.den_emulate(P, fixture_inputs["y"], fixture_inputs["lx"])
     assert abs(ea[0] + 6.25832785) < 1e-6 and abs(eb[0] + 6.25832785) < 1e-6
 

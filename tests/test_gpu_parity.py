@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box; reference CUDA = oracle/_ref sm100fix build, see oracle/Makefile): the CUDA path, called through the reference-facing surface
+"""GPU parity tests (run on the H100; reference CUDA = oracle/_ref patched build, see oracle/Makefile): the CUDA path, called through the reference-facing surface
 (ctc_crf.CTC_CRF_LOSS / _C.gpu_den / _C.gpu_ctc -> C ABI), against the fp64 oracle, the committed golden
 vectors, and the reference's own CUDA code (oracle/_ref) on the same seeded inputs.
 
@@ -114,7 +114,7 @@ def test_ctc_vs_oracle(N, T, V, lens, ly):
 
 
 @pytest.mark.parametrize("env", ["CCB_ARCS_IN_GLOBAL", "CCB_W1_IN_GLOBAL", "CCB_NO_PAIRS", "HUBS", "HUBS+CCB_ARCS_IN_GLOBAL",
-                                 "CCB_NO_TMA", "CCB_RING_ROWS=8", "CCB_ARCS_IN_GLOBAL+CCB_NO_TMA", "CCB_NO_MERGE", "CCB_NO_MERGE+CCB_NO_TMA",
+                                 "CCB_NO_TMA", "CCB_ARCS_IN_GLOBAL+CCB_NO_TMA", "CCB_NO_MERGE", "CCB_NO_MERGE+CCB_NO_TMA",
                                  "CCB_NO_OWN", "CCB_NO_OWN+CCB_NO_TMA"])
 def test_fallback_paths(tmp_graphs, monkeypatch, env):
     """Arc tiles streamed from global memory (graphs too large for shared memory: through per-warp bulk-copy rings next to
@@ -316,6 +316,19 @@ def test_sliced_batches_and_padded_frames(tmp_graphs, monkeypatch):
     _close_loss(loss, ref_loss, 1e-6)
     assert np.abs(grad - ref_grad).max() < 1e-6
     del ctx
+
+
+def test_vs_reference_cuda_golden():
+    """The CUDA path against the reference's own CUDA outputs recorded in tests/golden/ref_cuda_golden.npz
+    (tests/golden/make_ref_golden.py): needs nothing outside the repository."""
+    from conftest import GOLDEN
+    z = np.load(os.path.join(GOLDEN, "ref_cuda_golden.npz"), allow_pickle=False)
+    for c in sorted({k.split("/")[0] for k in z.files}):
+        ctx = _ctx(os.path.join(GOLDEN, str(z[f"{c}/graph"])))
+        loss, grad = _run_ours(z[f"{c}/y"], z[f"{c}/labels"], z[f"{c}/lx"], z[f"{c}/ly"], float(z[f"{c}/lamb"]))
+        _close_loss(loss, float(z[f"{c}/ref_loss"]))
+        assert np.abs(grad - z[f"{c}/ref_grad"]).max() < GRAD_ATOL, c
+        del ctx
 
 
 def test_vs_reference_cuda(tmp_path):

@@ -89,7 +89,7 @@ def test_assembly_matches_reference_formula(tmp_graphs):
 
 
 def test_against_reference_cuda_golden():
-    """Golden vectors produced by the reference's own CUDA code (oracle/_ref) on the B200 box with
+    """Golden vectors produced by the reference's own CUDA code (oracle/_ref) on the GPU with
     tests/golden/make_ref_golden.py: the oracle must reproduce the reference's outputs."""
     path = os.path.join(GOLDEN, "ref_cuda_golden.npz")
     if not os.path.exists(path):

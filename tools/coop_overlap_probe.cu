@@ -1,7 +1,7 @@
-// Probe: can two COOPERATIVE (persistent, grid-synchronising) kernels of 148 CTAs each be co-resident, one CTA of each per
+// Probe: can two COOPERATIVE (persistent, grid-synchronising) kernels of one CTA per SM each be co-resident, one CTA of each per
 // SM, when launched on two streams?  (Needed for running the forward and the backward recursion concurrently.)
 // Each kernel does `iters` rounds of {spin ~2 us, grid barrier}.  Prints the time of A alone, B alone, and A||B.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/coop_overlap_probe tools/coop_overlap_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/coop_overlap_probe tools/coop_overlap_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -5,7 +5,7 @@
 //   bulk   : ONE lane issues cp.async.bulk (TMA 1-D copy, mbarrier complete_tx) for the whole row, up to 32 rows per
 //            warp instruction; the warp then reads the ring with LDS.
 // Every variant consumes the data the way the recursion does (two FMAs per lane and row).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/l2_bulk_gather_bench tools/l2_bulk_gather_bench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/l2_bulk_gather_bench tools/l2_bulk_gather_bench.cu
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>

@@ -1,7 +1,7 @@
-// Micro-benchmark: L2 -> SM random ROW gather bandwidth on B200 (the resource that bounds the den kernels).
+// Micro-benchmark: L2 -> SM random ROW gather bandwidth on the GPU (the resource that bounds the den kernels).
 // A [rows][row_floats] fp32 table that fits L2 is gathered by random row index, one row per warp-load
 // (row_floats = 32*U floats, each lane loads a float{U} with ld.global.cg), B loads in flight per warp.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/l2_gather_bench tools/l2_gather_bench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/l2_gather_bench tools/l2_gather_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -62,7 +62,7 @@ int main() {
     run<1, 8>(rows, 512, 1, sms);  run<1, 16>(rows, 512, 1, sms); run<1, 16>(rows, 1024, 1, sms); run<1, 16>(rows, 1024, 2, sms);
     run<2, 8>(rows, 512, 1, sms);  run<2, 16>(rows, 512, 1, sms); run<2, 8>(rows, 1024, 1, sms);  run<2, 16>(rows, 1024, 1, sms); run<2, 16>(rows, 1024, 2, sms);
     run<4, 4>(rows, 512, 1, sms);  run<4, 8>(rows, 512, 1, sms);  run<4, 8>(rows, 1024, 1, sms);  run<4, 8>(rows, 1024, 2, sms);
-    run<2, 16>(400000, 1024, 2, sms);   // 100 MB table: mostly L2 still (126 MB)
+    run<2, 16>(400000, 1024, 2, sms);   // 100 MB table: twice the 50 MB L2 of an H100
     run<2, 16>(4000000, 1024, 2, sms);  // 1 GB table: HBM random rows
     return 0;
 }

@@ -1,6 +1,6 @@
 // Micro-benchmark 2: random ROW gathers from a table that every SM REWRITES between passes (the den recursion's
 // access pattern: rows produced by other SMs one frame earlier), versus a table written once (read-mostly).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/l2_pingpong_bench tools/l2_pingpong_bench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/l2_pingpong_bench tools/l2_pingpong_bench.cu
 #include <cstdio>
 #include <vector>
 #include <cuda_runtime.h>
@@ -38,7 +38,7 @@ __global__ void rewrite(float *tab, int rows, float val) {
 
 template <int U, int B>
 void run(int rows, int threads, int sms, bool pingpong) {
-    const int per_warp = 512;   // ~ one den frame per launch: 148*16*512 = 1.2M row gathers
+    const int per_warp = 512;   // ~ one den frame per launch: SMs x 16 warps x 512 row gathers
     const int warps = sms * threads / 32;
     float *tab, *out; unsigned *idx;
     cudaMalloc(&tab, (size_t)rows * 32 * U * 4); cudaMemset(tab, 0, (size_t)rows * 32 * U * 4);

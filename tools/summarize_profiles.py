@@ -3,7 +3,7 @@
 import collections, csv, json, os, subprocess, sys
 tag, launches, rep, bench = sys.argv[1:5]
 ref = sys.argv[5] if len(sys.argv) > 5 else None
-out = [f"# {tag}: ncu + bench summary (B200, sm_100a)\n"]
+out = [f"# {tag}: ncu + bench summary (H100, sm_90a)\n"]
 j = json.load(open(bench))
 out.append("## bench.py line (N=1)\n```json\n" + json.dumps(j, indent=1)[:6000] + "\n```\n")
 if ref and os.path.exists(ref):

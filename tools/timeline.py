@@ -17,7 +17,8 @@ y = torch.log_softmax(3 * torch.randn(N, T, V, device="cuda"), -1)
 lens = torch.full((N,), T, dtype=torch.int32, device="cuda")
 alpha = torch.empty(int(L.ccb_den_alpha_floats(N, T)), device="cuda"); aux = torch.empty(int(L.ccb_den_aux_bytes(N, T)), dtype=torch.uint8, device="cuda")
 grad = torch.zeros(N, T, V, device="cuda"); logz = torch.empty(N, device="cuda")
-n_chunks = 148 * int(os.environ.get("CCB_DEN_WARPS", "16")); steps, step0 = 16, T // 2
+n_ctas = torch.cuda.get_device_properties(0).multi_processor_count   # one CTA per SM (den_graph.cc)
+n_chunks = n_ctas * int(os.environ.get("CCB_DEN_WARPS", "16")); steps, step0 = 16, T // 2
 stream = torch.cuda.current_stream().cuda_stream
 def run():
     rc = L.ccb_den_forward_backward(y.data_ptr(), 0, T * V, V, N, T, V, lens.data_ptr(), alpha.data_ptr(), aux.data_ptr(), grad.data_ptr(), T * V, V, 1.0, logz.data_ptr(), None, stream)
@@ -40,6 +41,6 @@ for name, r in out.items():
     work = (r[:, :, 2] - r[:, :, 1]).astype(np.float64); total = (r[:, :, 3] - r[:, :, 1]).astype(np.float64)
     g0 = r[:, :, 0].astype(np.float64); step_ns = np.diff(g0.min(1))
     print(f"{name}: frame period {step_ns.mean()/1e3:.2f} us (globaltimer); per-warp work cycles mean {work.mean():.0f} p50 {np.median(work):.0f} p99 {np.percentile(work,99):.0f} max {work.max():.0f}; frame cycles mean {total.mean():.0f}")
-    cta = work.reshape(steps, 148, -1).max(2)
+    cta = work.reshape(steps, n_ctas, -1).max(2)
     print(f"   slowest warp per CTA: mean {cta.mean():.0f} max {cta.max():.0f} min {cta.min():.0f}; start skew across CTAs (ns) p50 {np.median(g0.max(1)-g0.min(1)):.0f}")
     print("   work/frame ratio mean %.2f ; (max work)/frame %.2f" % ((work/total).mean(), (work.max(1)/total.mean(1)).mean()))
