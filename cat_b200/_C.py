@@ -12,6 +12,7 @@ Addition: ``ctc_crf_loss_fwd`` -- the fused, synchronisation-free entry used by 
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional, Tuple
 
 import torch
@@ -199,27 +200,62 @@ def _scratch_budget(dev, need: int = 0) -> int:
     return budget
 
 
+CKPT_WIDTH = 32                  # a slice whose alpha spill does not fit is halved while it is wider than this (and halving
+                                 # shrinks its lane padding); at or below it, it runs with checkpointed alpha instead
+                                 # (DESIGN.md "Checkpointed α": on an H100, config 4's graph, T=2000, one checkpointed slice
+                                 # of 64 took 0.90 s against 0.87 s for two full-spill halves; of 32, 0.61 s against 0.80 s)
+_ckpt_k_override = None          # test hook: run every slice checkpointed with this interval K
+
+
+def ckpt_interval(tmax: int) -> int:
+    """Checkpoint interval of a slice walking `tmax` frames: ceil(sqrt(tmax)), which about minimises checkpoints + segment."""
+    return max(1, math.isqrt(max(1, tmax) - 1) + 1)
+
+
+def _slice_need(L, n, tmax, maxl, k):
+    alpha = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
+    return int(alpha) * 4 + int(L.ccb_den_aux_bytes(n, tmax)) + int(L.ccb_ctc_workspace_bytes(n, tmax, maxl))
+
+
 def _plan_slices(L, lx, ly, N, V, dev):
     """Split the batch into contiguous slices whose scratch (alpha spill etc.) fits the free device memory.
-    Each slice walks only max(lx[slice]) frames."""
+    Each slice walks only max(lx[slice]) frames.  Returns (n0, n1, tmax, maxl, K) per slice; K = 0 keeps every alpha
+    frame, K > 0 keeps every K-th and recomputes the rest in the backward pass.
+    A slice whose full alpha spill does not fit is halved while it is wider than CKPT_WIDTH and halving shrinks its lane
+    padding (the spill is proportional to the padding); otherwise it runs checkpointed with K = ceil(sqrt(tmax)), and is
+    halved further only if that does not fit either."""
     budget = _scratch_budget(dev)
     slices, n0 = [], 0
     while n0 < N:
         n1 = min(N, n0 + MAX_UTTS_PER_CALL)
         while True:
+            n = n1 - n0
+            half = max(1, n // 2)
             tmax = max(1, int(lx[n0:n1].max()))
             maxl = int(ly[n0:n1].max())
-            need = (int(L.ccb_den_alpha_floats(n1 - n0, tmax)) * 4 + int(L.ccb_den_aux_bytes(n1 - n0, tmax))
-                    + int(L.ccb_ctc_workspace_bytes(n1 - n0, tmax, maxl)))
+            k = 0 if _ckpt_k_override is None else int(_ckpt_k_override)
+            need = _slice_need(L, n, tmax, maxl, k)
             if need > budget:
                 budget = _scratch_budget(dev, need)     # a stale (cached) figure must not split a batch needlessly
-            if need <= budget or n1 - n0 == 1:
+            if need <= budget:
                 break
-            n1 = n0 + max(1, (n1 - n0) // 2)
-        if need > budget:
-            raise RuntimeError(f"CTC-CRF scratch for a single utterance of {tmax} frames needs {need >> 20} MiB, "
-                               f"only {budget >> 20} MiB free")
-        slices.append((n0, n1, tmax, maxl))
+            full = need
+            if k == 0 and n > CKPT_WIDTH and int(L.ccb_den_alpha_floats(half, tmax)) < int(L.ccb_den_alpha_floats(n, tmax)):
+                n1 = n0 + half
+                continue
+            if k == 0:
+                k = ckpt_interval(tmax)
+                need = _slice_need(L, n, tmax, maxl, k)
+                if need > budget:
+                    budget = _scratch_budget(dev, need)
+                if need <= budget:
+                    break
+            if n == 1:
+                raise RuntimeError(f"CTC-CRF scratch for a single utterance of {tmax} frames needs {full >> 20} MiB with every "
+                                   f"alpha frame kept and {need >> 20} MiB checkpointed every {k} frames, "
+                                   f"only {budget >> 20} MiB free")
+            n1 = n0 + half
+        slices.append((n0, n1, tmax, maxl, k))
         n0 = n1
     return slices
 
@@ -234,6 +270,7 @@ def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tenso
     (grad = d loss / d raw logits), replacing cat/ctc/train.py:173-174."""
     L = _lib.lib()
     entry = L.ccb_ctc_crf_loss_logits_fwd if from_logits else L.ccb_ctc_crf_loss_fwd
+    ckpt_entry = L.ccb_ctc_crf_loss_logits_ckpt_fwd if from_logits else L.ccb_ctc_crf_loss_ckpt_fwd
     assert logits.is_cuda and logits.dim() == 3 and logits.is_contiguous()
     if logits.dtype not in _DTYPES:
         raise RuntimeError(f"unsupported logits dtype {logits.dtype}")
@@ -253,17 +290,22 @@ def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tenso
         def run_slices():
             slices = _plan_slices(L, lx, ly, N, V, dev)
             losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
-            for i, (n0, n1, tmax, maxl) in enumerate(slices):
+            for i, (n0, n1, tmax, maxl, k) in enumerate(slices):
                 n = n1 - n0
-                alpha_ws = torch.empty(int(L.ccb_den_alpha_floats(n, tmax)), dtype=torch.float32, device=dev)
+                alpha_floats = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
+                alpha_ws = torch.empty(int(alpha_floats), dtype=torch.float32, device=dev)
                 aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
                 ctc_ws = torch.empty(int(L.ccb_ctc_workspace_bytes(n, tmax, maxl)), dtype=torch.uint8, device=dev)
                 sub_parts = torch.empty(2 * n, dtype=torch.float32, device=dev) if want_parts else None
-                rc = entry(logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype], n, T, V, tmax,
-                           p_labels, p_off + 4 * n0, p_ly + 4 * n0, p_lx + 4 * n0, maxl, float(lamb),
-                           float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(), ctc_ws.data_ptr(),
-                           grad.data_ptr() + n0 * T * V * 4, losses.data_ptr() + 4 * i,
-                           sub_parts.data_ptr() if want_parts else None, stream)
+                args = (p_labels, p_off + 4 * n0, p_ly + 4 * n0, p_lx + 4 * n0, maxl, float(lamb),
+                        float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(), ctc_ws.data_ptr(),
+                        grad.data_ptr() + n0 * T * V * 4, losses.data_ptr() + 4 * i,
+                        sub_parts.data_ptr() if want_parts else None, stream)
+                y_ptr = logits.data_ptr() + n0 * T * V * esz
+                if k:
+                    rc = ckpt_entry(y_ptr, _DTYPES[logits.dtype], n, T, V, tmax, k, *args)
+                else:
+                    rc = entry(y_ptr, _DTYPES[logits.dtype], n, T, V, tmax, *args)
                 _check(rc, "ctc_crf_loss_fwd")
                 if want_parts:
                     parts[n0:n1] = sub_parts[:n]

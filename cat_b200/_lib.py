@@ -24,6 +24,7 @@ SYMBOLS = [
     "ccb_ctc_workspace_bytes", "ccb_den_forward_backward", "ccb_ctc_forward_backward", "ccb_ctc_crf_loss_fwd",
     "ccb_ctc_crf_loss_logits_fwd", "ccb_ctc_loss_fwd", "ccb_ctc_align_workspace_bytes", "ccb_ctc_align",
     "ccb_launch_count", "ccb_debug_timeline", "ccb_plan_create", "ccb_plan_destroy", "ccb_plan_info", "ccb_plan_copy",
+    "ccb_den_ckpt_alpha_floats", "ccb_ctc_crf_loss_ckpt_fwd", "ccb_ctc_crf_loss_logits_ckpt_fwd",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -66,6 +67,12 @@ def lib() -> C.CDLL:
     L.ccb_ctc_crf_loss_fwd.restype = C.c_int
     L.ccb_ctc_crf_loss_logits_fwd.argtypes = L.ccb_ctc_crf_loss_fwd.argtypes
     L.ccb_ctc_crf_loss_logits_fwd.restype = C.c_int
+    L.ccb_den_ckpt_alpha_floats.argtypes = [C.c_int, C.c_int, C.c_int]; L.ccb_den_ckpt_alpha_floats.restype = C.c_size_t
+    L.ccb_ctc_crf_loss_ckpt_fwd.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int,
+                                            C.c_float, C.c_float, vp, vp, vp, vp, vp, vp, vp]
+    L.ccb_ctc_crf_loss_ckpt_fwd.restype = C.c_int
+    L.ccb_ctc_crf_loss_logits_ckpt_fwd.argtypes = L.ccb_ctc_crf_loss_ckpt_fwd.argtypes
+    L.ccb_ctc_crf_loss_logits_ckpt_fwd.restype = C.c_int
     L.ccb_ctc_loss_fwd.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,
                                    C.c_float, vp, vp, vp, vp, vp]
     L.ccb_ctc_loss_fwd.restype = C.c_int

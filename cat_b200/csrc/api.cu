@@ -263,6 +263,8 @@ DenParams BaseParams(const DeviceGraph &g, const void *y, int dtype, long sn, lo
     p.y = y; p.y_bf16 = (dtype == CCB_DTYPE_BF16); p.sn = sn; p.st = st;
     p.N = N; p.Npad = L.Npad; p.Tmax = T; p.V = V; p.len = len;
     p.alpha = alpha;
+    p.a_frames = T + 1 + (g.P > 0 ? 2 : 0);   // full spill (a_base = a_ring = 0: frame t at position t)
+    p.t_lo = 0; p.t_hi = T;
     p.bh = reinterpret_cast<float *>(a + L.bh);
     p.colsum_a = reinterpret_cast<float *>(a + L.colsum_a);
     p.colsum_b = reinterpret_cast<float *>(a + L.colsum_b);
@@ -287,10 +289,20 @@ int CheckDen(const DeviceGraph &g, int dtype, int N, int T, int V) {
     return 0;
 }
 
+// Checkpointed alpha (ckpt_k = K > 0): the workspace holds CkptSegFrames positions (the first pass's ring, later one
+// segment of frames), then CkptCount checkpoint frames, then the backward pass's carried log-scales (Npad doubles).
+void SetCkpt(DenParams &p, const DeviceGraph &g, int T, int K) {
+    const size_t frame = (size_t)g.S * p.Npad;
+    p.ckpt_k = CkptK(T, K);
+    p.ckpt = p.alpha + (size_t)CkptSegFrames(T, K) * frame;
+    p.runlog_b = reinterpret_cast<double *>(p.ckpt + (size_t)CkptCount(T, K) * frame);
+}
+
 // forward part: zero aux, frame max, alpha recursion; logz_a lands in aux
 // raw: `y` holds unnormalised logits; the log-normalisers go to aux (lz, lnorm) and logZ comes out normalised
+// ckpt_k > 0: alpha on a ring of kAlphaRing frames, checkpoints every ckpt_k frames (see SetCkpt)
 int DenForward(const DeviceGraph &g, const void *y, int dtype, long sn, long st, int N, int T, int V, const int *len,
-               float *alpha, void *aux, cudaStream_t stream, bool raw = false) {
+               float *alpha, void *aux, cudaStream_t stream, bool raw = false, int ckpt_k = 0) {
     const DenAuxLayout L = MakeDenAuxLayout(g.S, N, T, g.small_ok);
     char *a = reinterpret_cast<char *>(aux);
     CCB_CUDA(cudaMemsetAsync(a, 0, L.zero_bytes, stream));
@@ -302,15 +314,21 @@ int DenForward(const DeviceGraph &g, const void *y, int dtype, long sn, long st,
     if (raw) p.lnorm = reinterpret_cast<const double *>(a + L.lnorm);
     p.barrier = reinterpret_cast<unsigned *>(a + L.barrier);
     p.logz = reinterpret_cast<float *>(a + L.logz_a);
+    if (ckpt_k > 0) {
+        SetCkpt(p, g, T, ckpt_k);
+        p.ckpt_mode = 1; p.a_ring = kAlphaRing; p.a_frames = kAlphaRing + 2;
+    }
     std::string err;
     rc = LaunchDenForward(g, p, stream, &err);
     if (rc) return Fail(err);
     return 0;
 }
 
+// backward part (beta recursion, occupancies, logz_b).  ckpt_k > 0: one segment of ckpt_k frames at a time, from the last
+// to the first, each first recomputed from its checkpoint into the segment positions by a forward launch.
 int DenBackward(const DeviceGraph &g, const void *y, int dtype, long sn, long st, int N, int T, int V, const int *len,
                 float *alpha, void *aux, float *grad, long gsn, long gst, float grad_scale, cudaStream_t stream,
-                bool raw = false) {
+                bool raw = false, int ckpt_k = 0) {
     const DenAuxLayout L = MakeDenAuxLayout(g.S, N, T, g.small_ok);
     char *a = reinterpret_cast<char *>(aux);
     DenParams p = BaseParams(g, y, dtype, sn, st, N, T, V, len, alpha, aux, L);
@@ -322,10 +340,31 @@ int DenBackward(const DeviceGraph &g, const void *y, int dtype, long sn, long st
     // backward pass over the same forward pass (or a reused aux buffer) starts clean instead of relying on DenForward's memset
     CCB_CUDA(cudaMemsetAsync(a + L.colsum_b, 0, L.zsum - L.colsum_b, stream));
     CCB_CUDA(cudaMemsetAsync(a + L.b0, 0, (size_t)L.Npad * 4, stream));
-    CCB_CUDA(cudaMemsetAsync(a + L.barrier + 128, 0, 128, stream));
     std::string err;
-    int rc = LaunchDenBackward(g, p, stream, &err);
-    if (rc) return Fail(err);
+    int rc = 0;
+    if (ckpt_k <= 0) {
+        CCB_CUDA(cudaMemsetAsync(a + L.barrier + 128, 0, 128, stream));
+        rc = LaunchDenBackward(g, p, stream, &err);
+        if (rc) return Fail(err);
+    } else {
+        SetCkpt(p, g, T, ckpt_k);
+        const int K = p.ckpt_k;
+        for (int j = CkptCount(T, ckpt_k) - 1; j >= 0; --j) {
+            const int lo = j * K, hi = std::min(lo + K, T);
+            DenParams f = BaseParams(g, y, dtype, sn, st, N, T, V, len, alpha, aux, L);   // recompute frames (lo, hi]
+            SetCkpt(f, g, T, ckpt_k);
+            f.ckpt_mode = 2; f.a_base = lo; f.a_frames = CkptSegFrames(T, ckpt_k);
+            f.t_lo = lo; f.t_hi = hi;
+            f.barrier = reinterpret_cast<unsigned *>(a + L.barrier);
+            CCB_CUDA(cudaMemsetAsync(a + L.barrier, 0, 128, stream));
+            rc = LaunchDenForward(g, f, stream, &err);
+            if (rc) return Fail(err);
+            p.a_base = lo; p.t_lo = lo; p.t_hi = hi;   // tau = hi .. lo + 1 (tau = 0 epilogue with the first segment)
+            CCB_CUDA(cudaMemsetAsync(a + L.barrier + 128, 0, 128, stream));
+            rc = LaunchDenBackward(g, p, stream, &err);
+            if (rc) return Fail(err);
+        }
+    }
     rc = LaunchDenGradNormalize(grad, gsn, gst, p.absum, len, N, L.Npad, T, V, grad_scale, stream);
     if (rc) return FailCuda("den_grad_normalize", (cudaError_t)rc);
     return 0;
@@ -408,6 +447,16 @@ size_t ccb_den_alpha_floats(int N, int T) {
     // T+1 frames of S real rows; the virtual pair-sum rows of a frame are parked two frames ahead (den_kernels.cu), so two
     // more frames at the end when the plan has pairs
     return (size_t)(T + 1 + (P > 0 ? 2 : 0)) * (size_t)S * (size_t)PadLanes(N, small_ok);
+}
+
+size_t ccb_den_ckpt_alpha_floats(int N, int T, int K) {
+    if (K <= 0 || T <= 0) return ccb_den_alpha_floats(N, T);
+    int S, P;
+    bool small_ok;
+    CurrentSizes(&S, &P, &small_ok);
+    // segment / ring positions + checkpoints of S real rows each, then Npad doubles of carried log-scales
+    const size_t npad = (size_t)PadLanes(N, small_ok);
+    return ((size_t)CkptSegFrames(T, K) + (size_t)CkptCount(T, K)) * (size_t)S * npad + 2 * npad;
 }
 
 size_t ccb_den_aux_bytes(int N, int T) {
@@ -556,7 +605,7 @@ int ccb_ctc_align(const void *logits, int dtype, long sn, long st, int N, int T,
     return 0;
 }
 
-static int LossFwdImpl(bool raw, const void *logits, int dtype, int N, int T, int V, int Tmax,
+static int LossFwdImpl(bool raw, const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k,
                        const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
                        const int *len_dev, int max_label_len, float lamb, float scale,
                        float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
@@ -565,6 +614,7 @@ static int LossFwdImpl(bool raw, const void *logits, int dtype, int N, int T, in
     DeviceGraph *g;
     if (CurrentGraph(&g)) return 1;
     if (Tmax <= 0 || Tmax > T) return Fail("ctc_crf_loss_fwd: Tmax must lie in [1, T]");
+    if (ckpt_k < 0) return Fail("ctc_crf_loss_fwd: checkpoint interval must be >= 0");
     if (CheckDen(*g, dtype, N, Tmax, V)) return 1;
     if (!alpha_ws || !aux_ws || !ctc_ws || !grad || !loss) return Fail("ctc_crf_loss_fwd: missing buffer");
     cudaStream_t s = (cudaStream_t)stream;
@@ -602,10 +652,10 @@ static int LossFwdImpl(bool raw, const void *logits, int dtype, int N, int T, in
     }
     CCB_CUDA(cudaMemsetAsync(grad, 0, sizeof(float) * (size_t)N * T * V, s));
     if (sd && sd->trace) cudaEventRecord(sd->tr[3], s);
-    if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw)) rc = 1;
+    if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw, ckpt_k)) rc = 1;
     if (sd && sd->trace) cudaEventRecord(sd->tr[4], s);
     if (sd && sd->order != 0 && side_numerator()) return 1;
-    if (!rc && DenBackward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, grad, sn, st, scale, s, raw)) rc = 1;
+    if (!rc && DenBackward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, grad, sn, st, scale, s, raw, ckpt_k)) rc = 1;
     if (sd && sd->trace) {
         cudaEventRecord(sd->tr[5], s);
         cudaDeviceSynchronize();
@@ -648,7 +698,7 @@ int ccb_ctc_crf_loss_fwd(const void *logits, int dtype, int N, int T, int V, int
                          const int *len_dev, int max_label_len, float lamb, float scale,
                          float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
                          void *stream) {
-    return LossFwdImpl(false, logits, dtype, N, T, V, Tmax, labels_dev, label_off_dev, label_len_dev, len_dev, max_label_len,
+    return LossFwdImpl(false, logits, dtype, N, T, V, Tmax, 0, labels_dev, label_off_dev, label_len_dev, len_dev, max_label_len,
                        lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
 }
 
@@ -657,8 +707,26 @@ int ccb_ctc_crf_loss_logits_fwd(const void *logits, int dtype, int N, int T, int
                                 const int *len_dev, int max_label_len, float lamb, float scale,
                                 float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
                                 void *stream) {
-    return LossFwdImpl(true, logits, dtype, N, T, V, Tmax, labels_dev, label_off_dev, label_len_dev, len_dev, max_label_len,
+    return LossFwdImpl(true, logits, dtype, N, T, V, Tmax, 0, labels_dev, label_off_dev, label_len_dev, len_dev, max_label_len,
                        lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
+}
+
+int ccb_ctc_crf_loss_ckpt_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k,
+                              const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                              const int *len_dev, int max_label_len, float lamb, float scale,
+                              float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
+                              void *stream) {
+    return LossFwdImpl(false, logits, dtype, N, T, V, Tmax, ckpt_k, labels_dev, label_off_dev, label_len_dev, len_dev,
+                       max_label_len, lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
+}
+
+int ccb_ctc_crf_loss_logits_ckpt_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k,
+                                     const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                                     const int *len_dev, int max_label_len, float lamb, float scale,
+                                     float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
+                                     void *stream) {
+    return LossFwdImpl(true, logits, dtype, N, T, V, Tmax, ckpt_k, labels_dev, label_off_dev, label_len_dev, len_dev,
+                       max_label_len, lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
 }
 
 /* ---- gpu_ctc/ctc.h surface ------------------------------------------------------------------- */

@@ -97,6 +97,16 @@ struct alignas(64) DenParams {
     const int *len;       // [N] device
     // workspaces
     float *alpha;         // [(Tmax+3)][S][Npad] scaled-linear alpha spill; the pair-sum rows of frame t are parked in frame t+2
+    // Frame addressing of `alpha` (den_kernels.cu alpha_pos): frame t sits at position t - a_base, modulo a_ring when
+    // a_ring > 0.  The full spill is a_base = a_ring = 0, the identity.  a_frames = positions the buffer holds.
+    int a_base, a_ring, a_frames;
+    // Checkpointed denominator (DESIGN.md "Checkpointed alpha"): ckpt_mode 0 = full spill; 1 = first forward pass on a
+    // ring, storing the real rows of every ckpt_k-th frame in `ckpt` and logZ frame by frame; 2 = recompute of the frames
+    // (t_lo, t_hi] from the checkpoint of frame t_lo, reading colsum_a and writing no logZ
+    int ckpt_mode, ckpt_k;
+    float *ckpt;          // [ceil(Tmax/ckpt_k)][S][Npad] real rows of frames 0, K, 2K, ...
+    int t_lo, t_hi;       // frames (t_lo, t_hi] walked by this launch (one launch per pass: 0, Tmax)
+    double *runlog_b;     // [Npad] backward log-scale books carried from one segment launch to the next
     float *bh;            // [2][S][Npad]          backward ping-pong (emission-weighted beta)
     float *colsum_a;      // [(Tmax+2)][Npad]
     float *colsum_b;      // [(Tmax+2)][Npad]
@@ -146,6 +156,12 @@ int LaunchFrameLse(const void *y, int y_bf16, long sn, long st, int N, int T, in
                    float *lz, double *lnorm, int Npad, cudaStream_t stream);
 int LaunchLogitGrad(const void *z, int z_bf16, long sn, long st, int N, int T, int V, const int *len, const float *lz,
                     int Npad, float *grad, long gsn, long gst, cudaStream_t stream);
+// Checkpointed alpha workspace for K = ckpt_k (0: the full spill): frame positions of the first pass's ring / of one
+// segment, then the checkpoints, then the backward pass's carried log-scales (see den_kernels.cu alpha_pos)
+constexpr int kAlphaRing = 4;
+inline int CkptK(int T, int K) { return K < T ? K : T; }
+inline int CkptSegFrames(int T, int K) { const int k = CkptK(T, K); return (k + 1 > kAlphaRing ? k + 1 : kAlphaRing) + 2; }
+inline int CkptCount(int T, int K) { const int k = CkptK(T, K); return (T + k - 1) / k; }
 int LaunchDenForward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err);
 int LaunchDenBackward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err);
 // fills *tm with the 2-D view [rows][Npad] fp32 of `base`, box = 1 row x box_cols columns; false if the driver entry

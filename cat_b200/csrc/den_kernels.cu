@@ -656,6 +656,45 @@ __device__ __noinline__ void forward_partial_row(const int *state_label, const i
     }
 }
 
+// Position of alpha frame t in DenParams::alpha.  Full spill: t.  Recompute of a segment: t - a_base (frames a_base ..
+// a_base + K, plus two for the parked rows of the last ones).  First checkpointed pass: t mod a_ring on a ring of
+// a_ring = kAlphaRing positions followed by 2 slack positions.  The layout stays relative to the frame: frame t's pair-sum
+// rows are parked at row 2S + j of ITS base, i.e. in position p + 2 (p = its position, so the slack when p >= a_ring - 2),
+// and frame t's hub rows are zeroed during frame t - 1.  While frame t is computed the live positions are p(t-1) with its
+// parked rows at p(t-1) + 2 (read), p(t) and p(t) + 2 (written) and p(t+1) (hub rows zeroed); four ring positions keep
+// the writes off everything frame t reads (three would land frame t's parked rows on frame t-1 when p(t) = 0), and a
+// position is rewritten a_ring frames later, after every reader of it has passed a grid barrier.
+__device__ __forceinline__ int alpha_pos(const DenParams &P, int t) {
+    const int p = t - P.a_base;
+    return P.a_ring > 0 ? p % P.a_ring : p;
+}
+
+// First checkpointed pass, once frame t is complete (after its grid barrier): keep a copy of its real rows if it is a
+// checkpoint, and add sum_q final(q) alpha_t(q, n) to zsum for the utterances that end at frame t (their frame is gone
+// from the ring by the end of the pass).  (Inlined: a call in the frame loop would save its live registers around it.)
+__device__ __forceinline__ void ckpt_frame_done(const DenParams &P, int t, const float *fr, int sb, int se, int lane) {
+    const size_t frame_elems = (size_t)P.S * P.Npad;
+    if (t % P.ckpt_k == 0 && t < P.Tmax) {   // (S * Npad is a multiple of 16 floats)
+        const float4 *src = reinterpret_cast<const float4 *>(fr);
+        float4 *dst = reinterpret_cast<float4 *>(P.ckpt + (size_t)(t / P.ckpt_k) * frame_elems);
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < frame_elems / 4; i += (size_t)gridDim.x * blockDim.x)
+            __stcg(dst + i, __ldcg(src + i));
+    }
+    for (int gc = 0; gc < (P.Npad + 31) / 32; ++gc) {
+        const int n = gc * 32 + lane;
+        const bool ends = n < P.N && __ldg(P.len + n) == t;
+        if (!__any_sync(kFull, ends)) continue;
+        float zs = 0.f;
+        if (ends) {
+            for (int q = sb; q < se; ++q) {
+                const float f = __ldg(P.final_lin + q);
+                if (f != 0.f) zs = fmaf(f, __ldcg(fr + (size_t)q * P.Npad + n), zs);
+            }
+        }
+        if (zs != 0.f) atomicAdd(P.zsum + n, zs);
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // forward: alpha recursion + logZ
 // ------------------------------------------------------------------------------------------------
@@ -740,27 +779,31 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
     }
     for (int i = tid; i < Npad; i += NT) s_sum[i] = 0.f;
 
-    // t = 0: alpha_0 = indicator(start) (virtual rows: the pair sum); column sum 1
-    for (int q = sb; q < se; ++q)
-        for (int n = lane; n < Npad; n += 32) __stcg(P.alpha + (size_t)q * Npad + n, q == P.start ? 1.f : 0.f);
+    // t = 0: alpha_0 = indicator(start) (virtual rows: the pair sum); column sum 1.  Recompute of a segment: frame t_lo is
+    // its checkpoint's real rows, and its pair-sum rows are rebuilt from them (the same fp32 sum the frame's row ends formed)
     {
+        const bool recompute = P.ckpt_mode == 2;
+        const float *src = recompute ? P.ckpt + (size_t)(P.t_lo / P.ckpt_k) * frame_elems : nullptr;
+        float *a0 = P.alpha + (size_t)alpha_pos(P, P.t_lo) * frame_elems;
+        auto first = [&](int q, int n) { return recompute ? __ldcg(src + (size_t)q * Npad + n) : (q == P.start ? 1.f : 0.f); };
+        for (int q = sb; q < se; ++q)
+            for (int n = lane; n < Npad; n += 32) __stcg(a0 + (size_t)q * Npad + n, first(q, n));
         int vj = vj0;
         for (int q = sb; q < se; ++q) {
             if (__ldg(P.state_pos + q) == 0) {   // q, q+1 are a pair
-                const float v = (q == P.start || q + 1 == P.start) ? 1.f : 0.f;
-                for (int n = lane; n < Npad; n += 32) __stcg(P.alpha + (size_t)(virt0 + vj) * Npad + n, v);
+                for (int n = lane; n < Npad; n += 32) __stcg(a0 + (size_t)(virt0 + vj) * Npad + n, first(q, n) + first(q + 1, n));
                 ++vj;
             }
         }
+        if (cta == 0 && !recompute) for (int n = tid; n < Npad; n += NT) __stcg(P.colsum_a + n, 1.f);
     }
-    if (cta == 0) for (int n = tid; n < Npad; n += NT) __stcg(P.colsum_a + n, 1.f);
     // rows of high in-degree states are accumulated with atomics from several parts: zero them one frame ahead
     auto zero_hub_rows = [&](int frame) {
-        float *fr = P.alpha + (size_t)frame * frame_elems;
+        float *fr = P.alpha + (size_t)alpha_pos(P, frame) * frame_elems;
         for (int i = cta * NT + tid; i < P.n_hubs * Npad; i += gridDim.x * NT)
             __stcg(fr + (size_t)__ldg(P.hub_states + i / Npad) * Npad + (i % Npad), 0.f);
     };
-    if (HUBS && P.Tmax >= 1) zero_hub_rows(1);
+    if (HUBS && P.t_lo < P.t_hi) zero_hub_rows(P.t_lo + 1);
     const int my_len = (cta == 0 && tid < P.N) ? __ldg(P.len + tid) : 0;   // CTA 0 keeps log-scale books
     int len0[U];   // lengths of this lane's utterances in lane group 0 (the only group for N <= 32*U)
 #pragma unroll
@@ -768,12 +811,14 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
     double runlog = 0.0;
     if (TMA) fence_proxy_async_global();
     grid_barrier(P.barrier, (++epoch) * gridDim.x);
+    if (P.ckpt_mode == 1) ckpt_frame_done(P, 0, P.alpha, sb, se, lane);
 
-    for (int t = 1; t <= P.Tmax; ++t) {
+    for (int t = P.t_lo + 1; t <= P.t_hi; ++t) {
         tl_mark(P, t, chunk, n_chunks, 0, lane);
         if (TMA) fence_proxy_async_global();
-        const float *a_prev = P.alpha + (size_t)(t - 1) * frame_elems;
-        float *a_cur = P.alpha + (size_t)t * frame_elems;
+        const int p_prev = alpha_pos(P, t - 1);
+        const float *a_prev = P.alpha + (size_t)p_prev * frame_elems;
+        float *a_cur = P.alpha + (size_t)alpha_pos(P, t) * frame_elems;
         for (int gc = 0; gc < (LPR == 32 ? Npad / (32 * U) : 1); ++gc) {
             const int n0 = gc * 32 * U + ul * U;
             bool act[U];
@@ -914,7 +959,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
             };
             if (TMA && LPR < 32) {
                 float acc[1] = {0.f};
-                walk_arcs_tma_small<LPR, 2>(arc4, n_batches, P.alpha, (t - 1) * S, ring, lane, frame_scalars,
+                walk_arcs_tma_small<LPR, 2>(arc4, n_batches, P.alpha, p_prev * S, ring, lane, frame_scalars,
                                             [&](const uint4 *quad, const float *v, uint32_t) {
                     const uint4 wq = quad[1];
                     constexpr int STEPS = LPR / 8, SUBS = 32 / LPR;
@@ -972,12 +1017,12 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
                 if (act[u] && sub == 0 && sum[u] != 0.f) atomicAdd(&s_sum[n0 + u], sum[u]);
         }
         tl_mark(P, t, chunk, n_chunks, 1, lane);
-        if (HUBS && t < P.Tmax) zero_hub_rows(t + 1);
+        if (HUBS && t < P.t_hi) zero_hub_rows(t + 1);
         if (TMA) fence_proxy_async_global();   // this frame's rows are read through the async proxy after the barrier
         __syncthreads();
-        for (int i = tid; i < Npad; i += NT) {
+        for (int i = tid; i < Npad; i += NT) {   // (a recompute reads the first pass's column sums, it does not add to them)
             const float v = s_sum[i];
-            if (v != 0.f) { atomicAdd(P.colsum_a + (size_t)t * Npad + i, v); s_sum[i] = 0.f; }
+            if (v != 0.f) { if (P.ckpt_mode != 2) atomicAdd(P.colsum_a + (size_t)t * Npad + i, v); s_sum[i] = 0.f; }
         }
         // arrive first, then the log-scale books of CTA 0 (two L2 round trips nobody waits for) in the barrier's shadow
         const bool split_barrier = !CCB_DBG(P, 2) && !CCB_DBG(P, 8);
@@ -991,10 +1036,14 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
         else if (!CCB_DBG(P, 2)) grid_barrier(P.barrier, (++epoch) * gridDim.x);
         else __syncthreads();
         tl_mark(P, t, chunk, n_chunks, 2, lane);
+        // (frame t's position is rewritten kAlphaRing frames later)
+        if (P.ckpt_mode == 1) ckpt_frame_done(P, t, P.alpha + (size_t)alpha_pos(P, t) * frame_elems, sb, se, lane);
     }
+    if (P.ckpt_mode == 2) return;   // a recompute only refills the segment's frames
 
     // logZ[n] = log sum_q alpha_len(q) final(q) + accumulated log scale      (den_calculate.cu:105-161)
-    for (int gc = 0; gc < (Npad + 31) / 32; ++gc) {
+    // (first checkpointed pass: already summed into zsum frame by frame, ckpt_frame_done)
+    for (int gc = 0; gc < (P.ckpt_mode == 0 ? (Npad + 31) / 32 : 0); ++gc) {
         const int n = gc * 32 + lane;
         const int ln = (n < P.N) ? __ldg(P.len + n) : -1;
         float zs = 0.f;
@@ -1114,14 +1163,18 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
 #pragma unroll
     for (int u = 0; u < U; ++u) len0[u] = (ul * U + u < P.N) ? __ldg(P.len + ul * U + u) : 0;
     double runlog = 0.0;
+    // segmented backward pass (checkpointed alpha): beta-hat, colsum_b and absum carry over in global memory, the
+    // log-scale books through runlog_b
+    if (P.t_hi < P.Tmax && cta == 0 && tid < P.N) runlog = P.runlog_b[tid];
     __syncthreads();
 
-    for (int tau = P.Tmax; tau >= 1; --tau) {
+    for (int tau = P.t_hi; tau > P.t_lo; --tau) {
         tl_mark(P, P.Tmax - tau, chunk, n_chunks, 0, lane);
         if (TMA) fence_proxy_async_global();
         const float *bh_next = P.bh + (size_t)((tau + 1) & 1) * frame_elems;
         float *bh_cur = P.bh + (size_t)(tau & 1) * frame_elems;
-        const float *a_row = P.alpha + (size_t)tau * alpha_frame;
+        // alpha_pos without the ring (a_ring = 0 for every backward launch): frame tau - 1 is the position before frame tau
+        const float *a_row = P.alpha + (size_t)(tau - P.a_base) * alpha_frame;
         if (tau > 1 && se > sb) {   // pull next step's alpha rows of this chunk towards L2
             const char *nb = reinterpret_cast<const char *>(a_row - alpha_frame + (size_t)sb * Npad);
             const size_t bytes = (size_t)(se - sb) * Npad * 4;
@@ -1348,6 +1401,10 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
     }
 
     if (STREAM) arc_ring_drain(aring);
+    if (P.t_lo > 0) {   // a later segment launch continues from here
+        if (cta == 0 && tid < P.N) P.runlog_b[tid] = runlog;
+        return;
+    }
     // tau = 0: beta_0(start) only -> logZ recomputed from the backward pass (den_calculate.cu:177-187,255-261)
     if (cta == 0 && warp == 0) {
         const float *bh1 = P.bh + (size_t)(1 & 1) * frame_elems;
@@ -1479,7 +1536,7 @@ int Dispatch(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_sme
     int U = LaneWidth(p.Npad);
     if (backward && U == 4) U = kBwdMaxLaneWidth;
     const float *table = backward ? p.bh : p.alpha;
-    const size_t rows = backward ? (size_t)2 * g.S : (size_t)(p.Tmax + 1 + (g.P > 0 ? 2 : 0)) * g.S;
+    const size_t rows = backward ? (size_t)2 * g.S : (size_t)p.a_frames * g.S;
     if (p.Npad < 32) {   // small batch: the lane padding promised the small-batch TMA kernels (DeviceGraph::small_ok)
         const int LPR = p.Npad;
         const size_t ring_off = (smem + 127) & ~(size_t)127;

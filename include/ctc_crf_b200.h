@@ -141,6 +141,24 @@ int ccb_ctc_crf_loss_logits_fwd(const void *logits, int dtype, int N, int T, int
                                 float *alpha_ws, void *aux_ws, void *ctc_ws,
                                 float *grad, float *loss, float *parts, void *stream);
 
+/* Checkpointed denominator: the two fused entries above with the alpha memory bounded.  The forward pass keeps alpha on a
+ * ring of a few frames plus a copy of every ckpt_k-th frame; the backward pass walks segments of ckpt_k frames from the last
+ * to the first, recomputing each from its checkpoint first (one more forward recursion in total).  alpha_ws holds
+ * ccb_den_ckpt_alpha_floats(N, Tmax, ckpt_k) floats, about (ceil(Tmax/K) + K + 3) frames of S x PadLanes(N) floats;
+ * ckpt_k = 0 is the full spill (ccb_den_alpha_floats).  Same results as the full spill to fp32 rounding.  Costs one more
+ * forward recursion: +40 % step time at N=64, T=1500 on an H100 (DESIGN.md "Checkpointed α"). */
+size_t ccb_den_ckpt_alpha_floats(int N, int T, int ckpt_k);
+int ccb_ctc_crf_loss_ckpt_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k,
+                              const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                              const int *len_dev, int max_label_len, float lamb, float scale,
+                              float *alpha_ws, void *aux_ws, void *ctc_ws,
+                              float *grad, float *loss, float *parts, void *stream);
+int ccb_ctc_crf_loss_logits_ckpt_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k,
+                                     const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                                     const int *len_dev, int max_label_len, float lamb, float scale,
+                                     float *alpha_ws, void *aux_ws, void *ctc_ws,
+                                     float *grad, float *loss, float *parts, void *stream);
+
 /* CTC-only loss (replaces the numerator-only path ctc_crf/__init__.py:25-56 = WARP_CTC_LOSS) on an (N,T,V) block of
  * log-probs, read in place (no (T,N,V) transpose copy, cf. __init__.py:31):
  *   logp[n] = log p(l_n | x_n)  (N,) device out;   loss[0] = -scale * sum_n logp[n];
