@@ -12,7 +12,7 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-LIB = os.path.join(HERE, os.environ.get("CCB_LIB_NAME", "libctc_crf_b200.so"))   # (name/defines: tuning builds only)
+LIB = os.path.join(HERE, "libctc_crf_b200.so")
 SOURCES = ["api.cu", "den_kernels.cu", "ctc_kernels.cu", "den_graph.cc"]
 HEADERS = ["common.cuh", "den_graph.h", os.path.join("..", "..", "include", "ctc_crf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -34,8 +34,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
         raise RuntimeError("nvcc not found: cannot build cat_b200/libctc_crf_b200.so")
-    defs = os.environ.get("CCB_NVCC_DEFS", "").split()
-    cmd = [nvcc, *NVCC_FLAGS, *defs, "-o", LIB + ".tmp", *[os.path.join(CSRC, s) for s in SOURCES]]
+    cmd = [nvcc, *NVCC_FLAGS, "-o", LIB + ".tmp", *[os.path.join(CSRC, s) for s in SOURCES]]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
     subprocess.check_call(cmd, cwd=CSRC)

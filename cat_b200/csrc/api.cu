@@ -42,48 +42,6 @@ struct LegacyScratch {
 };
 LegacyScratch g_legacy[kMaxDevices];
 
-// Side stream of the fused loss (OPT-IN, CCB_OVERLAP=1 at Init; off by default):
-// the numerator's alpha || beta chains (a latency-bound ~1 ms on 2N small CTAs) run here next to the den forward pass, whose
-// persistent CTAs leave room for one of them per SM.  Co-residence is not profitable: either the cooperative den grid is
-// admitted only after the numerator, or both run at once and both slow down until the numerator is through.
-// Created at Init, destroyed by Release.
-struct SideStream {
-    cudaStream_t s = nullptr;
-    cudaEvent_t fork = nullptr, join = nullptr;
-    bool ok = false;
-    int order = 0;                     // CCB_OVERLAP_ORDER (tuning): 0 numerator launched before the den forward pass, 1 after it
-    bool carve = true;                 // CCB_OVERLAP_CARVE=0 (tuning): leave the numerator kernel's L1 / shared-memory split at its default
-    bool trace = false;                // CCB_OVERLAP_TRACE=1 (diagnostics): timed events around each part, printed to stderr (synchronises!)
-    cudaEvent_t tr[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-};
-SideStream g_side[kMaxDevices];
-
-void FreeSide(SideStream &sd) {
-    if (sd.fork) cudaEventDestroy(sd.fork);
-    if (sd.join) cudaEventDestroy(sd.join);
-    if (sd.s) cudaStreamDestroy(sd.s);
-    for (cudaEvent_t e : sd.tr) if (e) cudaEventDestroy(e);
-    sd = SideStream();
-}
-
-void MakeSide(SideStream &sd) {   // (current device); failure just leaves the single-stream path
-    FreeSide(sd);
-    const char *e = getenv("CCB_OVERLAP");
-    if (!(e && e[0] == '1')) return;
-    if (cudaStreamCreateWithFlags(&sd.s, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&sd.fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&sd.join, cudaEventDisableTiming) != cudaSuccess) {
-        cudaGetLastError();
-        FreeSide(sd);
-        return;
-    }
-    sd.ok = true;
-    { const char *o = getenv("CCB_OVERLAP_ORDER"); sd.order = o ? atoi(o) : 0; }
-    { const char *c = getenv("CCB_OVERLAP_CARVE"); sd.carve = !(c && c[0] == '0'); }
-    { const char *t = getenv("CCB_OVERLAP_TRACE"); sd.trace = t && t[0] == '1'; }
-    if (sd.trace) for (cudaEvent_t &e : sd.tr) if (cudaEventCreate(&e) != cudaSuccess) { sd.trace = false; break; }
-}
-
 // profiling aid (ccb_debug_timeline)
 unsigned long long *g_timeline = nullptr;
 int g_tl_step0 = 0, g_tl_steps = 0;
@@ -155,15 +113,6 @@ int CurrentGraph(DeviceGraph **out) {
     return 0;
 }
 
-// warps per CTA of the persistent den kernels (512 threads, one CTA per SM); tuning builds: CCB_DEN_WARPS=8 for experiments
-int DenWarps() {
-#ifdef CCB_TUNING
-    const char *e = getenv("CCB_DEN_WARPS");
-    if (e && (atoi(e) == 8 || atoi(e) == 24)) return atoi(e);
-#endif
-    return 16;
-}
-
 int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
     std::lock_guard<std::mutex> lk(g_mu);
     if (!fst_name || n_gpus <= 0 || !gpus) return Fail("Init: bad arguments");
@@ -179,7 +128,7 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
     cudaDeviceProp prop;
     CCB_CUDA(cudaGetDeviceProperties(&prop, gpus[0]));
     if (!prop.cooperativeLaunch) return Fail("device does not support cooperative launch");
-    if (!BuildDenPlan(fst, prop.multiProcessorCount, DenWarps(), &g_plan, &err)) return Fail(err);
+    if (!BuildDenPlan(fst, prop.multiProcessorCount, kDenThreads / 32, &g_plan, &err)) return Fail(err);
     g_plan_valid = true;
     DEN_NUM_STATES = g_plan.num_states + g_plan.num_pairs;   // rows per alpha frame (what binding.cpp sizes scratch with)
     DEN_NUM_ARCS = (int)g_plan.fwd.arcs.size();
@@ -224,7 +173,7 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
         d.n_hubs = (int)g_plan.hub_states.size();
         d.start_final = g_plan.final_lin[(size_t)g_plan.start];
         d.loaded = (rc == 0);
-        if (rc == 0) { ++g_refs[gpus[i]]; MakeSide(g_side[gpus[i]]); }
+        if (rc == 0) ++g_refs[gpus[i]];
     }
     cudaSetDevice(prev);
     return rc;
@@ -240,7 +189,6 @@ int ReleaseImpl(int n_gpus, const int *gpus) {
         if (cudaSetDevice(gpus[i]) != cudaSuccess) continue;
         cudaDeviceSynchronize();
         FreeDevice(g_dev[gpus[i]]);
-        FreeSide(g_side[gpus[i]]);
         LegacyScratch &ls = g_legacy[gpus[i]];
         cudaFree(ls.aux); cudaFree(ls.alpha); cudaFree(ls.ctc);
         ls = LegacyScratch();
@@ -273,9 +221,6 @@ DenParams BaseParams(const DeviceGraph &g, const void *y, int dtype, long sn, lo
     p.b0 = reinterpret_cast<float *>(a + L.b0);
     p.fmax = reinterpret_cast<float *>(a + L.fmax);
     p.timeline = g_timeline; p.tl_step0 = g_tl_step0; p.tl_steps = g_tl_steps;
-#ifdef CCB_TUNING   // timing-experiment switches (skip row ends / barriers: WRONG RESULTS) exist in tuning builds only
-    { const char *e = getenv("CCB_DEBUG"); p.debug = e ? atoi(e) : 0; }
-#endif
     return p;
 }
 
@@ -538,17 +483,6 @@ int ccb_den_forward_backward(const void *logits, int dtype, long sn, long st, in
     return 0;
 }
 
-#ifdef CCB_TUNING
-/* tuning builds only: the backward pass alone over the spill of an earlier forward pass (overlap experiments) */
-int ccb_debug_den_backward(const void *logits, int dtype, long sn, long st, int N, int T, int V, const int *len_dev,
-                           float *alpha_ws, void *aux_ws, float *grad, long gsn, long gst, void *stream) {
-    g_err.clear();
-    DeviceGraph *g;
-    if (CurrentGraph(&g)) return 1;
-    return DenBackward(*g, logits, dtype, sn, st, N, T, V, len_dev, alpha_ws, aux_ws, grad, gsn, gst, 1.f, (cudaStream_t)stream);
-}
-#endif
-
 int ccb_ctc_forward_backward(const void *logits, int dtype, long sn, long st, int N, int T, int V,
                              const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
                              const int *len_dev, int max_label_len, int blank, void *workspace,
@@ -621,63 +555,18 @@ static int LossFwdImpl(bool raw, const void *logits, int dtype, int N, int T, in
     const long sn = (long)T * V, st = V;     // the (N,T,V) block is addressed in place; only Tmax frames are walked
     const DenAuxLayout L = MakeDenAuxLayout(g->S, N, Tmax, g->small_ok);
     float *logz = reinterpret_cast<float *>((char *)aux_ws + L.logz_a);
-    // log p(l|x) per utterance: behind the numerator's cells in ITS workspace (not in the den aux block: the numerator may run
-    // concurrently with the den passes)
+    // log p(l|x) per utterance: the numerator's output, kept behind its cells in ITS workspace (ccb_ctc_workspace_bytes
+    // counts it)
     float *logp = reinterpret_cast<float *>(reinterpret_cast<double *>(ctc_ws) +
                                             (size_t)N * (2 * (size_t)Tmax * (2 * (size_t)max_label_len + 1) + 1) + 32);
     const double *lnorm = raw ? reinterpret_cast<const double *>((char *)aux_ws + L.lnorm) : nullptr;
-    std::string err;
-    int dev = 0;
-    CCB_CUDA(cudaGetDevice(&dev));
-    // Fork: the numerator's chains need only y and the labels.  (raw-logit entry: they also need the frame normalisers the den
-    // prologue computes on the caller's stream -- kept in line there.)
-    SideStream *sd = (!raw && dev < kMaxDevices && g_side[dev].ok) ? &g_side[dev] : nullptr;
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    if (sd && (cudaStreamIsCapturing(s, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone)) { cudaGetLastError(); sd = nullptr; }
-    int rc = 0;
-    auto side_numerator = [&]() -> int {
-        if (sd->trace) cudaEventRecord(sd->tr[1], sd->s);
-        int r = LaunchCtcAlphaBeta(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
-                                   max_label_len, 0, reinterpret_cast<float *>(ctc_ws), true, logp, nullptr, sd->s, &err, sd->carve);
-        if (r) return Fail(err);
-        if (sd->trace) cudaEventRecord(sd->tr[2], sd->s);
-        CCB_CUDA(cudaEventRecord(sd->join, sd->s));
-        return 0;
-    };
-    if (sd) {
-        if (sd->trace) cudaEventRecord(sd->tr[0], s);
-        CCB_CUDA(cudaEventRecord(sd->fork, s));
-        CCB_CUDA(cudaStreamWaitEvent(sd->s, sd->fork, 0));
-        if (sd->order == 0 && side_numerator()) return 1;
-    }
     CCB_CUDA(cudaMemsetAsync(grad, 0, sizeof(float) * (size_t)N * T * V, s));
-    if (sd && sd->trace) cudaEventRecord(sd->tr[3], s);
-    if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw, ckpt_k)) rc = 1;
-    if (sd && sd->trace) cudaEventRecord(sd->tr[4], s);
-    if (sd && sd->order != 0 && side_numerator()) return 1;
-    if (!rc && DenBackward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, grad, sn, st, scale, s, raw, ckpt_k)) rc = 1;
-    if (sd && sd->trace) {
-        cudaEventRecord(sd->tr[5], s);
-        cudaDeviceSynchronize();
-        float a0 = 0, a1 = 0, f0 = 0, f1 = 0, b1 = 0;
-        cudaEventElapsedTime(&a0, sd->tr[0], sd->tr[1]); cudaEventElapsedTime(&a1, sd->tr[0], sd->tr[2]);
-        cudaEventElapsedTime(&f0, sd->tr[0], sd->tr[3]); cudaEventElapsedTime(&f1, sd->tr[0], sd->tr[4]);
-        cudaEventElapsedTime(&b1, sd->tr[0], sd->tr[5]);
-        fprintf(stderr, "ccb overlap trace (ms from fork): numerator %.3f..%.3f  den forward %.3f..%.3f  den backward ..%.3f\n", a0, a1, f0, f1, b1);
-    }
-    if (sd) {   // join even on failure: the side stream must never outlive the call's buffers unordered
-        const std::string keep = g_err;
-        if (cudaStreamWaitEvent(s, sd->join, 0) != cudaSuccess && !rc) return FailCuda("cudaStreamWaitEvent(join)", cudaGetLastError());
-        g_err = keep;
-    }
-    if (rc) return 1;
-    if (!sd) {
-        rc = LaunchCtcAlphaBeta(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
-                                max_label_len, 0, reinterpret_cast<float *>(ctc_ws), true, logp, lnorm, s, &err, false);
-        if (rc) return Fail(err);
-    }
-    rc = LaunchCtcGamma(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
-                        max_label_len, 0, reinterpret_cast<float *>(ctc_ws), grad, sn, st, -(1.f + lamb) * scale, s, &err);
+    if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw, ckpt_k)) return 1;
+    if (DenBackward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, grad, sn, st, scale, s, raw, ckpt_k)) return 1;
+    // the numerator accumulates into the gradient after the den passes have normalised their part of it
+    std::string err;
+    int rc = LaunchCtc(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+                       max_label_len, 0, reinterpret_cast<float *>(ctc_ws), grad, sn, st, -(1.f + lamb) * scale, logp, lnorm, s, &err);
     if (rc) return Fail(err);
     if (raw) {   // chain through log_softmax: dL/dz = g - softmax(z) * sum_k g_k
         rc = LaunchLogitGrad(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, len_dev,

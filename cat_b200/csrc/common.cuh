@@ -18,6 +18,8 @@ constexpr uint32_t kOobRow = 0x40000000u;   // a TMA row coordinate no gather ta
 // backward arc bytes per CTA tile (12 per slot) above which a graph also gets the streamed-arc copy of its quads: below it
 // the stream fits shared memory next to the deepest rings at every batch width
 constexpr size_t kStreamTierArcBytes = 72 * 1024;
+// threads per CTA of the persistent den kernels: 16 warps, one CTA per SM (the den plan is built for 16 warps per CTA)
+constexpr int kDenThreads = 512;
 
 struct DevicePass {
     Arc *arcs = nullptr;
@@ -127,7 +129,6 @@ struct alignas(64) DenParams {
     // optional per-warp timeline (profiling aid, normally null)
     unsigned long long *timeline;
     int tl_step0, tl_steps;
-    int debug;            // CCB_DEBUG bit 0: skip row-end work, bit 1: skip the grid barrier (TIMING EXPERIMENTS ONLY)
 };
 
 // workspace carving (all offsets in bytes, 256-aligned)
@@ -173,14 +174,6 @@ int LaunchCtc(const void *y, int y_bf16, long sn, long st, int N, int T, int V, 
               const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
               float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, float *logp,
               const double *lnorm, cudaStream_t stream, std::string *err, int overwrite = 0, int Tfull = 0);
-int LaunchCtcAlphaBeta(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
-                       const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
-                       float *alpha_ws, bool want_beta, float *logp, const double *lnorm, cudaStream_t stream,
-                       std::string *err, bool share_sm);
-int LaunchCtcGamma(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
-                   const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
-                   float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, cudaStream_t stream,
-                   std::string *err, int overwrite = 0, int Tfull = 0);
 int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStream_t stream);
 int LaunchCtcViterbi(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
                      const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,

@@ -367,15 +367,12 @@ __global__ void assemble_loss_kernel(const float *logz, const float *logp, int N
     if (threadIdx.x == 0) loss[0] = (float)(acc * (double)scale);
 }
 
-}  // namespace
-
-// The two halves of the numerator, separately launchable: the alpha || beta chains read only y and the labels and write
-// the cell workspace + logp, so the fused loss runs them on a side stream next to the den forward pass (api.cu); the
-// occupancy kernel accumulates into the gradient and therefore follows the den normalisation pass.
+// The two halves of the numerator: the alpha || beta chains write the cell workspace + logp, the occupancy kernel turns
+// the cells into the gradient.
 int LaunchCtcAlphaBeta(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
                        const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                        float *alpha_ws, bool want_beta, float *logp, const double *lnorm, cudaStream_t stream,
-                       std::string *err, bool share_sm) {
+                       std::string *err) {
     if (N == 0) return 0;
     const int ScMax = 2 * max_label_len + 1;
     int threads = ((max_label_len + 1 + 31) / 32) * 32;
@@ -384,12 +381,6 @@ int LaunchCtcAlphaBeta(const void *y, int y_bf16, long sn, long st, int N, int T
     if (smem > 200 * 1024 || (size_t)V * 4 > 200 * 1024) { *err = "label sequence too long for the numerator kernel's shared memory"; return 1; }
     cudaError_t e = cudaFuncSetAttribute(ctc_alpha_beta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc): ") + cudaGetErrorString(e); return (int)e; }
-    // share_sm: these CTAs are meant to sit NEXT to a persistent den CTA (166-182 KB of shared memory) on the same SM.  An SM
-    // cannot change its L1 / shared-memory split while a CTA is resident, so both kernels must ask for the same split or the
-    // later one waits for the earlier one to drain: prefer the maximum carve-out here as the den kernels need it anyway.
-    e = cudaFuncSetAttribute(ctc_alpha_beta_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
-                             share_sm ? (int)cudaSharedmemCarveoutMaxShared : (int)cudaSharedmemCarveoutDefault);
-    if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc carve-out): ") + cudaGetErrorString(e); return (int)e; }
     ctc_alpha_beta_kernel<<<2 * N, threads, smem, stream>>>(y, y_bf16, sn, st, T, V, labels, label_off, label_len, len,
                                                             max_label_len, blank, alpha_ws, want_beta, logp, lnorm);
     CountLaunch();
@@ -418,12 +409,14 @@ int LaunchCtcGamma(const void *y, int y_bf16, long sn, long st, int N, int T, in
     return 0;
 }
 
+}  // namespace
+
 int LaunchCtc(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
               const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
               float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, float *logp,
               const double *lnorm, cudaStream_t stream, std::string *err, int overwrite, int Tfull) {
     int rc = LaunchCtcAlphaBeta(y, y_bf16, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws,
-                                grad != nullptr, logp, lnorm, stream, err, false);
+                                grad != nullptr, logp, lnorm, stream, err);
     if (rc || grad == nullptr) return rc;
     return LaunchCtcGamma(y, y_bf16, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws, grad, gsn,
                           gst, grad_scale, stream, err, overwrite, Tfull);

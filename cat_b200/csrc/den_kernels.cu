@@ -19,14 +19,6 @@
 
 #include "common.cuh"
 
-// timing-experiment switches (DenParams::debug: skip row ends / barriers -- WRONG RESULTS) exist in tuning builds only; the
-// shipped kernels do not even test the word
-#ifdef CCB_TUNING
-#define CCB_DBG(P, bit) (((P).debug & (bit)) != 0)
-#else
-#define CCB_DBG(P, bit) false
-#endif
-
 namespace ccb {
 
 namespace {
@@ -43,23 +35,17 @@ constexpr unsigned kFull = 0xffffffffu;
 // frame ends in the grid barrier's gpu-scope acquire fence + bar.sync, after which ordinary loads must observe the other
 // CTAs' released writes (the same contract cooperative-groups grid.sync() gives), and no row is re-read within a frame
 // after being rewritten.  Against ld.global.cg this makes the zero-weight padding slots (which repeat the address of
-// the preceding arc) L1 hits.  -DCCB_GATHER_CG restores
-// the L2-only loads for A/B runs.
-#ifdef CCB_GATHER_CG
-#define CCB_GATHER_LOAD(p) __ldcg(p)
-#else
-#define CCB_GATHER_LOAD(p) (*(p))
-#endif
+// the preceding arc) L1 hits.
 template <int U> struct Vec;
 template <> struct Vec<1> {
     float v[1];
-    __device__ __forceinline__ static Vec ld_row(const float *p) { Vec r; r.v[0] = CCB_GATHER_LOAD(p); return r; }
+    __device__ __forceinline__ static Vec ld_row(const float *p) { Vec r; r.v[0] = *p; return r; }
     __device__ __forceinline__ void stcg(float *p) const { __stcg(p, v[0]); }
 };
 template <> struct Vec<2> {
     float v[2];
     __device__ __forceinline__ static Vec ld_row(const float *p) {
-        float2 t = CCB_GATHER_LOAD(reinterpret_cast<const float2 *>(p));
+        float2 t = *reinterpret_cast<const float2 *>(p);
         Vec r; r.v[0] = t.x; r.v[1] = t.y; return r;
     }
     __device__ __forceinline__ void stcg(float *p) const { __stcg(reinterpret_cast<float2 *>(p), make_float2(v[0], v[1])); }
@@ -67,7 +53,7 @@ template <> struct Vec<2> {
 template <> struct Vec<4> {
     float v[4];
     __device__ __forceinline__ static Vec ld_row(const float *p) {
-        float4 t = CCB_GATHER_LOAD(reinterpret_cast<const float4 *>(p));
+        float4 t = *reinterpret_cast<const float4 *>(p);
         Vec r; r.v[0] = t.x; r.v[1] = t.y; r.v[2] = t.z; r.v[3] = t.w; return r;
     }
     __device__ __forceinline__ void stcg(float *p) const {
@@ -216,7 +202,7 @@ __global__ void logit_grad_kernel(const void *z, int bf16, long sn, long st, int
 // ------------------------------------------------------------------------------------------------
 // The arc walk shared by both passes: a software-pipelined stream over the warp's chunk of arcs.
 //   * arcs come a quad at a time: one LDS.128 of four peers for the gathers, one LDS.128 of four weights for the FMAs;
-//   * BATCH row gathers (CCB_GATHER_LOAD, 32*U*4 bytes each, one per arc) are issued for batch k+1 BEFORE batch k
+//   * BATCH row gathers (plain loads, 32*U*4 bytes each, one per arc) are issued for batch k+1 BEFORE batch k
 //     is consumed, so a warp keeps BATCH..2*BATCH loads in flight (the recursion is latency-bound on L2);
 //   * weights are applied as |w|; the sign bit of a quad's 4th weight marks the end of a segment and the sign bits
 //     of its 3rd/2nd weights the event code (den_graph.h kEv*): `seg_end(acc, event)` runs (warp-uniform branch).
@@ -427,51 +413,6 @@ template <> __device__ __forceinline__ Vec<4> lds_row<4>(uint32_t addr) {
     return r;
 }
 
-// The arc walk with TMA-staged rows.  `arcs`: the chunk's quads in shared memory, WPQ 16-byte words per quad
-// {row index 0..3}{w0..3}[{w1 0..3}]; n_batches = chunk arcs / R.  One batch = R/4 quads, issued by lanes 0..R-1 (one
-// row each).  `consume_quad(words of the quad, rows v[4])` does the FMAs and the segment-end work.
-template <int U, int R, int WPQ, typename Prologue, typename ConsumeQuad>
-__device__ __forceinline__ void walk_arcs_tma(const uint4 *arcs, int n_batches, const CUtensorMap *tm, int col, int row_base,
-                                              TmaRing &ring, int lane, Prologue &&prologue, ConsumeQuad &&consume_quad) {
-    constexpr int QB = R / kQuad;   // (two stages)
-    constexpr uint32_t ROWB = 32u * U * 4u;
-    static_assert(R % kQuad == 0 && kChunkArcPad % R == 0 && R <= 32, "a batch is whole quads, divides the chunk padding, one row per lane");
-    auto issue = [&](int k, int s) {
-        const uint32_t bar = ring.bar + 8u * s;
-        if (lane == 0) mbar_expect_tx(bar, R * ROWB);
-        __syncwarp();
-        if (lane < R) {
-            const uint4 pr = arcs[(size_t)WPQ * (k * QB + lane / kQuad)];
-            tma_row(ring.buf + (uint32_t)(s * R + lane) * ROWB, tm, col, row_base + quad_row(pr, lane % kQuad), bar);
-        }
-    };
-    auto consume = [&](int k, int s) {
-        mbar_wait(ring.bar + 8u * s, (ring.phase >> s) & 1u);
-        ring.phase ^= 1u << s;
-        const uint32_t base = ring.buf + (uint32_t)(s * R) * ROWB + (uint32_t)lane * (U * 4u);
-#pragma unroll
-        for (int q = 0; q < QB; ++q) {
-            Vec<U> v[kQuad];
-#pragma unroll
-            for (int j = 0; j < kQuad; ++j) v[j] = lds_row<U>(base + (uint32_t)(q * kQuad + j) * ROWB);
-            consume_quad(arcs + (size_t)WPQ * (k * QB + q), v);
-        }
-        __syncwarp();   // every lane is done with the stage before it is refilled
-    };
-    if (n_batches <= 0) { prologue(); return; }
-    issue(0, 0);
-    if (n_batches > 1) issue(1, 1);
-    prologue();   // per-frame scalars are fetched while the first rows are in flight
-    for (int k = 0; k < n_batches; k += 2) {
-        consume(k, 0);
-        if (k + 2 < n_batches) issue(k + 2, 0);
-        if (k + 1 < n_batches) {
-            consume(k + 1, 1);
-            if (k + 3 < n_batches) issue(k + 3, 1);
-        }
-    }
-}
-
 // Streamed arcs (graphs whose arc stream does not fit shared memory, BASELINE config 4: 5 M arcs): the chunk's quads are
 // not resident; they flow through a per-warp ring of kArcStages batches, filled by 1-D bulk copies (`cp.async.bulk`, SASS
 // UBLKCP: the stream is sequential and the same every frame) from DevicePass::tq, each stage completing its own mbarrier.
@@ -506,11 +447,15 @@ __device__ __forceinline__ void arc_ring_drain(ArcRing &ar) {
         ++ar.done;
     }
 }
+// The arc walk with TMA-staged rows over the streamed quads (WPQ 16-byte words each, {row index 0..3}{w0..3}{w1 0..3}):
+// n_batches = chunk arcs / R, one batch = R/4 quads whose rows lanes 0..R-1 request (one row each).  `consume_quad(words of
+// the quad, rows v[4])` does the FMAs and the group-end work.
 template <int U, int R, int WPQ, typename Prologue, typename ConsumeQuad>
 __device__ __forceinline__ void walk_arcs_tma_stream(ArcRing &ar, int n_batches, const CUtensorMap *tm, int col, int row_base,
                                                      TmaRing &ring, int lane, Prologue &&prologue, ConsumeQuad &&consume_quad) {
     constexpr int QB = R / kQuad, AW = QB * WPQ;
     constexpr uint32_t ROWB = 32u * U * 4u;
+    static_assert(R % kQuad == 0 && kChunkArcPad % R == 0 && R <= 32, "a batch is whole quads, divides the chunk padding, one row per lane");
     const uint32_t g0 = ar.done;
     auto issue = [&](int k, int s) {
         const uint32_t g = g0 + (uint32_t)k, st = g % kArcStages;
@@ -700,13 +645,13 @@ __device__ __forceinline__ void ckpt_frame_done(const DenParams &P, int t, const
 // ------------------------------------------------------------------------------------------------
 // HUBS: the plan contains high in-degree rows split into parts (kEvPartial segments); the common case compiles the
 // partial-row path out entirely so that it costs the hot row-end code nothing.
-// TMA: the gathered rows are staged in shared memory by TMA row copies (walk_arcs_tma) instead of register gathers; needs
-// the arc tile in shared memory (SMEM_ARCS) and DenParams::tmap.
-// LPR < 32 (8 or 16 lanes per row): the small-batch variant, see walk_arcs_tma_small (TMA, U = 1, no hub rows).
-template <int NT, int U, int BATCH, bool SMEM_ARCS, bool HUBS, bool TMA = false, int LPR = 32>
-__global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(const __grid_constant__ DenParams P) {
-    static_assert(!TMA || SMEM_ARCS, "the TMA walk reads the arc tile from shared memory");
-    static_assert(LPR == 32 || (TMA && U == 1 && !HUBS && (LPR == 8 || LPR == 16)), "small-batch variant: TMA, one utterance per lane, no hubs");
+// LPR = 32: rows are gathered into registers (walk_arcs).  LPR < 32 (8 or 16 lanes per row): the small-batch variant, whose
+// rows are staged in shared memory by bulk copies (TMA, walk_arcs_tma_small); needs the arc tile in shared memory
+// (SMEM_ARCS), one utterance per lane and no hub rows.
+template <int U, int BATCH, bool SMEM_ARCS, bool HUBS, int LPR = 32>
+__global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __grid_constant__ DenParams P) {
+    constexpr bool TMA = LPR < 32;
+    static_assert(!TMA || (SMEM_ARCS && U == 1 && !HUBS && (LPR == 8 || LPR == 16)), "small-batch variant: arc tile in shared memory, one utterance per lane, no hubs");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float *s_sum = reinterpret_cast<float *>(smem_raw);                                  // [Npad]
     int *s_label = reinterpret_cast<int *>(s_sum + P.Npad);                              // [tile_rows] label per row
@@ -738,17 +683,16 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
     int labp0 = -1, labp1 = -1;
     for (int q = se - 1; q >= sb; --q) { if (__ldg(P.state_pos + q)) labp1 = __ldg(P.state_label + q); else labp0 = __ldg(P.state_label + q); }
     unsigned epoch = 0;
-    const int n_batches = (ae - ab) / (TMA && LPR < 32 ? 16 : BATCH);   // (TMA: BATCH = rows per ring stage)
+    const int n_batches = (ae - ab) / (TMA ? 16 : BATCH);   // (small batches: 16 rows per ring stage)
     const uint4 *const arc4 = SMEM_ARCS ? reinterpret_cast<const uint4 *>(s_arcs + (ab - tile_a0))
                                         : reinterpret_cast<const uint4 *>(P.arcs + ab);
     TmaRing ring{0u, 0u, 0u};
     if (TMA) {
-        constexpr int kStages = LPR == 32 ? 2 : kSmallStages;
-        constexpr uint32_t kRingBytes = LPR == 32 ? 2u * BATCH * 32u * U * 4u : (uint32_t)kSmallStages * 16u * LPR * 4u;
+        constexpr uint32_t kRingBytes = (uint32_t)kSmallStages * 16u * LPR * 4u;
         ring.buf = smem_u32(smem_raw + P.ring_off) + (uint32_t)warp * kRingBytes;
-        ring.bar = smem_u32(smem_raw + P.bar_off) + (uint32_t)warp * 8u * kStages;
+        ring.bar = smem_u32(smem_raw + P.bar_off) + (uint32_t)warp * 8u * kSmallStages;
         if (lane == 0) {
-            for (int st = 0; st < kStages; ++st) mbar_init(ring.bar + 8u * st, 1);
+            for (int st = 0; st < kSmallStages; ++st) mbar_init(ring.bar + 8u * st, 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
         __syncwarp();
@@ -756,16 +700,16 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
 
     // per-row metadata lives in shared memory: L1 is invalidated at every grid barrier, and a global load on the
     // row-end path would cost an L2 round trip per row
-    for (int i = tid; i < tile_s1 - tile_s0; i += NT) s_label[i] = __ldg(P.state_label + tile_s0 + i);
+    for (int i = tid; i < tile_s1 - tile_s0; i += kDenThreads) s_label[i] = __ldg(P.state_label + tile_s0 + i);
     const uint32_t row_bytes = (uint32_t)Npad * 4u;
     if (SMEM_ARCS) {   // stage the tile once, quad-wise transposed: {byte offset 0..3}{w0..3}
         uint4 *sq = reinterpret_cast<uint4 *>(s_arcs);
         const uint4 *src = reinterpret_cast<const uint4 *>(P.arcs + tile_a0);
-        for (int i = tid; i < (tile_a1 - tile_a0) / kQuad; i += NT) {
+        for (int i = tid; i < (tile_a1 - tile_a0) / kQuad; i += kDenThreads) {
             const uint4 m0 = __ldg(src + 2 * i), m1 = __ldg(src + 2 * i + 1);
             const uint32_t mul = TMA ? 1u : row_bytes;   // TMA: row coordinates; register gathers: byte offsets
             uint4 pr = make_uint4(fwd_row(m0.x, S) * mul, fwd_row(m0.z, S) * mul, fwd_row(m1.x, S) * mul, fwd_row(m1.z, S) * mul);
-            if (TMA && !HUBS) {
+            if (TMA) {
                 // zero-weight padding slots name a row coordinate beyond the tensor: the TMA unit zero-fills them in shared
                 // memory without touching L2 (17 % of the forward stream; the register path gets these from L1 instead)
                 if ((m0.y & 0x7fffffffu) == 0u) pr.x = kOobRow;
@@ -777,7 +721,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
             sq[2 * i + 1] = make_uint4(m0.y, m0.w, m1.y, m1.w);
         }
     }
-    for (int i = tid; i < Npad; i += NT) s_sum[i] = 0.f;
+    for (int i = tid; i < Npad; i += kDenThreads) s_sum[i] = 0.f;
 
     // t = 0: alpha_0 = indicator(start) (virtual rows: the pair sum); column sum 1.  Recompute of a segment: frame t_lo is
     // its checkpoint's real rows, and its pair-sum rows are rebuilt from them (the same fp32 sum the frame's row ends formed)
@@ -795,12 +739,12 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
                 ++vj;
             }
         }
-        if (cta == 0 && !recompute) for (int n = tid; n < Npad; n += NT) __stcg(P.colsum_a + n, 1.f);
+        if (cta == 0 && !recompute) for (int n = tid; n < Npad; n += kDenThreads) __stcg(P.colsum_a + n, 1.f);
     }
     // rows of high in-degree states are accumulated with atomics from several parts: zero them one frame ahead
     auto zero_hub_rows = [&](int frame) {
         float *fr = P.alpha + (size_t)alpha_pos(P, frame) * frame_elems;
-        for (int i = cta * NT + tid; i < P.n_hubs * Npad; i += gridDim.x * NT)
+        for (int i = cta * kDenThreads + tid; i < P.n_hubs * Npad; i += gridDim.x * kDenThreads)
             __stcg(fr + (size_t)__ldg(P.hub_states + i / Npad) * Npad + (i % Npad), 0.f);
     };
     if (HUBS && P.t_lo < P.t_hi) zero_hub_rows(P.t_lo + 1);
@@ -869,7 +813,6 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
             bool ec0_fresh = false;   // merged pairs: the first members' common emission, refreshed at the frame's first pair
             auto seg_end = [&](float *acc, int ev, bool new_label, const uint4 *quad, const float *a2, const Vec<U> &v3, float w3) {
                 const bool k1 = ev != kEvRowPos0;
-                if (CCB_DBG(P, 1)) { sum[0] += acc[0]; acc[0] = 0.f; return; }
                 if (!HUBS && ev == kEvPairMerged) {
                     // BOTH rows of a pair (den_graph.h DenPlan::fwd_merged): the second member's sum is everything but the last
                     // slot (a2), the first member's single arc is the last slot (w3 * v3); rows out_row, out_row + 1
@@ -917,7 +860,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
 #pragma unroll
                     for (int u = 0; u < U; ++u) { part.v[u] = acc[u]; acc[u] = 0.f; }
                     // byte offset of the target row (last slot of the segment)
-                    const uint32_t tgt_off = TMA ? quad[0].w * row_bytes : load_quad_peers<SMEM_ARCS>(quad, row_bytes, (uint32_t)S).w;
+                    const uint32_t tgt_off = load_quad_peers<SMEM_ARCS>(quad, row_bytes, (uint32_t)S).w;
                     forward_partial_row<U>(P.state_label, P.len, P.colsum_a + (size_t)(t - 1) * Npad, P.fmax + (size_t)(t - 1) * Npad,
                                            P.y, P.y_bf16, P.sn, (long)(t - 1) * P.st, P.N, t, n0, part, tgt_off, row_bytes, a_cur, s_sum, P.scale_exp);
                     if (tgt_off == out_row * row_bytes) { ++out_row; ++ql; }   // the part that lives in the row's own group
@@ -957,7 +900,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
                 ++ql;
                 own_prefetch(out_row);
             };
-            if (TMA && LPR < 32) {
+            if (TMA) {
                 float acc[1] = {0.f};
                 walk_arcs_tma_small<LPR, 2>(arc4, n_batches, P.alpha, p_prev * S, ring, lane, frame_scalars,
                                             [&](const uint4 *quad, const float *v, uint32_t) {
@@ -987,27 +930,6 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
                         seg_end(acc, ev, (int)wq.x < 0, quad, a2, v3, 1.f);
                     }
                 });
-            } else if (TMA) {
-                float acc[U];
-#pragma unroll
-                for (int u = 0; u < U; ++u) acc[u] = 0.f;
-                auto consume_quad = [&](const uint4 *quad, const Vec<U> *v) {
-                    const uint4 wq = quad[1];
-                    const float w0 = fabsf(__uint_as_float(wq.x)), w1 = fabsf(__uint_as_float(wq.y));
-                    const float w2 = fabsf(__uint_as_float(wq.z)), w3 = fabsf(__uint_as_float(wq.w));
-                    float a2[U];   // the sums without the quad's last slot (kEvPairMerged)
-#pragma unroll
-                    for (int u = 0; u < U; ++u) {
-                        acc[u] = fmaf(w0, v[0].v[u], acc[u]);
-                        acc[u] = fmaf(w1, v[1].v[u], acc[u]);
-                        acc[u] = fmaf(w2, v[2].v[u], acc[u]);
-                        a2[u] = acc[u];
-                        acc[u] = fmaf(w3, v[3].v[u], acc[u]);
-                    }
-                    if ((int)wq.w < 0)   // warp-uniform: a segment ends at this quad
-                        seg_end(acc, (int)(((wq.z >> 31) << 1) | (wq.y >> 31)), (int)wq.x < 0, quad, a2, v[3], w3);
-                };
-                walk_arcs_tma<U, BATCH, 2>(arc4, n_batches, &P.tmap, gc * 32 * U, (t - 1) * S, ring, lane, frame_scalars, consume_quad);
             } else {
                 walk_arcs<U, BATCH, SMEM_ARCS>(arc4, n_batches, row_bytes, (uint32_t)S, reinterpret_cast<const char *>(a_prev + n0), lane_act,
                                                frame_scalars, seg_end);
@@ -1020,21 +942,18 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
         if (HUBS && t < P.t_hi) zero_hub_rows(t + 1);
         if (TMA) fence_proxy_async_global();   // this frame's rows are read through the async proxy after the barrier
         __syncthreads();
-        for (int i = tid; i < Npad; i += NT) {   // (a recompute reads the first pass's column sums, it does not add to them)
+        for (int i = tid; i < Npad; i += kDenThreads) {   // (a recompute reads the first pass's column sums, it does not add to them)
             const float v = s_sum[i];
             if (v != 0.f) { if (P.ckpt_mode != 2) atomicAdd(P.colsum_a + (size_t)t * Npad + i, v); s_sum[i] = 0.f; }
         }
         // arrive first, then the log-scale books of CTA 0 (two L2 round trips nobody waits for) in the barrier's shadow
-        const bool split_barrier = !CCB_DBG(P, 2) && !CCB_DBG(P, 8);
-        if (split_barrier) grid_barrier_arrive(P.barrier);
+        grid_barrier_arrive(P.barrier);
         if (cta == 0 && tid < P.N && t <= my_len) {
             int sh;
             (void)scale_from_sum(__ldcg(P.colsum_a + (size_t)(t - 1) * Npad + tid), &sh, P.scale_exp);
             runlog += (double)__ldg(P.fmax + (size_t)(t - 1) * Npad + tid) - (double)sh * 0.6931471805599453;
         }
-        if (split_barrier) grid_barrier_wait(P.barrier, (++epoch) * gridDim.x);
-        else if (!CCB_DBG(P, 2)) grid_barrier(P.barrier, (++epoch) * gridDim.x);
-        else __syncthreads();
+        grid_barrier_wait(P.barrier, (++epoch) * gridDim.x);
         tl_mark(P, t, chunk, n_chunks, 2, lane);
         // (frame t's position is rewritten kAlphaRing frames later)
         if (P.ckpt_mode == 1) ckpt_frame_done(P, t, P.alpha + (size_t)alpha_pos(P, t) * frame_elems, sb, se, lane);
@@ -1056,7 +975,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
         if (zs != 0.f) atomicAdd(&s_sum[n], zs);
     }
     __syncthreads();
-    for (int i = tid; i < Npad; i += NT) {
+    for (int i = tid; i < Npad; i += kDenThreads) {
         const float v = s_sum[i];
         if (v != 0.f) atomicAdd(P.zsum + i, v);
     }
@@ -1067,11 +986,14 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_forward_kernel(cons
 // ------------------------------------------------------------------------------------------------
 // backward: beta recursion, occupancies, logZ from beta
 // ------------------------------------------------------------------------------------------------
-template <int NT, int U, int BATCH, bool SMEM_ARCS, bool W1_SMEM = SMEM_ARCS, bool TMA = false, int LPR = 32, bool STREAM = false>
-__global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(const __grid_constant__ DenParams P) {
-    static_assert(!TMA || STREAM || (SMEM_ARCS && (W1_SMEM || LPR < 32)), "the TMA walk reads the offsets (and, at full width, both weights) from shared memory");
-    static_assert(!STREAM || (TMA && !SMEM_ARCS && LPR == 32), "streamed arcs: TMA, full-width rows");
-    static_assert(LPR == 32 || (TMA && U == 1 && (LPR == 8 || LPR == 16)), "small-batch variant: TMA, one utterance per lane");
+// Rows are gathered into registers (walk_arcs_dual) except in two TMA variants: LPR < 32, the small-batch variant
+// (walk_arcs_tma_small, arc tile in shared memory, one utterance per lane), and STREAM, the streamed-arc tier
+// (walk_arcs_tma_stream, full-width rows, arcs flowing through per-warp rings).
+template <int U, int BATCH, bool SMEM_ARCS, bool W1_SMEM = SMEM_ARCS, int LPR = 32, bool STREAM = false>
+__global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __grid_constant__ DenParams P) {
+    constexpr bool TMA = LPR < 32 || STREAM;
+    static_assert(LPR == 32 || (SMEM_ARCS && U == 1 && (LPR == 8 || LPR == 16)), "small-batch variant: arc tile in shared memory, one utterance per lane");
+    static_assert(!STREAM || (!SMEM_ARCS && LPR == 32), "streamed arcs: not resident, full-width rows");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int Npad = P.Npad, S = P.S;
     float *s_sum = reinterpret_cast<float *>(smem_raw);            // [2][Npad]: colsum_b, absum
@@ -1098,7 +1020,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
     const int cl_lab1 = __ldg(P.cta_labels + cta * 4 + 2), cl_n1 = __ldg(P.cta_labels + cta * 4 + 3);
     int labp0 = -1, labp1 = -1;
     for (int q = se - 1; q >= sb; --q) { if (__ldg(P.state_pos + q)) labp1 = __ldg(P.state_label + q); else labp0 = __ldg(P.state_label + q); }
-    const int n_batches = (ae - ab) / (TMA && LPR < 32 ? 16 : BATCH);   // (TMA: BATCH = rows per ring stage)
+    const int n_batches = (ae - ab) / (LPR < 32 ? 16 : BATCH);   // (small batches: 16 rows per ring stage; streamed arcs: BATCH)
     // shared memory: 3 words of 16 bytes per quad {byte offsets}{w0}{w1}; global fallback: AoS arcs + w1 array
     constexpr int kW = W1_SMEM ? 3 : 2;   // 16-byte words per staged quad
     const uint4 *const arc4 = SMEM_ARCS ? reinterpret_cast<const uint4 *>(s_arcs) + kW * ((ab - tile_a0) / kQuad)
@@ -1109,7 +1031,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
     const size_t alpha_frame = (size_t)S * Npad;                          // alpha spill: real rows only (see den_forward_kernel)
     unsigned epoch = 0;
 
-    for (int i = tid; i < tile_s1 - tile_s0; i += NT) {
+    for (int i = tid; i < tile_s1 - tile_s0; i += kDenThreads) {
         s_label[i] = __ldg(P.state_label + tile_s0 + i);
         s_final[i] = __ldg(P.final_lin + tile_s0 + i);
     }
@@ -1118,7 +1040,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
         uint4 *sq = reinterpret_cast<uint4 *>(s_arcs);
         const uint4 *src = reinterpret_cast<const uint4 *>(P.arcs + tile_a0);
         const uint4 *src1 = reinterpret_cast<const uint4 *>(P.w1 + tile_a0);
-        for (int i = tid; i < (tile_a1 - tile_a0) / kQuad; i += NT) {
+        for (int i = tid; i < (tile_a1 - tile_a0) / kQuad; i += kDenThreads) {
             const uint4 m0 = __ldg(src + 2 * i), m1 = __ldg(src + 2 * i + 1);
             const uint32_t mul = TMA ? 1u : row_bytes;   // TMA: row coordinates; register gathers: byte offsets
             uint4 pr = make_uint4(m0.x * mul, m0.z * mul, m1.x * mul, m1.z * mul);
@@ -1157,7 +1079,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
         aring.src = P.tq + (size_t)3 * (ab / kQuad);
         arc_ring_fill<kAW>(aring, lane);
     }
-    for (int i = tid; i < (2 + P.gacc_rows) * Npad; i += NT) s_sum[i] = 0.f;
+    for (int i = tid; i < (2 + P.gacc_rows) * Npad; i += kDenThreads) s_sum[i] = 0.f;
     const int my_len = (cta == 0 && tid < P.N) ? __ldg(P.len + tid) : 0;
     int len0[U];
 #pragma unroll
@@ -1279,7 +1201,6 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
                 ++ql;
             };
             auto group_end = [&](float *acc0, float *acc1, bool pair, bool new0, bool new1) {
-                if (CCB_DBG(P, 1)) { sum_b[0] += acc0[0] + acc1[0]; acc0[0] = 0.f; acc1[0] = 0.f; return; }
                 if (own) {
 #pragma unroll
                     for (int u = 0; u < U; ++u) {
@@ -1303,7 +1224,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
                 a_q1 = ((int)out_row + 1 < se && lane_act) ? gather_row<U>(a_base, (out_row + 1) * row_bytes) : vec_zero<U>();
                 own_prefetch(out_row);
             };
-            if (TMA && LPR < 32) {
+            if (LPR < 32) {
                 float acc0[1] = {0.f}, acc1[1] = {0.f};
                 const uint32_t w1buf = smem_u32(smem_raw + P.bar_off) + (uint32_t)P.n_warps * 8u * kSmallStages + (uint32_t)warp * 64u * kSmallStages;
                 walk_arcs_tma_small<LPR, W1_SMEM ? 3 : 2, !W1_SMEM>(arc4, n_batches, P.bh, ((tau + 1) & 1) * S, ring, lane, frame_scalars,
@@ -1325,7 +1246,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
                         group_end(acc0, acc1, (int)wq.z < 0, (int)wq.x < 0, (int)wq.y < 0);
                     }
                 }, reinterpret_cast<const float *>(w1g), w1buf);
-            } else if (TMA) {
+            } else if (STREAM) {
                 float acc0[U], acc1[U];
 #pragma unroll
                 for (int u = 0; u < U; ++u) { acc0[u] = 0.f; acc1[u] = 0.f; }
@@ -1346,8 +1267,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
                     if ((int)wq.w < 0)   // warp-uniform: the group ends at this quad
                         group_end(acc0, acc1, (int)wq.z < 0, (int)wq.x < 0, (int)wq.y < 0);
                 };
-                if (STREAM) walk_arcs_tma_stream<U, BATCH, 3>(aring, n_batches, &P.tmap, gc * 32 * U, ((tau + 1) & 1) * S, ring, lane, frame_scalars, consume_quad);
-                else walk_arcs_tma<U, BATCH, 3>(arc4, n_batches, &P.tmap, gc * 32 * U, ((tau + 1) & 1) * S, ring, lane, frame_scalars, consume_quad);
+                walk_arcs_tma_stream<U, BATCH, 3>(aring, n_batches, &P.tmap, gc * 32 * U, ((tau + 1) & 1) * S, ring, lane, frame_scalars, consume_quad);
             } else {
                 walk_arcs_dual<U, BATCH, SMEM_ARCS, W1_SMEM>(arc4, w1g, n_batches, row_bytes, reinterpret_cast<const char *>(bh_next + n0),
                                                              lane_gat, frame_scalars, group_end);
@@ -1365,20 +1285,19 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
         tl_mark(P, P.Tmax - tau, chunk, n_chunks, 1, lane);
         if (TMA) fence_proxy_async_global();   // this frame's rows are read through the async proxy after the barrier
         __syncthreads();
-        for (int i = tid; i < Npad; i += NT) {   // the next frame's scale: must be out before this CTA arrives
+        for (int i = tid; i < Npad; i += kDenThreads) {   // the next frame's scale: must be out before this CTA arrives
             const float vb = s_sum[i];
             if (vb != 0.f) { atomicAdd(P.colsum_b + (size_t)tau * Npad + i, vb); s_sum[i] = 0.f; }
         }
         // Everything the next frame reads is written: arrive now, and flush what only the end of the kernel needs
         // (occupancy sums, the label accumulator) in the shadow of the barrier latency.
-        const bool split_barrier = !CCB_DBG(P, 2) && !CCB_DBG(P, 8);
-        if (split_barrier) grid_barrier_arrive(P.barrier);
-        for (int i = tid; i < Npad; i += NT) {
+        grid_barrier_arrive(P.barrier);
+        for (int i = tid; i < Npad; i += kDenThreads) {
             const float vab = s_sum[Npad + i];
             if (vab != 0.f) { atomicAdd(P.absum + (size_t)tau * Npad + i, vab); s_sum[Npad + i] = 0.f; }
         }
         if (use_gacc) {
-            for (int i = tid; i < (cl_n0 + cl_n1) * Npad; i += NT) {
+            for (int i = tid; i < (cl_n0 + cl_n1) * Npad; i += kDenThreads) {
                 const float g = s_gacc[i];
                 if (g != 0.f) {
                     const int n = i % Npad, row = i / Npad;
@@ -1394,9 +1313,7 @@ __global__ void __launch_bounds__(NT, NT == 256 ? 2 : 1) den_backward_kernel(con
             (void)scale_from_sum(__ldcg(P.colsum_b + (size_t)(tau + 1) * Npad + tid), &sh, P.scale_exp);
             runlog += (double)__ldg(P.fmax + (size_t)tau * Npad + tid) - (double)sh * 0.6931471805599453;
         }
-        if (split_barrier) grid_barrier_wait(P.barrier, (++epoch) * gridDim.x);
-        else if (!CCB_DBG(P, 2)) grid_barrier(P.barrier, (++epoch) * gridDim.x);
-        else __syncthreads();
+        grid_barrier_wait(P.barrier, (++epoch) * gridDim.x);
         tl_mark(P, P.Tmax - tau, chunk, n_chunks, 2, lane);
     }
 
@@ -1448,49 +1365,49 @@ __global__ void den_grad_normalize_kernel(float *grad, long gsn, long gst, const
 // ------------------------------------------------------------------------------------------------
 // launch plumbing
 // ------------------------------------------------------------------------------------------------
-int LaunchCoop(const void *fn, int NT, const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
+int LaunchCoop(const void *fn, const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
     cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(e); return (int)e; }
     int per_sm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, NT, smem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kDenThreads, smem);
     if (e != cudaSuccess || per_sm < 1) {
         *err = "den kernel does not fit on an SM (smem=" + std::to_string(smem) + ")";
         return e != cudaSuccess ? (int)e : 1;
     }
     DenParams pc = p;
     void *args[] = {&pc};
-    e = cudaLaunchCooperativeKernel(fn, dim3(n_ctas), dim3(NT), args, smem, stream);
+    e = cudaLaunchCooperativeKernel(fn, dim3(n_ctas), dim3(kDenThreads), args, smem, stream);
     if (e != cudaSuccess) { *err = std::string("cooperative launch failed: ") + cudaGetErrorString(e); return (int)e; }
     CountLaunch();
     return 0;
 }
 
-template <int NT, int U, int BATCH, bool SMEM_ARCS>
+template <int U, int BATCH, bool SMEM_ARCS>
 int LaunchFwd(const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    const void *fn = p.n_hubs > 0 ? (const void *)den_forward_kernel<NT, U, BATCH, SMEM_ARCS, true>
-                                  : (const void *)den_forward_kernel<NT, U, BATCH, SMEM_ARCS, false>;
-    return LaunchCoop(fn, NT, p, n_ctas, smem, stream, err);
+    const void *fn = p.n_hubs > 0 ? (const void *)den_forward_kernel<U, BATCH, SMEM_ARCS, true>
+                                  : (const void *)den_forward_kernel<U, BATCH, SMEM_ARCS, false>;
+    return LaunchCoop(fn, p, n_ctas, smem, stream, err);
 }
-template <int NT, int U, int BATCH, bool SMEM_ARCS>
+template <int U, int BATCH, bool SMEM_ARCS>
 int LaunchBwd(bool w1_smem, const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    const void *fn = SMEM_ARCS && !w1_smem ? (const void *)den_backward_kernel<NT, U, BATCH, SMEM_ARCS, false>
-                                           : (const void *)den_backward_kernel<NT, U, BATCH, SMEM_ARCS>;
-    return LaunchCoop(fn, NT, p, n_ctas, smem, stream, err);
+    const void *fn = SMEM_ARCS && !w1_smem ? (const void *)den_backward_kernel<U, BATCH, SMEM_ARCS, false>
+                                           : (const void *)den_backward_kernel<U, BATCH, SMEM_ARCS>;
+    return LaunchCoop(fn, p, n_ctas, smem, stream, err);
 }
 
 // backward pass with the arc stream flowing through per-warp rings instead of being resident (walk_arcs_tma_stream)
-template <int NT, int U, int R>
+template <int U, int R>
 int LaunchTmaStreamBwd(const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    return LaunchCoop((const void *)den_backward_kernel<NT, U, R, false, true, true, 32, true>, NT, p, n_ctas, smem, stream, err);
+    return LaunchCoop((const void *)den_backward_kernel<U, R, false, true, 32, true>, p, n_ctas, smem, stream, err);
 }
 
 // small batches: rows of LPR = 8 / 16 floats (see walk_arcs_tma_small)
-template <int NT, int LPR>
+template <int LPR>
 int LaunchTmaSmall(bool backward, bool w1_smem, const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    const void *fn = !backward ? (const void *)den_forward_kernel<NT, 1, 16, true, false, true, LPR>
-                     : w1_smem ? (const void *)den_backward_kernel<NT, 1, 16, true, true, true, LPR>
-                               : (const void *)den_backward_kernel<NT, 1, 16, true, false, true, LPR>;
-    return LaunchCoop(fn, NT, p, n_ctas, smem, stream, err);
+    const void *fn = !backward ? (const void *)den_forward_kernel<1, 16, true, false, LPR>
+                     : w1_smem ? (const void *)den_backward_kernel<1, 16, true, true, LPR>
+                               : (const void *)den_backward_kernel<1, 16, true, false, LPR>;
+    return LaunchCoop(fn, p, n_ctas, smem, stream, err);
 }
 
 constexpr int kBwdMaxLaneWidth = 2;   // four utterances per lane spill the backward pass's two accumulators
@@ -1500,20 +1417,21 @@ constexpr int kBwdMaxLaneWidth = 2;   // four utterances per lane spill the back
 template <int U> struct FwdBatch { static constexpr int value = U == 4 ? 8 : 16; };
 constexpr int kBwdBatch = 8;
 
-template <int NT, int U>
+template <int U>
 int DispatchU(bool backward, bool tma, bool smem_arcs, bool w1_smem, const DenParams &p, int n_ctas, size_t smem,
               cudaStream_t stream, std::string *err) {
-    if (tma) return LaunchTmaStreamBwd<NT, U, TmaShape<U>::R>(p, n_ctas, smem, stream, err);
+    if (tma) return LaunchTmaStreamBwd<U, TmaShape<U>::R>(p, n_ctas, smem, stream, err);
     if (backward)
-        return smem_arcs ? LaunchBwd<NT, U, kBwdBatch, true>(w1_smem, p, n_ctas, smem, stream, err)
-                         : LaunchBwd<NT, U, kBwdBatch, false>(w1_smem, p, n_ctas, smem, stream, err);
-    return smem_arcs ? LaunchFwd<NT, U, FwdBatch<U>::value, true>(p, n_ctas, smem, stream, err)
-                     : LaunchFwd<NT, U, FwdBatch<U>::value, false>(p, n_ctas, smem, stream, err);
+        return smem_arcs ? LaunchBwd<U, kBwdBatch, true>(w1_smem, p, n_ctas, smem, stream, err)
+                         : LaunchBwd<U, kBwdBatch, false>(w1_smem, p, n_ctas, smem, stream, err);
+    return smem_arcs ? LaunchFwd<U, FwdBatch<U>::value, true>(p, n_ctas, smem, stream, err)
+                     : LaunchFwd<U, FwdBatch<U>::value, false>(p, n_ctas, smem, stream, err);
 }
 
-template <int NT>
 int Dispatch(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_smem, cudaStream_t stream,
              std::string *err) {
+    if (p.Npad > g.n_warps * 32) { *err = "batch too large for the den kernel's bookkeeping CTA (N <= " + std::to_string(g.n_warps * 32) + ")"; return 1; }
+    if (g.n_warps * 32 != kDenThreads) { *err = "unsupported warps per CTA for den kernels (" + std::to_string(kDenThreads / 32) + ")"; return 1; }
     const DevicePass &pass = backward ? g.bwd : g.fwd;
     // Tiers by graph size, for batches of more than 16 utterances.  (1) The whole arc stream in shared memory (8 bytes per
     // forward slot, 12 per backward slot), rows gathered into registers: on an H100 this beats staging the rows by one TMA
@@ -1552,8 +1470,8 @@ int Dispatch(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_sme
             return 1;
         }
         p.use_tma = 1; p.ring_off = (int)ring_off; p.bar_off = (int)bar_off;
-        return LPR == 8 ? LaunchTmaSmall<NT, 8>(backward, w1_smem, p, g.n_ctas, total, stream, err)
-                        : LaunchTmaSmall<NT, 16>(backward, w1_smem, p, g.n_ctas, total, stream, err);
+        return LPR == 8 ? LaunchTmaSmall<8>(backward, w1_smem, p, g.n_ctas, total, stream, err)
+                        : LaunchTmaSmall<16>(backward, w1_smem, p, g.n_ctas, total, stream, err);
     }
     bool tma = false;
     p.use_tma = 0;
@@ -1577,21 +1495,9 @@ int Dispatch(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_sme
             smem = total;
         }
     }
-    if (U == 1) return DispatchU<NT, 1>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
-    if (U == 2) return DispatchU<NT, 2>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
-    return DispatchU<NT, 4>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
-}
-
-int DispatchThreads(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_smem, cudaStream_t stream,
-                    std::string *err) {
-    if (p.Npad > g.n_warps * 32) { *err = "batch too large for the den kernel's bookkeeping CTA (N <= " + std::to_string(g.n_warps * 32) + ")"; return 1; }
-    if (g.n_warps == 16) return Dispatch<512>(backward, g, p, fixed_smem, stream, err);
-#ifdef CCB_TUNING
-    if (g.n_warps == 8) return Dispatch<256>(backward, g, p, fixed_smem, stream, err);   // two co-resident CTAs per SM (experiments)
-    if (g.n_warps == 24) return Dispatch<768>(backward, g, p, fixed_smem, stream, err);
-#endif
-    *err = "unsupported warps per CTA for den kernels (16)";
-    return 1;
+    if (U == 1) return DispatchU<1>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
+    if (U == 2) return DispatchU<2>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
+    return DispatchU<4>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
 }
 
 }  // namespace
@@ -1681,7 +1587,7 @@ int LaunchDenForward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, st
     p.own_c = g.fwd.own_c; p.own = g.own_rows ? 1 : 0;
     p.tile_rows = g.fwd.max_tile_rows;
     const size_t fixed = (((size_t)(p.Npad + p.tile_rows) * 4 + 15) & ~(size_t)15);
-    return DispatchThreads(false, g, p, fixed, stream, err);
+    return Dispatch(false, g, p, fixed, stream, err);
 }
 
 int LaunchDenBackward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err) {
@@ -1693,7 +1599,7 @@ int LaunchDenBackward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, s
     p.gacc_rows = gacc_bytes <= 64 * 1024 ? g.bwd.max_tile_labels : 0;
     p.tile_rows = g.bwd.max_tile_rows;
     const size_t fixed = ((((size_t)(2 + p.gacc_rows) * p.Npad + 2 * (size_t)p.tile_rows) * 4 + 15) & ~(size_t)15);
-    return DispatchThreads(true, g, p, fixed, stream, err);
+    return Dispatch(true, g, p, fixed, stream, err);
 }
 
 int LaunchDenGradNormalize(float *grad, long gsn, long gst, const float *absum, const int *len, int N, int Npad,

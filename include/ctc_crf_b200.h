@@ -123,8 +123,7 @@ int ccb_ctc_forward_backward(const void *logits, int dtype, long sn, long st, in
  * scale = 1/batch for size_average (the caller may split a batch into several calls and sum the losses).
  * Tmax <= T is the number of frames actually walked (max input length of the block); workspaces are sized with
  * ccb_*_floats/bytes(N, Tmax).  parts (optional, may be NULL): 2N floats = [logZ_den | logp_ctc].
- * Everything is enqueued on `stream`.  (Opt-in, CCB_OVERLAP=1 at Init: the numerator's alpha || beta chains are forked onto a
- * library-owned side stream and joined back before the call's last kernels -- one such call per device at a time.) */
+ * Everything is enqueued on `stream`. */
 int ccb_ctc_crf_loss_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax,
                          const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
                          const int *len_dev, int max_label_len, float lamb, float scale,

@@ -48,7 +48,7 @@ def test_status_strings_and_workspace_query():
 def test_ctc_workspace_holds_cells_and_loglikelihoods():
     """ccb_ctc_workspace_bytes: per utterance the alpha and beta cells [T][2L+1] in double + the fp64 log-likelihood, then
     32 doubles of slack, then N floats -- where the fused loss keeps log p(l|x) (api.cu LossFwdImpl places them at double
-    offset N * per_utt + 32; the numerator may run while the den aux block is busy, so they cannot live there)."""
+    offset N * per_utt + 32: the numerator's output lives in the numerator's workspace, not in the den aux block)."""
     from cat_b200 import _lib
     L = _lib.lib()
     L.ccb_ctc_workspace_bytes.restype = C.c_size_t

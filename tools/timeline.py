@@ -18,7 +18,7 @@ lens = torch.full((N,), T, dtype=torch.int32, device="cuda")
 alpha = torch.empty(int(L.ccb_den_alpha_floats(N, T)), device="cuda"); aux = torch.empty(int(L.ccb_den_aux_bytes(N, T)), dtype=torch.uint8, device="cuda")
 grad = torch.zeros(N, T, V, device="cuda"); logz = torch.empty(N, device="cuda")
 n_ctas = torch.cuda.get_device_properties(0).multi_processor_count   # one CTA per SM (den_graph.cc)
-n_chunks = n_ctas * int(os.environ.get("CCB_DEN_WARPS", "16")); steps, step0 = 16, T // 2
+n_chunks = n_ctas * 16; steps, step0 = 16, T // 2   # 16 warps per CTA, one chunk each
 stream = torch.cuda.current_stream().cuda_stream
 def run():
     rc = L.ccb_den_forward_backward(y.data_ptr(), 0, T * V, V, N, T, V, lens.data_ptr(), alpha.data_ptr(), aux.data_ptr(), grad.data_ptr(), T * V, V, 1.0, logz.data_ptr(), None, stream)
