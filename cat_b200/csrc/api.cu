@@ -70,17 +70,8 @@ void FreeDevice(DeviceGraph &d) {
 }
 
 int UploadPass(const PassPlan &h, DevicePass *d) {
-    if (Upload(&d->arcs, h.arcs)) return 1;
-    if (Upload(&d->chunk_state, h.chunk_state)) return 1;
-    if (Upload(&d->chunk_arc, h.chunk_arc)) return 1;
-    if (Upload(&d->chunk_pair, h.chunk_pair)) return 1;
-    if (Upload(&d->cta_labels, h.cta_labels)) return 1;
-    if (Upload(&d->w1, h.w1)) return 1;
-    d->num_arcs = (int)h.arcs.size();
-    d->max_tile_arcs = h.max_tile_arcs;
-    d->max_tile_labels = h.max_tile_labels;
-    d->max_tile_rows = h.max_tile_rows;
-    return 0;
+    return Upload(&d->arcs, h.arcs) || Upload(&d->chunk_state, h.chunk_state) || Upload(&d->chunk_arc, h.chunk_arc) ||
+           Upload(&d->chunk_pair, h.chunk_pair) || Upload(&d->cta_labels, h.cta_labels) || Upload(&d->w1, h.w1);
 }
 
 // The backward pass's quads as the streamed-arc TMA kernel reads them (DevicePass::tq): per quad {row coordinate of slot 0..3}
@@ -143,7 +134,7 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
         d.device = gpus[i];
         d.S = g_plan.num_states; d.P = g_plan.num_pairs; d.start = g_plan.start; d.num_labels = g_plan.num_labels;
         d.scale_exp = g_plan.scale_exp;
-        d.n_ctas = g_plan.n_ctas; d.n_warps = g_plan.n_warps;
+        d.n_ctas = g_plan.n_ctas;
         d.max_smem_optin = (int)p2.sharedMemPerBlockOptin;
         rc = Upload(&d.state_label, g_plan.state_label) || Upload(&d.state_pos, g_plan.state_pos) ||
              Upload(&d.final_lin, g_plan.final_lin) || Upload(&d.start_arcs, g_plan.start_arcs) ||
@@ -151,26 +142,14 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
              UploadPass(g_plan.fwd, &d.fwd) || UploadPass(g_plan.bwd, &d.bwd) ||
              Upload(&d.fwd.own_c, g_plan.own_fwd) || Upload(&d.bwd.own_c, g_plan.own_bwd);
         d.own_rows = g_plan.own_rows;
-        { const char *e = getenv("CCB_ARCS_IN_GLOBAL"); d.tune_arcs_in_global = e && e[0] == '1'; }
-        { const char *e = getenv("CCB_W1_IN_GLOBAL"); d.tune_w1_in_global = e && e[0] == '1'; }
-        { const char *e = getenv("CCB_NO_TMA"); d.tune_no_tma = e && e[0] == '1'; }   // A/B: register gathers instead of TMA row staging
-        // streamed-arc tier: only graphs whose arc stream may not fit shared memory next to the TMA rings carry the copy
-        if (rc == 0 && g_plan.hub_states.empty() && !d.tune_no_tma &&
-            (d.tune_arcs_in_global || (size_t)d.bwd.max_tile_arcs * 12 > kStreamTierArcBytes))
-            rc = UploadTransposedQuads(g_plan.bwd, &d.bwd);   // (the forward pass of such graphs keeps register gathers)
-        if (d.tune_arcs_in_global || d.tune_w1_in_global)
+        auto on = [](const char *name) { const char *e = getenv(name); return e && e[0] == '1'; };
+        d.hooks.arcs_in_global = on("CCB_ARCS_IN_GLOBAL"); d.hooks.w1_in_global = on("CCB_W1_IN_GLOBAL"); d.hooks.no_tma = on("CCB_NO_TMA");
+        d.shape = ShapeOf(g_plan, d.hooks);
+        if (rc == 0 && d.shape.streamed_quads) rc = UploadTransposedQuads(g_plan.bwd, &d.bwd);
+        if (d.hooks.arcs_in_global || d.hooks.w1_in_global)
             fprintf(stderr, "ctc_crf_b200: CCB_ARCS_IN_GLOBAL / CCB_W1_IN_GLOBAL set -- den arc tiles forced out of shared memory (test hook, slow)\n");
-        {   // small-batch kernels: both arc streams in shared memory next to 4 KB (8 KB) of rings per warp, no hub rows
-            const size_t budget = (size_t)d.max_smem_optin > 2048 ? (size_t)d.max_smem_optin - 1024 : 0;
-            // (the backward pass may keep only offsets + first weights resident, 8 bytes per slot, and stream the second weights)
-            const size_t ring = (size_t)d.n_warps * (4 * 16 * 64 + 4 * (8 + 64));
-            const size_t fwd_need = (size_t)d.fwd.max_tile_arcs * sizeof(Arc) + (size_t)(16 + d.fwd.max_tile_rows) * 4 + ring + 512;
-            const size_t bwd_need = (size_t)d.bwd.max_tile_arcs * 8 + ((size_t)(2 + d.bwd.max_tile_labels) * 16 + 2 * (size_t)d.bwd.max_tile_rows) * 4 + ring + 512;
-            d.small_ok = !d.tune_no_tma && !d.tune_arcs_in_global && g_plan.hub_states.empty() &&
-                         fwd_need <= budget && bwd_need <= budget && getenv("CCB_NO_SMALL") == nullptr;
-        }
+        d.small_ok = SmallBatchOk(d.shape, d.max_smem_optin, d.hooks);
         d.n_start_arcs = (int)g_plan.start_arcs.size();
-        d.n_hubs = (int)g_plan.hub_states.size();
         d.start_final = g_plan.final_lin[(size_t)g_plan.start];
         d.loaded = (rc == 0);
         if (rc == 0) ++g_refs[gpus[i]];
@@ -204,8 +183,8 @@ DenParams BaseParams(const DeviceGraph &g, const void *y, int dtype, long sn, lo
     char *a = reinterpret_cast<char *>(aux);
     p.state_label = g.state_label; p.state_pos = g.state_pos; p.final_lin = g.final_lin;
     p.start_arcs = g.start_arcs; p.n_start_arcs = g.n_start_arcs;
-    p.hub_states = g.hub_states; p.n_hubs = g.n_hubs;
-    p.S = g.S; p.num_pairs = g.P; p.start = g.start; p.n_warps = g.n_warps;
+    p.hub_states = g.hub_states; p.n_hubs = g.shape.n_hubs;
+    p.S = g.S; p.num_pairs = g.P; p.start = g.start; p.n_warps = g.shape.n_warps;
     p.scale_exp = g.scale_exp;
     p.start_final = g.start_final;
     p.y = y; p.y_bf16 = (dtype == CCB_DTYPE_BF16); p.sn = sn; p.st = st;
@@ -230,7 +209,7 @@ int CheckDen(const DeviceGraph &g, int dtype, int N, int T, int V) {
     if (V < g.num_labels)
         return Fail("den graph uses label " + std::to_string(g.num_labels - 1) + " but logits have only " + std::to_string(V) + " classes");
     if ((size_t)(2 * (size_t)g.S + g.P) * (size_t)PadLanes(N, g.small_ok) * 4 >= ((size_t)1 << 32)) return Fail("den: states x batch too large for 32-bit row offsets; split the batch");
-    if (PadLanes(N, g.small_ok) > g.n_warps * 32) return Fail("den: batch larger than " + std::to_string(g.n_warps * 32) + " utterances per call; split the batch");
+    if (PadLanes(N, g.small_ok) > g.shape.n_warps * 32) return Fail("den: batch larger than " + std::to_string(g.shape.n_warps * 32) + " utterances per call; split the batch");
     return 0;
 }
 
@@ -264,7 +243,7 @@ int DenForward(const DeviceGraph &g, const void *y, int dtype, long sn, long st,
         p.ckpt_mode = 1; p.a_ring = kAlphaRing; p.a_frames = kAlphaRing + 2;
     }
     std::string err;
-    rc = LaunchDenForward(g, p, stream, &err);
+    rc = LaunchDen(false, g, p, stream, &err);
     if (rc) return Fail(err);
     return 0;
 }
@@ -289,7 +268,7 @@ int DenBackward(const DeviceGraph &g, const void *y, int dtype, long sn, long st
     int rc = 0;
     if (ckpt_k <= 0) {
         CCB_CUDA(cudaMemsetAsync(a + L.barrier + 128, 0, 128, stream));
-        rc = LaunchDenBackward(g, p, stream, &err);
+        rc = LaunchDen(true, g, p, stream, &err);
         if (rc) return Fail(err);
     } else {
         SetCkpt(p, g, T, ckpt_k);
@@ -302,11 +281,11 @@ int DenBackward(const DeviceGraph &g, const void *y, int dtype, long sn, long st
             f.t_lo = lo; f.t_hi = hi;
             f.barrier = reinterpret_cast<unsigned *>(a + L.barrier);
             CCB_CUDA(cudaMemsetAsync(a + L.barrier, 0, 128, stream));
-            rc = LaunchDenForward(g, f, stream, &err);
+            rc = LaunchDen(false, g, f, stream, &err);
             if (rc) return Fail(err);
             p.a_base = lo; p.t_lo = lo; p.t_hi = hi;   // tau = hi .. lo + 1 (tau = 0 epilogue with the first segment)
             CCB_CUDA(cudaMemsetAsync(a + L.barrier + 128, 0, 128, stream));
-            rc = LaunchDenBackward(g, p, stream, &err);
+            rc = LaunchDen(true, g, p, stream, &err);
             if (rc) return Fail(err);
         }
     }
@@ -739,6 +718,20 @@ int ccb_plan_copy(void *plan, int which, void *dst, size_t dst_bytes) {
     }
     if (bytes > dst_bytes) return 2;
     memcpy(dst, src, bytes);
+    return 0;
+}
+
+int ccb_plan_launch(void *plan, int N, int backward, int smem_optin, int hooks, long *out) {
+    g_err.clear();
+    if (!plan || !out || N <= 0) return Fail("ccb_plan_launch: bad arguments");
+    const DenHooks h{(hooks & 1) != 0, (hooks & 2) != 0, (hooks & 4) != 0};
+    const DenGraphShape g = ShapeOf(*reinterpret_cast<const DenPlan *>(plan), h);
+    const int Npad = PadLanes(N, SmallBatchOk(g, smem_optin, h));
+    DenLaunch L;
+    if (!ChooseDenLaunch(g, Npad, backward != 0, smem_optin, h, &L, &g_err)) return 1;
+    const long v[] = {L.tier, L.lanes_per_row, L.U, L.batch, L.w1_smem, Npad, L.tile_rows, L.gacc_rows, (long)L.arcs_off,
+                      (long)L.ring_off, (long)L.bar_off, (long)L.w1_off, (long)L.abar_off, (long)L.aring_off, (long)L.total};
+    memcpy(out, v, sizeof(v));
     return 0;
 }
 

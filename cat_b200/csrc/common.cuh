@@ -7,7 +7,7 @@
 #include <cstdint>
 #include <string>
 
-#include "den_graph.h"
+#include "den_launch.h"
 
 namespace ccb {
 
@@ -15,11 +15,6 @@ namespace ccb {
 // Device copy of the den plan (one per GPU listed in Init()).
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kOobRow = 0x40000000u;   // a TMA row coordinate no gather table reaches (tables are limited to 2^30 rows)
-// backward arc bytes per CTA tile (12 per slot) above which a graph also gets the streamed-arc copy of its quads: below it
-// the stream fits shared memory next to the deepest rings at every batch width
-constexpr size_t kStreamTierArcBytes = 72 * 1024;
-// threads per CTA of the persistent den kernels: 16 warps, one CTA per SM (the den plan is built for 16 warps per CTA)
-constexpr int kDenThreads = 512;
 
 struct DevicePass {
     Arc *arcs = nullptr;
@@ -29,14 +24,9 @@ struct DevicePass {
     int *cta_labels = nullptr;
     float *w1 = nullptr;      // backward pass: second weight per slot
     float *own_c = nullptr;   // [2S + 4] own-row coefficients of this pass (DenPlan::own_fwd / own_bwd)
-    // Streamed-arc tier (backward pass of graphs whose arc stream does not fit shared memory): the pass's quads as the TMA
-    // kernel stages them, 3 16-byte words per quad {row coordinate 0..3}{w0 0..3}{w1 0..3}; built at Init when the graph is
-    // large enough to need it, else null
+    // streamed-arc tier (DenGraphShape::streamed_quads, else null): the backward quads as the TMA kernel stages them, 3
+    // 16-byte words per quad {row coordinate 0..3}{w0 0..3}{w1 0..3}
     uint4 *tq = nullptr;
-    int num_arcs = 0;
-    int max_tile_arcs = 0;
-    int max_tile_labels = 0;
-    int max_tile_rows = 0;
 };
 
 struct DeviceGraph {
@@ -44,21 +34,19 @@ struct DeviceGraph {
     int device = -1;
     int S = 0, P = 0, start = 0, num_labels = 0;   // S states, P pairs (gather-table rows S..S+P-1 = virtual pair-sum rows)
     int scale_exp = 56;
-    int n_ctas = 0, n_warps = 0;
+    int n_ctas = 0;
+    DenGraphShape shape;   // what the kernel launch is chosen on (den_launch.h)
     int *state_label = nullptr;
     int *state_pos = nullptr;
     float *final_lin = nullptr;
     DevicePass fwd, bwd;
     Arc *start_arcs = nullptr;   // out-arcs of the start state
     int n_start_arcs = 0;
-    int *hub_states = nullptr;   // states whose forward row is accumulated from parts
-    int n_hubs = 0;
+    int *hub_states = nullptr;   // states whose forward row is accumulated from parts (shape.n_hubs)
     float start_final = 0.f;
     int max_smem_optin = 0;
-    // test hooks, read ONCE at Init (never on the per-call path): force the large-graph tiers on a small graph
-    bool tune_arcs_in_global = false, tune_w1_in_global = false, tune_no_tma = false;
-    // batches of <= 16 utterances run the small-batch TMA kernels (rows of 8 / 16 floats): needs both arc streams in
-    // shared memory next to the rings, no hub rows, and a usable TMA descriptor -- decided once at Init
+    DenHooks hooks;        // test hooks, read ONCE at Init (never on the per-call path)
+    // batches of <= 16 utterances run the small-batch kernels (rows of 16 floats): SmallBatchOk, decided once at Init
     bool small_ok = false;
     bool own_rows = false;     // DenPlan::own_rows: own-row coefficients instead of own-row arcs (DevicePass::own_c)
 };
@@ -66,12 +54,14 @@ struct DeviceGraph {
 // Kernel parameter block shared by the two persistent den kernels (passed as a __grid_constant__ kernel parameter: the TMA
 // descriptor inside it is read by the hardware straight from parameter memory and must sit on a 64-byte boundary).
 struct alignas(64) DenParams {
-    // TMA view of the pass's gather table (forward: the alpha spill, backward: the beta ping-pong) as a 2-D tensor
-    // [rows][Npad] of fp32 with a box of one row x (32 * utterances per lane) columns; used by the full-width TMA kernels only
+    // TMA view of the backward gather table (the beta ping-pong) as a 2-D tensor [rows][Npad] of fp32 with a box of one
+    // row x (32 * utterances per lane) columns; used by the streamed-arc tier only
     CUtensorMap tmap;
-    int use_tma;          // 1: rows are staged in shared memory by TMA / bulk copies (den_kernels.cu), 0: register gathers
-    int ring_off;         // byte offset of the per-warp row rings in dynamic shared memory (128-byte aligned)
-    int bar_off;          // byte offset of the rings' mbarriers
+    // Byte offsets in dynamic shared memory (DenLaunch) of the streamed-arc tier's arc-ring mbarriers, the row rings and their
+    // mbarriers.  (Kept at these offsets: shifting the pointers below by 8 bytes makes ptxas spill in several variants.)
+    int abar_off;
+    int ring_off;
+    int bar_off;
     // graph
     const Arc *arcs;
     const float *w1;      // backward pass only
@@ -82,7 +72,7 @@ struct alignas(64) DenParams {
     const int *state_label;
     const int *state_pos;
     const uint4 *tq;          // streamed-arc tier: the pass's transposed quads in global memory (DevicePass::tq)
-    int aring_off, abar_off;  // ... byte offsets in dynamic shared memory of the per-warp arc rings and their mbarriers
+    int aring_off;            // ... byte offset in dynamic shared memory of the per-warp rings they flow through
     const float *final_lin;
     const Arc *start_arcs;
     int n_start_arcs;
@@ -137,9 +127,8 @@ struct DenAuxLayout {
     size_t colsum_a = 0, colsum_b = 0, absum = 0, zsum = 0, b0 = 0, barrier = 0, zero_bytes = 0;
     size_t fmax = 0, bh = 0, logz_a = 0, logz_b = 0, lz = 0, lnorm = 0, total = 0;
 };
-// Lane padding of a batch: whole 32-lane groups carrying 1, 2 or 4 utterances per lane; batches of <= 16 utterances
-// on a graph that supports the small-batch kernels (DeviceGraph::small_ok) use 8- or 16-float rows instead, with the
-// lanes of a warp spread over (arc of the quad) x (utterance)  (den_kernels.cu, LPR template parameter).
+// Lane padding of a batch: whole 32-lane groups carrying 1, 2 or 4 utterances per lane; batches of <= 16 utterances on a
+// graph that supports the small-batch kernels (DeviceGraph::small_ok) use 16-float rows instead (den_kernels.cu SMALL).
 inline int PadLanes(int N, bool small_ok) {
     // (16-float rows even for N <= 8: the row copies are bound by their count, not by their bytes)
     if (small_ok && N <= 16) return 16;
@@ -148,7 +137,6 @@ inline int PadLanes(int N, bool small_ok) {
     return g * 32;
 }
 DenAuxLayout MakeDenAuxLayout(int S, int N, int T, bool small_ok);
-inline int LaneWidth(int Npad) { int g = Npad / 32; return g >= 4 ? 4 : (g < 1 ? 1 : g); }
 
 // host launchers; return cudaError_t-compatible int (0 = ok) and fill *err
 int LaunchFrameMax(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *len, float *fmax,
@@ -163,11 +151,8 @@ constexpr int kAlphaRing = 4;
 inline int CkptK(int T, int K) { return K < T ? K : T; }
 inline int CkptSegFrames(int T, int K) { const int k = CkptK(T, K); return (k + 1 > kAlphaRing ? k + 1 : kAlphaRing) + 2; }
 inline int CkptCount(int T, int K) { const int k = CkptK(T, K); return (T + k - 1) / k; }
-int LaunchDenForward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err);
-int LaunchDenBackward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err);
-// fills *tm with the 2-D view [rows][Npad] fp32 of `base`, box = 1 row x box_cols columns; false if the driver entry
-// point is unavailable or refuses the shape (the callers then keep the register-gather kernels)
-bool EncodeRowTensorMap(CUtensorMap *tm, const float *base, size_t rows, int Npad, int box_cols);
+// one persistent den pass (the forward or the backward recursion) with the launch den_launch.h chooses
+int LaunchDen(bool backward, const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err);
 int LaunchDenGradNormalize(float *grad, long gsn, long gst, const float *absum, const int *len, int N, int Npad,
                            int T, int V, float scale, cudaStream_t stream);
 int LaunchCtc(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,

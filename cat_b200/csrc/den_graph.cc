@@ -1,5 +1,6 @@
-// Host-side den-graph loader and kernel plan.  See den_graph.h.
+// Host-side den-graph loader, kernel plan and kernel launch decision.  See den_graph.h and den_launch.h.
 #include "den_graph.h"
+#include "den_launch.h"
 
 #include <algorithm>
 #include <cmath>
@@ -221,11 +222,10 @@ static bool BuildDenPlanImpl(const HostFst &fst, int n_ctas, int n_warps, bool a
 
 bool BuildDenPlan(const HostFst &fst, int n_ctas, int n_warps, DenPlan *plan, std::string *err) {
     if (!BuildDenPlanImpl(fst, n_ctas, n_warps, true, plan, err)) return false;
-    // Own-row terms are for graphs that run the main tier (arc streams resident in shared memory next to the TMA rings).  A
-    // graph whose backward stream exceeds kOwnRowsMaxTileBytes per CTA runs the large-graph tiers (register gathers forwards,
-    // streamed arcs backwards), where the extra row loads and registers cost more than the dropped padding returns
-    // (5.1 M-arc graph, N=128, T=2000: 615 ms per step with own-row terms against 575 ms without): build it without them.
-    if (plan->own_rows && (size_t)plan->bwd.max_tile_arcs * 12 > kOwnRowsMaxTileBytes) {
+    // Own-row terms are for graphs that run the main tier.  On the large-graph tiers (LargeGraphTiers: register gathers forwards,
+    // streamed arcs backwards) the extra row loads and registers cost more than the dropped padding returns (5.1 M-arc
+    // graph, N=128, T=2000: 615 ms per step with own-row terms against 575 ms without): build such a graph without them.
+    if (plan->own_rows && LargeGraphTiers(plan->bwd.max_tile_arcs)) {
         *plan = DenPlan();
         return BuildDenPlanImpl(fst, n_ctas, n_warps, false, plan, err);
     }
@@ -754,6 +754,75 @@ static bool BuildDenPlanImpl(const HostFst &fst, int n_ctas, int n_warps, bool a
     Layout(fgroups, (int)S, plan->state_label, plan->state_pos, n_ctas, n_warps, chunk_group, false, &plan->fwd);
     Layout(bgroups, (int)S, plan->state_label, plan->state_pos, n_ctas, n_warps, chunk_group, true, &plan->bwd);
     return true;
+}
+
+// ---- launch of the persistent den kernels (den_launch.h) ----
+bool ChooseDenLaunch(const DenGraphShape &g, int Npad, bool backward, int smem_optin, const DenHooks &hooks, DenLaunch *out,
+                     std::string *why) {
+    if (g.n_warps * 32 != kDenThreads || Npad > kDenThreads || (Npad != kSmallLanes && Npad != 32 && Npad != 64 && (Npad <= 0 || Npad % 128))) {
+        *why = "den: no kernel for " + std::to_string(Npad) + " lanes at " + std::to_string(g.n_warps) + " warps per CTA (16, N <= 512)";
+        return false;
+    }
+    const DenPassShape &pass = backward ? g.bwd : g.fwd;
+    auto up128 = [](size_t x) { return (x + 127) & ~(size_t)127; };
+    const size_t budget = (size_t)smem_optin > 2048 ? (size_t)smem_optin - 1024 : 0, nw = (size_t)g.n_warps;
+    DenLaunch L;
+    L.tile_rows = pass.max_tile_rows;   // and backward, the label accumulator in shared memory if the CTA's label range is small
+    L.gacc_rows = backward && (size_t)pass.max_tile_labels * Npad * 4 <= 64 * 1024 ? pass.max_tile_labels : 0;
+    L.arcs_off = backward ? BwdArcsOff(Npad, L.gacc_rows, L.tile_rows) : FwdArcsOff(Npad, L.tile_rows);
+    // Tiers by graph size, for batches of more than 16 utterances.  (1) The whole arc stream in shared memory (8 bytes per
+    // forward slot, 12 per backward slot), rows gathered into registers: on an H100 this beats staging the rows by one TMA
+    // copy each at every batch width (N = 32 / 64 / 128, T = 1500, 1.02 M arcs: 46.7 / 79.9 / 160.1 ms per step against
+    // 56.0 / 87.5 / 175.1 ms, 700 W, 1980 MHz); (2) backward only: offsets + first weights in shared memory, second weights
+    // streamed from L2, or the streamed-arc TMA tier below; (3) everything from L2.
+    // Small batches: the arc stream must fit NEXT TO the small-batch rings; the 12-byte backward form gives way to the 8-byte
+    // one when only that leaves them room.
+    const bool small = Npad == kSmallLanes;
+    const size_t small_extra = small ? 128 + nw * (kSmallRingWarpBytes + kSmallBarWarpBytes + kSmallW1WarpBytes) : 0;
+    bool w1_smem = backward && !hooks.w1_in_global;
+    size_t arc_bytes = (size_t)pass.max_tile_arcs * (w1_smem ? 12 : sizeof(Arc));
+    if (w1_smem && L.arcs_off + arc_bytes + small_extra > budget) { w1_smem = false; arc_bytes = (size_t)pass.max_tile_arcs * sizeof(Arc); }
+    const bool smem_arcs = L.arcs_off + arc_bytes + small_extra <= budget && !hooks.arcs_in_global;
+    if (small) {   // one utterance per lane, 16 lanes per row; needs the arc tile resident and no hub rows
+        L.tier = kTierSmall; L.lanes_per_row = kSmallLanes; L.batch = kSmallRows; L.w1_smem = w1_smem;
+        L.ring_off = up128(L.arcs_off + (smem_arcs ? arc_bytes : 0)); L.bar_off = L.ring_off + nw * kSmallRingWarpBytes;
+        L.w1_off = SmallW1Off((uint32_t)L.bar_off, g.n_warps); L.total = L.w1_off + nw * kSmallW1WarpBytes;   // (forward too)
+        *out = L;
+        if (smem_arcs && L.total <= budget && g.n_hubs == 0 && !hooks.no_tma) return true;
+        *why = "den: no small-batch kernels for this graph/device (smem " + std::to_string(L.total) + "/" + std::to_string(budget) + ")";
+        return false;
+    }
+    // utterances per lane: the widest row segment the batch allows, except that the backward pass (two accumulators per
+    // utterance) spills at 4 -- it walks 64-utterance groups instead
+    L.U = Npad >= 128 ? (backward ? 2 : 4) : Npad / 32;
+    // Streamed-arc TMA tier, BACKWARD pass only: the stream does not fit (or the test hook says so) but the graph carries the
+    // transposed copy.  The forward pass of such graphs keeps the register gathers with the arcs read from L2: its 8-byte
+    // slots would make 128-byte bulk copies, one per 16 rows.
+    if (backward && !(smem_arcs && w1_smem) && g.streamed_quads && g.n_hubs == 0 && !hooks.no_tma) {
+        DenLaunch S = L;
+        S.tier = kTierStreamed; S.batch = kStreamRows;
+        S.ring_off = up128(S.arcs_off); S.bar_off = S.ring_off + nw * StreamRingWarpBytes(S.U);
+        S.abar_off = S.bar_off + nw * kStreamBarWarpBytes; S.aring_off = up128(S.abar_off + nw * kArcBarWarpBytes);
+        S.total = S.aring_off + nw * kArcRingWarpBytes;
+        if (S.total <= budget) { *out = S; return true; }
+    }
+    L.tier = smem_arcs ? kTierShared : kTierGlobal; L.w1_smem = smem_arcs && w1_smem;
+    L.batch = backward ? kBwdBatch : FwdBatch(L.U); L.total = L.arcs_off + (smem_arcs ? arc_bytes : 0);
+    *out = L;
+    return true;
+}
+
+bool SmallBatchOk(const DenGraphShape &g, int smem_optin, const DenHooks &hooks) {
+    DenLaunch L;
+    std::string why;
+    return ChooseDenLaunch(g, kSmallLanes, false, smem_optin, hooks, &L, &why) && ChooseDenLaunch(g, kSmallLanes, true, smem_optin, hooks, &L, &why);
+}
+
+DenGraphShape ShapeOf(const DenPlan &plan, const DenHooks &hooks) {
+    const int n_hubs = (int)plan.hub_states.size();
+    return {{plan.fwd.max_tile_arcs, plan.fwd.max_tile_rows, plan.fwd.max_tile_labels},
+            {plan.bwd.max_tile_arcs, plan.bwd.max_tile_rows, plan.bwd.max_tile_labels}, n_hubs, plan.n_warps,
+            n_hubs == 0 && !hooks.no_tma && (hooks.arcs_in_global || LargeGraphTiers(plan.bwd.max_tile_arcs))};
 }
 
 }  // namespace ccb

@@ -33,8 +33,6 @@ static constexpr int kEvPairMerged = 3;  // forward only, plans WITHOUT high in-
                                          // contain): the segment ends BOTH rows of a pair.  Slots 0 .. n-2 are the in-arcs of the second
                                          // member, the LAST slot is the single in-arc of the first member (DenPlan::fwd_merged);
                                          // with own-row terms (DenPlan::own_rows) there is no such tail slot: all slots are the second member's
-static constexpr size_t kOwnRowsMaxTileBytes = 72 * 1024;   // (= common.cuh kStreamTierArcBytes: the backward stream, 12 bytes per slot and
-                                                            //  CTA, up to which a graph runs the main tier at every batch width)
 static constexpr int kHubInArcs = 384;   // rows with more in-arcs than this are split into parts of kPartArcs arcs that
 static constexpr int kPartArcs = 191;    // any warp of the grid can own (real n-gram den graphs have such states)
 

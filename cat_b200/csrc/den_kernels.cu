@@ -390,11 +390,6 @@ __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence
 struct TmaRing {
     uint32_t buf, bar, phase;
 };
-// rows per ring stage (two stages per warp) of the streamed-arc backward tier
-template <int U> struct TmaShape;
-template <> struct TmaShape<1> { static constexpr int R = 16; };
-template <> struct TmaShape<2> { static constexpr int R = 16; };
-template <> struct TmaShape<4> { static constexpr int R = 8; };
 
 template <int U> __device__ __forceinline__ Vec<U> lds_row(uint32_t addr);
 template <> __device__ __forceinline__ Vec<1> lds_row<1>(uint32_t addr) {
@@ -407,11 +402,6 @@ template <> __device__ __forceinline__ Vec<2> lds_row<2>(uint32_t addr) {
     asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(r.v[0]), "=f"(r.v[1]) : "r"(addr));
     return r;
 }
-template <> __device__ __forceinline__ Vec<4> lds_row<4>(uint32_t addr) {
-    Vec<4> r;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]) : "r"(addr));
-    return r;
-}
 
 // Streamed arcs (graphs whose arc stream does not fit shared memory, BASELINE config 4: 5 M arcs): the chunk's quads are
 // not resident; they flow through a per-warp ring of kArcStages batches, filled by 1-D bulk copies (`cp.async.bulk`, SASS
@@ -419,7 +409,6 @@ template <> __device__ __forceinline__ Vec<4> lds_row<4>(uint32_t addr) {
 // The ring is topped up after every consumed batch and runs across frames and lane groups: the first kArcStages batches
 // of the NEXT walk are requested at the end of this one, so they are in shared memory before the grid barrier opens.
 // Batches are counted from the start of the kernel (stage = count % kArcStages, parity = count / kArcStages & 1).
-constexpr int kArcStages = 8;
 struct ArcRing {
     const uint4 *buf;        // this warp's ring in shared memory ...
     uint32_t buf_s, bar;     // ... its shared-memory address, and its first mbarrier
@@ -498,16 +487,13 @@ __device__ __forceinline__ void walk_arcs_tma_stream(ArcRing &ar, int n_batches,
     }
 }
 
-// Small batches (Npad = LPR = 8 or 16 utterances): a row of the gather table is 32 / 64 bytes, and the lanes of a warp are
-// spread over (arc of the quad) x (utterance): the four rows of a quad lie back to back in the ring (4 * LPR floats), so
-// ONE `LDS.32` per lane reads 32 / LPR arcs x LPR utterances at once (LPR = 8: a whole quad per instruction; 16: two
-// instructions), each lane multiplies by the weight of ITS arc, and the partial sums of the 32 / LPR lane groups are
-// combined with one or two shuffles when a segment ends.  A warp thus spends 4x (2x) fewer instructions and rows of L2
-// traffic per utterance than with 24 (16) of 32 lanes idle -- the per-GPU share of a batch sharded over 8 GPUs is 8-32
-// utterances (SURVEY.md 8e).  Rings: kSmallStages stages of 16 rows per warp.  Rows this short sit below the 128-byte
-// alignment a tensor copy's destination needs, so each row is a 1-D bulk copy from `table` (16-byte alignment), one per
-// lane, and the lane of a padding slot (kOobRow) zero-fills its row with shared stores instead.
-constexpr int kSmallStages = 4;
+// Small batches (Npad = 16 utterances): a row of the gather table is 64 bytes, and the lanes of a warp are spread over (arc
+// of the quad) x (utterance): the four rows of a quad lie back to back in the ring, so two `LDS.32` per lane read 2 arcs x
+// 16 utterances each, each lane multiplies by the weight of ITS arc, and the two lane groups' partial sums are combined with
+// one shuffle when a segment ends: half the instructions and rows of L2 traffic per utterance of 16 idle lanes (the per-GPU
+// share of a batch sharded over 8 GPUs is 8-32 utterances, SURVEY.md 8e).  Rings: kSmallStages stages of kSmallRows rows
+// per warp.  Rows this short sit below the 128-byte alignment a tensor copy's destination needs, so each row is a 1-D bulk
+// copy from `table` (16-byte alignment), one per lane; the lane of a padding slot (kOobRow) zero-fills its row instead.
 __device__ __forceinline__ float lds_f32(uint32_t addr) {
     float r;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(r) : "r"(addr));
@@ -516,12 +502,12 @@ __device__ __forceinline__ float lds_f32(uint32_t addr) {
 // W1_STREAM (backward pass of graphs whose 12-byte slots do not fit shared memory): the SECOND weights of a batch -- 16
 // consecutive floats of DenPlan::bwd.w1 -- are not resident; they ride along with the batch's rows as one 64-byte bulk copy
 // into `w1buf` (one 64-byte slot per stage) on the same mbarrier, and `consume_quad` receives their shared-memory address.
-template <int LPR, int WPQ, bool W1_STREAM = false, typename Prologue, typename ConsumeQuad>
+template <int WPQ, bool W1_STREAM = false, typename Prologue, typename ConsumeQuad>
 __device__ __forceinline__ void walk_arcs_tma_small(const uint4 *arcs, int n_batches, const float *table, int row_base,
                                                     TmaRing &ring, int lane, Prologue &&prologue, ConsumeQuad &&consume_quad,
                                                     const float *w1g = nullptr, uint32_t w1buf = 0u) {
-    constexpr int R = 16, QB = R / kQuad, STEPS = LPR / 8;      // LDS steps per quad: 1 (LPR = 8) or 2 (LPR = 16)
-    constexpr uint32_t ROWB = LPR * 4u;
+    constexpr int R = kSmallRows, QB = R / kQuad;
+    constexpr uint32_t ROWB = kSmallLanes * 4u;
     auto issue = [&](int k, int s) {
         const uint32_t bar = ring.bar + 8u * s, dst = ring.buf + (uint32_t)(s * R + lane) * ROWB;
         const uint32_t row = lane < R ? (uint32_t)quad_row(arcs[(size_t)WPQ * (k * QB + lane / kQuad)], lane % kQuad) : kOobRow;
@@ -537,7 +523,7 @@ __device__ __forceinline__ void walk_arcs_tma_small(const uint4 *arcs, int n_bat
             if (W1_STREAM) bulk_g2s(w1buf + 64u * s, w1g + (size_t)k * R, R * 4u, bar);
         }
         __syncwarp();   // (also orders the zero stores before every lane's reads of the stage)
-        if (row != kOobRow) bulk_g2s(dst, table + (size_t)(row_base + (int)row) * LPR, ROWB, bar);
+        if (row != kOobRow) bulk_g2s(dst, table + (size_t)(row_base + (int)row) * kSmallLanes, ROWB, bar);
     };
     if (n_batches <= 0) { prologue(); return; }
     for (int k = 0; k < kSmallStages && k < n_batches; ++k) issue(k, k);
@@ -549,9 +535,9 @@ __device__ __forceinline__ void walk_arcs_tma_small(const uint4 *arcs, int n_bat
         const uint32_t base = ring.buf + (uint32_t)(s * R) * ROWB + (uint32_t)lane * 4u;
 #pragma unroll
         for (int q = 0; q < QB; ++q) {
-            float v[STEPS];
+            float v[2];   // slots sub and 2 + sub (two LDS steps per quad)
 #pragma unroll
-            for (int st = 0; st < STEPS; ++st) v[st] = lds_f32(base + (uint32_t)q * (kQuad * ROWB) + (uint32_t)st * 128u);
+            for (int st = 0; st < 2; ++st) v[st] = lds_f32(base + (uint32_t)q * (kQuad * ROWB) + (uint32_t)st * 128u);
             consume_quad(arcs + (size_t)WPQ * (k * QB + q), v, w1buf + 64u * s + 16u * q);
         }
         __syncwarp();
@@ -645,17 +631,17 @@ __device__ __forceinline__ void ckpt_frame_done(const DenParams &P, int t, const
 // ------------------------------------------------------------------------------------------------
 // HUBS: the plan contains high in-degree rows split into parts (kEvPartial segments); the common case compiles the
 // partial-row path out entirely so that it costs the hot row-end code nothing.
-// LPR = 32: rows are gathered into registers (walk_arcs).  LPR < 32 (8 or 16 lanes per row): the small-batch variant, whose
-// rows are staged in shared memory by bulk copies (TMA, walk_arcs_tma_small); needs the arc tile in shared memory
+// Rows are gathered into registers (walk_arcs), except in the small-batch variant (SMALL: 16 lanes per row), whose rows
+// are staged in shared memory by bulk copies (TMA, walk_arcs_tma_small); it needs the arc tile in shared memory
 // (SMEM_ARCS), one utterance per lane and no hub rows.
-template <int U, int BATCH, bool SMEM_ARCS, bool HUBS, int LPR = 32>
+template <int U, int BATCH, bool SMEM_ARCS, bool HUBS, bool SMALL = false>
 __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __grid_constant__ DenParams P) {
-    constexpr bool TMA = LPR < 32;
-    static_assert(!TMA || (SMEM_ARCS && U == 1 && !HUBS && (LPR == 8 || LPR == 16)), "small-batch variant: arc tile in shared memory, one utterance per lane, no hubs");
+    constexpr int LPR = SMALL ? kSmallLanes : 32;   // lanes per row
+    static_assert(!SMALL || (SMEM_ARCS && U == 1 && !HUBS), "small-batch variant: arc tile in shared memory, one utterance per lane, no hubs");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float *s_sum = reinterpret_cast<float *>(smem_raw);                                  // [Npad]
     int *s_label = reinterpret_cast<int *>(s_sum + P.Npad);                              // [tile_rows] label per row
-    Arc *s_arcs = reinterpret_cast<Arc *>(smem_raw + (((size_t)(P.Npad + P.tile_rows) * 4 + 15) & ~(size_t)15));
+    Arc *s_arcs = reinterpret_cast<Arc *>(smem_raw + FwdArcsOff(P.Npad, P.tile_rows));
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(kFull, tid >> 5, 0);   // (through a shuffle: lets ptxas keep warp-derived addresses in uniform registers)
@@ -683,14 +669,13 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
     int labp0 = -1, labp1 = -1;
     for (int q = se - 1; q >= sb; --q) { if (__ldg(P.state_pos + q)) labp1 = __ldg(P.state_label + q); else labp0 = __ldg(P.state_label + q); }
     unsigned epoch = 0;
-    const int n_batches = (ae - ab) / (TMA ? 16 : BATCH);   // (small batches: 16 rows per ring stage)
+    const int n_batches = (ae - ab) / (SMALL ? kSmallRows : BATCH);   // (small batches: kSmallRows rows per ring stage)
     const uint4 *const arc4 = SMEM_ARCS ? reinterpret_cast<const uint4 *>(s_arcs + (ab - tile_a0))
                                         : reinterpret_cast<const uint4 *>(P.arcs + ab);
     TmaRing ring{0u, 0u, 0u};
-    if (TMA) {
-        constexpr uint32_t kRingBytes = (uint32_t)kSmallStages * 16u * LPR * 4u;
-        ring.buf = smem_u32(smem_raw + P.ring_off) + (uint32_t)warp * kRingBytes;
-        ring.bar = smem_u32(smem_raw + P.bar_off) + (uint32_t)warp * 8u * kSmallStages;
+    if (SMALL) {
+        ring.buf = smem_u32(smem_raw + P.ring_off) + (uint32_t)warp * kSmallRingWarpBytes;
+        ring.bar = smem_u32(smem_raw + P.bar_off) + (uint32_t)warp * kSmallBarWarpBytes;
         if (lane == 0) {
             for (int st = 0; st < kSmallStages; ++st) mbar_init(ring.bar + 8u * st, 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -707,9 +692,9 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
         const uint4 *src = reinterpret_cast<const uint4 *>(P.arcs + tile_a0);
         for (int i = tid; i < (tile_a1 - tile_a0) / kQuad; i += kDenThreads) {
             const uint4 m0 = __ldg(src + 2 * i), m1 = __ldg(src + 2 * i + 1);
-            const uint32_t mul = TMA ? 1u : row_bytes;   // TMA: row coordinates; register gathers: byte offsets
+            const uint32_t mul = SMALL ? 1u : row_bytes;   // TMA: row coordinates; register gathers: byte offsets
             uint4 pr = make_uint4(fwd_row(m0.x, S) * mul, fwd_row(m0.z, S) * mul, fwd_row(m1.x, S) * mul, fwd_row(m1.z, S) * mul);
-            if (TMA) {
+            if (SMALL) {
                 // zero-weight padding slots name a row coordinate beyond the tensor: the TMA unit zero-fills them in shared
                 // memory without touching L2 (17 % of the forward stream; the register path gets these from L1 instead)
                 if ((m0.y & 0x7fffffffu) == 0u) pr.x = kOobRow;
@@ -753,13 +738,13 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
 #pragma unroll
     for (int u = 0; u < U; ++u) len0[u] = (ul * U + u < P.N) ? __ldg(P.len + ul * U + u) : 0;
     double runlog = 0.0;
-    if (TMA) fence_proxy_async_global();
+    if (SMALL) fence_proxy_async_global();
     grid_barrier(P.barrier, (++epoch) * gridDim.x);
     if (P.ckpt_mode == 1) ckpt_frame_done(P, 0, P.alpha, sb, se, lane);
 
     for (int t = P.t_lo + 1; t <= P.t_hi; ++t) {
         tl_mark(P, t, chunk, n_chunks, 0, lane);
-        if (TMA) fence_proxy_async_global();
+        if (SMALL) fence_proxy_async_global();
         const int p_prev = alpha_pos(P, t - 1);
         const float *a_prev = P.alpha + (size_t)p_prev * frame_elems;
         float *a_cur = P.alpha + (size_t)alpha_pos(P, t) * frame_elems;
@@ -787,7 +772,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
                 if (!own || (int)row >= se) return;
                 c01 = __ldg(reinterpret_cast<const float2 *>(P.own_c) + row);
                 c23 = __ldg(reinterpret_cast<const float2 *>(P.own_c) + row + 1);
-                if (TMA || lane_act) {
+                if (SMALL || lane_act) {
                     xa = gather_row<U>(x_base, row * row_bytes);
                     if ((int)row + 1 < se) xb = gather_row<U>(x_base, (row + 1u) * row_bytes);
                 }
@@ -838,13 +823,13 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
                         const float s1 = own ? fmaf(c23.x, xa.v[u], fmaf(c23.y, xb.v[u], acc[u])) : a2[u];
                         o0.v[u] = s0 * ec0[u] * r[u];   // (no own terms: same operation order as a one-arc row, fma(w, v, 0) * e * r)
                         o1.v[u] = s1 * ec1[u] * r[u];
-                        if (TMA && !act[u]) { o0.v[u] = 0.f; o1.v[u] = 0.f; }
+                        if (SMALL && !act[u]) { o0.v[u] = 0.f; o1.v[u] = 0.f; }
                         ov.v[u] = o0.v[u] + o1.v[u];
                         sum[u] += o0.v[u];
                         sum[u] += o1.v[u];
                         acc[u] = 0.f;
                     }
-                    if ((TMA || lane_act) && sub == 0) {
+                    if ((SMALL || lane_act) && sub == 0) {
                         o0.stcg(row_ptr<U>(out_base, out_row, row_bytes));
                         o1.stcg(row_ptr<U>(out_base, out_row + 1u, row_bytes));
                         ov.stcg(row_ptr<U>(out_base, virt_row, row_bytes));
@@ -884,48 +869,45 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
                     out.v[u] = acc[u] * (k1 ? ec1[u] : ec0[u]) * r[u];   // ec is 0 for inactive utterances
                     // TMA rows are read by every lane, whatever its utterances do: inactive columns are kept at a clean 0
                     // (the register path never loads them)
-                    if (TMA && !act[u]) out.v[u] = 0.f;
+                    if (SMALL && !act[u]) out.v[u] = 0.f;
                     sum[u] += out.v[u];
                     acc[u] = 0.f;
                 }
-                if ((TMA || lane_act) && sub == 0) out.stcg(row_ptr<U>(out_base, out_row, row_bytes));
+                if ((SMALL || lane_act) && sub == 0) out.stcg(row_ptr<U>(out_base, out_row, row_bytes));
                 if (ev == kEvRowPos0) cacc = out;
                 else if (ev == kEvRowPos1) {   // the pair's virtual row: what the next frame gathers instead of both
 #pragma unroll
                     for (int u = 0; u < U; ++u) cacc.v[u] += out.v[u];
-                    if ((TMA || lane_act) && sub == 0) cacc.stcg(row_ptr<U>(out_base, virt_row, row_bytes));
+                    if ((SMALL || lane_act) && sub == 0) cacc.stcg(row_ptr<U>(out_base, virt_row, row_bytes));
                     ++virt_row;
                 }
                 ++out_row;
                 ++ql;
                 own_prefetch(out_row);
             };
-            if (TMA) {
+            if (SMALL) {
                 float acc[1] = {0.f};
-                walk_arcs_tma_small<LPR, 2>(arc4, n_batches, P.alpha, p_prev * S, ring, lane, frame_scalars,
-                                            [&](const uint4 *quad, const float *v, uint32_t) {
+                walk_arcs_tma_small<2>(arc4, n_batches, P.alpha, p_prev * S, ring, lane, frame_scalars,
+                                       [&](const uint4 *quad, const float *v, uint32_t) {
                     const uint4 wq = quad[1];
-                    constexpr int STEPS = LPR / 8, SUBS = 32 / LPR;
-                    float before = acc[0];   // the lane's sum before the quad's last LDS step (slot 3 = last step of the last lane group)
+                    float before = acc[0];   // the lane's sum before the quad's last LDS step (slot 3 = last step of lane group 1)
 #pragma unroll
-                    for (int st = 0; st < STEPS; ++st) {
-                        if (st == STEPS - 1) before = acc[0];
-                        acc[0] = fmaf(fabsf(__uint_as_float(quad_word(wq, st * SUBS + sub))), v[st], acc[0]);
+                    for (int st = 0; st < 2; ++st) {
+                        if (st == 1) before = acc[0];
+                        acc[0] = fmaf(fabsf(__uint_as_float(quad_word(wq, st * 2 + sub))), v[st], acc[0]);
                     }
                     if ((int)wq.w < 0) {   // warp-uniform: a segment ends at this quad -> combine the lane groups' partial sums
                         const int ev = (int)(((wq.z >> 31) << 1) | (wq.y >> 31));
                         float a2[1] = {0.f};
                         Vec<U> v3 = vec_zero<U>();   // (U == 1 on this path)
                         if (ev == kEvPairMerged && !own) {   // slot 3 (the pair's first member) apart from the rest (its second member)
-                            const bool last = sub == SUBS - 1;
+                            const bool last = sub == 1;
                             a2[0] = last ? before : acc[0];
-                            v3.v[0] = last ? fabsf(__uint_as_float(wq.w)) * v[STEPS - 1] : 0.f;
+                            v3.v[0] = last ? fabsf(__uint_as_float(wq.w)) * v[1] : 0.f;
                             a2[0] += __shfl_xor_sync(kFull, a2[0], 16);
                             v3.v[0] += __shfl_xor_sync(kFull, v3.v[0], 16);
-                            if (LPR == 8) { a2[0] += __shfl_xor_sync(kFull, a2[0], 8); v3.v[0] += __shfl_xor_sync(kFull, v3.v[0], 8); }
                         } else {
                             acc[0] += __shfl_xor_sync(kFull, acc[0], 16);
-                            if (LPR == 8) acc[0] += __shfl_xor_sync(kFull, acc[0], 8);
                         }
                         seg_end(acc, ev, (int)wq.x < 0, quad, a2, v3, 1.f);
                     }
@@ -940,7 +922,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
         }
         tl_mark(P, t, chunk, n_chunks, 1, lane);
         if (HUBS && t < P.t_hi) zero_hub_rows(t + 1);
-        if (TMA) fence_proxy_async_global();   // this frame's rows are read through the async proxy after the barrier
+        if (SMALL) fence_proxy_async_global();   // this frame's rows are read through the async proxy after the barrier
         __syncthreads();
         for (int i = tid; i < Npad; i += kDenThreads) {   // (a recompute reads the first pass's column sums, it does not add to them)
             const float v = s_sum[i];
@@ -986,21 +968,22 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
 // ------------------------------------------------------------------------------------------------
 // backward: beta recursion, occupancies, logZ from beta
 // ------------------------------------------------------------------------------------------------
-// Rows are gathered into registers (walk_arcs_dual) except in two TMA variants: LPR < 32, the small-batch variant
-// (walk_arcs_tma_small, arc tile in shared memory, one utterance per lane), and STREAM, the streamed-arc tier
-// (walk_arcs_tma_stream, full-width rows, arcs flowing through per-warp rings).
-template <int U, int BATCH, bool SMEM_ARCS, bool W1_SMEM = SMEM_ARCS, int LPR = 32, bool STREAM = false>
+// Rows are gathered into registers (walk_arcs_dual) except in two TMA variants: SMALL, the small-batch variant
+// (walk_arcs_tma_small, 16 lanes per row, arc tile in shared memory, one utterance per lane), and STREAM, the streamed-arc
+// tier (walk_arcs_tma_stream, full-width rows, arcs flowing through per-warp rings).
+template <int U, int BATCH, bool SMEM_ARCS, bool W1_SMEM = SMEM_ARCS, bool SMALL = false, bool STREAM = false>
 __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __grid_constant__ DenParams P) {
-    constexpr bool TMA = LPR < 32 || STREAM;
-    static_assert(LPR == 32 || (SMEM_ARCS && U == 1 && (LPR == 8 || LPR == 16)), "small-batch variant: arc tile in shared memory, one utterance per lane");
-    static_assert(!STREAM || (!SMEM_ARCS && LPR == 32), "streamed arcs: not resident, full-width rows");
+    constexpr bool TMA = SMALL || STREAM;
+    constexpr int LPR = SMALL ? kSmallLanes : 32;   // lanes per row
+    static_assert(!SMALL || (SMEM_ARCS && U == 1), "small-batch variant: arc tile in shared memory, one utterance per lane");
+    static_assert(!STREAM || (!SMEM_ARCS && !SMALL), "streamed arcs: not resident, full-width rows");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int Npad = P.Npad, S = P.S;
     float *s_sum = reinterpret_cast<float *>(smem_raw);            // [2][Npad]: colsum_b, absum
     float *s_gacc = s_sum + 2 * Npad;                              // [gacc_rows][Npad]
     int *s_label = reinterpret_cast<int *>(s_gacc + (size_t)P.gacc_rows * Npad);   // [tile_rows]
     float *s_final = reinterpret_cast<float *>(s_label + P.tile_rows);             // [tile_rows]
-    Arc *s_arcs = reinterpret_cast<Arc *>(smem_raw + ((((size_t)(2 + P.gacc_rows) * Npad + 2 * (size_t)P.tile_rows) * 4 + 15) & ~(size_t)15));
+    Arc *s_arcs = reinterpret_cast<Arc *>(smem_raw + BwdArcsOff(Npad, P.gacc_rows, P.tile_rows));
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(kFull, tid >> 5, 0);   // (through a shuffle: lets ptxas keep warp-derived addresses in uniform registers)
@@ -1020,7 +1003,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
     const int cl_lab1 = __ldg(P.cta_labels + cta * 4 + 2), cl_n1 = __ldg(P.cta_labels + cta * 4 + 3);
     int labp0 = -1, labp1 = -1;
     for (int q = se - 1; q >= sb; --q) { if (__ldg(P.state_pos + q)) labp1 = __ldg(P.state_label + q); else labp0 = __ldg(P.state_label + q); }
-    const int n_batches = (ae - ab) / (LPR < 32 ? 16 : BATCH);   // (small batches: 16 rows per ring stage; streamed arcs: BATCH)
+    const int n_batches = (ae - ab) / (SMALL ? kSmallRows : BATCH);   // (small batches: kSmallRows rows per ring stage; streamed arcs: BATCH)
     // shared memory: 3 words of 16 bytes per quad {byte offsets}{w0}{w1}; global fallback: AoS arcs + w1 array
     constexpr int kW = W1_SMEM ? 3 : 2;   // 16-byte words per staged quad
     const uint4 *const arc4 = SMEM_ARCS ? reinterpret_cast<const uint4 *>(s_arcs) + kW * ((ab - tile_a0) / kQuad)
@@ -1058,13 +1041,12 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
     }
     TmaRing ring{0u, 0u, 0u};
     if (TMA) {
-        constexpr int kStages = LPR == 32 ? 2 : kSmallStages;
-        constexpr uint32_t kRingBytes = LPR == 32 ? 2u * BATCH * 32u * U * 4u : (uint32_t)kSmallStages * 16u * LPR * 4u;
-        ring.buf = smem_u32(smem_raw + P.ring_off) + (uint32_t)warp * kRingBytes;
-        ring.bar = smem_u32(smem_raw + P.bar_off) + (uint32_t)warp * 8u * kStages;
+        constexpr int kStages = SMALL ? kSmallStages : 2;
+        ring.buf = smem_u32(smem_raw + P.ring_off) + (uint32_t)warp * (SMALL ? kSmallRingWarpBytes : StreamRingWarpBytes(U));
+        ring.bar = smem_u32(smem_raw + P.bar_off) + (uint32_t)warp * (SMALL ? kSmallBarWarpBytes : kStreamBarWarpBytes);
         if (lane == 0) {
             for (int st = 0; st < kStages; ++st) mbar_init(ring.bar + 8u * st, 1);
-            if (STREAM) for (int st = 0; st < kArcStages; ++st) mbar_init(smem_u32(smem_raw + P.abar_off) + (uint32_t)(warp * kArcStages + st) * 8u, 1);
+            if (STREAM) for (int st = 0; st < kArcStages; ++st) mbar_init(smem_u32(smem_raw + P.abar_off) + (uint32_t)(warp * (kArcBarWarpBytes / 8) + st) * 8u, 1);
             asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         }
         __syncwarp();
@@ -1072,9 +1054,9 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
     ArcRing aring{nullptr, 0u, 0u, 0u, 0u, 0u, 0u, nullptr};
     if (STREAM) {
         constexpr int kAW = BATCH / kQuad * 3;   // 16-byte words per batch
-        aring.buf = reinterpret_cast<const uint4 *>(smem_raw + P.aring_off) + (size_t)warp * kArcStages * kAW;
+        aring.buf = reinterpret_cast<const uint4 *>(smem_raw + P.aring_off) + (size_t)warp * (kArcRingWarpBytes / 16);
         aring.buf_s = smem_u32(aring.buf);
-        aring.bar = smem_u32(smem_raw + P.abar_off) + (uint32_t)warp * kArcStages * 8u;
+        aring.bar = smem_u32(smem_raw + P.abar_off) + (uint32_t)warp * kArcBarWarpBytes;
         aring.n = (uint32_t)n_batches;
         aring.src = P.tq + (size_t)3 * (ab / kQuad);
         arc_ring_fill<kAW>(aring, lane);
@@ -1224,25 +1206,24 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
                 a_q1 = ((int)out_row + 1 < se && lane_act) ? gather_row<U>(a_base, (out_row + 1) * row_bytes) : vec_zero<U>();
                 own_prefetch(out_row);
             };
-            if (LPR < 32) {
+            if (SMALL) {
                 float acc0[1] = {0.f}, acc1[1] = {0.f};
-                const uint32_t w1buf = smem_u32(smem_raw + P.bar_off) + (uint32_t)P.n_warps * 8u * kSmallStages + (uint32_t)warp * 64u * kSmallStages;
-                walk_arcs_tma_small<LPR, W1_SMEM ? 3 : 2, !W1_SMEM>(arc4, n_batches, P.bh, ((tau + 1) & 1) * S, ring, lane, frame_scalars,
-                                            [&](const uint4 *quad, const float *v, uint32_t w1s) {
+                const uint32_t w1buf = SmallW1Off(smem_u32(smem_raw + P.bar_off), P.n_warps) + (uint32_t)warp * kSmallW1WarpBytes;
+                walk_arcs_tma_small<W1_SMEM ? 3 : 2, !W1_SMEM>(arc4, n_batches, P.bh, ((tau + 1) & 1) * S, ring, lane, frame_scalars,
+                                                               [&](const uint4 *quad, const float *v, uint32_t w1s) {
                     const uint4 wq = quad[1];
                     uint4 t1;
                     if (W1_SMEM) t1 = quad[2];
                     else asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(t1.x), "=r"(t1.y), "=r"(t1.z), "=r"(t1.w) : "r"(w1s));
 #pragma unroll
-                    for (int st = 0; st < LPR / 8; ++st) {
-                        const int j = st * (32 / LPR) + sub;
+                    for (int st = 0; st < 2; ++st) {
+                        const int j = st * 2 + sub;
                         acc0[0] = fmaf(fabsf(__uint_as_float(quad_word(wq, j))), v[st], acc0[0]);
                         acc1[0] = fmaf(__uint_as_float(quad_word(t1, j)), v[st], acc1[0]);
                     }
                     if ((int)wq.w < 0) {   // warp-uniform: the group ends at this quad -> combine the lane groups' partial sums
                         acc0[0] += __shfl_xor_sync(kFull, acc0[0], 16);
                         acc1[0] += __shfl_xor_sync(kFull, acc1[0], 16);
-                        if (LPR == 8) { acc0[0] += __shfl_xor_sync(kFull, acc0[0], 8); acc1[0] += __shfl_xor_sync(kFull, acc1[0], 8); }
                         group_end(acc0, acc1, (int)wq.z < 0, (int)wq.x < 0, (int)wq.y < 0);
                     }
                 }, reinterpret_cast<const float *>(w1g), w1buf);
@@ -1382,122 +1363,51 @@ int LaunchCoop(const void *fn, const DenParams &p, int n_ctas, size_t smem, cuda
     return 0;
 }
 
-template <int U, int BATCH, bool SMEM_ARCS>
-int LaunchFwd(const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    const void *fn = p.n_hubs > 0 ? (const void *)den_forward_kernel<U, BATCH, SMEM_ARCS, true>
-                                  : (const void *)den_forward_kernel<U, BATCH, SMEM_ARCS, false>;
-    return LaunchCoop(fn, p, n_ctas, smem, stream, err);
-}
-template <int U, int BATCH, bool SMEM_ARCS>
-int LaunchBwd(bool w1_smem, const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    const void *fn = SMEM_ARCS && !w1_smem ? (const void *)den_backward_kernel<U, BATCH, SMEM_ARCS, false>
-                                           : (const void *)den_backward_kernel<U, BATCH, SMEM_ARCS>;
-    return LaunchCoop(fn, p, n_ctas, smem, stream, err);
-}
-
-// backward pass with the arc stream flowing through per-warp rings instead of being resident (walk_arcs_tma_stream)
-template <int U, int R>
-int LaunchTmaStreamBwd(const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    return LaunchCoop((const void *)den_backward_kernel<U, R, false, true, 32, true>, p, n_ctas, smem, stream, err);
-}
-
-// small batches: rows of LPR = 8 / 16 floats (see walk_arcs_tma_small)
-template <int LPR>
-int LaunchTmaSmall(bool backward, bool w1_smem, const DenParams &p, int n_ctas, size_t smem, cudaStream_t stream, std::string *err) {
-    const void *fn = !backward ? (const void *)den_forward_kernel<1, 16, true, false, LPR>
-                     : w1_smem ? (const void *)den_backward_kernel<1, 16, true, true, LPR>
-                               : (const void *)den_backward_kernel<1, 16, true, false, LPR>;
-    return LaunchCoop(fn, p, n_ctas, smem, stream, err);
+// 2-D view [rows][Npad] fp32 of `base` with a box of 1 row x box_cols columns, by cuTensorMapEncodeTiled through the
+// runtime's driver entry point (no link-time dependency on libcuda); false if that is unavailable or refuses the shape
+bool EncodeRowTensorMap(CUtensorMap *tm, const float *base, size_t rows, int Npad, int box_cols) {
+    typedef CUresult (*EncodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
+                                    const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    static EncodeTiled encode = []() -> EncodeTiled {
+        void *fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+            cudaGetLastError();
+            return nullptr;
+        }
+        return (EncodeTiled)fn;
+    }();
+    if (!encode || !base || rows == 0 || box_cols > 256 || (reinterpret_cast<uintptr_t>(base) & 15)) return false;
+    cuuint64_t dims[2] = {(cuuint64_t)Npad, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)Npad * 4};
+    cuuint32_t box[2] = {(cuuint32_t)box_cols, 1};
+    cuuint32_t estr[2] = {1, 1};
+    return encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-constexpr int kBwdMaxLaneWidth = 2;   // four utterances per lane spill the backward pass's two accumulators
-
-// Gathers per batch (two batches are in flight per warp), fixed per variant by the register budget at 512 threads:
-// forward 2x16 rows (2x8 at four utterances per lane), backward 2x8.
-template <int U> struct FwdBatch { static constexpr int value = U == 4 ? 8 : 16; };
-constexpr int kBwdBatch = 8;
-
+// the kernel instantiation a launch names (den_launch.h DenLaunch)
 template <int U>
-int DispatchU(bool backward, bool tma, bool smem_arcs, bool w1_smem, const DenParams &p, int n_ctas, size_t smem,
-              cudaStream_t stream, std::string *err) {
-    if (tma) return LaunchTmaStreamBwd<U, TmaShape<U>::R>(p, n_ctas, smem, stream, err);
-    if (backward)
-        return smem_arcs ? LaunchBwd<U, kBwdBatch, true>(w1_smem, p, n_ctas, smem, stream, err)
-                         : LaunchBwd<U, kBwdBatch, false>(w1_smem, p, n_ctas, smem, stream, err);
-    return smem_arcs ? LaunchFwd<U, FwdBatch<U>::value, true>(p, n_ctas, smem, stream, err)
-                     : LaunchFwd<U, FwdBatch<U>::value, false>(p, n_ctas, smem, stream, err);
+const void *ForwardKernel(const DenLaunch &L, bool hubs) {
+    constexpr int B = FwdBatch(U);
+    if (L.tier == kTierShared) return hubs ? (const void *)den_forward_kernel<U, B, true, true> : (const void *)den_forward_kernel<U, B, true, false>;
+    return hubs ? (const void *)den_forward_kernel<U, B, false, true> : (const void *)den_forward_kernel<U, B, false, false>;
 }
-
-int Dispatch(bool backward, const DeviceGraph &g, DenParams &p, size_t fixed_smem, cudaStream_t stream,
-             std::string *err) {
-    if (p.Npad > g.n_warps * 32) { *err = "batch too large for the den kernel's bookkeeping CTA (N <= " + std::to_string(g.n_warps * 32) + ")"; return 1; }
-    if (g.n_warps * 32 != kDenThreads) { *err = "unsupported warps per CTA for den kernels (" + std::to_string(kDenThreads / 32) + ")"; return 1; }
-    const DevicePass &pass = backward ? g.bwd : g.fwd;
-    // Tiers by graph size, for batches of more than 16 utterances.  (1) The whole arc stream in shared memory (8 bytes per
-    // forward slot, 12 per backward slot), rows gathered into registers: on an H100 this beats staging the rows by one TMA
-    // copy each at every batch width (N = 32 / 64 / 128, T = 1500, 1.02 M arcs: 46.7 / 79.9 / 160.1 ms per step against
-    // 56.0 / 87.5 / 175.1 ms, 700 W, 1980 MHz); (2) backward only: offsets + first weights in shared memory, second weights
-    // streamed from L2, or the streamed-arc TMA tier below; (3) everything from L2.
-    const size_t budget = (size_t)g.max_smem_optin > 2048 ? (size_t)g.max_smem_optin - 1024 : 0;
-    const bool no_smem = g.tune_arcs_in_global;   // test hooks (read once at Init): exercise the large-graph tiers
-    bool w1_smem = backward && !g.tune_w1_in_global;
-    size_t arc_bytes = (size_t)pass.max_tile_arcs * (backward && w1_smem ? 12 : sizeof(Arc));
-    // small batches: the arc stream must fit NEXT TO the small-batch rings (the same sum DeviceGraph::small_ok was decided on at
-    // Init: 8 bytes per backward slot with the second weights streamed) -- without this the 12-byte form could be kept although
-    // only the 8-byte form leaves room for the rings, and the launch below refused a batch that had been padded for it
-    const size_t small_extra = p.Npad < 32 ? 128 + (size_t)g.n_warps * kSmallStages * (16 * (size_t)p.Npad * 4 + 8 + 64) : 0;
-    if (backward && w1_smem && fixed_smem + arc_bytes + small_extra > budget) { w1_smem = false; arc_bytes = (size_t)pass.max_tile_arcs * sizeof(Arc); }
-    const bool smem_arcs = fixed_smem + arc_bytes + small_extra <= budget && !no_smem;
-    size_t smem = fixed_smem + (smem_arcs ? arc_bytes : 0);
-    // utterances per lane: the widest row segment the batch allows, except that the backward pass (two accumulators per
-    // utterance) runs out of registers at 4 -- it walks 64-utterance groups instead.
-    int U = LaneWidth(p.Npad);
-    if (backward && U == 4) U = kBwdMaxLaneWidth;
-    const float *table = backward ? p.bh : p.alpha;
-    const size_t rows = backward ? (size_t)2 * g.S : (size_t)p.a_frames * g.S;
-    if (p.Npad < 32) {   // small batch: the lane padding promised the small-batch TMA kernels (DeviceGraph::small_ok)
-        const int LPR = p.Npad;
-        const size_t ring_off = (smem + 127) & ~(size_t)127;
-        const size_t bar_off = ring_off + (size_t)g.n_warps * kSmallStages * 16 * LPR * 4;
-        // mbarriers, then (backward, second weights streamed) one 64-byte slot per stage and warp for the bulk-copied w1 words
-        const size_t total = bar_off + (size_t)g.n_warps * kSmallStages * (8 + 64);
-        const bool fits = g.small_ok && smem_arcs && total <= budget && p.n_hubs == 0 && (LPR == 8 || LPR == 16) && rows < ((size_t)1 << 30);
-        if (!fits || !EncodeRowTensorMap(&p.tmap, table, rows, p.Npad, LPR)) {
-            *err = "den: small-batch kernels unavailable for this graph/device although the batch was padded for them (" +
-                   std::string(backward ? "backward" : "forward") + ": small_ok=" + std::to_string((int)g.small_ok) + " smem_arcs=" + std::to_string((int)smem_arcs) +
-                   " smem=" + std::to_string(total) + "/" + std::to_string(budget) + " hubs=" + std::to_string(p.n_hubs) + " rows=" + std::to_string(rows) +
-                   (fits ? " tensor map rejected)" : ")");
-            return 1;
-        }
-        p.use_tma = 1; p.ring_off = (int)ring_off; p.bar_off = (int)bar_off;
-        return LPR == 8 ? LaunchTmaSmall<8>(backward, w1_smem, p, g.n_ctas, total, stream, err)
-                        : LaunchTmaSmall<16>(backward, w1_smem, p, g.n_ctas, total, stream, err);
-    }
-    bool tma = false;
-    p.use_tma = 0;
-    // Streamed-arc TMA tier, BACKWARD pass only: the stream does not fit (or the test hook says so) but the graph carries the
-    // transposed copy.  The forward pass of such graphs keeps the register gathers with the arcs read from L2: its 8-byte
-    // slots would make 128-byte bulk copies, one per 16 rows.
-    bool smem_arcs_eff = smem_arcs;
-    if (backward && !(smem_arcs && w1_smem) && pass.tq != nullptr && p.n_hubs == 0 && !g.tune_no_tma && rows < ((size_t)1 << 30) &&
-        EncodeRowTensorMap(&p.tmap, table, rows, p.Npad, 32 * U)) {
-        const int R = U == 4 ? TmaShape<4>::R : 16;
-        const size_t ring_off = (fixed_smem + 127) & ~(size_t)127;
-        const size_t bar_off = ring_off + (size_t)g.n_warps * 2 * R * 32 * U * 4;
-        const size_t abar_off = bar_off + (size_t)g.n_warps * 2 * 8;
-        const size_t aring_off = (abar_off + (size_t)g.n_warps * kArcStages * 8 + 127) & ~(size_t)127;
-        const size_t arc_ring = (size_t)g.n_warps * kArcStages * (R / kQuad) * 3 * 16;
-        const size_t total = aring_off + arc_ring;
-        if (total <= budget) {
-            tma = true; smem_arcs_eff = false;
-            p.use_tma = 1; p.ring_off = (int)ring_off; p.bar_off = (int)bar_off;
-            p.abar_off = (int)abar_off; p.aring_off = (int)aring_off; p.tq = pass.tq;
-            smem = total;
-        }
-    }
-    if (U == 1) return DispatchU<1>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
-    if (U == 2) return DispatchU<2>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
-    return DispatchU<4>(backward, tma, smem_arcs_eff, w1_smem, p, g.n_ctas, smem, stream, err);
+template <int U>
+const void *BackwardKernel(const DenLaunch &L) {
+    if (L.tier == kTierStreamed) return (const void *)den_backward_kernel<U, kStreamRows, false, true, false, true>;
+    if (L.tier == kTierGlobal) return (const void *)den_backward_kernel<U, kBwdBatch, false>;
+    return L.w1_smem ? (const void *)den_backward_kernel<U, kBwdBatch, true, true> : (const void *)den_backward_kernel<U, kBwdBatch, true, false>;
+}
+const void *DenKernel(bool backward, const DenLaunch &L, bool hubs) {
+    if (L.tier == kTierSmall)
+        return !backward ? (const void *)den_forward_kernel<1, kSmallRows, true, false, true>
+             : L.w1_smem ? (const void *)den_backward_kernel<1, kSmallRows, true, true, true>
+                         : (const void *)den_backward_kernel<1, kSmallRows, true, false, true>;
+    if (backward) return L.U == 1 ? BackwardKernel<1>(L) : BackwardKernel<2>(L);
+    return L.U == 1 ? ForwardKernel<1>(L, hubs) : L.U == 2 ? ForwardKernel<2>(L, hubs) : ForwardKernel<4>(L, hubs);
 }
 
 }  // namespace
@@ -1556,50 +1466,24 @@ int LaunchLogitGrad(const void *z, int z_bf16, long sn, long st, int N, int T, i
     return (int)cudaGetLastError();
 }
 
-// cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time dependency on libcuda)
-bool EncodeRowTensorMap(CUtensorMap *tm, const float *base, size_t rows, int Npad, int box_cols) {
-    typedef CUresult (*EncodeTiled)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                    const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static EncodeTiled encode = []() -> EncodeTiled {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
-            cudaGetLastError();
-            return nullptr;
-        }
-        return (EncodeTiled)fn;
-    }();
-    if (!encode || !base || rows == 0 || box_cols > 256 || (reinterpret_cast<uintptr_t>(base) & 15)) return false;
-    cuuint64_t dims[2] = {(cuuint64_t)Npad, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)Npad * 4};
-    cuuint32_t box[2] = {(cuuint32_t)box_cols, 1};
-    cuuint32_t estr[2] = {1, 1};
-    return encode(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-int LaunchDenForward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err) {
-    p.arcs = g.fwd.arcs; p.chunk_state = g.fwd.chunk_state; p.chunk_arc = g.fwd.chunk_arc;
-    p.chunk_pair = g.fwd.chunk_pair; p.cta_labels = g.fwd.cta_labels;
-    p.gacc_rows = 0;
-    p.own_c = g.fwd.own_c; p.own = g.own_rows ? 1 : 0;
-    p.tile_rows = g.fwd.max_tile_rows;
-    const size_t fixed = (((size_t)(p.Npad + p.tile_rows) * 4 + 15) & ~(size_t)15);
-    return Dispatch(false, g, p, fixed, stream, err);
-}
-
-int LaunchDenBackward(const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err) {
-    p.arcs = g.bwd.arcs; p.chunk_state = g.bwd.chunk_state; p.chunk_arc = g.bwd.chunk_arc;
-    p.chunk_pair = g.bwd.chunk_pair; p.cta_labels = g.bwd.cta_labels; p.w1 = g.bwd.w1;
-    p.own_c = g.bwd.own_c; p.own = g.own_rows ? 1 : 0;
-    // label accumulator in shared memory when the per-CTA label range is small enough
-    size_t gacc_bytes = (size_t)g.bwd.max_tile_labels * p.Npad * 4;
-    p.gacc_rows = gacc_bytes <= 64 * 1024 ? g.bwd.max_tile_labels : 0;
-    p.tile_rows = g.bwd.max_tile_rows;
-    const size_t fixed = ((((size_t)(2 + p.gacc_rows) * p.Npad + 2 * (size_t)p.tile_rows) * 4 + 15) & ~(size_t)15);
-    return Dispatch(true, g, p, fixed, stream, err);
+int LaunchDen(bool backward, const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err) {
+    const DevicePass &pass = backward ? g.bwd : g.fwd;
+    p.arcs = pass.arcs; p.chunk_state = pass.chunk_state; p.chunk_arc = pass.chunk_arc;
+    p.chunk_pair = pass.chunk_pair; p.cta_labels = pass.cta_labels; p.w1 = backward ? pass.w1 : nullptr;
+    p.own_c = pass.own_c; p.own = g.own_rows ? 1 : 0;
+    DenHooks hooks = g.hooks;   // (a copy: a launch without a tensor map is chosen as without TMA)
+    DenLaunch L;
+    if (!ChooseDenLaunch(g.shape, p.Npad, backward, g.max_smem_optin, hooks, &L, err)) return 1;
+    const size_t rows = backward ? (size_t)2 * g.S : (size_t)p.a_frames * g.S;   // TMA row coordinates stay below kOobRow
+    if (L.tier == kTierSmall && rows >= kOobRow) { *err = "den: small-batch kernels: gather table of " + std::to_string(rows) + " rows"; return 1; }
+    if (L.tier == kTierStreamed && !(rows < kOobRow && EncodeRowTensorMap(&p.tmap, p.bh, rows, p.Npad, 32 * L.U))) {
+        hooks.no_tma = true;
+        if (!ChooseDenLaunch(g.shape, p.Npad, backward, g.max_smem_optin, hooks, &L, err)) return 1;
+    }
+    p.tq = L.tier == kTierStreamed ? pass.tq : nullptr;
+    p.tile_rows = L.tile_rows; p.gacc_rows = L.gacc_rows;
+    p.ring_off = (int)L.ring_off; p.bar_off = (int)L.bar_off; p.abar_off = (int)L.abar_off; p.aring_off = (int)L.aring_off;
+    return LaunchCoop(DenKernel(backward, L, g.shape.n_hubs > 0), p, g.n_ctas, L.total, stream, err);
 }
 
 int LaunchDenGradNormalize(float *grad, long gsn, long gst, const float *absum, const int *len, int N, int Npad,

@@ -134,9 +134,10 @@ def test_fallback_paths(tmp_graphs, monkeypatch, env):
     path, g, V = tmp_graphs["tlm_mid"]
     ctx = _ctx(path)
     T = 30
-    # 20: one utterance per lane (second weights prefetched with the gathers); 12 / 5: the small-batch kernels (16- / 8-float
+    # 20: one utterance per lane (second weights prefetched with the gathers); 12 / 5: the small-batch kernels (16-float
     # rows), whose backward pass then streams the second weights with bulk copies next to the TMA row gathers
-    # ARCS_IN_GLOBAL: 1, 2 and 4 utterances per lane of the streamed-arc kernels (two lane groups in the backward pass at 130)
+    # ARCS_IN_GLOBAL: 1 and 2 utterances per lane of the streamed-arc backward kernels (two lane groups at 130), 1, 2 and 4 of
+    # the forward kernels reading their arcs from L2 (tests/test_den_launch.py pins these tiers)
     for N in ((40, 20, 12, 5) if "W1" in env else (40, 12, 130) if "ARCS" in env else (40, 64) if "RING" in env else (40, 12, 64) if ("MERGE" in env or "OWN" in env) else (40,)):
         lens = np.maximum(1, T - (np.arange(N) * 5) % T).astype(np.int32)
         y, _, lens, _ = oracle.synth_batch(N, T, V, seed=8, lens=lens)
