@@ -7,7 +7,8 @@ and the work is enqueued on the current CUDA stream of the tensors' device.  Dif
 installed (binding.cpp has none, SURVEY.md 8b) and native errors raise ``RuntimeError`` instead of being
 ignored (binding.cpp:105,111) or exiting the process (den_calculate.cu:16-25).
 
-Addition: ``ctc_crf_loss_fwd`` -- the fused, synchronisation-free entry used by ``CTC_CRF_LOSS``.
+Addition: ``ctc_crf_loss_fwd`` -- the fused, synchronisation-free entry used by ``CTC_CRF_LOSS``; ``ctc_crf_loss_fwd_only``
+and ``ctc_loss_fwd_only`` -- the losses without a gradient, used when grad mode is off.
 """
 from __future__ import annotations
 
@@ -324,6 +325,73 @@ def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tenso
     return loss, grad, parts
 
 
+def _fwd_only_need(L, n, tmax):
+    return (int(L.ccb_den_fwd_alpha_floats(n)) * 4 + int(L.ccb_den_aux_bytes(n, tmax))
+            + int(L.ccb_num_fwd_only_bytes(n)))
+
+
+def _plan_fwd_only_slices(L, lx, ly, N, dev):
+    """Slices of the forward-only loss: contiguous runs of at most MAX_UTTS_PER_CALL utterances, each walking its own
+    max(lx).  Its alpha is a ring of a few frames whose size does not depend on the length, so a slice is never halved or
+    checkpointed; one whose scratch does not fit the free device memory is an error.  Returns (n0, n1, tmax, maxl)."""
+    budget = _scratch_budget(dev)
+    slices = []
+    for n0 in range(0, N, MAX_UTTS_PER_CALL):
+        n1 = min(N, n0 + MAX_UTTS_PER_CALL)
+        tmax = max(1, int(lx[n0:n1].max()))
+        need = _fwd_only_need(L, n1 - n0, tmax)
+        if need > budget:
+            budget = _scratch_budget(dev, need)
+        if need > budget:
+            raise RuntimeError(f"forward-only CTC-CRF scratch for {n1 - n0} utterances of up to {tmax} frames needs "
+                               f"{need >> 20} MiB (alpha ring {int(L.ccb_den_fwd_alpha_floats(n1 - n0)) * 4 >> 20} MiB), "
+                               f"only {budget >> 20} MiB free")
+        slices.append((n0, n1, tmax, int(ly[n0:n1].max())))
+    return slices
+
+
+def ctc_crf_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
+                          lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False
+                          ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """The loss of ``ctc_crf_loss_fwd`` without its gradient, for evaluation: (loss[1] fp32 CUDA, parts[2N] or None).
+    The den forward pass keeps alpha on a ring of frames, the numerator writes no cells, and no (N,T,V) buffer is
+    allocated, so the scratch is a few frames of the den graph per slice whatever the lengths.  Never synchronises the
+    host.  Arguments as for ``ctc_crf_loss_fwd``."""
+    L = _lib.lib()
+    N, T, V = _check_batch_args(logits, labels, lx, ly)
+    dev = logits.device
+    esz = logits.element_size()
+    scale = 1.0 / N if size_average else 1.0
+    with torch.cuda.device(dev):
+        meta, sum_l, _ = upload_meta(labels, lx, ly, dev)
+        base = meta.data_ptr()
+        p_labels, p_off = base, base + 4 * sum_l
+        p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
+        parts = torch.empty(2 * N, dtype=torch.float32, device=dev) if want_parts else None
+        stream = _stream(dev)
+        slices = _plan_fwd_only_slices(L, lx, ly, N, dev)
+        losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
+        for i, (n0, n1, tmax, maxl) in enumerate(slices):
+            n = n1 - n0
+            alpha_ws = torch.empty(int(L.ccb_den_fwd_alpha_floats(n)), dtype=torch.float32, device=dev)
+            aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
+            num_ws = torch.empty(int(L.ccb_num_fwd_only_bytes(n)), dtype=torch.uint8, device=dev)
+            sub_parts = torch.empty(2 * n, dtype=torch.float32, device=dev) if want_parts else None
+            rc = L.ccb_ctc_crf_loss_fwd_only(logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype], int(from_logits),
+                                             n, T, V, tmax, p_labels, p_off + 4 * n0, p_ly + 4 * n0, p_lx + 4 * n0, maxl,
+                                             float(lamb), float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(),
+                                             num_ws.data_ptr(), losses.data_ptr() + 4 * i,
+                                             sub_parts.data_ptr() if want_parts else None, stream)
+            _check(rc, "ctc_crf_loss_fwd_only")
+            if want_parts:
+                parts[n0:n1] = sub_parts[:n]
+                parts[N + n0:N + n1] = sub_parts[n:]
+            del alpha_ws, aux_ws, num_ws      # stream-ordered reuse by the caching allocator for the next slice
+        loss = losses.sum().reshape(1) if len(slices) > 1 else losses
+        meta.record_stream(torch.cuda.current_stream(dev))
+    return loss, parts
+
+
 def _check_batch_args(logits, labels, lx, ly):
     assert logits.is_cuda and logits.dim() == 3 and logits.is_contiguous()
     if logits.dtype not in _DTYPES:
@@ -367,6 +435,29 @@ def ctc_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, l
         _check(rc, "ctc_loss_fwd")
         meta.record_stream(torch.cuda.current_stream(dev))
     return loss, grad, logp
+
+
+def ctc_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
+                      size_average: bool, blank: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The loss of ``ctc_loss_fwd`` without its gradient: (loss[1], logp[N]) on the device, the same values, from one alpha
+    chain per utterance that writes no cells.  No workspace, no (N,T,V) buffer, no host synchronisation."""
+    L = _lib.lib()
+    N, T, V = _check_batch_args(logits, labels, lx, ly)
+    dev = logits.device
+    scale = 1.0 / N if size_average else 1.0
+    with torch.cuda.device(dev):
+        meta, sum_l, maxl = upload_meta(labels, lx, ly, dev)
+        base = meta.data_ptr()
+        p_labels, p_off = base, base + 4 * sum_l
+        p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
+        tmax = max(1, int(lx.max()))
+        loss = torch.empty(1, dtype=torch.float32, device=dev)
+        logp = torch.empty(N, dtype=torch.float32, device=dev)
+        rc = L.ccb_ctc_loss_fwd_only(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx,
+                                     maxl, int(blank), float(scale), loss.data_ptr(), logp.data_ptr(), _stream(dev))
+        _check(rc, "ctc_loss_fwd_only")
+        meta.record_stream(torch.cuda.current_stream(dev))
+    return loss, logp
 
 
 def ctc_align(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, blank: int = 0

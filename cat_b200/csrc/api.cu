@@ -222,11 +222,20 @@ void SetCkpt(DenParams &p, const DeviceGraph &g, int T, int K) {
     p.runlog_b = reinterpret_cast<double *>(p.ckpt + (size_t)CkptCount(T, K) * frame);
 }
 
+// Forward-only loss: the first checkpointed pass with ckpt_k = T, so frame 0 is the only checkpoint; it sits right behind
+// the kAlphaRing + 2 ring positions (ccb_den_fwd_alpha_floats).  No backward pass follows: no carried log-scales.
+void SetFwdOnly(DenParams &p, const DeviceGraph &g, int T) {
+    p.ckpt_k = T;
+    p.ckpt = p.alpha + (size_t)(kAlphaRing + 2) * g.S * p.Npad;
+    p.runlog_b = nullptr;
+}
+
 // forward part: zero aux, frame max, alpha recursion; logz_a lands in aux
 // raw: `y` holds unnormalised logits; the log-normalisers go to aux (lz, lnorm) and logZ comes out normalised
 // ckpt_k > 0: alpha on a ring of kAlphaRing frames, checkpoints every ckpt_k frames (see SetCkpt)
+// fwd_only: alpha on the ring, logZ only (see SetFwdOnly; ckpt_k is ignored)
 int DenForward(const DeviceGraph &g, const void *y, int dtype, long sn, long st, int N, int T, int V, const int *len,
-               float *alpha, void *aux, cudaStream_t stream, bool raw = false, int ckpt_k = 0) {
+               float *alpha, void *aux, cudaStream_t stream, bool raw = false, int ckpt_k = 0, bool fwd_only = false) {
     const DenAuxLayout L = MakeDenAuxLayout(g.S, N, T, g.small_ok);
     char *a = reinterpret_cast<char *>(aux);
     CCB_CUDA(cudaMemsetAsync(a, 0, L.zero_bytes, stream));
@@ -238,8 +247,9 @@ int DenForward(const DeviceGraph &g, const void *y, int dtype, long sn, long st,
     if (raw) p.lnorm = reinterpret_cast<const double *>(a + L.lnorm);
     p.barrier = reinterpret_cast<unsigned *>(a + L.barrier);
     p.logz = reinterpret_cast<float *>(a + L.logz_a);
-    if (ckpt_k > 0) {
-        SetCkpt(p, g, T, ckpt_k);
+    if (ckpt_k > 0 || fwd_only) {
+        if (fwd_only) SetFwdOnly(p, g, T);
+        else SetCkpt(p, g, T, ckpt_k);
         p.ckpt_mode = 1; p.a_ring = kAlphaRing; p.a_frames = kAlphaRing + 2;
     }
     std::string err;
@@ -382,6 +392,16 @@ size_t ccb_den_ckpt_alpha_floats(int N, int T, int K) {
     const size_t npad = (size_t)PadLanes(N, small_ok);
     return ((size_t)CkptSegFrames(T, K) + (size_t)CkptCount(T, K)) * (size_t)S * npad + 2 * npad;
 }
+
+size_t ccb_den_fwd_alpha_floats(int N) {
+    int S, P;
+    bool small_ok;
+    CurrentSizes(&S, &P, &small_ok);
+    // the ring's kAlphaRing + 2 positions, then the one checkpoint (frame 0) of SetFwdOnly, S real rows each; no T in it
+    return (size_t)(kAlphaRing + 2 + 1) * (size_t)S * (size_t)PadLanes(N, small_ok);
+}
+
+size_t ccb_num_fwd_only_bytes(int N) { return (size_t)(N > 0 ? N : 0) * sizeof(float); }
 
 size_t ccb_den_aux_bytes(int N, int T) {
     int S, P;
@@ -595,6 +615,65 @@ int ccb_ctc_crf_loss_logits_ckpt_fwd(const void *logits, int dtype, int N, int T
                                      void *stream) {
     return LossFwdImpl(true, logits, dtype, N, T, V, Tmax, ckpt_k, labels_dev, label_off_dev, label_len_dev, len_dev,
                        max_label_len, lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
+}
+
+/* Forward-only CTC-CRF loss: the same loss (and parts) as LossFwdImpl without the gradient.  The den forward pass keeps
+ * alpha on the ring (SetFwdOnly), the numerator walks its alpha chains without writing cells, and nothing touches an (N,T,V)
+ * buffer but the logits.  Launches: frame max (raw: frame log-sum-exp + normalisers), den forward, numerator, loss. */
+static int LossFwdOnlyImpl(bool raw, const void *logits, int dtype, int N, int T, int V, int Tmax,
+                           const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                           const int *len_dev, int max_label_len, float lamb, float scale,
+                           float *alpha_ws, void *aux_ws, void *num_ws, float *loss, float *parts, void *stream) {
+    g_err.clear();
+    DeviceGraph *g;
+    if (CurrentGraph(&g)) return 1;
+    if (Tmax <= 0 || Tmax > T) return Fail("ctc_crf_loss_fwd_only: Tmax must lie in [1, T]");
+    if (CheckDen(*g, dtype, N, Tmax, V)) return 1;
+    if (!alpha_ws || !aux_ws || !num_ws || !loss) return Fail("ctc_crf_loss_fwd_only: missing buffer");
+    cudaStream_t s = (cudaStream_t)stream;
+    const long sn = (long)T * V, st = V;
+    const DenAuxLayout L = MakeDenAuxLayout(g->S, N, Tmax, g->small_ok);
+    float *logz = reinterpret_cast<float *>((char *)aux_ws + L.logz_a);
+    float *logp = reinterpret_cast<float *>(num_ws);
+    const double *lnorm = raw ? reinterpret_cast<const double *>((char *)aux_ws + L.lnorm) : nullptr;
+    if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw, 0, /*fwd_only=*/true)) return 1;
+    std::string err;
+    int rc = LaunchCtcLogp(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev,
+                           len_dev, max_label_len, 0, logp, lnorm, s, &err);
+    if (rc) return Fail(err);
+    rc = LaunchAssembleLoss(logz, logp, N, lamb, scale, loss, s);
+    if (rc) return FailCuda("assemble_loss", (cudaError_t)rc);
+    if (parts) {
+        CCB_CUDA(cudaMemcpyAsync(parts, logz, sizeof(float) * N, cudaMemcpyDeviceToDevice, s));
+        CCB_CUDA(cudaMemcpyAsync(parts + N, logp, sizeof(float) * N, cudaMemcpyDeviceToDevice, s));
+    }
+    return 0;
+}
+
+int ccb_ctc_crf_loss_fwd_only(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax,
+                              const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                              const int *len_dev, int max_label_len, float lamb, float scale,
+                              float *alpha_ws, void *aux_ws, void *num_ws, float *loss, float *parts, void *stream) {
+    return LossFwdOnlyImpl(from_logits != 0, logits, dtype, N, T, V, Tmax, labels_dev, label_off_dev, label_len_dev, len_dev,
+                           max_label_len, lamb, scale, alpha_ws, aux_ws, num_ws, loss, parts, stream);
+}
+
+int ccb_ctc_loss_fwd_only(const void *logits, int dtype, int N, int T, int V, int Tmax,
+                          const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                          int max_label_len, int blank, float scale, float *loss, float *logp, void *stream) {
+    g_err.clear();
+    if (N <= 0 || T <= 0 || V <= 0 || !logits || !loss || !logp) return Fail("ctc_loss_fwd_only: bad arguments");
+    if (Tmax <= 0 || Tmax > T) return Fail("ctc_loss_fwd_only: Tmax must lie in [1, T]");
+    if (dtype != CCB_DTYPE_F32 && dtype != CCB_DTYPE_BF16) return Fail("ctc_loss_fwd_only: unsupported logits dtype");
+    if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
+    cudaStream_t s = (cudaStream_t)stream;
+    std::string err;
+    int rc = LaunchCtcLogp(logits, dtype == CCB_DTYPE_BF16, (long)T * V, V, N, Tmax, V, labels_dev, label_off_dev, label_len_dev,
+                           len_dev, max_label_len, blank, logp, nullptr, s, &err);
+    if (rc) return Fail(err);
+    rc = LaunchSumScale(logp, N, -scale, loss, s);
+    if (rc) return FailCuda("sum_scale", (cudaError_t)rc);
+    return 0;
 }
 
 /* ---- gpu_ctc/ctc.h surface ------------------------------------------------------------------- */

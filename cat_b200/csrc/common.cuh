@@ -159,6 +159,11 @@ int LaunchCtc(const void *y, int y_bf16, long sn, long st, int N, int T, int V, 
               const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
               float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, float *logp,
               const double *lnorm, cudaStream_t stream, std::string *err, int overwrite = 0, int Tfull = 0);
+// forward-only numerator: logp[n] = log p(l_n | x_n) (normalised by lnorm[n] when given) from the alpha chains alone, one
+// CTA per utterance, no workspace; infeasible utterances get -inf
+int LaunchCtcLogp(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+                  const int *label_off, const int *label_len, const int *len, int max_label_len, int blank, float *logp,
+                  const double *lnorm, cudaStream_t stream, std::string *err);
 int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStream_t stream);
 int LaunchCtcViterbi(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
                      const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,

@@ -57,7 +57,8 @@ __device__ __forceinline__ double log_add3_d(double a, double b, double c) {
 }
 
 struct CtcWorkspace {
-    double *a, *b, *logp;
+    double *a = nullptr, *b = nullptr, *logp = nullptr;
+    __device__ CtcWorkspace() {}
     __device__ CtcWorkspace(float *base, int n, int T, int ScMax) {
         const size_t cells = (size_t)T * ScMax;
         double *p = reinterpret_cast<double *>(base) + (size_t)n * (2 * cells + 1);
@@ -68,13 +69,16 @@ struct CtcWorkspace {
 };
 
 // shared memory carve-up: a[2][ScMax] doubles | lab[Lmax+1] ints | yrow[2][V] floats
+// SPILL = false (forward-only loss): one CTA per utterance walks the alpha chain and writes only logp_out; no cell, no
+// workspace.  The arithmetic is the same, so logp_out is bit-identical to the spilling launch's.
+template <bool SPILL>
 __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long st, int T, int V,
                                       const int *labels, const int *label_off, const int *label_len, const int *len,
                                       int max_label_len, int blank, float *alpha_ws, bool want_beta, float *logp_out,
                                       const double *lnorm) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    const int n = blockIdx.x >> 1;
-    const unsigned role = blockIdx.x & 1;   // 0: alpha pass, 1: beta pass
+    const int n = SPILL ? blockIdx.x >> 1 : blockIdx.x;
+    const unsigned role = SPILL ? blockIdx.x & 1 : 0;   // 0: alpha pass, 1: beta pass
     const int tid = threadIdx.x, NT = blockDim.x;
     const int L = label_len[n], Tn = len[n];
     const int Sc = 2 * L + 1, L1 = L + 1;
@@ -82,7 +86,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
     double *s_a = reinterpret_cast<double *>(smem_raw);                        // [2][ScMax]
     int *s_lab = reinterpret_cast<int *>(s_a + 2 * ScMax);                     // [max_label_len + 1] label of cell 2i+1
     float *s_y = reinterpret_cast<float *>(s_lab + max_label_len + 1);         // [2][V]
-    CtcWorkspace W(alpha_ws, n, T, ScMax);
+    const CtcWorkspace W = SPILL ? CtcWorkspace(alpha_ws, n, T, ScMax) : CtcWorkspace();
     const int *lab = labels + label_off[n];
 
     // feasibility (gpu_ctc_kernels.h:108-109)
@@ -94,7 +98,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
     if (rep) atomicAdd(&s_rep, rep);
     __syncthreads();
     if (Tn <= 0 || L + s_rep > Tn) {
-        if (tid == 0 && role == 0) { logp_out[n] = -INFINITY; *W.logp = -INFINITY; }
+        if (tid == 0 && role == 0) { logp_out[n] = -INFINITY; if (SPILL) *W.logp = -INFINITY; }
         return;
     }
     if (!want_beta && role == 1) return;   // likelihood only
@@ -114,7 +118,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
         if (s == 0) v = (double)s_y[blank];
         else if (s == 1) v = (double)s_y[s_lab[0]];
         s_a[s] = v;
-        ws[s] = v;
+        if (SPILL) ws[s] = v;
     }
     // Row prefetch: the emission row of frame t+1 is loaded into registers while frame t is computed and parked in
     // shared memory afterwards, so no frame waits on a global-memory round trip (V <= kRowRegs * blockDim).
@@ -142,7 +146,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
             if (i > 0) vb = log_add_d(vb, prev[sb - 1]);
             vb += (double)yc[blank];
             cur[sb] = vb;
-            ws[(size_t)t * ScMax + sb] = vb;
+            if (SPILL) ws[(size_t)t * ScMax + sb] = vb;
             if (i < L) {   // label cell 2i+1
                 const int sl = sb + 1;
                 const int li = s_lab[i];
@@ -150,7 +154,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
                 double vl = log_add3_d(prev[sl], prev[sb], skip ? prev[sl - 2] : -INFINITY);
                 vl += (double)yc[li];
                 cur[sl] = vl;
-                ws[(size_t)t * ScMax + sl] = vl;
+                if (SPILL) ws[(size_t)t * ScMax + sl] = vl;
             }
         }
         if (row_in_regs && t + 1 < Tn) {   // park row t+1 in the slot last read during frame t-1
@@ -166,9 +170,9 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
         if (Sc > 1) lp = log_add_d(lp, last[Sc - 2]);
         // raw-logit entry: the reported log-likelihood is normalised; everything else stays in the raw domain
         logp_out[n] = (float)(lp - (lnorm ? lnorm[n] : 0.0));
-        *W.logp = lp;
+        if (SPILL) *W.logp = lp;
     }
-    } else {
+    } else if (SPILL) {
     // ---- beta pass (the utterance's second CTA), concurrent with the alpha pass -------------------------
     {
         const int t = Tn - 1;
@@ -368,7 +372,7 @@ __global__ void assemble_loss_kernel(const float *logz, const float *logp, int N
 }
 
 // The two halves of the numerator: the alpha || beta chains write the cell workspace + logp, the occupancy kernel turns
-// the cells into the gradient.
+// the cells into the gradient.  alpha_ws = null: the forward-only launch (the alpha chains alone, logp only).
 int LaunchCtcAlphaBeta(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
                        const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                        float *alpha_ws, bool want_beta, float *logp, const double *lnorm, cudaStream_t stream,
@@ -379,10 +383,16 @@ int LaunchCtcAlphaBeta(const void *y, int y_bf16, long sn, long st, int N, int T
     threads = threads < 64 ? 64 : (threads > 1024 ? 1024 : threads);
     const size_t smem = (size_t)2 * ScMax * 8 + (size_t)(max_label_len + 1) * 4 + (size_t)2 * V * 4 + 16;
     if (smem > 200 * 1024 || (size_t)V * 4 > 200 * 1024) { *err = "label sequence too long for the numerator kernel's shared memory"; return 1; }
-    cudaError_t e = cudaFuncSetAttribute(ctc_alpha_beta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const bool spill = alpha_ws != nullptr;
+    const void *kernel = spill ? (const void *)ctc_alpha_beta_kernel<true> : (const void *)ctc_alpha_beta_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc): ") + cudaGetErrorString(e); return (int)e; }
-    ctc_alpha_beta_kernel<<<2 * N, threads, smem, stream>>>(y, y_bf16, sn, st, T, V, labels, label_off, label_len, len,
-                                                            max_label_len, blank, alpha_ws, want_beta, logp, lnorm);
+    if (spill)
+        ctc_alpha_beta_kernel<true><<<2 * N, threads, smem, stream>>>(y, y_bf16, sn, st, T, V, labels, label_off, label_len, len,
+                                                                      max_label_len, blank, alpha_ws, want_beta, logp, lnorm);
+    else
+        ctc_alpha_beta_kernel<false><<<N, threads, smem, stream>>>(y, y_bf16, sn, st, T, V, labels, label_off, label_len, len,
+                                                                   max_label_len, blank, nullptr, false, logp, lnorm);
     CountLaunch();
     e = cudaGetLastError();
     if (e != cudaSuccess) { *err = std::string("ctc launch: ") + cudaGetErrorString(e); return (int)e; }
@@ -420,6 +430,13 @@ int LaunchCtc(const void *y, int y_bf16, long sn, long st, int N, int T, int V, 
     if (rc || grad == nullptr) return rc;
     return LaunchCtcGamma(y, y_bf16, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws, grad, gsn,
                           gst, grad_scale, stream, err, overwrite, Tfull);
+}
+
+int LaunchCtcLogp(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+                  const int *label_off, const int *label_len, const int *len, int max_label_len, int blank, float *logp,
+                  const double *lnorm, cudaStream_t stream, std::string *err) {
+    return LaunchCtcAlphaBeta(y, y_bf16, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, nullptr,
+                              false, logp, lnorm, stream, err);
 }
 
 int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStream_t stream) {

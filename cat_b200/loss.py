@@ -110,6 +110,11 @@ class CTC_CRF_LOSS(Module):
         _assert_no_grad(labels)
         _assert_no_grad(lx)
         _assert_no_grad(ly)
+        if not torch.is_grad_enabled():
+            # evaluation (torch.no_grad / inference_mode): the loss alone, with the den alpha on a ring of frames and no
+            # gradient.  Keyed on grad mode, not on logits.requires_grad: with grad mode on the gradient is always computed.
+            return core.ctc_crf_loss_fwd_only(logits.contiguous(), labels, lx, ly, self.lamb, self.size_average,
+                                              from_logits=self.from_logits)[0]
         return self.ctc_crf(logits, labels, lx, ly, self.lamb, self.size_average)
 
 
@@ -126,6 +131,8 @@ class WARP_CTC_LOSS(Module):
         _assert_no_grad(labels)
         _assert_no_grad(input_lengths)
         _assert_no_grad(label_lengths)
+        if not torch.is_grad_enabled():   # evaluation: the loss alone (see CTC_CRF_LOSS.forward)
+            return core.ctc_loss_fwd_only(logits.contiguous(), labels, input_lengths, label_lengths, self.size_average)[0]
         return self.ctc(logits, labels, input_lengths, label_lengths, self.size_average)
 
 

@@ -158,6 +158,22 @@ int ccb_ctc_crf_loss_logits_ckpt_fwd(const void *logits, int dtype, int N, int T
                                      float *alpha_ws, void *aux_ws, void *ctc_ws,
                                      float *grad, float *loss, float *parts, void *stream);
 
+/* Forward-only CTC-CRF loss, for evaluation without a gradient (CTC_CRF_LOSS under torch.no_grad): the loss and parts of
+ * the two fused entries above, from_logits != 0 selecting the raw-logit one, and nothing else.
+ *   loss[0] = scale * sum_n (logZ_den[n] - (1+lamb) logp_ctc[n]);   parts (optional, may be NULL): 2N floats [logZ_den | logp_ctc]
+ * The den forward pass keeps alpha on a ring of a few frames and sums logZ at each utterance's last frame, so its memory does
+ * not grow with Tmax: alpha_ws holds ccb_den_fwd_alpha_floats(N) floats (7 frames of S x PadLanes(N) floats).  There is no
+ * backward pass, no numerator cell spill and no (N,T,V) gradient.  aux_ws: ccb_den_aux_bytes(N, Tmax) bytes; num_ws:
+ * ccb_num_fwd_only_bytes(N) bytes, the numerator's log-likelihoods.  logp_ctc is bit-identical to the fused entries', logZ_den
+ * equal to fp32 rounding.  Everything is enqueued on `stream`. */
+size_t ccb_den_fwd_alpha_floats(int N);
+size_t ccb_num_fwd_only_bytes(int N);
+int ccb_ctc_crf_loss_fwd_only(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax,
+                              const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                              const int *len_dev, int max_label_len, float lamb, float scale,
+                              float *alpha_ws, void *aux_ws, void *num_ws,
+                              float *loss, float *parts, void *stream);
+
 /* CTC-only loss (replaces the numerator-only path ctc_crf/__init__.py:25-56 = WARP_CTC_LOSS) on an (N,T,V) block of
  * log-probs, read in place (no (T,N,V) transpose copy, cf. __init__.py:31):
  *   logp[n] = log p(l_n | x_n)  (N,) device out;   loss[0] = -scale * sum_n logp[n];
@@ -168,6 +184,11 @@ int ccb_ctc_loss_fwd(const void *logits, int dtype, int N, int T, int V, int Tma
                      const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
                      int max_label_len, int blank, float scale, void *ctc_ws, float *grad, float *loss, float *logp,
                      void *stream);
+/* Its forward-only counterpart (WARP_CTC_LOSS under torch.no_grad): logp and loss as above, bit-identical; no workspace and
+ * no gradient (one alpha chain per utterance, no cells written). */
+int ccb_ctc_loss_fwd_only(const void *logits, int dtype, int N, int T, int V, int Tmax,
+                          const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                          int max_label_len, int blank, float scale, float *loss, float *logp, void *stream);
 
 /* Best-path (Viterbi) alignment over the numerator lattice -- the forced alignment that comes with the CTC numerator
  * (SURVEY.md 8f-4).  align: (N,T) int32 device out, the token emitted at every frame t < len (blank included), -1 beyond
