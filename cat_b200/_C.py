@@ -21,7 +21,9 @@ import torch
 from . import _lib
 from ._lib import ctcOptions
 
-_DTYPES = {torch.float32: 0, torch.bfloat16: 1}
+# logits dtype -> CCB_DTYPE_* code (include/ctc_crf_b200.h).  The fused entries read the logits in place in this type and
+# compute in fp32; gpu_den / gpu_ctc keep the reference's fp32 contract.
+_DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 
 
 def _check(rc: int, what: str) -> None:
@@ -264,7 +266,7 @@ def _plan_slices(L, lx, ly, N, V, dev):
 def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
                      lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False
                      ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
-    """Fused CTC-CRF loss.  logits (N,T,V) fp32 or bf16 CUDA contiguous log-probs; labels/lx/ly int32 CPU.
+    """Fused CTC-CRF loss.  logits (N,T,V) fp32, bf16 or fp16 CUDA contiguous log-probs; labels/lx/ly int32 CPU.
     Returns (loss[1] fp32 CUDA, grad (N,T,V) fp32 CUDA, parts[2N] or None).  Never synchronises the host.
     Batches whose scratch does not fit the free memory (or > 512 utterances) are processed in slices.
     from_logits: `logits` are the RAW encoder outputs; log_softmax and its Jacobian are applied inside
@@ -462,8 +464,8 @@ def ctc_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tens
 
 def ctc_align(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, blank: int = 0
               ) -> Tuple[torch.Tensor, torch.Tensor]:
-    """Best-path (Viterbi) forced alignment over the numerator lattice (SURVEY 8f-4).  logits (N,T,V) fp32/bf16 CUDA
-    log-probs; labels/lx/ly int32 CPU as for the loss.  Returns (align (N,T) int32 CUDA: the token of every frame
+    """Best-path (Viterbi) forced alignment over the numerator lattice (SURVEY 8f-4).  logits (N,T,V) fp32/bf16/fp16
+    CUDA log-probs; labels/lx/ly int32 CPU as for the loss.  Returns (align (N,T) int32 CUDA: the token of every frame
     t < lx[n], blank included, -1 beyond; score (N,) fp32 CUDA: log-probability of that path, -inf if infeasible)."""
     L = _lib.lib()
     N, T, V = _check_batch_args(logits, labels, lx, ly)

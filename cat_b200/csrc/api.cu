@@ -49,6 +49,13 @@ int g_tl_step0 = 0, g_tl_steps = 0;
 int Fail(const std::string &m) { g_err = m; return 1; }
 int FailCuda(const char *what, cudaError_t e) { g_err = std::string(what) + ": " + cudaGetErrorString(e); return (int)e ? (int)e : 1; }
 
+// the logits dtypes the kernels read (common.cuh load_y); any other code is refused before a kernel sees it
+bool KnownDtype(int dtype) { return dtype == CCB_DTYPE_F32 || dtype == CCB_DTYPE_BF16 || dtype == CCB_DTYPE_F16; }
+int FailDtype(const char *what, int dtype) {
+    return Fail(std::string(what) + ": unsupported logits dtype code " + std::to_string(dtype) +
+                " (CCB_DTYPE_F32 0, CCB_DTYPE_BF16 1, CCB_DTYPE_F16 2)");
+}
+
 #define CCB_CUDA(call)                                                   \
     do {                                                                 \
         cudaError_t e__ = (call);                                        \
@@ -187,7 +194,7 @@ DenParams BaseParams(const DeviceGraph &g, const void *y, int dtype, long sn, lo
     p.S = g.S; p.num_pairs = g.P; p.start = g.start; p.n_warps = g.shape.n_warps;
     p.scale_exp = g.scale_exp;
     p.start_final = g.start_final;
-    p.y = y; p.y_bf16 = (dtype == CCB_DTYPE_BF16); p.sn = sn; p.st = st;
+    p.y = y; p.y_dtype = dtype; p.sn = sn; p.st = st;
     p.N = N; p.Npad = L.Npad; p.Tmax = T; p.V = V; p.len = len;
     p.alpha = alpha;
     p.a_frames = T + 1 + (g.P > 0 ? 2 : 0);   // full spill (a_base = a_ring = 0: frame t at position t)
@@ -205,7 +212,7 @@ DenParams BaseParams(const DeviceGraph &g, const void *y, int dtype, long sn, lo
 
 int CheckDen(const DeviceGraph &g, int dtype, int N, int T, int V) {
     if (N <= 0 || T <= 0 || V <= 0) return Fail("den: empty batch");
-    if (dtype != CCB_DTYPE_F32 && dtype != CCB_DTYPE_BF16) return Fail("den: unsupported logits dtype");
+    if (!KnownDtype(dtype)) return FailDtype("den", dtype);
     if (V < g.num_labels)
         return Fail("den graph uses label " + std::to_string(g.num_labels - 1) + " but logits have only " + std::to_string(V) + " classes");
     if ((size_t)(2 * (size_t)g.S + g.P) * (size_t)PadLanes(N, g.small_ok) * 4 >= ((size_t)1 << 32)) return Fail("den: states x batch too large for 32-bit row offsets; split the batch");
@@ -239,9 +246,9 @@ int DenForward(const DeviceGraph &g, const void *y, int dtype, long sn, long st,
     const DenAuxLayout L = MakeDenAuxLayout(g.S, N, T, g.small_ok);
     char *a = reinterpret_cast<char *>(aux);
     CCB_CUDA(cudaMemsetAsync(a, 0, L.zero_bytes, stream));
-    int rc = raw ? LaunchFrameLse(y, dtype == CCB_DTYPE_BF16, sn, st, N, T, V, len, reinterpret_cast<float *>(a + L.fmax),
+    int rc = raw ? LaunchFrameLse(y, dtype, sn, st, N, T, V, len, reinterpret_cast<float *>(a + L.fmax),
                                   reinterpret_cast<float *>(a + L.lz), reinterpret_cast<double *>(a + L.lnorm), L.Npad, stream)
-                 : LaunchFrameMax(y, dtype == CCB_DTYPE_BF16, sn, st, N, T, V, len, reinterpret_cast<float *>(a + L.fmax), L.Npad, stream);
+                 : LaunchFrameMax(y, dtype, sn, st, N, T, V, len, reinterpret_cast<float *>(a + L.fmax), L.Npad, stream);
     if (rc) return FailCuda("frame_max", (cudaError_t)rc);
     DenParams p = BaseParams(g, y, dtype, sn, st, N, T, V, len, alpha, aux, L);
     if (raw) p.lnorm = reinterpret_cast<const double *>(a + L.lnorm);
@@ -488,9 +495,10 @@ int ccb_ctc_forward_backward(const void *logits, int dtype, long sn, long st, in
                              float *grad, long gsn, long gst, float grad_scale, float *logp, void *stream) {
     g_err.clear();
     if (N <= 0 || T <= 0 || V <= 0 || !logits || !workspace || !logp) return Fail("ctc: bad arguments");
+    if (!KnownDtype(dtype)) return FailDtype("ctc", dtype);
     if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
     std::string err;
-    int rc = LaunchCtc(logits, dtype == CCB_DTYPE_BF16, sn, st, N, T, V, labels_dev, label_off_dev, label_len_dev,
+    int rc = LaunchCtc(logits, dtype, sn, st, N, T, V, labels_dev, label_off_dev, label_len_dev,
                        len_dev, max_label_len, blank, reinterpret_cast<float *>(workspace), grad, gsn, gst, grad_scale,
                        logp, nullptr, (cudaStream_t)stream, &err);
     if (rc) return Fail(err);
@@ -506,12 +514,12 @@ int ccb_ctc_loss_fwd(const void *logits, int dtype, int N, int T, int V, int Tma
     g_err.clear();
     if (N <= 0 || T <= 0 || V <= 0 || !logits || !ctc_ws || !grad || !loss || !logp) return Fail("ctc_loss_fwd: bad arguments");
     if (Tmax <= 0 || Tmax > T) return Fail("ctc_loss_fwd: Tmax must lie in [1, T]");
-    if (dtype != CCB_DTYPE_F32 && dtype != CCB_DTYPE_BF16) return Fail("ctc_loss_fwd: unsupported logits dtype");
+    if (!KnownDtype(dtype)) return FailDtype("ctc_loss_fwd", dtype);
     if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
     cudaStream_t s = (cudaStream_t)stream;
     const long sn = (long)T * V, st = V;
     std::string err;
-    int rc = LaunchCtc(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+    int rc = LaunchCtc(logits, dtype, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
                        max_label_len, blank, reinterpret_cast<float *>(ctc_ws), grad, sn, st, -scale, logp, nullptr, s, &err,
                        /*overwrite=*/1, /*Tfull=*/T);
     if (rc) return Fail(err);
@@ -529,10 +537,10 @@ int ccb_ctc_align(const void *logits, int dtype, long sn, long st, int N, int T,
                   int max_label_len, int blank, void *workspace, int *align, float *score, void *stream) {
     g_err.clear();
     if (N <= 0 || T <= 0 || V <= 0 || !logits || !workspace || !align) return Fail("ctc_align: bad arguments");
-    if (dtype != CCB_DTYPE_F32 && dtype != CCB_DTYPE_BF16) return Fail("ctc_align: unsupported logits dtype");
+    if (!KnownDtype(dtype)) return FailDtype("ctc_align", dtype);
     if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
     std::string err;
-    int rc = LaunchCtcViterbi(logits, dtype == CCB_DTYPE_BF16, sn, st, N, T, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+    int rc = LaunchCtcViterbi(logits, dtype, sn, st, N, T, V, labels_dev, label_off_dev, label_len_dev, len_dev,
                               max_label_len, blank, reinterpret_cast<unsigned char *>(workspace), align, score, (cudaStream_t)stream, &err);
     if (rc) return Fail(err);
     return 0;
@@ -564,11 +572,11 @@ static int LossFwdImpl(bool raw, const void *logits, int dtype, int N, int T, in
     if (DenBackward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, grad, sn, st, scale, s, raw, ckpt_k)) return 1;
     // the numerator accumulates into the gradient after the den passes have normalised their part of it
     std::string err;
-    int rc = LaunchCtc(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+    int rc = LaunchCtc(logits, dtype, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
                        max_label_len, 0, reinterpret_cast<float *>(ctc_ws), grad, sn, st, -(1.f + lamb) * scale, logp, lnorm, s, &err);
     if (rc) return Fail(err);
     if (raw) {   // chain through log_softmax: dL/dz = g - softmax(z) * sum_k g_k
-        rc = LaunchLogitGrad(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, len_dev,
+        rc = LaunchLogitGrad(logits, dtype, sn, st, N, Tmax, V, len_dev,
                              reinterpret_cast<const float *>((char *)aux_ws + L.lz), L.Npad, grad, sn, st, s);
         if (rc) return FailCuda("logit_grad", (cudaError_t)rc);
     }
@@ -638,7 +646,7 @@ static int LossFwdOnlyImpl(bool raw, const void *logits, int dtype, int N, int T
     const double *lnorm = raw ? reinterpret_cast<const double *>((char *)aux_ws + L.lnorm) : nullptr;
     if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw, 0, /*fwd_only=*/true)) return 1;
     std::string err;
-    int rc = LaunchCtcLogp(logits, dtype == CCB_DTYPE_BF16, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev,
+    int rc = LaunchCtcLogp(logits, dtype, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev,
                            len_dev, max_label_len, 0, logp, lnorm, s, &err);
     if (rc) return Fail(err);
     rc = LaunchAssembleLoss(logz, logp, N, lamb, scale, loss, s);
@@ -664,11 +672,11 @@ int ccb_ctc_loss_fwd_only(const void *logits, int dtype, int N, int T, int V, in
     g_err.clear();
     if (N <= 0 || T <= 0 || V <= 0 || !logits || !loss || !logp) return Fail("ctc_loss_fwd_only: bad arguments");
     if (Tmax <= 0 || Tmax > T) return Fail("ctc_loss_fwd_only: Tmax must lie in [1, T]");
-    if (dtype != CCB_DTYPE_F32 && dtype != CCB_DTYPE_BF16) return Fail("ctc_loss_fwd_only: unsupported logits dtype");
+    if (!KnownDtype(dtype)) return FailDtype("ctc_loss_fwd_only", dtype);
     if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
     cudaStream_t s = (cudaStream_t)stream;
     std::string err;
-    int rc = LaunchCtcLogp(logits, dtype == CCB_DTYPE_BF16, (long)T * V, V, N, Tmax, V, labels_dev, label_off_dev, label_len_dev,
+    int rc = LaunchCtcLogp(logits, dtype, (long)T * V, V, N, Tmax, V, labels_dev, label_off_dev, label_len_dev,
                            len_dev, max_label_len, blank, logp, nullptr, s, &err);
     if (rc) return Fail(err);
     rc = LaunchSumScale(logp, N, -scale, loss, s);

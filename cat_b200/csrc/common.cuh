@@ -2,11 +2,13 @@
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <cstdint>
 #include <string>
 
+#include "../../include/ctc_crf_b200.h"
 #include "den_launch.h"
 
 namespace ccb {
@@ -82,8 +84,8 @@ struct alignas(64) DenParams {
     int scale_exp;        // column sums are renormalised to ~2^scale_exp (DenPlan::scale_exp)
     float start_final;
     // problem
-    const void *y;        // (N,T,V) log-probs, fp32 or bf16
-    int y_bf16;
+    const void *y;        // (N,T,V) log-probs, fp32, bf16 or fp16
+    int y_dtype;          // CCB_DTYPE_* code of y (load_y)
     long sn, st;          // element strides of y
     int N, Npad, Tmax, V;
     const int *len;       // [N] device
@@ -139,11 +141,11 @@ inline int PadLanes(int N, bool small_ok) {
 DenAuxLayout MakeDenAuxLayout(int S, int N, int T, bool small_ok);
 
 // host launchers; return cudaError_t-compatible int (0 = ok) and fill *err
-int LaunchFrameMax(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *len, float *fmax,
+int LaunchFrameMax(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *len, float *fmax,
                    int Npad, cudaStream_t stream);
-int LaunchFrameLse(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *len, float *fmax,
+int LaunchFrameLse(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *len, float *fmax,
                    float *lz, double *lnorm, int Npad, cudaStream_t stream);
-int LaunchLogitGrad(const void *z, int z_bf16, long sn, long st, int N, int T, int V, const int *len, const float *lz,
+int LaunchLogitGrad(const void *z, int z_dtype, long sn, long st, int N, int T, int V, const int *len, const float *lz,
                     int Npad, float *grad, long gsn, long gst, cudaStream_t stream);
 // Checkpointed alpha workspace for K = ckpt_k (0: the full spill): frame positions of the first pass's ring / of one
 // segment, then the checkpoints, then the backward pass's carried log-scales (see den_kernels.cu alpha_pos)
@@ -155,17 +157,17 @@ inline int CkptCount(int T, int K) { const int k = CkptK(T, K); return (T + k - 
 int LaunchDen(bool backward, const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err);
 int LaunchDenGradNormalize(float *grad, long gsn, long gst, const float *absum, const int *len, int N, int Npad,
                            int T, int V, float scale, cudaStream_t stream);
-int LaunchCtc(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+int LaunchCtc(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
               const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
               float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, float *logp,
               const double *lnorm, cudaStream_t stream, std::string *err, int overwrite = 0, int Tfull = 0);
 // forward-only numerator: logp[n] = log p(l_n | x_n) (normalised by lnorm[n] when given) from the alpha chains alone, one
 // CTA per utterance, no workspace; infeasible utterances get -inf
-int LaunchCtcLogp(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+int LaunchCtcLogp(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                   const int *label_off, const int *label_len, const int *len, int max_label_len, int blank, float *logp,
                   const double *lnorm, cudaStream_t stream, std::string *err);
 int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStream_t stream);
-int LaunchCtcViterbi(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+int LaunchCtcViterbi(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                      const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                      unsigned char *bp_ws, int *align, float *score, cudaStream_t stream, std::string *err);
 int LaunchAssembleLoss(const float *logz, const float *logp, int N, float lamb, float scale, float *loss,
@@ -176,9 +178,12 @@ void CountLaunch(int n = 1);
 // device helpers
 // ------------------------------------------------------------------------------------------------
 #ifdef __CUDACC__
-__device__ __forceinline__ float load_y(const void *y, int bf16, long idx) {
-    return bf16 ? __bfloat162float(reinterpret_cast<const __nv_bfloat16 *>(y)[idx])
-                : __ldg(reinterpret_cast<const float *>(y) + idx);
+// Element idx of the logits as float.  dtype is a CCB_DTYPE_* code: fp32 is read as is; bf16 and fp16 share one 16-bit
+// load and differ only in the convert (callers accept no other code).
+__device__ __forceinline__ float load_y(const void *y, int dtype, long idx) {
+    if (dtype == CCB_DTYPE_F32) return __ldg(reinterpret_cast<const float *>(y) + idx);
+    const unsigned short h = reinterpret_cast<const unsigned short *>(y)[idx];
+    return dtype == CCB_DTYPE_BF16 ? __bfloat162float(__ushort_as_bfloat16(h)) : __half2float(__ushort_as_half(h));
 }
 
 __device__ __forceinline__ void red_release_add_u32(unsigned *p, unsigned v) {

@@ -72,7 +72,7 @@ struct CtcWorkspace {
 // SPILL = false (forward-only loss): one CTA per utterance walks the alpha chain and writes only logp_out; no cell, no
 // workspace.  The arithmetic is the same, so logp_out is bit-identical to the spilling launch's.
 template <bool SPILL>
-__global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long st, int T, int V,
+__global__ void ctc_alpha_beta_kernel(const void *y, int y_dtype, long sn, long st, int T, int V,
                                       const int *labels, const int *label_off, const int *label_len, const int *len,
                                       int max_label_len, int blank, float *alpha_ws, bool want_beta, float *logp_out,
                                       const double *lnorm) {
@@ -111,7 +111,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
 
     if (role == 0) {
     // ---- forward ---------------------------------------------------------------------------------
-    for (int k = tid; k < V; k += NT) s_y[k] = load_y(y, y_bf16, ybase + k);
+    for (int k = tid; k < V; k += NT) s_y[k] = load_y(y, y_dtype, ybase + k);
     __syncthreads();
     for (int s = tid; s < Sc; s += NT) {
         double v = -INFINITY;
@@ -124,7 +124,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
     // shared memory afterwards, so no frame waits on a global-memory round trip (V <= kRowRegs * blockDim).
     if (row_in_regs && Tn > 1) {
 #pragma unroll
-        for (int j = 0; j < kRowRegs; ++j) { const int k = tid + j * NT; yreg[j] = k < V ? load_y(y, y_bf16, ybase + st + k) : 0.f; }
+        for (int j = 0; j < kRowRegs; ++j) { const int k = tid + j * NT; yreg[j] = k < V ? load_y(y, y_dtype, ybase + st + k) : 0.f; }
 #pragma unroll
         for (int j = 0; j < kRowRegs; ++j) { const int k = tid + j * NT; if (k < V) s_y[V + k] = yreg[j]; }
     }
@@ -133,10 +133,10 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
         float *yc = s_y + (t & 1) * V;
         const double *prev = s_a + ((t - 1) & 1) * ScMax;
         double *cur = s_a + (t & 1) * ScMax;
-        if (!row_in_regs) for (int k = tid; k < V; k += NT) yc[k] = load_y(y, y_bf16, ybase + (long)t * st + k);
+        if (!row_in_regs) for (int k = tid; k < V; k += NT) yc[k] = load_y(y, y_dtype, ybase + (long)t * st + k);
         else if (t + 1 < Tn) {
 #pragma unroll
-            for (int j = 0; j < kRowRegs; ++j) { const int k = tid + j * NT; yreg[j] = k < V ? load_y(y, y_bf16, ybase + (long)(t + 1) * st + k) : 0.f; }
+            for (int j = 0; j < kRowRegs; ++j) { const int k = tid + j * NT; yreg[j] = k < V ? load_y(y, y_dtype, ybase + (long)(t + 1) * st + k) : 0.f; }
         }
         __syncthreads();
         for (int i = tid; i < L1; i += NT) {
@@ -177,7 +177,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
     {
         const int t = Tn - 1;
         float *yc = s_y + (t & 1) * V;
-        for (int k = tid; k < V; k += NT) yc[k] = load_y(y, y_bf16, ybase + (long)t * st + k);
+        for (int k = tid; k < V; k += NT) yc[k] = load_y(y, y_dtype, ybase + (long)t * st + k);
     }
     for (int t = Tn - 1; t >= 0; --t) {
         float *yc = s_y + (t & 1) * V;
@@ -185,7 +185,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
         const double *nxt = s_a + ((t + 1) & 1) * ScMax;
         if (t > 0 && row_in_regs) {   // issue the loads for frame t-1 now; they are parked after this frame's work
 #pragma unroll
-            for (int j = 0; j < kRowRegs; ++j) { const int k = tid + j * NT; yreg[j] = k < V ? load_y(y, y_bf16, ybase + (long)(t - 1) * st + k) : 0.f; }
+            for (int j = 0; j < kRowRegs; ++j) { const int k = tid + j * NT; yreg[j] = k < V ? load_y(y, y_dtype, ybase + (long)(t - 1) * st + k) : 0.f; }
         }
         __syncthreads();   // the only barrier of the frame: publishes row t and beta_{t+1}
         double *bl = wsb + (size_t)t * ScMax;
@@ -222,7 +222,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
 #pragma unroll
                 for (int j = 0; j < kRowRegs; ++j) { const int k = tid + j * NT; if (k < V) yn[k] = yreg[j]; }
             } else {
-                for (int k = tid; k < V; k += NT) yn[k] = load_y(y, y_bf16, ybase + (long)(t - 1) * st + k);
+                for (int k = tid; k < V; k += NT) yn[k] = load_y(y, y_dtype, ybase + (long)(t - 1) * st + k);
             }
         }
     }
@@ -233,7 +233,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_bf16, long sn, long s
 // Occupancies from the two spills: one warp per (utterance, frame), label accumulator [V] per warp in shared memory.
 //   gamma_t[k] = sum_{s: l'_s = k} exp(alpha_t(s) + beta_t(s) - y_t(k) - log p)   (gpu_ctc_kernels.h:337-453)
 // accumulated with the caller's scale into grad[n][t][:] (which may already hold the denominator part).
-__global__ void ctc_gamma_kernel(const void *y, int y_bf16, long sn, long st, int N, int T, int V,
+__global__ void ctc_gamma_kernel(const void *y, int y_dtype, long sn, long st, int N, int T, int V,
                                  const int *labels, const int *label_off, const int *label_len, const int *len,
                                  int max_label_len, int blank, float *alpha_ws,
                                  float *grad, long gsn, long gst, float grad_scale, int overwrite, int Tfull) {
@@ -261,7 +261,7 @@ __global__ void ctc_gamma_kernel(const void *y, int y_bf16, long sn, long st, in
     float occ_blank = 0.f;
     for (int s = lane; s < Sc; s += 32) {   // lane parity == cell parity: even lanes take blanks, odd lanes labels
         const int li = (s & 1) ? __ldg(lab + (s >> 1)) : blank;
-        const float o = (float)(al[s] + bl[s] - (double)load_y(y, y_bf16, yrow + li) - logp_d);
+        const float o = (float)(al[s] + bl[s] - (double)load_y(y, y_dtype, yrow + li) - logp_d);
         const float e = (o == -INFINITY || o != o) ? 0.f : expf(o);
         if (s & 1) { if (e != 0.f) atomicAdd(&g[li], e); }
         else occ_blank += e;
@@ -294,7 +294,7 @@ __global__ void sum_scale_kernel(const float *logp, int N, float scale, float *l
 // walks it back.  align[n][t] = the token emitted at frame t (blank included), -1 for t >= len or an infeasible utterance.
 // Ties are broken towards the smaller predecessor index (stay < s-1 < s-2).
 // shared memory: lab[Lmax] ints | v[2][ScMax] floats
-__global__ void ctc_viterbi_kernel(const void *y, int y_bf16, long sn, long st, int T, int V,
+__global__ void ctc_viterbi_kernel(const void *y, int y_dtype, long sn, long st, int T, int V,
                                    const int *labels, const int *label_off, const int *label_len, const int *len,
                                    int max_label_len, int blank, unsigned char *bp_ws, int *align, float *score) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -320,8 +320,8 @@ __global__ void ctc_viterbi_kernel(const void *y, int y_bf16, long sn, long st, 
     const long ybase = n * sn;
     for (int s = tid; s < Sc; s += NT) {
         float v = -INFINITY;
-        if (s == 0) v = load_y(y, y_bf16, ybase + blank);
-        else if (s == 1) v = load_y(y, y_bf16, ybase + s_lab[0]);
+        if (s == 0) v = load_y(y, y_dtype, ybase + blank);
+        else if (s == 1) v = load_y(y, y_dtype, ybase + s_lab[0]);
         s_v[s] = v;
         bp[s] = 0;
     }
@@ -336,7 +336,7 @@ __global__ void ctc_viterbi_kernel(const void *y, int y_bf16, long sn, long st, 
             float vb = prev[sb];
             unsigned char kb = 0;
             if (i > 0 && prev[sb - 1] > vb) { vb = prev[sb - 1]; kb = 1; }
-            cur[sb] = vb + load_y(y, y_bf16, yrow + blank);
+            cur[sb] = vb + load_y(y, y_dtype, yrow + blank);
             b[sb] = kb;
             if (i < L) {
                 const int sl = sb + 1, li = s_lab[i];
@@ -344,7 +344,7 @@ __global__ void ctc_viterbi_kernel(const void *y, int y_bf16, long sn, long st, 
                 unsigned char kl = 0;
                 if (prev[sb] > vl) { vl = prev[sb]; kl = 1; }
                 if (i > 0 && li != s_lab[i - 1] && prev[sl - 2] > vl) { vl = prev[sl - 2]; kl = 2; }
-                cur[sl] = vl + load_y(y, y_bf16, yrow + li);
+                cur[sl] = vl + load_y(y, y_dtype, yrow + li);
                 b[sl] = kl;
             }
         }
@@ -373,7 +373,7 @@ __global__ void assemble_loss_kernel(const float *logz, const float *logp, int N
 
 // The two halves of the numerator: the alpha || beta chains write the cell workspace + logp, the occupancy kernel turns
 // the cells into the gradient.  alpha_ws = null: the forward-only launch (the alpha chains alone, logp only).
-int LaunchCtcAlphaBeta(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+int LaunchCtcAlphaBeta(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                        const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                        float *alpha_ws, bool want_beta, float *logp, const double *lnorm, cudaStream_t stream,
                        std::string *err) {
@@ -388,10 +388,10 @@ int LaunchCtcAlphaBeta(const void *y, int y_bf16, long sn, long st, int N, int T
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc): ") + cudaGetErrorString(e); return (int)e; }
     if (spill)
-        ctc_alpha_beta_kernel<true><<<2 * N, threads, smem, stream>>>(y, y_bf16, sn, st, T, V, labels, label_off, label_len, len,
+        ctc_alpha_beta_kernel<true><<<2 * N, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len, len,
                                                                       max_label_len, blank, alpha_ws, want_beta, logp, lnorm);
     else
-        ctc_alpha_beta_kernel<false><<<N, threads, smem, stream>>>(y, y_bf16, sn, st, T, V, labels, label_off, label_len, len,
+        ctc_alpha_beta_kernel<false><<<N, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len, len,
                                                                    max_label_len, blank, nullptr, false, logp, lnorm);
     CountLaunch();
     e = cudaGetLastError();
@@ -399,7 +399,7 @@ int LaunchCtcAlphaBeta(const void *y, int y_bf16, long sn, long st, int N, int T
     return 0;
 }
 
-int LaunchCtcGamma(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+int LaunchCtcGamma(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                    const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                    float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, cudaStream_t stream,
                    std::string *err, int overwrite, int Tfull) {
@@ -411,7 +411,7 @@ int LaunchCtcGamma(const void *y, int y_bf16, long sn, long st, int N, int T, in
     if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc gamma): ") + cudaGetErrorString(e); return (int)e; }
     const long rows = (long)N * (overwrite ? Tfull : T);
     ctc_gamma_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, gsm, stream>>>(
-        y, y_bf16, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws, grad, gsn, gst, grad_scale,
+        y, y_dtype, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws, grad, gsn, gst, grad_scale,
         overwrite, Tfull);
     CountLaunch();
     e = cudaGetLastError();
@@ -421,21 +421,21 @@ int LaunchCtcGamma(const void *y, int y_bf16, long sn, long st, int N, int T, in
 
 }  // namespace
 
-int LaunchCtc(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+int LaunchCtc(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
               const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
               float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, float *logp,
               const double *lnorm, cudaStream_t stream, std::string *err, int overwrite, int Tfull) {
-    int rc = LaunchCtcAlphaBeta(y, y_bf16, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws,
+    int rc = LaunchCtcAlphaBeta(y, y_dtype, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws,
                                 grad != nullptr, logp, lnorm, stream, err);
     if (rc || grad == nullptr) return rc;
-    return LaunchCtcGamma(y, y_bf16, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws, grad, gsn,
+    return LaunchCtcGamma(y, y_dtype, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws, grad, gsn,
                           gst, grad_scale, stream, err, overwrite, Tfull);
 }
 
-int LaunchCtcLogp(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+int LaunchCtcLogp(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                   const int *label_off, const int *label_len, const int *len, int max_label_len, int blank, float *logp,
                   const double *lnorm, cudaStream_t stream, std::string *err) {
-    return LaunchCtcAlphaBeta(y, y_bf16, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, nullptr,
+    return LaunchCtcAlphaBeta(y, y_dtype, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, nullptr,
                               false, logp, lnorm, stream, err);
 }
 
@@ -445,7 +445,7 @@ int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStrea
     return (int)cudaGetLastError();
 }
 
-int LaunchCtcViterbi(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *labels,
+int LaunchCtcViterbi(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                      const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                      unsigned char *bp_ws, int *align, float *score, cudaStream_t stream, std::string *err) {
     if (N == 0) return 0;
@@ -456,7 +456,7 @@ int LaunchCtcViterbi(const void *y, int y_bf16, long sn, long st, int N, int T, 
     if (smem > 200 * 1024) { *err = "label sequence too long for the alignment kernel's shared memory"; return 1; }
     cudaError_t e = cudaFuncSetAttribute(ctc_viterbi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc viterbi): ") + cudaGetErrorString(e); return (int)e; }
-    ctc_viterbi_kernel<<<N, threads, smem, stream>>>(y, y_bf16, sn, st, T, V, labels, label_off, label_len, len, max_label_len,
+    ctc_viterbi_kernel<<<N, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len, len, max_label_len,
                                                      blank, bp_ws, align, score);
     CountLaunch();
     e = cudaGetLastError();

@@ -125,7 +125,7 @@ __device__ __forceinline__ void prefetch_l2(const void *p) {
 // ------------------------------------------------------------------------------------------------
 // per-frame emission shift  m[t][n] = max_k y[n][t][k]
 // ------------------------------------------------------------------------------------------------
-__global__ void frame_max_kernel(const void *y, int bf16, long sn, long st, int N, int T, int V,
+__global__ void frame_max_kernel(const void *y, int dtype, long sn, long st, int N, int T, int V,
                                  const int *len, float *fmax, int Npad) {
     const int warps_per_block = blockDim.x >> 5;
     const long row = (long)blockIdx.x * warps_per_block + (threadIdx.x >> 5);
@@ -135,7 +135,7 @@ __global__ void frame_max_kernel(const void *y, int bf16, long sn, long st, int 
     if (t >= len[n]) return;
     float m = -INFINITY;
     const long base = n * sn + t * st;
-    for (int k = lane; k < V; k += 32) m = fmaxf(m, load_y(y, bf16, base + k));
+    for (int k = lane; k < V; k += 32) m = fmaxf(m, load_y(y, dtype, base + k));
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(kFull, m, o));
     if (lane == 0) fmax[(size_t)t * Npad + n] = (m == -INFINITY) ? 0.f : m;
@@ -144,7 +144,7 @@ __global__ void frame_max_kernel(const void *y, int bf16, long sn, long st, int 
 // Raw-logit entry (SURVEY 8f-1): per valid frame the max AND the log-normaliser lz = log sum_k exp(z_k) of the raw
 // encoder outputs.  The recursions then run on z as if it were log-probs (emissions are shifted by the row max either
 // way, and a per-frame constant does not change any occupancy); only the log-likelihoods need lz, summed per utterance.
-__global__ void frame_lse_kernel(const void *y, int bf16, long sn, long st, int N, int T, int V,
+__global__ void frame_lse_kernel(const void *y, int dtype, long sn, long st, int N, int T, int V,
                                  const int *len, float *fmax, float *lz, int Npad) {
     const int warps_per_block = blockDim.x >> 5;
     const long row = (long)blockIdx.x * warps_per_block + (threadIdx.x >> 5);
@@ -154,12 +154,12 @@ __global__ void frame_lse_kernel(const void *y, int bf16, long sn, long st, int 
     if (t >= len[n]) return;
     float m = -INFINITY;
     const long base = n * sn + t * st;
-    for (int k = lane; k < V; k += 32) m = fmaxf(m, load_y(y, bf16, base + k));
+    for (int k = lane; k < V; k += 32) m = fmaxf(m, load_y(y, dtype, base + k));
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(kFull, m, o));
     if (m == -INFINITY) m = 0.f;
     float s = 0.f;
-    for (int k = lane; k < V; k += 32) s += expf(load_y(y, bf16, base + k) - m);
+    for (int k = lane; k < V; k += 32) s += expf(load_y(y, dtype, base + k) - m);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
     if (lane == 0) {
@@ -181,7 +181,7 @@ __global__ void lnorm_kernel(const float *lz, const int *len, int N, int Npad, d
 
 // Softmax Jacobian of the raw-logit entry: g = dL/dy (y = log_softmax z) -> dL/dz_k = g_k - softmax(z)_k * sum_j g_j,
 // in place, one warp per valid frame (cat/ctc/train.py:173-174 does this through autograd of log_softmax).
-__global__ void logit_grad_kernel(const void *z, int bf16, long sn, long st, int N, int T, int V, const int *len,
+__global__ void logit_grad_kernel(const void *z, int dtype, long sn, long st, int N, int T, int V, const int *len,
                                   const float *lz, int Npad, float *grad, long gsn, long gst) {
     const int warps_per_block = blockDim.x >> 5;
     const long row = (long)blockIdx.x * warps_per_block + (threadIdx.x >> 5);
@@ -196,7 +196,7 @@ __global__ void logit_grad_kernel(const void *z, int bf16, long sn, long st, int
     for (int o = 16; o > 0; o >>= 1) gs += __shfl_xor_sync(kFull, gs, o);
     const float l = lz[(size_t)t * Npad + n];
     const long base = n * sn + t * st;
-    for (int k = lane; k < V; k += 32) g[k] -= expf(load_y(z, bf16, base + k) - l) * gs;
+    for (int k = lane; k < V; k += 32) g[k] -= expf(load_y(z, dtype, base + k) - l) * gs;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -568,7 +568,7 @@ __device__ __forceinline__ void tl_mark(const DenParams &P, int step_index, int 
 // it recomputes the few per-frame scalars it needs so that the hot row-end path keeps its registers.
 template <int U>
 __device__ __noinline__ void forward_partial_row(const int *state_label, const int *len, const float *colsum_prev,
-                                                 const float *fmax_prev, const void *y, int y_bf16, long sn, long yt_off,
+                                                 const float *fmax_prev, const void *y, int y_dtype, long sn, long yt_off,
                                                  int N, int t, int n0, Vec<U> part, uint32_t tgt_off, uint32_t row_bytes,
                                                  float *a_cur, float *s_sum, int scale_exp) {
     const int tgt = (int)(tgt_off / row_bytes);
@@ -580,7 +580,7 @@ __device__ __noinline__ void forward_partial_row(const int *state_label, const i
         if (n < N && t <= __ldg(len + n)) {
             int sh;
             const float r = scale_from_sum(__ldcg(colsum_prev + n), &sh, scale_exp);
-            const float e = expf(load_y(y, y_bf16, n * sn + yt_off + lab) - __ldg(fmax_prev + n));
+            const float e = expf(load_y(y, y_dtype, n * sn + yt_off + lab) - __ldg(fmax_prev + n));
             const float o = part.v[u] * e * r;
             if (o != 0.f) { atomicAdd(dst + u, o); atomicAdd(&s_sum[n], o); }
         }
@@ -786,8 +786,8 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
                     fm[u] = act[u] ? __ldg(P.fmax + (size_t)(t - 1) * Npad + n0 + u) : 0.f;
                     // emissions of the chunk's first labels: issued now, consumed at the first row ends
                     const long yb = (n0 + u) * P.sn + (long)(t - 1) * P.st;
-                    ypre0[u] = (act[u] && labp0 >= 0) ? load_y(P.y, P.y_bf16, yb + labp0) : 0.f;
-                    ypre1[u] = (act[u] && labp1 >= 0) ? load_y(P.y, P.y_bf16, yb + labp1) : 0.f;
+                    ypre0[u] = (act[u] && labp0 >= 0) ? load_y(P.y, P.y_dtype, yb + labp0) : 0.f;
+                    ypre1[u] = (act[u] && labp1 >= 0) ? load_y(P.y, P.y_dtype, yb + labp1) : 0.f;
                 }
             };
             int ql = sb - tile_s0;                               // row index inside the CTA tile
@@ -806,7 +806,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
 #pragma unroll
                         for (int u = 0; u < U; ++u) {
                             const float yv = (lab == labp1) ? ypre1[u]
-                                             : (act[u] ? load_y(P.y, P.y_bf16, (n0 + u) * P.sn + (long)(t - 1) * P.st + lab) : 0.f);
+                                             : (act[u] ? load_y(P.y, P.y_dtype, (n0 + u) * P.sn + (long)(t - 1) * P.st + lab) : 0.f);
                             ec1[u] = act[u] ? expf(yv - fm[u]) : 0.f;
                         }
                     }
@@ -847,7 +847,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
                     // byte offset of the target row (last slot of the segment)
                     const uint32_t tgt_off = load_quad_peers<SMEM_ARCS>(quad, row_bytes, (uint32_t)S).w;
                     forward_partial_row<U>(P.state_label, P.len, P.colsum_a + (size_t)(t - 1) * Npad, P.fmax + (size_t)(t - 1) * Npad,
-                                           P.y, P.y_bf16, P.sn, (long)(t - 1) * P.st, P.N, t, n0, part, tgt_off, row_bytes, a_cur, s_sum, P.scale_exp);
+                                           P.y, P.y_dtype, P.sn, (long)(t - 1) * P.st, P.N, t, n0, part, tgt_off, row_bytes, a_cur, s_sum, P.scale_exp);
                     if (tgt_off == out_row * row_bytes) { ++out_row; ++ql; }   // the part that lives in the row's own group
                     return;
                 }
@@ -857,7 +857,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
 #pragma unroll
                     for (int u = 0; u < U; ++u) {
                         const float yv = (lab == lp) ? (k1 ? ypre1[u] : ypre0[u])
-                                         : (act[u] ? load_y(P.y, P.y_bf16, (n0 + u) * P.sn + (long)(t - 1) * P.st + lab) : 0.f);
+                                         : (act[u] ? load_y(P.y, P.y_dtype, (n0 + u) * P.sn + (long)(t - 1) * P.st + lab) : 0.f);
                         const float en = act[u] ? expf(yv - fm[u]) : 0.f;
                         if (k1) ec1[u] = en; else ec0[u] = en;
                     }
@@ -1110,8 +1110,8 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
                     rb[u] = gat[u] ? scale_from_sum(__ldcg(P.colsum_b + (size_t)(tau + 1) * Npad + n0 + u), &sh, P.scale_exp) : 1.f;
                     fm[u] = act[u] ? __ldg(P.fmax + (size_t)(tau - 1) * Npad + n0 + u) : 0.f;
                     const long yb = (n0 + u) * P.sn + (long)(tau - 1) * P.st;
-                    ypre0[u] = (act[u] && labp0 >= 0) ? load_y(P.y, P.y_bf16, yb + labp0) : 0.f;
-                    ypre1[u] = (act[u] && labp1 >= 0) ? load_y(P.y, P.y_bf16, yb + labp1) : 0.f;
+                    ypre0[u] = (act[u] && labp0 >= 0) ? load_y(P.y, P.y_dtype, yb + labp0) : 0.f;
+                    ypre1[u] = (act[u] && labp1 >= 0) ? load_y(P.y, P.y_dtype, yb + labp1) : 0.f;
                 }
             };
             int curlab0 = -1, curlab1 = -1;
@@ -1160,7 +1160,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
 #pragma unroll
                     for (int u = 0; u < U; ++u) {
                         const float yv = (lab == lp) ? (k1 ? ypre1[u] : ypre0[u])
-                                         : (act[u] ? load_y(P.y, P.y_bf16, (n0 + u) * P.sn + (long)(tau - 1) * P.st + lab) : 0.f);
+                                         : (act[u] ? load_y(P.y, P.y_dtype, (n0 + u) * P.sn + (long)(tau - 1) * P.st + lab) : 0.f);
                         const float en = act[u] ? expf(yv - fm[u]) : 0.f;
                         if (k1) ec1[u] = en; else ec0[u] = en;
                     }
@@ -1435,33 +1435,33 @@ DenAuxLayout MakeDenAuxLayout(int S, int N, int T, bool small_ok) {
     return L;
 }
 
-int LaunchFrameMax(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *len, float *fmax,
+int LaunchFrameMax(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *len, float *fmax,
                    int Npad, cudaStream_t stream) {
     const long rows = (long)N * T;
     if (rows == 0) return 0;
     const int wpb = 8;
-    frame_max_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(y, y_bf16, sn, st, N, T, V, len, fmax, Npad);
+    frame_max_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(y, y_dtype, sn, st, N, T, V, len, fmax, Npad);
     CountLaunch();
     return (int)cudaGetLastError();
 }
 
-int LaunchFrameLse(const void *y, int y_bf16, long sn, long st, int N, int T, int V, const int *len, float *fmax,
+int LaunchFrameLse(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *len, float *fmax,
                    float *lz, double *lnorm, int Npad, cudaStream_t stream) {
     const long rows = (long)N * T;
     if (rows == 0) return 0;
     const int wpb = 8;
-    frame_lse_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(y, y_bf16, sn, st, N, T, V, len, fmax, lz, Npad);
+    frame_lse_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(y, y_dtype, sn, st, N, T, V, len, fmax, lz, Npad);
     lnorm_kernel<<<N, 32, 0, stream>>>(lz, len, N, Npad, lnorm);
     CountLaunch(2);
     return (int)cudaGetLastError();
 }
 
-int LaunchLogitGrad(const void *z, int z_bf16, long sn, long st, int N, int T, int V, const int *len, const float *lz,
+int LaunchLogitGrad(const void *z, int z_dtype, long sn, long st, int N, int T, int V, const int *len, const float *lz,
                     int Npad, float *grad, long gsn, long gst, cudaStream_t stream) {
     const long rows = (long)N * T;
     if (rows == 0) return 0;
     const int wpb = 8;
-    logit_grad_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(z, z_bf16, sn, st, N, T, V, len, lz, Npad, grad, gsn, gst);
+    logit_grad_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(z, z_dtype, sn, st, N, T, V, len, lz, Npad, grad, gsn, gst);
     CountLaunch();
     return (int)cudaGetLastError();
 }

@@ -96,14 +96,15 @@ class CTC_CRF_LOSS(Module):
     def forward(self, logits, labels, lx, ly) -> torch.FloatTensor:
         """
         logits (torch.FloatTensor): size (N, T, V), log-probabilities, on GPU device.
-            (torch.bfloat16 is accepted too; accumulation is fp32 -- the reference asserts fp32.)
+            (torch.bfloat16 and torch.float16 are accepted too, read in place with fp32 arithmetic -- the reference asserts
+            fp32.  With from_logits=True this takes the fp16 output of an fp16 autocast encoder as is.)
         labels (torch.IntTensor)  : size (sum {Ui}, ) flattened without paddings, on CPU.
         lx (torch.IntTensor) : size (N, ), on CPU
         ly (torch.IntTensor) : size (N, ), on CPU
         """
         assert len(labels.size()) == 1
-        assert logits.dtype in (torch.float, torch.bfloat16), \
-            f"expect logits to be torch.float (or torch.bfloat16) object, instead: {logits.dtype}"
+        assert logits.dtype in (torch.float, torch.bfloat16, torch.float16), \
+            f"expect logits to be torch.float (or torch.bfloat16 / torch.float16) object, instead: {logits.dtype}"
         assert labels.dtype == torch.int, f"expect labels to be torch.int object, instead: {labels.dtype}"
         assert lx.dtype == torch.int, f"expect lx to be torch.int object, instead: {lx.dtype}"
         assert ly.dtype == torch.int, f"expect ly to be torch.int object, instead: {ly.dtype}"

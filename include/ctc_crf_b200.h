@@ -89,8 +89,13 @@ ctcStatus_t get_workspace_size(const int *const label_lengths, const int *const 
 /* ------------------------------------------------------------------------------------------------
  * Section 2 -- fused entry and helpers (additions)
  * ---------------------------------------------------------------------------------------------- */
+/* Logits dtype codes, the `dtype` argument of every section-2 entry that takes one: the (N,T,V) block is read in this type
+ * and converted to fp32 element by element; the arithmetic and every output (loss, parts, gradient, score) stay fp32.  fp16
+ * is what CAT's `--amp` encoder returns (torch.cuda.amp autocast); bf16 what a bf16 autocast returns.  Any other code fails
+ * with a message.  Section 1 takes fp32 only, as the reference does. */
 #define CCB_DTYPE_F32 0
 #define CCB_DTYPE_BF16 1
+#define CCB_DTYPE_F16 2
 
 const char *ccb_last_error(void);            /* thread-local message of the last failure ("" if none) */
 int ccb_den_loaded(int device);              /* 1 if Init() covered this device */

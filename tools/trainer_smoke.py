@@ -11,6 +11,12 @@ are restated here in behaviour, each with its source line:
   * the unified trainer's SECOND criterion call on the same batch inside one step (cat/ctc/train_unified.py:248,267);
   * the step: ``autocast(enabled=use_amp)`` around the model, ``loss.data = loss.detach() * (local_bs * world / global_bs)``
     then ``backward()`` (cat/shared/manager.py:524-547);
+  * CAT's mixed precision, with ``--amp --amp-dtype float16``: fp16, not bf16.  The manager imports ``autocast, GradScaler``
+    from ``torch.cuda.amp`` (manager.py:29) and builds ``GradScaler(enabled=args.amp)`` (:280); ``autocast(enabled=use_amp)``
+    (:533) is fp16 by default, so the encoder's last Linear returns fp16 logits; the step is ``scaler.scale(loss).backward()``
+    (:547), then ``scaler.unscale_(optimizer)``, ``clip_grad_norm_(..., grad_norm)`` (default 2.0, coreutils.py:277-280),
+    ``scaler.step(optimizer)``, ``scaler.update()`` (:620-627).  ``--amp`` alone keeps a bf16 autocast and a plain
+    ``backward()`` + ``step()``;
   * process spawning: one process per GPU with ``mp.spawn``, ``torch.cuda.set_device(gpu)``, ``init_process_group('nccl')``,
     DistributedDataParallel (cat/shared/coreutils.py:493-504, cat/ctc/train.py:45-56,352).
 
@@ -21,6 +27,7 @@ small random phone LM composed natively (cat_b200.fst.compose_ctc_lm).
     python tools/trainer_smoke.py --steps 30                    # 1 GPU
     python tools/trainer_smoke.py --steps 30 --gpus 8           # DDP x 8 (mp.spawn, NCCL)
     python tools/trainer_smoke.py --steps 30 --from-logits      # CTC_CRF_LOSS(from_logits=True): raw encoder outputs in
+    python tools/trainer_smoke.py --steps 30 --from-logits --amp --amp-dtype float16   # CAT's --amp: fp16 logits, GradScaler
 """
 from __future__ import annotations
 
@@ -86,7 +93,7 @@ class AMTrainer(nn.Module):
         if self._crf_ctx is None:                              # lazy init, train.py:180-182
             self.register_crf_ctx(self.den_lm)
         with autocast("cuda", enabled=False):                  # train.py:184
-            # the reference passes logits.float(); the raw-logit entry takes the encoder's own dtype (bf16 under AMP)
+            # the reference passes logits.float(); the raw-logit entry takes the encoder's own dtype (bf16 or fp16 under AMP)
             loss = self.criterion(logits if self.from_logits else logits.float(),
                                   labels.to(torch.int), lx.to(torch.int), ly.to(torch.int))
         if self.unified:                                       # train_unified.py:248-273: a second pass over the same batch
@@ -139,19 +146,29 @@ def train(gpu: int, world: int, args, den_lm: str, log: List[float]) -> None:
     model = AMTrainer(TinyEncoder(), den_lm, lamb=0.01, from_logits=args.from_logits, unified=not args.no_unified).cuda(gpu)
     net = nn.parallel.DistributedDataParallel(model, device_ids=[gpu]) if world > 1 else model   # train.py:352
     opt = torch.optim.Adam(net.parameters(), lr=5e-3)
+    amp_dtype = getattr(torch, args.amp_dtype)
+    cat_amp = args.amp and amp_dtype == torch.float16          # CAT's fp16 step with its GradScaler (manager.py:29,280)
+    scaler = torch.amp.GradScaler("cuda", enabled=cat_amp)
     rng = np.random.default_rng(100 + gpu)
     emb = np.random.default_rng(7).standard_normal((V, FEAT)).astype(np.float32)
     local_bs, global_bs = args.batch, args.batch * world
     for step in range(args.steps):
         feats, lx, labels, ly = make_batch(rng, emb, local_bs)
         feats = feats.cuda(gpu, non_blocking=True)
-        with autocast("cuda", dtype=torch.bfloat16, enabled=args.amp):      # manager.py:533
+        with autocast("cuda", dtype=amp_dtype, enabled=args.amp):            # manager.py:533
             loss = net(feats, lx, labels, ly)
         raw = loss.detach().clone()
         loss.data = loss.detach() * (feats.size(0) * world / global_bs)       # manager.py:546
         opt.zero_grad(set_to_none=True)
-        loss.backward()
-        opt.step()
+        if cat_amp:
+            scaler.scale(loss).backward()                                     # manager.py:547
+            scaler.unscale_(opt)                                              # manager.py:620-627
+            torch.nn.utils.clip_grad_norm_(net.parameters(), args.grad_norm, error_if_nonfinite=False)
+            scaler.step(opt)
+            scaler.update()
+        else:
+            loss.backward()
+            opt.step()
         if world > 1:
             dist.all_reduce(raw)
             raw /= world
@@ -184,7 +201,7 @@ def run(args) -> List[float]:
         mp.spawn(_worker, nprocs=args.gpus, args=(args.gpus, args, den_lm, out))   # coreutils.py:493-504
         log = list(np.load(out))
     first, last = float(np.mean(log[:5])), float(np.mean(log[-5:]))
-    print(f"[trainer_smoke] gpus={args.gpus} amp={args.amp} from_logits={args.from_logits} unified={not args.no_unified}: "
+    print(f"[trainer_smoke] gpus={args.gpus} amp={args.amp and args.amp_dtype} from_logits={args.from_logits} unified={not args.no_unified}: "
           f"loss {first:.4f} -> {last:.4f} over {len(log)} steps")
     if not last < first - 0.1 * abs(first):
         raise SystemExit(f"loss did not decrease: {first} -> {last}")
@@ -197,7 +214,10 @@ def parse(argv=None):
     ap.add_argument("--batch", type=int, default=16)
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--port", type=int, default=29531)
-    ap.add_argument("--amp", action="store_true", help="bf16 autocast around the model (the loss stays under autocast(enabled=False))")
+    ap.add_argument("--amp", action="store_true", help="autocast around the model (the loss stays under autocast(enabled=False))")
+    ap.add_argument("--amp-dtype", default="bfloat16", choices=["bfloat16", "float16"],
+                    help="autocast dtype of --amp; float16 is CAT's (torch.cuda.amp), with its GradScaler step")
+    ap.add_argument("--grad-norm", type=float, default=2.0, help="gradient clipping of the float16 step (CAT's default)")
     ap.add_argument("--from-logits", action="store_true")
     ap.add_argument("--no-unified", action="store_true", help="one criterion call per step instead of two")
     return ap.parse_args(argv)
