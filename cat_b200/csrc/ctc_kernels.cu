@@ -381,8 +381,19 @@ int LaunchCtcAlphaBeta(const void *y, int y_dtype, long sn, long st, int N, int 
     const int ScMax = 2 * max_label_len + 1;
     int threads = ((max_label_len + 1 + 31) / 32) * 32;
     threads = threads < 64 ? 64 : (threads > 1024 ? 1024 : threads);
-    const size_t smem = (size_t)2 * ScMax * 8 + (size_t)(max_label_len + 1) * 4 + (size_t)2 * V * 4 + 16;
-    if (smem > 200 * 1024 || (size_t)V * 4 > 200 * 1024) { *err = "label sequence too long for the numerator kernel's shared memory"; return 1; }
+    // two emission rows of V floats are staged in shared memory, so V bounds the vocabulary: at most 25 505 classes with
+    // label sequences of up to 20 (the lattice rows take 16 * (2 Lmax + 1) + 4 * (Lmax + 1) + 16 bytes of the 200 KB)
+    constexpr size_t kSmemLimit = 200 * 1024;
+    const size_t lattice = (size_t)2 * ScMax * 8 + (size_t)(max_label_len + 1) * 4 + 16;
+    const size_t smem = lattice + (size_t)2 * V * 4;
+    if (smem > kSmemLimit) {
+        const long v_max = lattice < kSmemLimit ? (long)((kSmemLimit - lattice) / 8) : 0;
+        *err = "numerator kernel: V = " + std::to_string(V) + " classes with label sequences of up to " +
+               std::to_string(max_label_len) + " need " + std::to_string(smem) + " bytes of shared memory (two emission rows " +
+               "of V floats plus the lattice), above its limit of " + std::to_string(kSmemLimit) + " bytes; at this label " +
+               "length V may be at most " + std::to_string(v_max);
+        return 1;
+    }
     const bool spill = alpha_ws != nullptr;
     const void *kernel = spill ? (const void *)ctc_alpha_beta_kernel<true> : (const void *)ctc_alpha_beta_kernel<false>;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -30,12 +30,21 @@ class Plan:
         self.L.ccb_plan_destroy(self.h)
 
 
+# Large-vocabulary T-compose-LM graphs: few states per label, so a CTA's tile spans many labels and the backward label
+# accumulator ([labels][Npad] floats, at most 64 KB) stops fitting at some batch width
+WIDE_LABEL_GRAPHS = {"G4k": (3000, 8, 4000), "G20k": (6000, 8, 20000)}
+
+
 @pytest.fixture(scope="module")
 def plans(tmp_graphs, fixture_fst, tmp_path_factory):
     paths = {"fixture": fixture_fst, **{k: v[0] for k, v in tmp_graphs.items()}}
-    big = str(tmp_path_factory.mktemp("launch") / "big.fst")
+    d = tmp_path_factory.mktemp("launch")
+    big = str(d / "big.fst")
     fst.write_fst(big, fst.make_synthetic_den(4000, 24, 60, seed=7))
     paths["synthetic_4000"] = big
+    for name, (H, deg, V) in WIDE_LABEL_GRAPHS.items():
+        paths[name] = str(d / f"{name}.fst")
+        fst.write_fst(paths[name], fst.make_synthetic_den(H, deg, V, seed=7))
     out = {k: Plan(p) for k, p in paths.items()}
     yield out
     for p in out.values():
@@ -82,3 +91,24 @@ def test_tiers_the_fallback_tests_run(plans):
         L = p.launch(64, backward)
         assert (L["tier"], L["U"], L["w1_smem"]) == (TIER_SHARED, 2, int(backward))
     assert p.launch(130, False)["U"] == 4 and p.launch(130, True)["U"] == 2
+
+
+def test_label_accumulator_by_batch_width(plans):
+    """Where the backward pass keeps its per-label occupancy sums in shared memory and where it adds them straight into the
+    gradient with global atomics (gacc_rows = 0), at 132 CTAs.  The accumulator holds the CTA tile's label range for every
+    lane, so its rows are fixed by the graph and it drops out once rows x Npad x 4 bytes pass 64 KB.
+    tests/test_gpu_regimes.py runs both sides of the line on these graphs."""
+    widths = {16: (1, 16), 32: (17, 32), 64: (33, 64), 128: (65, 128), 256: (129, 256), 384: (257, 384), 512: (385, 512)}
+    want = {"tlm_mid": {w: 3 for w in widths},                                        # phone-shaped: 3 labels per tile
+            "G4k": {**{w: 50 for w in (16, 32, 64, 128, 256)}, 384: 0, 512: 0},       # 50 x 384 x 4 B > 64 KB
+            "G20k": {**{w: 213 for w in (16, 32, 64)}, 128: 0, 256: 0, 384: 0, 512: 0}}
+    for name, rows in want.items():
+        p = plans[name]
+        for Npad, (n_lo, n_hi) in widths.items():
+            for N in (n_lo, n_hi):
+                L = p.launch(N, True)
+                assert (L["Npad"], L["gacc_rows"]) == (Npad, rows[Npad]), (name, N, L)
+                assert L["gacc_rows"] * Npad * 4 <= 64 * 1024
+                assert p.launch(N, False)["gacc_rows"] == 0                           # the forward pass has none
+        # the two wide graphs walk 4 and 2 utterances per lane at every width from 128 on, accumulator or not
+        assert (p.launch(512, False)["U"], p.launch(512, True)["U"]) == (4, 2)
