@@ -8,7 +8,9 @@ installed (binding.cpp has none, SURVEY.md 8b) and native errors raise ``Runtime
 ignored (binding.cpp:105,111) or exiting the process (den_calculate.cu:16-25).
 
 Addition: ``ctc_crf_loss_fwd`` -- the fused, synchronisation-free entry used by ``CTC_CRF_LOSS``; ``ctc_crf_loss_fwd_only``
-and ``ctc_loss_fwd_only`` -- the losses without a gradient, used when grad mode is off.
+and ``ctc_loss_fwd_only`` -- the losses without a gradient, used when grad mode is off.  Every loss function takes
+``reduction`` (None: the scalar of ``size_average``; 'none': one cost per utterance) and ``zero_infinity``;
+``grad_rows_scale`` is the backward of the per-utterance costs.
 """
 from __future__ import annotations
 
@@ -24,6 +26,14 @@ from ._lib import ctcOptions
 # logits dtype -> CCB_DTYPE_* code (include/ctc_crf_b200.h).  The fused entries read the logits in place in this type and
 # compute in fp32; gpu_den / gpu_ctc keep the reference's fp32 contract.
 _DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+
+
+def check_reduction(reduction) -> None:
+    """reduction None keeps the scalar loss of ``size_average`` (the sum, or the mean over the batch); 'none' returns the
+    (N,) costs.  There is no second spelling of the sum or the mean."""
+    if reduction is not None and reduction != "none":
+        raise ValueError(f"reduction must be None or 'none', not {reduction!r}: for the batch sum or mean leave it None and "
+                         f"choose with size_average (False: sum, True: mean over the batch)")
 
 
 def _check(rc: int, what: str) -> None:
@@ -264,13 +274,21 @@ def _plan_slices(L, lx, ly, N, V, dev):
 
 
 def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
-                     lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False
+                     lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False,
+                     reduction: Optional[str] = None, zero_infinity: bool = False
                      ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
     """Fused CTC-CRF loss.  logits (N,T,V) fp32, bf16 or fp16 CUDA contiguous log-probs; labels/lx/ly int32 CPU.
     Returns (loss[1] fp32 CUDA, grad (N,T,V) fp32 CUDA, parts[2N] or None).  Never synchronises the host.
     Batches whose scratch does not fit the free memory (or > 512 utterances) are processed in slices.
     from_logits: `logits` are the RAW encoder outputs; log_softmax and its Jacobian are applied inside
-    (grad = d loss / d raw logits), replacing cat/ctc/train.py:173-174."""
+    (grad = d loss / d raw logits), replacing cat/ctc/train.py:173-174.
+    reduction 'none': the first result is costs (N,) fp32 CUDA, cost[n] = logZ_den[n] - (1+lamb) log p_ctc[n], and grad is
+    unscaled (grad[n] = d cost[n] / d logits[n]); size_average is then ignored.
+    zero_infinity: an utterance whose cost is not finite gets cost 0 and zero gradient rows (the divisor of size_average
+    stays N)."""
+    check_reduction(reduction)
+    per_utt = reduction == "none"
+    with_costs = per_utt or zero_infinity
     L = _lib.lib()
     entry = L.ccb_ctc_crf_loss_logits_fwd if from_logits else L.ccb_ctc_crf_loss_fwd
     ckpt_entry = L.ccb_ctc_crf_loss_logits_ckpt_fwd if from_logits else L.ccb_ctc_crf_loss_ckpt_fwd
@@ -280,13 +298,14 @@ def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tenso
     N, T, V = _check_batch_args(logits, labels, lx, ly)
     dev = logits.device
     esz = logits.element_size()
-    scale = 1.0 / N if size_average else 1.0
+    scale = 1.0 if per_utt else 1.0 / N if size_average else 1.0
     with torch.cuda.device(dev):
         meta, sum_l, _ = upload_meta(labels, lx, ly, dev)
         base = meta.data_ptr()
         p_labels, p_off = base, base + 4 * sum_l
         p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
         grad = torch.empty((N, T, V), dtype=torch.float32, device=dev)
+        costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
         parts = torch.empty(2 * N, dtype=torch.float32, device=dev) if want_parts else None
         stream = _stream(dev)
 
@@ -303,12 +322,16 @@ def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tenso
                 args = (p_labels, p_off + 4 * n0, p_ly + 4 * n0, p_lx + 4 * n0, maxl, float(lamb),
                         float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(), ctc_ws.data_ptr(),
                         grad.data_ptr() + n0 * T * V * 4, losses.data_ptr() + 4 * i,
-                        sub_parts.data_ptr() if want_parts else None, stream)
+                        sub_parts.data_ptr() if want_parts else None)
                 y_ptr = logits.data_ptr() + n0 * T * V * esz
-                if k:
-                    rc = ckpt_entry(y_ptr, _DTYPES[logits.dtype], n, T, V, tmax, k, *args)
+                if with_costs:      # each slice writes its own costs[n0:n1] in place
+                    rc = L.ccb_ctc_crf_loss_costs(y_ptr, _DTYPES[logits.dtype], int(from_logits), n, T, V, tmax, k, *args,
+                                                  costs.data_ptr() + 4 * n0 if per_utt else None, int(zero_infinity),
+                                                  stream)
+                elif k:
+                    rc = ckpt_entry(y_ptr, _DTYPES[logits.dtype], n, T, V, tmax, k, *args, stream)
                 else:
-                    rc = entry(y_ptr, _DTYPES[logits.dtype], n, T, V, tmax, *args)
+                    rc = entry(y_ptr, _DTYPES[logits.dtype], n, T, V, tmax, *args, stream)
                 _check(rc, "ctc_crf_loss_fwd")
                 if want_parts:
                     parts[n0:n1] = sub_parts[:n]
@@ -324,7 +347,7 @@ def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tenso
             slices, losses = run_slices()
         loss = losses.sum().reshape(1) if len(slices) > 1 else losses
         meta.record_stream(torch.cuda.current_stream(dev))
-    return loss, grad, parts
+    return (costs if per_utt else loss), grad, parts
 
 
 def _fwd_only_need(L, n, tmax):
@@ -353,23 +376,27 @@ def _plan_fwd_only_slices(L, lx, ly, N, dev):
 
 
 def ctc_crf_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
-                          lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False
+                          lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False,
+                          reduction: Optional[str] = None, zero_infinity: bool = False
                           ) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """The loss of ``ctc_crf_loss_fwd`` without its gradient, for evaluation: (loss[1] fp32 CUDA, parts[2N] or None).
     The den forward pass keeps alpha on a ring of frames, the numerator writes no cells, and no (N,T,V) buffer is
     allocated, so the scratch is a few frames of the den graph per slice whatever the lengths.  Never synchronises the
-    host.  Arguments as for ``ctc_crf_loss_fwd``."""
+    host.  Arguments as for ``ctc_crf_loss_fwd`` (reduction 'none': the first result is the (N,) costs)."""
+    check_reduction(reduction)
+    per_utt = reduction == "none"
     L = _lib.lib()
     N, T, V = _check_batch_args(logits, labels, lx, ly)
     dev = logits.device
     esz = logits.element_size()
-    scale = 1.0 / N if size_average else 1.0
+    scale = 1.0 if per_utt else 1.0 / N if size_average else 1.0
     with torch.cuda.device(dev):
         meta, sum_l, _ = upload_meta(labels, lx, ly, dev)
         base = meta.data_ptr()
         p_labels, p_off = base, base + 4 * sum_l
         p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
         parts = torch.empty(2 * N, dtype=torch.float32, device=dev) if want_parts else None
+        costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
         stream = _stream(dev)
         slices = _plan_fwd_only_slices(L, lx, ly, N, dev)
         losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
@@ -379,11 +406,15 @@ def ctc_crf_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.
             aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
             num_ws = torch.empty(int(L.ccb_num_fwd_only_bytes(n)), dtype=torch.uint8, device=dev)
             sub_parts = torch.empty(2 * n, dtype=torch.float32, device=dev) if want_parts else None
-            rc = L.ccb_ctc_crf_loss_fwd_only(logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype], int(from_logits),
-                                             n, T, V, tmax, p_labels, p_off + 4 * n0, p_ly + 4 * n0, p_lx + 4 * n0, maxl,
-                                             float(lamb), float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(),
-                                             num_ws.data_ptr(), losses.data_ptr() + 4 * i,
-                                             sub_parts.data_ptr() if want_parts else None, stream)
+            args = (logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype], int(from_logits),
+                    n, T, V, tmax, p_labels, p_off + 4 * n0, p_ly + 4 * n0, p_lx + 4 * n0, maxl,
+                    float(lamb), float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(),
+                    num_ws.data_ptr(), losses.data_ptr() + 4 * i, sub_parts.data_ptr() if want_parts else None)
+            if per_utt or zero_infinity:
+                rc = L.ccb_ctc_crf_loss_costs_fwd_only(*args, costs.data_ptr() + 4 * n0 if per_utt else None,
+                                                       int(zero_infinity), stream)
+            else:
+                rc = L.ccb_ctc_crf_loss_fwd_only(*args, stream)
             _check(rc, "ctc_crf_loss_fwd_only")
             if want_parts:
                 parts[n0:n1] = sub_parts[:n]
@@ -391,7 +422,7 @@ def ctc_crf_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.
             del alpha_ws, aux_ws, num_ws      # stream-ordered reuse by the caching allocator for the next slice
         loss = losses.sum().reshape(1) if len(slices) > 1 else losses
         meta.record_stream(torch.cuda.current_stream(dev))
-    return loss, parts
+    return (costs if per_utt else loss), parts
 
 
 def _check_batch_args(logits, labels, lx, ly):
@@ -413,14 +444,19 @@ def _check_batch_args(logits, labels, lx, ly):
 
 
 def ctc_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
-                 size_average: bool, blank: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                 size_average: bool, blank: int = 0, reduction: Optional[str] = None, zero_infinity: bool = False
+                 ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """CTC-only loss on the (N,T,V) log-probs in place (the native counterpart of ``_WARP_CTC_GPU``,
     ctc_crf/__init__.py:25-56): no (T,N,V) transpose copy, no zero fill, no host round trip for the costs.
-    Returns (loss[1], grad (N,T,V) fp32 = d loss / d logits, logp[N]) on the device; never synchronises the host."""
+    Returns (loss[1], grad (N,T,V) fp32 = d loss / d logits, logp[N]) on the device; never synchronises the host.
+    reduction 'none': the first result is costs (N,), cost[n] = -log p[n], and grad is unscaled; zero_infinity: a cost
+    that is not finite becomes 0 and its gradient rows zeros (as in ``ctc_crf_loss_fwd``)."""
+    check_reduction(reduction)
+    per_utt = reduction == "none"
     L = _lib.lib()
     N, T, V = _check_batch_args(logits, labels, lx, ly)
     dev = logits.device
-    scale = 1.0 / N if size_average else 1.0
+    scale = 1.0 if per_utt else 1.0 / N if size_average else 1.0
     with torch.cuda.device(dev):
         meta, sum_l, maxl = upload_meta(labels, lx, ly, dev)
         base = meta.data_ptr()
@@ -431,22 +467,30 @@ def ctc_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, l
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         logp = torch.empty(N, dtype=torch.float32, device=dev)
         ws = torch.empty(int(L.ccb_ctc_workspace_bytes(N, tmax, maxl)), dtype=torch.uint8, device=dev)
-        rc = L.ccb_ctc_loss_fwd(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx, maxl,
-                                int(blank), float(scale), ws.data_ptr(), grad.data_ptr(), loss.data_ptr(), logp.data_ptr(),
-                                _stream(dev))
+        args = (logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx, maxl,
+                int(blank), float(scale), ws.data_ptr(), grad.data_ptr(), loss.data_ptr(), logp.data_ptr())
+        if per_utt or zero_infinity:
+            costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
+            rc = L.ccb_ctc_loss_costs(*args, costs.data_ptr() if per_utt else None, int(zero_infinity), _stream(dev))
+        else:
+            rc = L.ccb_ctc_loss_fwd(*args, _stream(dev))
         _check(rc, "ctc_loss_fwd")
         meta.record_stream(torch.cuda.current_stream(dev))
-    return loss, grad, logp
+    return (costs if per_utt else loss), grad, logp
 
 
 def ctc_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
-                      size_average: bool, blank: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+                      size_average: bool, blank: int = 0, reduction: Optional[str] = None, zero_infinity: bool = False
+                      ) -> Tuple[torch.Tensor, torch.Tensor]:
     """The loss of ``ctc_loss_fwd`` without its gradient: (loss[1], logp[N]) on the device, the same values, from one alpha
-    chain per utterance that writes no cells.  No workspace, no (N,T,V) buffer, no host synchronisation."""
+    chain per utterance that writes no cells.  No workspace, no (N,T,V) buffer, no host synchronisation.
+    reduction and zero_infinity as for ``ctc_loss_fwd``."""
+    check_reduction(reduction)
+    per_utt = reduction == "none"
     L = _lib.lib()
     N, T, V = _check_batch_args(logits, labels, lx, ly)
     dev = logits.device
-    scale = 1.0 / N if size_average else 1.0
+    scale = 1.0 if per_utt else 1.0 / N if size_average else 1.0
     with torch.cuda.device(dev):
         meta, sum_l, maxl = upload_meta(labels, lx, ly, dev)
         base = meta.data_ptr()
@@ -455,11 +499,17 @@ def ctc_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tens
         tmax = max(1, int(lx.max()))
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         logp = torch.empty(N, dtype=torch.float32, device=dev)
-        rc = L.ccb_ctc_loss_fwd_only(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx,
-                                     maxl, int(blank), float(scale), loss.data_ptr(), logp.data_ptr(), _stream(dev))
+        if per_utt or zero_infinity:
+            costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
+            rc = L.ccb_ctc_loss_costs(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx,
+                                      maxl, int(blank), float(scale), None, None, loss.data_ptr(), logp.data_ptr(),
+                                      costs.data_ptr() if per_utt else None, int(zero_infinity), _stream(dev))
+        else:
+            rc = L.ccb_ctc_loss_fwd_only(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx,
+                                         maxl, int(blank), float(scale), loss.data_ptr(), logp.data_ptr(), _stream(dev))
         _check(rc, "ctc_loss_fwd_only")
         meta.record_stream(torch.cuda.current_stream(dev))
-    return loss, logp
+    return (costs if per_utt else loss), logp
 
 
 def ctc_align(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, blank: int = 0
@@ -483,6 +533,27 @@ def ctc_align(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: 
         _check(rc, "ctc_align")
         meta.record_stream(torch.cuda.current_stream(dev))
     return align, score
+
+
+def grad_rows_scale(grad: torch.Tensor, w: torch.Tensor, lx: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """Backward of the per-utterance costs: out[n] = w[n] * grad[n] in `dtype` (fp32, bf16 or fp16), rows t >= lx[n] zero,
+    in one pass over the (N,T,V) fp32 `grad` of a loss function called with reduction 'none'.  w: (N,) the gradient with
+    respect to each cost; lx: the int32 CPU input lengths of the forward call (uploaded asynchronously)."""
+    L = _lib.lib()
+    assert grad.is_cuda and grad.dtype == torch.float32 and grad.dim() == 3 and grad.is_contiguous()
+    if dtype not in _DTYPES:
+        raise RuntimeError(f"unsupported gradient dtype {dtype}")
+    N, T, V = grad.shape
+    dev = grad.device
+    with torch.cuda.device(dev):
+        w = w.to(device=dev, dtype=torch.float32).reshape(N).contiguous()
+        lens = _rings.setdefault(torch.device(dev).index, _PinnedRing()).stage([lx.to(torch.int32)], dev)
+        out = torch.empty((N, T, V), dtype=dtype, device=dev)
+        rc = L.ccb_grad_rows_scale(grad.data_ptr(), w.data_ptr(), lens.data_ptr(), N, T, V, out.data_ptr(), _DTYPES[dtype],
+                                   _stream(dev))
+        _check(rc, "grad_rows_scale")
+        lens.record_stream(torch.cuda.current_stream(dev))
+    return out
 
 
 def launch_count() -> int:

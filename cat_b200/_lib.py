@@ -27,6 +27,7 @@ SYMBOLS = [
     "ccb_plan_launch",
     "ccb_den_ckpt_alpha_floats", "ccb_ctc_crf_loss_ckpt_fwd", "ccb_ctc_crf_loss_logits_ckpt_fwd",
     "ccb_den_fwd_alpha_floats", "ccb_num_fwd_only_bytes", "ccb_ctc_crf_loss_fwd_only", "ccb_ctc_loss_fwd_only",
+    "ccb_ctc_crf_loss_costs", "ccb_ctc_crf_loss_costs_fwd_only", "ccb_ctc_loss_costs", "ccb_grad_rows_scale",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -86,6 +87,17 @@ def lib() -> C.CDLL:
     L.ccb_ctc_loss_fwd_only.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,
                                         C.c_float, vp, vp, vp]
     L.ccb_ctc_loss_fwd_only.restype = C.c_int
+    L.ccb_ctc_crf_loss_costs.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp,
+                                         C.c_int, C.c_float, C.c_float, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp]
+    L.ccb_ctc_crf_loss_costs.restype = C.c_int
+    L.ccb_ctc_crf_loss_costs_fwd_only.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp,
+                                                  C.c_int, C.c_float, C.c_float, vp, vp, vp, vp, vp, vp, C.c_int, vp]
+    L.ccb_ctc_crf_loss_costs_fwd_only.restype = C.c_int
+    L.ccb_ctc_loss_costs.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,
+                                     C.c_float, vp, vp, vp, vp, vp, C.c_int, vp]
+    L.ccb_ctc_loss_costs.restype = C.c_int
+    L.ccb_grad_rows_scale.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp]
+    L.ccb_grad_rows_scale.restype = C.c_int
     L.ccb_ctc_align_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
     L.ccb_ctc_align_workspace_bytes.restype = C.c_size_t
     L.ccb_ctc_align.argtypes = [vp, C.c_int, C.c_long, C.c_long, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,

@@ -506,25 +506,56 @@ int ccb_ctc_forward_backward(const void *logits, int dtype, long sn, long st, in
 }
 
 /* CTC-only loss (WARP_CTC_LOSS, ctc_crf/__init__.py:25-56) on the (N,T,V) block in place: one numerator pass, the gradient
- * rows all written by the occupancy kernel (no zero fill), the scalar assembled on the device (no host round trip). */
-int ccb_ctc_loss_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax,
-                     const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
-                     int max_label_len, int blank, float scale, void *ctc_ws, float *grad, float *loss, float *logp,
-                     void *stream) {
+ * rows all written by the occupancy kernel (no zero fill), the scalar assembled on the device (no host round trip).
+ * grad = null: the forward-only loss (one alpha chain per utterance, no cells written, ctc_ws unused). */
+static int CtcLossImpl(const char *what, const void *logits, int dtype, int N, int T, int V, int Tmax,
+                       const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                       int max_label_len, int blank, float scale, void *ctc_ws, float *grad, float *loss, float *logp,
+                       float *costs, int zero_inf, void *stream) {
     g_err.clear();
-    if (N <= 0 || T <= 0 || V <= 0 || !logits || !ctc_ws || !grad || !loss || !logp) return Fail("ctc_loss_fwd: bad arguments");
-    if (Tmax <= 0 || Tmax > T) return Fail("ctc_loss_fwd: Tmax must lie in [1, T]");
-    if (!KnownDtype(dtype)) return FailDtype("ctc_loss_fwd", dtype);
+    if (N <= 0 || T <= 0 || V <= 0 || !logits || (grad && !ctc_ws) || !loss || !logp)
+        return Fail(std::string(what) + ": bad arguments");
+    if (Tmax <= 0 || Tmax > T) return Fail(std::string(what) + ": Tmax must lie in [1, T]");
+    if (!KnownDtype(dtype)) return FailDtype(what, dtype);
     if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
     cudaStream_t s = (cudaStream_t)stream;
     const long sn = (long)T * V, st = V;
     std::string err;
-    int rc = LaunchCtc(logits, dtype, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
-                       max_label_len, blank, reinterpret_cast<float *>(ctc_ws), grad, sn, st, -scale, logp, nullptr, s, &err,
-                       /*overwrite=*/1, /*Tfull=*/T);
+    int rc = grad ? LaunchCtc(logits, dtype, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+                              max_label_len, blank, reinterpret_cast<float *>(ctc_ws), grad, sn, st, -scale, logp, nullptr, s,
+                              &err, /*overwrite=*/1, /*Tfull=*/T, /*logz=*/nullptr, zero_inf)
+                  : LaunchCtcLogp(logits, dtype, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+                                  max_label_len, blank, logp, nullptr, s, &err);
     if (rc) return Fail(err);
-    rc = LaunchSumScale(logp, N, -scale, loss, s);
+    rc = LaunchSumScale(logp, N, scale, loss, s, costs, zero_inf);
     if (rc) return FailCuda("sum_scale", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_ctc_loss_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax,
+                     const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                     int max_label_len, int blank, float scale, void *ctc_ws, float *grad, float *loss, float *logp,
+                     void *stream) {
+    if (!grad) return Fail("ctc_loss_fwd: bad arguments");
+    return CtcLossImpl("ctc_loss_fwd", logits, dtype, N, T, V, Tmax, labels_dev, label_off_dev, label_len_dev, len_dev,
+                       max_label_len, blank, scale, ctc_ws, grad, loss, logp, nullptr, 0, stream);
+}
+
+int ccb_ctc_loss_costs(const void *logits, int dtype, int N, int T, int V, int Tmax,
+                       const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                       int max_label_len, int blank, float scale, void *ctc_ws, float *grad, float *loss, float *logp,
+                       float *costs, int zero_inf, void *stream) {
+    return CtcLossImpl("ctc_loss_costs", logits, dtype, N, T, V, Tmax, labels_dev, label_off_dev, label_len_dev, len_dev,
+                       max_label_len, blank, scale, ctc_ws, grad, loss, logp, costs, zero_inf, stream);
+}
+
+int ccb_grad_rows_scale(const float *grad, const float *w, const int *len_dev, int N, int T, int V, void *out, int out_dtype,
+                        void *stream) {
+    g_err.clear();
+    if (N <= 0 || T <= 0 || V <= 0 || !grad || !w || !len_dev || !out) return Fail("grad_rows_scale: bad arguments");
+    if (!KnownDtype(out_dtype)) return FailDtype("grad_rows_scale", out_dtype);
+    int rc = LaunchGradRowsScale(grad, w, len_dev, N, T, V, out, out_dtype, (cudaStream_t)stream);
+    if (rc) return FailCuda("grad_rows_scale", (cudaError_t)rc);
     return 0;
 }
 
@@ -550,7 +581,7 @@ static int LossFwdImpl(bool raw, const void *logits, int dtype, int N, int T, in
                        const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
                        const int *len_dev, int max_label_len, float lamb, float scale,
                        float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
-                       void *stream) {
+                       float *costs, int zero_inf, void *stream) {
     g_err.clear();
     DeviceGraph *g;
     if (CurrentGraph(&g)) return 1;
@@ -570,17 +601,19 @@ static int LossFwdImpl(bool raw, const void *logits, int dtype, int N, int T, in
     CCB_CUDA(cudaMemsetAsync(grad, 0, sizeof(float) * (size_t)N * T * V, s));
     if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw, ckpt_k)) return 1;
     if (DenBackward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, grad, sn, st, scale, s, raw, ckpt_k)) return 1;
-    // the numerator accumulates into the gradient after the den passes have normalised their part of it
+    // the numerator accumulates into the gradient after the den passes have normalised their part of it (with zero_inf it
+    // overwrites the rows of an utterance whose logZ or log p is not finite with zeros instead)
     std::string err;
     int rc = LaunchCtc(logits, dtype, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev,
-                       max_label_len, 0, reinterpret_cast<float *>(ctc_ws), grad, sn, st, -(1.f + lamb) * scale, logp, lnorm, s, &err);
+                       max_label_len, 0, reinterpret_cast<float *>(ctc_ws), grad, sn, st, -(1.f + lamb) * scale, logp, lnorm, s, &err,
+                       /*overwrite=*/0, /*Tfull=*/0, logz, zero_inf);
     if (rc) return Fail(err);
-    if (raw) {   // chain through log_softmax: dL/dz = g - softmax(z) * sum_k g_k
+    if (raw) {   // chain through log_softmax: dL/dz = g - softmax(z) * sum_k g_k (a zero row stays zero)
         rc = LaunchLogitGrad(logits, dtype, sn, st, N, Tmax, V, len_dev,
                              reinterpret_cast<const float *>((char *)aux_ws + L.lz), L.Npad, grad, sn, st, s);
         if (rc) return FailCuda("logit_grad", (cudaError_t)rc);
     }
-    rc = LaunchAssembleLoss(logz, logp, N, lamb, scale, loss, s);
+    rc = LaunchAssembleLoss(logz, logp, N, lamb, scale, loss, s, costs, zero_inf);
     if (rc) return FailCuda("assemble_loss", (cudaError_t)rc);
     if (parts) {
         CCB_CUDA(cudaMemcpyAsync(parts, logz, sizeof(float) * N, cudaMemcpyDeviceToDevice, s));
@@ -595,7 +628,7 @@ int ccb_ctc_crf_loss_fwd(const void *logits, int dtype, int N, int T, int V, int
                          float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
                          void *stream) {
     return LossFwdImpl(false, logits, dtype, N, T, V, Tmax, 0, labels_dev, label_off_dev, label_len_dev, len_dev, max_label_len,
-                       lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
+                       lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, nullptr, 0, stream);
 }
 
 int ccb_ctc_crf_loss_logits_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax,
@@ -604,7 +637,7 @@ int ccb_ctc_crf_loss_logits_fwd(const void *logits, int dtype, int N, int T, int
                                 float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
                                 void *stream) {
     return LossFwdImpl(true, logits, dtype, N, T, V, Tmax, 0, labels_dev, label_off_dev, label_len_dev, len_dev, max_label_len,
-                       lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
+                       lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, nullptr, 0, stream);
 }
 
 int ccb_ctc_crf_loss_ckpt_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k,
@@ -613,7 +646,7 @@ int ccb_ctc_crf_loss_ckpt_fwd(const void *logits, int dtype, int N, int T, int V
                               float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
                               void *stream) {
     return LossFwdImpl(false, logits, dtype, N, T, V, Tmax, ckpt_k, labels_dev, label_off_dev, label_len_dev, len_dev,
-                       max_label_len, lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
+                       max_label_len, lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, nullptr, 0, stream);
 }
 
 int ccb_ctc_crf_loss_logits_ckpt_fwd(const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k,
@@ -622,7 +655,7 @@ int ccb_ctc_crf_loss_logits_ckpt_fwd(const void *logits, int dtype, int N, int T
                                      float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
                                      void *stream) {
     return LossFwdImpl(true, logits, dtype, N, T, V, Tmax, ckpt_k, labels_dev, label_off_dev, label_len_dev, len_dev,
-                       max_label_len, lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, stream);
+                       max_label_len, lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, nullptr, 0, stream);
 }
 
 /* Forward-only CTC-CRF loss: the same loss (and parts) as LossFwdImpl without the gradient.  The den forward pass keeps
@@ -631,7 +664,8 @@ int ccb_ctc_crf_loss_logits_ckpt_fwd(const void *logits, int dtype, int N, int T
 static int LossFwdOnlyImpl(bool raw, const void *logits, int dtype, int N, int T, int V, int Tmax,
                            const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
                            const int *len_dev, int max_label_len, float lamb, float scale,
-                           float *alpha_ws, void *aux_ws, void *num_ws, float *loss, float *parts, void *stream) {
+                           float *alpha_ws, void *aux_ws, void *num_ws, float *loss, float *parts, float *costs,
+                           int zero_inf, void *stream) {
     g_err.clear();
     DeviceGraph *g;
     if (CurrentGraph(&g)) return 1;
@@ -649,7 +683,7 @@ static int LossFwdOnlyImpl(bool raw, const void *logits, int dtype, int N, int T
     int rc = LaunchCtcLogp(logits, dtype, sn, st, N, Tmax, V, labels_dev, label_off_dev, label_len_dev,
                            len_dev, max_label_len, 0, logp, lnorm, s, &err);
     if (rc) return Fail(err);
-    rc = LaunchAssembleLoss(logz, logp, N, lamb, scale, loss, s);
+    rc = LaunchAssembleLoss(logz, logp, N, lamb, scale, loss, s, costs, zero_inf);
     if (rc) return FailCuda("assemble_loss", (cudaError_t)rc);
     if (parts) {
         CCB_CUDA(cudaMemcpyAsync(parts, logz, sizeof(float) * N, cudaMemcpyDeviceToDevice, s));
@@ -663,25 +697,32 @@ int ccb_ctc_crf_loss_fwd_only(const void *logits, int dtype, int from_logits, in
                               const int *len_dev, int max_label_len, float lamb, float scale,
                               float *alpha_ws, void *aux_ws, void *num_ws, float *loss, float *parts, void *stream) {
     return LossFwdOnlyImpl(from_logits != 0, logits, dtype, N, T, V, Tmax, labels_dev, label_off_dev, label_len_dev, len_dev,
-                           max_label_len, lamb, scale, alpha_ws, aux_ws, num_ws, loss, parts, stream);
+                           max_label_len, lamb, scale, alpha_ws, aux_ws, num_ws, loss, parts, nullptr, 0, stream);
+}
+
+int ccb_ctc_crf_loss_costs(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax, int ckpt_k,
+                           const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                           const int *len_dev, int max_label_len, float lamb, float scale,
+                           float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss, float *parts,
+                           float *costs, int zero_inf, void *stream) {
+    return LossFwdImpl(from_logits != 0, logits, dtype, N, T, V, Tmax, ckpt_k, labels_dev, label_off_dev, label_len_dev, len_dev,
+                       max_label_len, lamb, scale, alpha_ws, aux_ws, ctc_ws, grad, loss, parts, costs, zero_inf, stream);
+}
+
+int ccb_ctc_crf_loss_costs_fwd_only(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax,
+                                    const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                                    const int *len_dev, int max_label_len, float lamb, float scale,
+                                    float *alpha_ws, void *aux_ws, void *num_ws, float *loss, float *parts,
+                                    float *costs, int zero_inf, void *stream) {
+    return LossFwdOnlyImpl(from_logits != 0, logits, dtype, N, T, V, Tmax, labels_dev, label_off_dev, label_len_dev, len_dev,
+                           max_label_len, lamb, scale, alpha_ws, aux_ws, num_ws, loss, parts, costs, zero_inf, stream);
 }
 
 int ccb_ctc_loss_fwd_only(const void *logits, int dtype, int N, int T, int V, int Tmax,
                           const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
                           int max_label_len, int blank, float scale, float *loss, float *logp, void *stream) {
-    g_err.clear();
-    if (N <= 0 || T <= 0 || V <= 0 || !logits || !loss || !logp) return Fail("ctc_loss_fwd_only: bad arguments");
-    if (Tmax <= 0 || Tmax > T) return Fail("ctc_loss_fwd_only: Tmax must lie in [1, T]");
-    if (!KnownDtype(dtype)) return FailDtype("ctc_loss_fwd_only", dtype);
-    if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
-    cudaStream_t s = (cudaStream_t)stream;
-    std::string err;
-    int rc = LaunchCtcLogp(logits, dtype, (long)T * V, V, N, Tmax, V, labels_dev, label_off_dev, label_len_dev,
-                           len_dev, max_label_len, blank, logp, nullptr, s, &err);
-    if (rc) return Fail(err);
-    rc = LaunchSumScale(logp, N, -scale, loss, s);
-    if (rc) return FailCuda("sum_scale", (cudaError_t)rc);
-    return 0;
+    return CtcLossImpl("ctc_loss_fwd_only", logits, dtype, N, T, V, Tmax, labels_dev, label_off_dev, label_len_dev, len_dev,
+                       max_label_len, blank, scale, nullptr, nullptr, loss, logp, nullptr, 0, stream);
 }
 
 /* ---- gpu_ctc/ctc.h surface ------------------------------------------------------------------- */

@@ -157,21 +157,30 @@ inline int CkptCount(int T, int K) { const int k = CkptK(T, K); return (T + k - 
 int LaunchDen(bool backward, const DeviceGraph &g, DenParams &p, cudaStream_t stream, std::string *err);
 int LaunchDenGradNormalize(float *grad, long gsn, long gst, const float *absum, const int *len, int N, int Npad,
                            int T, int V, float scale, cudaStream_t stream);
+// zero_inf: an utterance whose cost is not finite (log p, or logz[n] when logz is given, not finite) gets zero gradient rows
+// t < len[n] -- written over whatever the den passes left there -- instead of its occupancies
 int LaunchCtc(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
               const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
               float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, float *logp,
-              const double *lnorm, cudaStream_t stream, std::string *err, int overwrite = 0, int Tfull = 0);
+              const double *lnorm, cudaStream_t stream, std::string *err, int overwrite = 0, int Tfull = 0,
+              const float *logz = nullptr, int zero_inf = 0);
 // forward-only numerator: logp[n] = log p(l_n | x_n) (normalised by lnorm[n] when given) from the alpha chains alone, one
 // CTA per utterance, no workspace; infeasible utterances get -inf
 int LaunchCtcLogp(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                   const int *label_off, const int *label_len, const int *len, int max_label_len, int blank, float *logp,
                   const double *lnorm, cudaStream_t stream, std::string *err);
-int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStream_t stream);
+// The loss assembly: cost[n] = -logp[n] (CTC) or logz[n] - (1+lamb) logp[n] (CTC-CRF), in fp64; loss[0] = scale * sum_n cost[n].
+// costs (N floats, may be null) receives every cost; zero_inf sets the costs that are not finite to 0 before both.
+int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStream_t stream, float *costs = nullptr,
+                   int zero_inf = 0);
 int LaunchCtcViterbi(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                      const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                      unsigned char *bp_ws, int *align, float *score, cudaStream_t stream, std::string *err);
 int LaunchAssembleLoss(const float *logz, const float *logp, int N, float lamb, float scale, float *loss,
-                       cudaStream_t stream);
+                       cudaStream_t stream, float *costs = nullptr, int zero_inf = 0);
+// out[n][t][:] = w[n] * grad[n][t][:] for t < len[n], 0 beyond (grad not read there); out in the CCB_DTYPE_* out_dtype
+int LaunchGradRowsScale(const float *grad, const float *w, const int *len, int N, int T, int V, void *out, int out_dtype,
+                        cudaStream_t stream);
 void CountLaunch(int n = 1);
 
 // ------------------------------------------------------------------------------------------------
@@ -184,6 +193,13 @@ __device__ __forceinline__ float load_y(const void *y, int dtype, long idx) {
     if (dtype == CCB_DTYPE_F32) return __ldg(reinterpret_cast<const float *>(y) + idx);
     const unsigned short h = reinterpret_cast<const unsigned short *>(y)[idx];
     return dtype == CCB_DTYPE_BF16 ? __bfloat162float(__ushort_as_bfloat16(h)) : __half2float(__ushort_as_half(h));
+}
+
+// The inverse of load_y: v stored as element idx of a buffer in the CCB_DTYPE_* code `dtype` (round to nearest even)
+__device__ __forceinline__ void store_y(void *out, int dtype, long idx, float v) {
+    if (dtype == CCB_DTYPE_F32) { reinterpret_cast<float *>(out)[idx] = v; return; }
+    reinterpret_cast<unsigned short *>(out)[idx] = dtype == CCB_DTYPE_BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(v))
+                                                                           : __half_as_ushort(__float2half_rn(v));
 }
 
 __device__ __forceinline__ void red_release_add_u32(unsigned *p, unsigned v) {

@@ -233,10 +233,14 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_dtype, long sn, long 
 // Occupancies from the two spills: one warp per (utterance, frame), label accumulator [V] per warp in shared memory.
 //   gamma_t[k] = sum_{s: l'_s = k} exp(alpha_t(s) + beta_t(s) - y_t(k) - log p)   (gpu_ctc_kernels.h:337-453)
 // accumulated with the caller's scale into grad[n][t][:] (which may already hold the denominator part).
+// zero_inf: this is the first launch after both halves of the loss, so it is where an utterance whose cost is not finite
+// (log p, or logz[n] when the den part is given, not finite) is masked: its rows t < len[n] are written with zeros, den
+// part included, instead of accumulated.
 __global__ void ctc_gamma_kernel(const void *y, int y_dtype, long sn, long st, int N, int T, int V,
                                  const int *labels, const int *label_off, const int *label_len, const int *len,
                                  int max_label_len, int blank, float *alpha_ws,
-                                 float *grad, long gsn, long gst, float grad_scale, int overwrite, int Tfull) {
+                                 float *grad, long gsn, long gst, float grad_scale, int overwrite, int Tfull,
+                                 const float *logz, int zero_inf) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
     const long row = (long)blockIdx.x * wpb + warp;
@@ -248,8 +252,12 @@ __global__ void ctc_gamma_kernel(const void *y, int y_dtype, long sn, long st, i
     const int L = label_len[n], Sc = 2 * L + 1, ScMax = 2 * max_label_len + 1;
     CtcWorkspace W(alpha_ws, n, T, ScMax);
     const double logp_d = *W.logp;
-    if (t >= len[n] || !(logp_d > -INFINITY)) {      // padding frame / infeasible utterance: no gradient
-        if (overwrite) { float *gz = grad + n * gsn + (long)t * gst; for (int k = lane; k < V; k += 32) gz[k] = 0.f; }
+    const bool masked = zero_inf && !(isfinite(logp_d) && (logz == nullptr || isfinite(logz[n])));
+    if (t >= len[n] || masked || !(logp_d > -INFINITY)) {      // padding frame / infeasible or masked utterance: no gradient
+        if (overwrite || (masked && t < len[n])) {
+            float *gz = grad + n * gsn + (long)t * gst;
+            for (int k = lane; k < V; k += 32) gz[k] = 0.f;
+        }
         return;
     }
     float *g = reinterpret_cast<float *>(smem_raw) + (size_t)warp * V;
@@ -279,13 +287,36 @@ __global__ void ctc_gamma_kernel(const void *y, int y_dtype, long sn, long st, i
     }
 }
 
-// loss[0] = scale * sum_n logp[n]   (CTC-only loss, ctc_crf/__init__.py:41-47: costs = -sum log p, / batch when averaging)
-__global__ void sum_scale_kernel(const float *logp, int N, float scale, float *loss) {
+// cost[n] = -logp[n];  loss[0] = scale * sum_n cost[n]   (CTC-only loss, ctc_crf/__init__.py:41-47: costs = -sum log p, / batch
+// when averaging).  costs (optional) receives each cost; zero_inf sets a cost that is not finite to 0 first.
+__global__ void sum_scale_kernel(const float *logp, int N, float scale, float *loss, float *costs, int zero_inf) {
     double acc = 0.0;
-    for (int n = threadIdx.x; n < N; n += 32) acc += (double)logp[n];
+    for (int n = threadIdx.x; n < N; n += 32) {
+        double c = -(double)logp[n];
+        if (zero_inf && !isfinite(c)) c = 0.0;
+        if (costs) costs[n] = (float)c;
+        acc += c;
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
     if (threadIdx.x == 0) loss[0] = (float)(acc * (double)scale);
+}
+
+// out[n][t][:] = w[n] * grad[n][t][:], converted to out_dtype, one warp per row; rows t >= len[n] are written with zeros
+// without reading grad.  The per-utterance weighted backward of a loss with reduction 'none'.
+__global__ void grad_rows_scale_kernel(const float *grad, const float *w, const int *len, int N, int T, int V, void *out,
+                                       int out_dtype) {
+    const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+    const long row = (long)blockIdx.x * wpb + (threadIdx.x >> 5);
+    if (row >= (long)N * T) return;
+    const int n = (int)(row / T), t = (int)(row % T);
+    const long base = row * V;
+    if (t >= len[n]) {
+        for (int k = lane; k < V; k += 32) store_y(out, out_dtype, base + k, 0.f);
+        return;
+    }
+    const float wn = __ldg(w + n);
+    for (int k = lane; k < V; k += 32) store_y(out, out_dtype, base + k, wn * __ldg(grad + base + k));
 }
 
 // Best-path (Viterbi) alignment over the same blank-expanded lattice: the forced alignment that is a by-product of the
@@ -362,10 +393,17 @@ __global__ void ctc_viterbi_kernel(const void *y, int y_dtype, long sn, long st,
     }
 }
 
-// loss[0] = scale * sum_n (logz[n] - (1+lamb) logp[n])      (ctc_crf/__init__.py:79-86)
-__global__ void assemble_loss_kernel(const float *logz, const float *logp, int N, float lamb, float scale, float *loss) {
+// cost[n] = logz[n] - (1+lamb) logp[n];  loss[0] = scale * sum_n cost[n]      (ctc_crf/__init__.py:79-86)
+// costs (optional) receives each cost; zero_inf sets a cost that is not finite to 0 first.
+__global__ void assemble_loss_kernel(const float *logz, const float *logp, int N, float lamb, float scale, float *loss,
+                                     float *costs, int zero_inf) {
     double acc = 0.0;
-    for (int n = threadIdx.x; n < N; n += 32) acc += (double)logz[n] - (1.0 + (double)lamb) * (double)logp[n];
+    for (int n = threadIdx.x; n < N; n += 32) {
+        double c = (double)logz[n] - (1.0 + (double)lamb) * (double)logp[n];
+        if (zero_inf && !isfinite(c)) c = 0.0;
+        if (costs) costs[n] = (float)c;
+        acc += c;
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
     if (threadIdx.x == 0) loss[0] = (float)(acc * (double)scale);
@@ -413,7 +451,7 @@ int LaunchCtcAlphaBeta(const void *y, int y_dtype, long sn, long st, int N, int 
 int LaunchCtcGamma(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                    const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                    float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, cudaStream_t stream,
-                   std::string *err, int overwrite, int Tfull) {
+                   std::string *err, int overwrite, int Tfull, const float *logz, int zero_inf) {
     if (N == 0) return 0;
     int wpb = 8;   // warps (= frames) per CTA of the occupancy kernel, bounded by the [V] accumulators
     while (wpb > 1 && (size_t)wpb * V * 4 > 48 * 1024) wpb >>= 1;
@@ -423,7 +461,7 @@ int LaunchCtcGamma(const void *y, int y_dtype, long sn, long st, int N, int T, i
     const long rows = (long)N * (overwrite ? Tfull : T);
     ctc_gamma_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, gsm, stream>>>(
         y, y_dtype, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws, grad, gsn, gst, grad_scale,
-        overwrite, Tfull);
+        overwrite, Tfull, logz, zero_inf);
     CountLaunch();
     e = cudaGetLastError();
     if (e != cudaSuccess) { *err = std::string("ctc gamma launch: ") + cudaGetErrorString(e); return (int)e; }
@@ -435,12 +473,13 @@ int LaunchCtcGamma(const void *y, int y_dtype, long sn, long st, int N, int T, i
 int LaunchCtc(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
               const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
               float *alpha_ws, float *grad, long gsn, long gst, float grad_scale, float *logp,
-              const double *lnorm, cudaStream_t stream, std::string *err, int overwrite, int Tfull) {
+              const double *lnorm, cudaStream_t stream, std::string *err, int overwrite, int Tfull, const float *logz,
+              int zero_inf) {
     int rc = LaunchCtcAlphaBeta(y, y_dtype, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws,
                                 grad != nullptr, logp, lnorm, stream, err);
     if (rc || grad == nullptr) return rc;
     return LaunchCtcGamma(y, y_dtype, sn, st, N, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws, grad, gsn,
-                          gst, grad_scale, stream, err, overwrite, Tfull);
+                          gst, grad_scale, stream, err, overwrite, Tfull, logz, zero_inf);
 }
 
 int LaunchCtcLogp(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
@@ -450,8 +489,18 @@ int LaunchCtcLogp(const void *y, int y_dtype, long sn, long st, int N, int T, in
                               false, logp, lnorm, stream, err);
 }
 
-int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStream_t stream) {
-    sum_scale_kernel<<<1, 32, 0, stream>>>(logp, N, scale, loss);
+int LaunchSumScale(const float *logp, int N, float scale, float *loss, cudaStream_t stream, float *costs, int zero_inf) {
+    sum_scale_kernel<<<1, 32, 0, stream>>>(logp, N, scale, loss, costs, zero_inf);
+    CountLaunch();
+    return (int)cudaGetLastError();
+}
+
+int LaunchGradRowsScale(const float *grad, const float *w, const int *len, int N, int T, int V, void *out, int out_dtype,
+                        cudaStream_t stream) {
+    const long rows = (long)N * T;
+    if (rows == 0) return 0;
+    const int wpb = 8;
+    grad_rows_scale_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, 0, stream>>>(grad, w, len, N, T, V, out, out_dtype);
     CountLaunch();
     return (int)cudaGetLastError();
 }
@@ -476,8 +525,8 @@ int LaunchCtcViterbi(const void *y, int y_dtype, long sn, long st, int N, int T,
 }
 
 int LaunchAssembleLoss(const float *logz, const float *logp, int N, float lamb, float scale, float *loss,
-                       cudaStream_t stream) {
-    assemble_loss_kernel<<<1, 32, 0, stream>>>(logz, logp, N, lamb, scale, loss);
+                       cudaStream_t stream, float *costs, int zero_inf) {
+    assemble_loss_kernel<<<1, 32, 0, stream>>>(logz, logp, N, lamb, scale, loss, costs, zero_inf);
     CountLaunch();
     return (int)cudaGetLastError();
 }

@@ -9,7 +9,7 @@ here ``_CTC_CRF.forward`` is ONE native call that writes the final gradient once
 from __future__ import annotations
 
 import os
-from typing import List, Union
+from typing import List, Optional, Union
 
 import torch
 from torch.autograd import Function
@@ -79,19 +79,80 @@ class _CTC_CRF_LOGITS(Function):
         return g.to(ctx.in_dtype), None, None, None, None, None, None
 
 
+class _CTC_CRF_COSTS(Function):
+    """The loss of ``_CTC_CRF`` / ``_CTC_CRF_LOGITS`` with ``reduction='none'`` (the (N,) costs
+    cost[n] = logZ_den[n] - (1+lamb) log p_ctc[n]) and / or ``zero_infinity``.  With 'none' the native call keeps the gradient
+    unscaled, G[n] = d cost[n] / d logits[n], and the backward is one pass that writes grad_output[n] * G[n] in the logits'
+    dtype (``_C.grad_rows_scale``)."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, input_lengths, label_lengths, lamb, size_average, from_logits, reduction, zero_infinity):
+        logits = logits.contiguous()
+        out, grads, _ = core.ctc_crf_loss_fwd(logits, labels, input_lengths, label_lengths, lamb, size_average,
+                                              from_logits=from_logits, reduction=reduction, zero_infinity=zero_infinity)
+        ctx.grads, ctx.lx, ctx.in_dtype, ctx.reduction = grads, input_lengths, logits.dtype, reduction
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        return (_costs_backward(ctx, grad_output),) + (None,) * 8
+
+
+class _WARP_CTC_COSTS(Function):
+    """``_WARP_CTC_GPU`` with ``reduction='none'`` (cost[n] = -log p[n]) and / or ``zero_infinity``; backward as in
+    ``_CTC_CRF_COSTS``."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, input_lengths, label_lengths, size_average, reduction, zero_infinity):
+        logits = logits.contiguous()
+        out, grads, _ = core.ctc_loss_fwd(logits, labels, input_lengths, label_lengths, size_average,
+                                          reduction=reduction, zero_infinity=zero_infinity)
+        ctx.grads, ctx.lx, ctx.in_dtype, ctx.reduction = grads, input_lengths, logits.dtype, reduction
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        return (_costs_backward(ctx, grad_output),) + (None,) * 6
+
+
+def _costs_backward(ctx, grad_output):
+    if ctx.reduction == "none":     # grad_logits[n] = grad_output[n] * G[n], in one pass, in the logits' dtype
+        return core.grad_rows_scale(ctx.grads, grad_output, ctx.lx, ctx.in_dtype)
+    return (ctx.grads * grad_output.to(ctx.grads.device)).to(ctx.in_dtype)
+
+
+def _loss_options(reduction, zero_infinity) -> dict:
+    """The keyword arguments the `_C` loss functions get for these settings: none at the defaults, so that the default
+    path calls exactly what it called before the two options existed."""
+    core.check_reduction(reduction)
+    if reduction is None and not zero_infinity:
+        return {}
+    return dict(reduction=reduction, zero_infinity=bool(zero_infinity))
+
+
 class CTC_CRF_LOSS(Module):
-    def __init__(self, lamb: float = 0.1, size_average: bool = True, from_logits: bool = False):
+    def __init__(self, lamb: float = 0.1, size_average: bool = True, from_logits: bool = False,
+                 reduction: Optional[str] = None, zero_infinity: bool = False):
         """
         lamb (float): weight for auxiliary CTC loss, final loss = lamb * loss_ctc + loss_crf
         size_average (bool): whether to do average over batch size dimension.
         from_logits (bool): addition to the reference signature -- ``forward`` takes the raw encoder outputs and
             applies log_softmax (and its backward) inside the fused call.  Default False = reference behaviour.
+        reduction (None or 'none'): addition -- None returns the scalar of the reference (the batch sum, or the mean
+            over the batch with size_average); 'none' returns the (N,) fp32 costs logZ_den[n] - (1+lamb) log p_ctc[n], to be
+            weighted, masked or normalised by the caller.  Any other value raises ValueError.
+        zero_infinity (bool): addition -- an utterance whose cost is not finite (an infeasible label sequence, an utterance
+            that cannot reach a final state of the den graph) gets cost 0 and a zero gradient instead of making the batch
+            loss inf or NaN.  With size_average the divisor stays N.
         """
         super(CTC_CRF_LOSS, self).__init__()
+        _loss_options(reduction, zero_infinity)      # an unknown reduction fails here, at construction
         self.ctc_crf = _CTC_CRF_LOGITS.apply if from_logits else _CTC_CRF.apply
         self.lamb = lamb
         self.size_average = size_average
         self.from_logits = from_logits
+        self.reduction = reduction
+        self.zero_infinity = zero_infinity
 
     def forward(self, logits, labels, lx, ly) -> torch.FloatTensor:
         """
@@ -111,29 +172,41 @@ class CTC_CRF_LOSS(Module):
         _assert_no_grad(labels)
         _assert_no_grad(lx)
         _assert_no_grad(ly)
+        opts = _loss_options(self.reduction, self.zero_infinity)    # read on every call: the attributes may be reassigned
         if not torch.is_grad_enabled():
             # evaluation (torch.no_grad / inference_mode): the loss alone, with the den alpha on a ring of frames and no
             # gradient.  Keyed on grad mode, not on logits.requires_grad: with grad mode on the gradient is always computed.
             return core.ctc_crf_loss_fwd_only(logits.contiguous(), labels, lx, ly, self.lamb, self.size_average,
-                                              from_logits=self.from_logits)[0]
+                                              from_logits=self.from_logits, **opts)[0]
+        if opts:
+            return _CTC_CRF_COSTS.apply(logits, labels, lx, ly, self.lamb, self.size_average, self.from_logits,
+                                        self.reduction, bool(self.zero_infinity))
         return self.ctc_crf(logits, labels, lx, ly, self.lamb, self.size_average)
 
 
 class WARP_CTC_LOSS(Module):
-    """__init__.py:128-144"""
+    """__init__.py:128-144.  reduction and zero_infinity (additions) as for CTC_CRF_LOSS, with cost[n] = -log p[n]."""
 
-    def __init__(self, size_average=True):
+    def __init__(self, size_average=True, reduction: Optional[str] = None, zero_infinity: bool = False):
         super(WARP_CTC_LOSS, self).__init__()
+        _loss_options(reduction, zero_infinity)      # an unknown reduction fails here, at construction
         self.ctc = _WARP_CTC_GPU.apply
         self.size_average = size_average
+        self.reduction = reduction
+        self.zero_infinity = zero_infinity
 
     def forward(self, logits, labels, input_lengths, label_lengths):
         assert len(labels.size()) == 1
         _assert_no_grad(labels)
         _assert_no_grad(input_lengths)
         _assert_no_grad(label_lengths)
+        opts = _loss_options(self.reduction, self.zero_infinity)
         if not torch.is_grad_enabled():   # evaluation: the loss alone (see CTC_CRF_LOSS.forward)
-            return core.ctc_loss_fwd_only(logits.contiguous(), labels, input_lengths, label_lengths, self.size_average)[0]
+            return core.ctc_loss_fwd_only(logits.contiguous(), labels, input_lengths, label_lengths, self.size_average,
+                                          **opts)[0]
+        if opts:
+            return _WARP_CTC_COSTS.apply(logits, labels, input_lengths, label_lengths, self.size_average, self.reduction,
+                                         bool(self.zero_infinity))
         return self.ctc(logits, labels, input_lengths, label_lengths, self.size_average)
 
 

@@ -195,6 +195,39 @@ int ccb_ctc_loss_fwd_only(const void *logits, int dtype, int N, int T, int V, in
                           const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
                           int max_label_len, int blank, float scale, float *loss, float *logp, void *stream);
 
+/* Per-utterance costs (reduction 'none') and zero_infinity.  The loss entries above with two more arguments:
+ *   costs    (optional, may be NULL): N floats out, cost[n] = logZ_den[n] - (1+lamb) logp_ctc[n] (CTC-CRF) or -logp[n] (CTC),
+ *            unscaled; loss[0] = scale * sum_n cost[n] as before.  A batch split into several calls passes costs + n0.
+ *   zero_inf (0 / 1): an utterance whose cost is not finite (+-inf or NaN: an infeasible label sequence, an utterance that
+ *            cannot reach a final state of the den graph, a length of 0) gets cost 0 in `costs` and in the sum, and zero
+ *            gradient rows -- den part included -- in every row t < len.  The mask is applied on the device, by the kernels
+ *            that already read both halves of the loss; nothing synchronises the host.
+ * With costs = NULL and zero_inf = 0 each is exactly the entry it extends.
+ * ccb_ctc_crf_loss_costs: ccb_ctc_crf_loss_fwd / _logits_fwd / _ckpt_fwd / _logits_ckpt_fwd, selected by from_logits != 0 and
+ * ckpt_k > 0 (ckpt_k = 0: the full alpha spill). */
+int ccb_ctc_crf_loss_costs(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax, int ckpt_k,
+                           const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                           const int *len_dev, int max_label_len, float lamb, float scale,
+                           float *alpha_ws, void *aux_ws, void *ctc_ws,
+                           float *grad, float *loss, float *parts, float *costs, int zero_inf, void *stream);
+/* ccb_ctc_crf_loss_fwd_only with costs and zero_inf (no gradient, so zero_inf masks the costs and the sum only). */
+int ccb_ctc_crf_loss_costs_fwd_only(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax,
+                                    const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                                    const int *len_dev, int max_label_len, float lamb, float scale,
+                                    float *alpha_ws, void *aux_ws, void *num_ws,
+                                    float *loss, float *parts, float *costs, int zero_inf, void *stream);
+/* ccb_ctc_loss_fwd with costs and zero_inf; grad = NULL is ccb_ctc_loss_fwd_only (ctc_ws is then not used, may be NULL). */
+int ccb_ctc_loss_costs(const void *logits, int dtype, int N, int T, int V, int Tmax,
+                       const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                       int max_label_len, int blank, float scale, void *ctc_ws, float *grad, float *loss, float *logp,
+                       float *costs, int zero_inf, void *stream);
+/* Backward of a loss with per-utterance costs: out[n][t][:] = w[n] * grad[n][t][:] for t < len[n], zeros beyond (grad is
+ * not read there), in one pass.  grad: (N,T,V) fp32, the unscaled gradient of the entries above (scale = 1); w: (N,) fp32,
+ * the gradient of the caller's objective with respect to each cost; out: (N,T,V) in the CCB_DTYPE_* code out_dtype (fp32,
+ * bf16 or fp16, rounded to nearest), not aliasing grad. */
+int ccb_grad_rows_scale(const float *grad, const float *w, const int *len_dev, int N, int T, int V, void *out, int out_dtype,
+                        void *stream);
+
 /* Best-path (Viterbi) alignment over the numerator lattice -- the forced alignment that comes with the CTC numerator
  * (SURVEY.md 8f-4).  align: (N,T) int32 device out, the token emitted at every frame t < len (blank included), -1 beyond
  * the length and for infeasible utterances; score (optional, may be NULL): (N,) log-probability of the best path.
