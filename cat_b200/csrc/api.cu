@@ -126,7 +126,16 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
     cudaDeviceProp prop;
     CCB_CUDA(cudaGetDeviceProperties(&prop, gpus[0]));
     if (!prop.cooperativeLaunch) return Fail("device does not support cooperative launch");
-    if (!BuildDenPlan(fst, prop.multiProcessorCount, kDenThreads / 32, &g_plan, &err)) return Fail(err);
+    int n_ctas = prop.multiProcessorCount;
+    if (const char *e = getenv("CCB_DEN_CTAS")) {   // test hook: the plan (and grid) of a part with fewer SMs
+        char *end = nullptr;
+        const long v = strtol(e, &end, 10);
+        if (end == e || *end != '\0' || v < 1 || v > prop.multiProcessorCount)
+            return Fail(std::string("Init: CCB_DEN_CTAS=") + e + " is not a CTA count in [1, " +
+                        std::to_string(prop.multiProcessorCount) + "] (the device's SM count)");
+        n_ctas = (int)v;
+    }
+    if (!BuildDenPlan(fst, n_ctas, kDenThreads / 32, &g_plan, &err)) return Fail(err);
     g_plan_valid = true;
     DEN_NUM_STATES = g_plan.num_states + g_plan.num_pairs;   // rows per alpha frame (what binding.cpp sizes scratch with)
     DEN_NUM_ARCS = (int)g_plan.fwd.arcs.size();
