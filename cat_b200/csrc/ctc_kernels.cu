@@ -322,7 +322,8 @@ __global__ void grad_rows_scale_kernel(const float *grad, const float *w, const 
 // Best-path (Viterbi) alignment over the same blank-expanded lattice: the forced alignment that is a by-product of the
 // numerator (SURVEY 8f-4).  One CTA per utterance; thread i owns cells 2i and 2i+1 as in the alpha pass; max replaces
 // log-add; a 2-bit back-pointer per cell and frame (0: stay, 1: from s-1, 2: from s-2) goes to the workspace, and thread 0
-// walks it back.  align[n][t] = the token emitted at frame t (blank included), -1 for t >= len or an infeasible utterance.
+// walks it back.  align[n][t] = the token emitted at frame t (blank included), -1 for t >= len or an utterance without a
+// path of finite score (too few frames for its labels, or every path through a -inf emission).
 // Ties are broken towards the smaller predecessor index (stay < s-1 < s-2).
 // shared memory: lab[Lmax] ints | v[2][ScMax] floats
 __global__ void ctc_viterbi_kernel(const void *y, int y_dtype, long sn, long st, int T, int V,
@@ -386,6 +387,8 @@ __global__ void ctc_viterbi_kernel(const void *y, int y_dtype, long sn, long st,
         int s = Sc - 1;
         if (Sc > 1 && last[Sc - 2] > last[Sc - 1]) s = Sc - 2;
         if (score) score[n] = last[s];
+        // every path killed by -inf emissions: the back-pointers lead nowhere, so the row keeps its -1s
+        if (last[s] == -INFINITY) return;
         for (int t = Tn - 1; t >= 0; --t) {
             arow[t] = (s & 1) ? s_lab[s >> 1] : blank;
             s -= bp[(size_t)t * ScMax + s];

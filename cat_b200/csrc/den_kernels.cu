@@ -194,6 +194,9 @@ __global__ void logit_grad_kernel(const void *z, int dtype, long sn, long st, in
     for (int k = lane; k < V; k += 32) gs += g[k];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) gs += __shfl_xor_sync(kFull, gs, o);
+    // a row whose entries sum to 0 loses nothing; skipping it keeps a zeroed row (zero_infinity) zero where the frame's
+    // logits are all -inf and expf(z - lz) = expf(-inf + inf) is NaN
+    if (gs == 0.f) return;
     const float l = lz[(size_t)t * Npad + n];
     const long base = n * sn + t * st;
     for (int k = lane; k < V; k += 32) g[k] -= expf(load_y(z, dtype, base + k) - l) * gs;

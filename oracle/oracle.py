@@ -105,10 +105,16 @@ def ctc_crf(graph, y, labels, lx, ly, lamb: float = 0.1, size_average: bool = Tr
 
 def ctc_crf_from_logits(graph, z, labels, lx, ly, lamb: float = 0.1, size_average: bool = True, nthreads: int = 0):
     """The loss on RAW encoder outputs z (N,T,V), as cat/ctc/train.py:173-174,184-190 composes it:
-    y = log_softmax(z) (fp64 here), loss = ctc_crf(y), d loss / d z = g - softmax(z) * sum_k g_k  (g = d loss / d y)."""
+    y = log_softmax(z) (fp64 here), loss = ctc_crf(y), d loss / d z = g - softmax(z) * sum_k g_k  (g = d loss / d y).
+    -inf logits are impossible tokens (log-prob -inf, softmax 0).  A frame whose logits are ALL -inf has no normaliser; it
+    is taken as a frame no path crosses (every log-prob -inf), so its utterance gets log p = logZ = -inf and no gradient."""
     z64 = np.asarray(z, np.float64)
-    lse = z64.max(-1, keepdims=True) + np.log(np.exp(z64 - z64.max(-1, keepdims=True)).sum(-1, keepdims=True))
-    y64 = z64 - lse
+    m = z64.max(-1, keepdims=True)
+    dead = m == -np.inf
+    m = np.where(dead, 0.0, m)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        lse = m + np.log(np.exp(z64 - m).sum(-1, keepdims=True))
+        y64 = np.where(dead, -np.inf, z64 - lse)
     loss, g, parts = ctc_crf(graph, y64.astype(np.float32), labels, lx, ly, lamb, size_average, nthreads)
     dz = g - np.exp(y64) * g.sum(-1, keepdims=True)
     return loss, dz, parts

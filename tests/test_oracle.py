@@ -188,3 +188,154 @@ def test_linear_domain_oracle_equals_log_domain_oracle(tmp_graphs, fixture_fst, 
     for u, v in zip(a, b):
         np.testing.assert_allclose(v, u, rtol=1e-12, atol=1e-12)
     assert abs(b[0][0] - (-6.25832785)) < 1e-6
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# -inf emissions (masked vocabularies, blank suppression, masked_fill before log_softmax): the oracle against first
+# principles -- every path enumerated in fp64, nothing shared with the lattice recursions
+# ---------------------------------------------------------------------------------------------------------------------
+def _brute_ctc(y, lab, blank=0):
+    """log p(l|x) and the occupancies of one utterance by enumerating all V^T frame-level token sequences and keeping those
+    that collapse (repeats merged, blanks dropped) to `lab` -- the definition of CTC, no lattice."""
+    import itertools
+    T, V = y.shape
+    y = y.astype(np.float64)
+    total, occ = 0.0, np.zeros((T, V))
+    rows = np.arange(T)
+    for seq in itertools.product(range(V), repeat=T):
+        if [k for i, k in enumerate(seq) if k != blank and (i == 0 or seq[i - 1] != k)] != list(lab):
+            continue
+        s = y[rows, seq].sum()
+        if s == -np.inf:
+            continue
+        total += np.exp(s)
+        occ[rows, seq] += np.exp(s)
+    return (np.log(total), occ / total) if total > 0 else (-np.inf, occ)
+
+
+def _brute_den(g, y):
+    """logZ and the occupancies of one utterance over the den graph `g`, path by path."""
+    src, dst, lab, lw = g.log_arcs()
+    ew = g.end_weight()
+    out = [[] for _ in range(g.num_states)]
+    for a in range(g.num_arcs):
+        out[src[a]].append(a)
+    T, V = y.shape
+    y = y.astype(np.float64)
+    acc = {"total": 0.0}
+    occ = np.zeros((T, V))
+
+    def walk(q, t, score, labs):
+        if score == -np.inf:
+            return
+        if t == T:
+            if np.isfinite(ew[q]):
+                p = np.exp(score + float(ew[q]))
+                acc["total"] += p
+                occ[np.arange(T), labs] += p
+            return
+        for a in out[q]:
+            walk(dst[a], t + 1, score + float(lw[a]) + y[t, lab[a]], labs + [int(lab[a])])
+
+    walk(g.start, 0, 0.0, [])
+    total = acc["total"]
+    return (np.log(total), occ / total) if total > 0 else (-np.inf, occ)
+
+
+def _masked_case(kind, T=6, V=4, seed=0):
+    """(log-probs y (1,T,V) float32 with -inf entries, labels).  Labels [1, 2] (blank 0, token 3 off the transcript)."""
+    rng = np.random.default_rng(seed)
+    z = rng.standard_normal((T, V)) * 1.5
+    mask = np.zeros((T, V), bool)
+    lab = [1, 2]
+    if kind == "off_path":          # the token outside the transcript masked everywhere, blank at one frame too
+        mask[:, 3] = True
+        mask[4, 0] = True
+    elif kind == "on_path":         # entries that alignments of [1, 2] do use: blank at frame 1, label 1 at frames 2-3,
+        mask[1, 0] = True           # label 2 at frame 1; other alignments remain
+        mask[2:4, 1] = True
+        mask[1, 2] = True
+    elif kind == "kill_all":        # frame 3 keeps only token 3: no path of the transcript survives
+        mask[3, :3] = True
+    elif kind == "dead_frame":      # frame 2 all -inf: no path at all, numerator or den
+        mask[2, :] = True
+    z = np.where(mask, -np.inf, z)
+    m = np.where(np.isfinite(z).any(-1, keepdims=True), z.max(-1, keepdims=True), 0.0)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        y = np.where(mask, -np.inf, z - m - np.log(np.exp(z - m).sum(-1, keepdims=True)))
+    return y[None].astype(np.float32), np.array(lab, np.int32)
+
+
+@pytest.fixture(scope="module")
+def tiny_den():
+    """A 5-state, 16-arc unstructured den graph over 4 labels, small enough to enumerate every path of 6 frames."""
+    return fst.make_random_den(5, 16, 4, seed=21)
+
+
+@pytest.mark.parametrize("kind", ["off_path", "on_path", "kill_all", "dead_frame"])
+def test_oracle_with_neg_inf_emissions_equals_brute_force(tiny_den, kind):
+    """oracle.ctc, oracle.den (log and linear domain) and the assembled gradient against path enumeration, with -inf
+    log-probs on and off the transcript's paths: log p, logZ and every occupancy finite and equal (an occupancy of a
+    -inf entry is exactly 0); torch's fp64 ctc_loss forward agrees on log p (its gradient has the same -inf + inf)."""
+    g = tiny_den
+    y, lab = _masked_case(kind)
+    T = y.shape[1]
+    lens, ly = np.array([T], np.int32), np.array([len(lab)], np.int32)
+    blp, bgam = _brute_ctc(y[0], lab)
+    if kind == "on_path":           # the mask removes alignments: unmasked, every masked entry carries occupancy
+        z = np.random.default_rng(0).standard_normal((T, 4)) * 1.5       # _masked_case's scores before the mask
+        _, free = _brute_ctc(z - np.log(np.exp(z).sum(-1, keepdims=True)), lab)
+        assert (free[np.isinf(y[0])] > 0).all()
+    lp, gam = oracle.ctc(y, lab, ly, lens)
+    assert (np.isfinite(blp), np.isfinite(lp[0])) == ({"kill_all": False, "dead_frame": False}.get(kind, True),) * 2
+    if np.isfinite(blp):
+        assert abs(lp[0] - blp) < 1e-9 * max(1.0, abs(blp))
+    else:
+        assert lp[0] == -np.inf
+    assert np.isfinite(gam).all()
+    np.testing.assert_allclose(gam[0], bgam, atol=1e-10)
+    assert not gam[0][np.isinf(y[0])].any()
+    nll = torch.nn.functional.ctc_loss(torch.tensor(y, dtype=torch.float64).transpose(0, 1), torch.tensor(lab).long(),
+                                       torch.tensor(lens).long(), torch.tensor(ly).long(), reduction="none")
+    assert float(nll[0]) == -lp[0] or abs(float(nll[0]) + lp[0]) < 1e-9 * max(1.0, abs(lp[0]))
+    bz, bocc = _brute_den(g, y[0])
+    assert np.isfinite(bz) == (kind != "dead_frame")
+    for fast in (False, True):
+        la, lb, gd = oracle.den(g, y, lens, fast=fast)
+        assert np.isfinite(gd).all(), fast
+        if np.isfinite(bz):
+            assert abs(la[0] - bz) < 1e-9 and abs(lb[0] - bz) < 1e-9, (fast, la, lb, bz)
+        else:
+            assert la[0] == -np.inf and lb[0] == -np.inf
+        np.testing.assert_allclose(gd[0], bocc, atol=1e-10)
+        assert not gd[0][np.isinf(y[0])].any()
+    loss, grad, parts = oracle.ctc_crf(g, y, lab, lens, ly, 0.1, size_average=False)
+    assert np.isfinite(grad).all()
+    np.testing.assert_allclose(grad[0], bocc - 1.1 * bgam, atol=1e-10)
+
+
+def test_oracle_from_logits_with_neg_inf_logits():
+    """oracle.ctc_crf_from_logits on raw logits holding -inf entries: the loss and d loss / d z are what torch's autograd
+    through an fp64 log_softmax gives from the oracle's own d loss / d y (softmax 0 at a -inf logit), and an utterance
+    with a valid frame whose logits are ALL -inf gets log p = logZ = -inf and an all-zero gradient, without touching the
+    other utterance."""
+    g = fst.make_random_den(5, 16, 4, seed=21)
+    rng = np.random.default_rng(5)
+    N, T, V = 2, 6, 4
+    z = (2.0 * rng.standard_normal((N, T, V)) + 3.0).astype(np.float32)
+    z[0, :, 3] = -np.inf
+    z[0, 1, 0] = -np.inf
+    z[1, 4, :] = -np.inf
+    labels, lx, ly = np.array([1, 2, 2, 1], np.int32), np.array([6, 5], np.int32), np.array([2, 2], np.int32)
+    _, dz, parts = oracle.ctc_crf_from_logits(g, z, labels, lx, ly, 0.05, size_average=False)
+    assert np.isfinite(dz).all() and not dz[1].any()
+    assert parts["logp_ctc"][1] == -np.inf and parts["logz_alpha"][1] == -np.inf
+    zt = torch.tensor(z[:1], dtype=torch.float64, requires_grad=True)
+    y = zt.log_softmax(-1)
+    oloss, gy, _ = oracle.ctc_crf(g, y.detach().numpy().astype(np.float32), labels[:2], lx[:1], ly[:1], 0.05,
+                                  size_average=False)
+    y.backward(torch.tensor(gy))
+    assert np.isfinite(oloss)
+    assert abs(parts["logz_alpha"][0] - 1.05 * parts["logp_ctc"][0] - oloss) < 1e-9
+    np.testing.assert_allclose(dz[0], zt.grad.numpy()[0], atol=1e-9)
+    assert not dz[0][np.isinf(z[0])].any()
