@@ -24,7 +24,7 @@ SYMBOLS = [
     "ccb_ctc_workspace_bytes", "ccb_den_forward_backward", "ccb_ctc_forward_backward", "ccb_ctc_crf_loss_fwd",
     "ccb_ctc_crf_loss_logits_fwd", "ccb_ctc_loss_fwd", "ccb_ctc_align_workspace_bytes", "ccb_ctc_align",
     "ccb_launch_count", "ccb_debug_timeline", "ccb_plan_create", "ccb_plan_destroy", "ccb_plan_info", "ccb_plan_copy",
-    "ccb_plan_launch",
+    "ccb_plan_launch", "ccb_plan_launch_own",
     "ccb_den_ckpt_alpha_floats", "ccb_ctc_crf_loss_ckpt_fwd", "ccb_ctc_crf_loss_logits_ckpt_fwd",
     "ccb_den_fwd_alpha_floats", "ccb_num_fwd_only_bytes", "ccb_ctc_crf_loss_fwd_only", "ccb_ctc_loss_fwd_only",
     "ccb_ctc_crf_loss_costs", "ccb_ctc_crf_loss_costs_fwd_only", "ccb_ctc_loss_costs", "ccb_grad_rows_scale",
@@ -111,6 +111,8 @@ def lib() -> C.CDLL:
     L.ccb_plan_copy.argtypes = [vp, C.c_int, vp, C.c_size_t]; L.ccb_plan_copy.restype = C.c_int
     L.ccb_plan_launch.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_long)]
     L.ccb_plan_launch.restype = C.c_int
+    L.ccb_plan_launch_own.argtypes = L.ccb_plan_launch.argtypes
+    L.ccb_plan_launch_own.restype = C.c_int
     _lib = L
     return L
 

@@ -160,6 +160,7 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
         d.own_rows = g_plan.own_rows;
         auto on = [](const char *name) { const char *e = getenv(name); return e && e[0] == '1'; };
         d.hooks.arcs_in_global = on("CCB_ARCS_IN_GLOBAL"); d.hooks.w1_in_global = on("CCB_W1_IN_GLOBAL"); d.hooks.no_tma = on("CCB_NO_TMA");
+        d.hooks.own_in_l2 = on("CCB_OWN_IN_L2");
         d.shape = ShapeOf(g_plan, d.hooks);
         if (rc == 0 && d.shape.streamed_quads) rc = UploadTransposedQuads(g_plan.bwd, &d.bwd);
         if (d.hooks.arcs_in_global || d.hooks.w1_in_global)
@@ -858,17 +859,33 @@ int ccb_plan_copy(void *plan, int which, void *dst, size_t dst_bytes) {
     return 0;
 }
 
+static int PlanLaunch(void *plan, int N, int backward, int smem_optin, int hooks, DenLaunch *L, int *Npad) {
+    const DenHooks h{(hooks & 1) != 0, (hooks & 2) != 0, (hooks & 4) != 0, (hooks & 8) != 0};
+    const DenGraphShape g = ShapeOf(*reinterpret_cast<const DenPlan *>(plan), h);
+    *Npad = PadLanes(N, SmallBatchOk(g, smem_optin, h));
+    return ChooseDenLaunch(g, *Npad, backward != 0, smem_optin, h, L, &g_err) ? 0 : 1;
+}
+
 int ccb_plan_launch(void *plan, int N, int backward, int smem_optin, int hooks, long *out) {
     g_err.clear();
     if (!plan || !out || N <= 0) return Fail("ccb_plan_launch: bad arguments");
-    const DenHooks h{(hooks & 1) != 0, (hooks & 2) != 0, (hooks & 4) != 0};
-    const DenGraphShape g = ShapeOf(*reinterpret_cast<const DenPlan *>(plan), h);
-    const int Npad = PadLanes(N, SmallBatchOk(g, smem_optin, h));
     DenLaunch L;
-    if (!ChooseDenLaunch(g, Npad, backward != 0, smem_optin, h, &L, &g_err)) return 1;
+    int Npad = 0;
+    if (PlanLaunch(plan, N, backward, smem_optin, hooks, &L, &Npad)) return 1;
     const long v[] = {L.tier, L.lanes_per_row, L.U, L.batch, L.w1_smem, Npad, L.tile_rows, L.gacc_rows, (long)L.arcs_off,
                       (long)L.ring_off, (long)L.bar_off, (long)L.w1_off, (long)L.abar_off, (long)L.aring_off, (long)L.total};
     memcpy(out, v, sizeof(v));
+    return 0;
+}
+
+int ccb_plan_launch_own(void *plan, int N, int backward, int smem_optin, int hooks, long *out) {
+    g_err.clear();
+    if (!plan || !out || N <= 0) return Fail("ccb_plan_launch_own: bad arguments");
+    DenLaunch L;
+    int Npad = 0;
+    if (PlanLaunch(plan, N, backward, smem_optin, hooks, &L, &Npad)) return 1;
+    out[0] = L.own_smem;
+    out[1] = (long)L.own_off;
     return 0;
 }
 

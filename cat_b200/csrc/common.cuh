@@ -112,6 +112,7 @@ struct alignas(64) DenParams {
     float *logz;          // [N] out (forward: logZ from alpha; backward: logZ from beta)
     const float *own_c;   // [2S + 4] own-row coefficients of this pass (den_graph.h DenPlan::own_rows), used when own != 0
     int own;
+    int own_off;          // byte offset in dynamic shared memory of the on-chip own rows (DenLaunch::own_smem; OWN_SMEM kernels)
     const double *lnorm;  // [N] or null: sum_t log-normaliser of raw logits, subtracted from logZ (raw-logit entry)
     // gradient (backward)
     float *grad;          // raw accumulation target, element (n,t,k) at n*gsn + t*gst + k

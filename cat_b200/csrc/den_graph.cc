@@ -808,6 +808,12 @@ bool ChooseDenLaunch(const DenGraphShape &g, int Npad, bool backward, int smem_o
     }
     L.tier = smem_arcs ? kTierShared : kTierGlobal; L.w1_smem = smem_arcs && w1_smem;
     L.batch = backward ? kBwdBatch : FwdBatch(L.U); L.total = L.arcs_off + (smem_arcs ? arc_bytes : 0);
+    // Own rows on chip: each warp reads back the rows it wrote one frame earlier (the own-row terms, 2 per pair) from a
+    // [tile_rows][Npad] copy behind the arc tile instead of from L2, where it fits (N = 64 at 132 CTAs: 78 KB)
+    const size_t own_off = (L.total + 15) & ~(size_t)15, own_bytes = (size_t)L.tile_rows * Npad * 4;
+    if (g.own_rows && !hooks.own_in_l2 && own_off + own_bytes <= budget) {
+        L.own_smem = true; L.own_off = own_off; L.total = own_off + own_bytes;
+    }
     *out = L;
     return true;
 }
@@ -822,7 +828,7 @@ DenGraphShape ShapeOf(const DenPlan &plan, const DenHooks &hooks) {
     const int n_hubs = (int)plan.hub_states.size();
     return {{plan.fwd.max_tile_arcs, plan.fwd.max_tile_rows, plan.fwd.max_tile_labels},
             {plan.bwd.max_tile_arcs, plan.bwd.max_tile_rows, plan.bwd.max_tile_labels}, n_hubs, plan.n_warps,
-            n_hubs == 0 && !hooks.no_tma && (hooks.arcs_in_global || LargeGraphTiers(plan.bwd.max_tile_arcs))};
+            n_hubs == 0 && !hooks.no_tma && (hooks.arcs_in_global || LargeGraphTiers(plan.bwd.max_tile_arcs)), plan.own_rows};
 }
 
 }  // namespace ccb

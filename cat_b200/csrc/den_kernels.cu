@@ -118,6 +118,23 @@ __device__ __forceinline__ float *row_ptr(float *lane_base, uint32_t row, uint32
     return reinterpret_cast<float *>(reinterpret_cast<char *>(lane_base) + (size_t)row * row_bytes);
 }
 
+// Own rows on chip (DenLaunch::own_smem, kernels OWN_SMEM): [tile row][Npad] floats in shared memory.  A lane addresses its
+// part of row q of the frame (q >= s0, the tile's first row) at base + q * row_bytes, with the same byte offsets as the frame
+// in global memory; base is a 32-bit shared address (unsigned arithmetic: wraps below the window, lands back inside it).
+__device__ __forceinline__ uint32_t own_lane_base(const float *s_own, int n0, int s0, uint32_t row_bytes) {
+    return (uint32_t)__cvta_generic_to_shared(s_own + n0) - (uint32_t)s0 * row_bytes;
+}
+template <int U> __device__ __forceinline__ void sts_row(uint32_t addr, const Vec<U> &r);
+template <> __device__ __forceinline__ void sts_row<1>(uint32_t addr, const Vec<1> &r) {
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(r.v[0]) : "memory");
+}
+template <> __device__ __forceinline__ void sts_row<2>(uint32_t addr, const Vec<2> &r) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(r.v[0]), "f"(r.v[1]) : "memory");
+}
+template <> __device__ __forceinline__ void sts_row<4>(uint32_t addr, const Vec<4> &r) {
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(r.v[0]), "f"(r.v[1]), "f"(r.v[2]), "f"(r.v[3]) : "memory");
+}
+
 __device__ __forceinline__ void prefetch_l2(const void *p) {
     asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
 }
@@ -405,6 +422,11 @@ template <> __device__ __forceinline__ Vec<2> lds_row<2>(uint32_t addr) {
     asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(r.v[0]), "=f"(r.v[1]) : "r"(addr));
     return r;
 }
+template <> __device__ __forceinline__ Vec<4> lds_row<4>(uint32_t addr) {
+    Vec<4> r;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]) : "r"(addr));
+    return r;
+}
 
 // Streamed arcs (graphs whose arc stream does not fit shared memory, BASELINE config 4: 5 M arcs): the chunk's quads are
 // not resident; they flow through a per-warp ring of kArcStages batches, filled by 1-D bulk copies (`cp.async.bulk`, SASS
@@ -636,15 +658,20 @@ __device__ __forceinline__ void ckpt_frame_done(const DenParams &P, int t, const
 // partial-row path out entirely so that it costs the hot row-end code nothing.
 // Rows are gathered into registers (walk_arcs), except in the small-batch variant (SMALL: 16 lanes per row), whose rows
 // are staged in shared memory by bulk copies (TMA, walk_arcs_tma_small); it needs the arc tile in shared memory
-// (SMEM_ARCS), one utterance per lane and no hub rows.
-template <int U, int BATCH, bool SMEM_ARCS, bool HUBS, bool SMALL = false>
+// (SMEM_ARCS), one utterance per lane and no hub rows.  OWN_SMEM: the own-row terms read the rows this warp wrote one frame
+// earlier from shared memory, not from L2 (plans with own-row terms have no hub rows).
+template <int U, int BATCH, bool SMEM_ARCS, bool HUBS, bool SMALL = false, bool OWN_SMEM = false>
 __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __grid_constant__ DenParams P) {
     constexpr int LPR = SMALL ? kSmallLanes : 32;   // lanes per row
     static_assert(!SMALL || (SMEM_ARCS && U == 1 && !HUBS), "small-batch variant: arc tile in shared memory, one utterance per lane, no hubs");
+    static_assert(!OWN_SMEM || (!SMALL && !HUBS), "own rows on chip: register gathers, no hub rows");
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float *s_sum = reinterpret_cast<float *>(smem_raw);                                  // [Npad]
     int *s_label = reinterpret_cast<int *>(s_sum + P.Npad);                              // [tile_rows] label per row
     Arc *s_arcs = reinterpret_cast<Arc *>(smem_raw + FwdArcsOff(P.Npad, P.tile_rows));
+    // own rows on chip: the tile's real rows of the last frame, [tile row][Npad], each value written and read back by one lane
+    constexpr bool own_smem = OWN_SMEM;
+    float *const s_own = reinterpret_cast<float *>(smem_raw + P.own_off);
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(kFull, tid >> 5, 0);   // (through a shuffle: lets ptxas keep warp-derived addresses in uniform registers)
@@ -719,7 +746,11 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
         float *a0 = P.alpha + (size_t)alpha_pos(P, P.t_lo) * frame_elems;
         auto first = [&](int q, int n) { return recompute ? __ldcg(src + (size_t)q * Npad + n) : (q == P.start ? 1.f : 0.f); };
         for (int q = sb; q < se; ++q)
-            for (int n = lane; n < Npad; n += 32) __stcg(a0 + (size_t)q * Npad + n, first(q, n));
+            for (int n = lane; n < Npad; n += 32) {
+                const float v = first(q, n);
+                __stcg(a0 + (size_t)q * Npad + n, v);
+                if (own_smem) s_own[(size_t)(q - tile_s0) * Npad + n] = v;   // (read by other lanes after the grid barrier)
+            }
         int vj = vj0;
         for (int q = sb; q < se; ++q) {
             if (__ldg(P.state_pos + q) == 0) {   // q, q+1 are a pair
@@ -766,16 +797,21 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
 #pragma unroll
             for (int u = 0; u < U; ++u) { r[u] = 1.f; fm[u] = 0.f; ypre0[u] = 0.f; ypre1[u] = 0.f; ec0[u] = 0.f; ec1[u] = 0.f; sum[u] = 0.f; }
             // own-row terms (den_graph.h DenPlan::own_rows): the previous frame's rows of the NEXT group to end (rows `row`,
-            // `row + 1`: this warp wrote them one frame ago) and their coefficients, fetched one group ahead of use
+            // `row + 1`: this warp wrote them one frame ago) and their coefficients, fetched one group ahead of use -- from
+            // shared memory with own_smem, where the lane's own values are always read before they are overwritten
             const bool own = P.own != 0;
             const char *const x_base = reinterpret_cast<const char *>(a_prev + n0);
+            const uint32_t own_base = own_smem ? own_lane_base(s_own, n0, tile_s0, row_bytes) : 0u;
             Vec<U> xa = vec_zero<U>(), xb = vec_zero<U>();
             float2 c01 = make_float2(0.f, 0.f), c23 = make_float2(0.f, 0.f);
             auto own_prefetch = [&](uint32_t row) {
                 if (!own || (int)row >= se) return;
                 c01 = __ldg(reinterpret_cast<const float2 *>(P.own_c) + row);
                 c23 = __ldg(reinterpret_cast<const float2 *>(P.own_c) + row + 1);
-                if (SMALL || lane_act) {
+                if (own_smem && lane_act) {
+                    xa = lds_row<U>(own_base + row * row_bytes);
+                    if ((int)row + 1 < se) xb = lds_row<U>(own_base + (row + 1u) * row_bytes);
+                } else if (SMALL || lane_act) {
                     xa = gather_row<U>(x_base, row * row_bytes);
                     if ((int)row + 1 < se) xb = gather_row<U>(x_base, (row + 1u) * row_bytes);
                 }
@@ -836,6 +872,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
                         o0.stcg(row_ptr<U>(out_base, out_row, row_bytes));
                         o1.stcg(row_ptr<U>(out_base, out_row + 1u, row_bytes));
                         ov.stcg(row_ptr<U>(out_base, virt_row, row_bytes));
+                        if (own_smem) { sts_row<U>(own_base + out_row * row_bytes, o0); sts_row<U>(own_base + (out_row + 1u) * row_bytes, o1); }
                     }
                     ++virt_row;
                     out_row += 2u;
@@ -876,7 +913,10 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
                     sum[u] += out.v[u];
                     acc[u] = 0.f;
                 }
-                if ((SMALL || lane_act) && sub == 0) out.stcg(row_ptr<U>(out_base, out_row, row_bytes));
+                if ((SMALL || lane_act) && sub == 0) {
+                    out.stcg(row_ptr<U>(out_base, out_row, row_bytes));
+                    if (own_smem) sts_row<U>(own_base + out_row * row_bytes, out);
+                }
                 if (ev == kEvRowPos0) cacc = out;
                 else if (ev == kEvRowPos1) {   // the pair's virtual row: what the next frame gathers instead of both
 #pragma unroll
@@ -974,9 +1014,11 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_forward_kernel(const __gri
 // Rows are gathered into registers (walk_arcs_dual) except in two TMA variants: SMALL, the small-batch variant
 // (walk_arcs_tma_small, 16 lanes per row, arc tile in shared memory, one utterance per lane), and STREAM, the streamed-arc
 // tier (walk_arcs_tma_stream, full-width rows, arcs flowing through per-warp rings).
-template <int U, int BATCH, bool SMEM_ARCS, bool W1_SMEM = SMEM_ARCS, bool SMALL = false, bool STREAM = false>
+// OWN_SMEM: own rows on chip, as in den_forward_kernel.
+template <int U, int BATCH, bool SMEM_ARCS, bool W1_SMEM = SMEM_ARCS, bool SMALL = false, bool STREAM = false, bool OWN_SMEM = false>
 __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __grid_constant__ DenParams P) {
     constexpr bool TMA = SMALL || STREAM;
+    static_assert(!OWN_SMEM || !TMA, "own rows on chip: register gathers");
     constexpr int LPR = SMALL ? kSmallLanes : 32;   // lanes per row
     static_assert(!SMALL || (SMEM_ARCS && U == 1), "small-batch variant: arc tile in shared memory, one utterance per lane");
     static_assert(!STREAM || (!SMEM_ARCS && !SMALL), "streamed arcs: not resident, full-width rows");
@@ -987,6 +1029,9 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
     int *s_label = reinterpret_cast<int *>(s_gacc + (size_t)P.gacc_rows * Npad);   // [tile_rows]
     float *s_final = reinterpret_cast<float *>(s_label + P.tile_rows);             // [tile_rows]
     Arc *s_arcs = reinterpret_cast<Arc *>(smem_raw + BwdArcsOff(Npad, P.gacc_rows, P.tile_rows));
+    // own rows on chip: the tile's beta-hat rows of the next frame, as in den_forward_kernel
+    constexpr bool own_smem = OWN_SMEM;
+    float *const s_own = reinterpret_cast<float *>(smem_raw + P.own_off);
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(kFull, tid >> 5, 0);   // (through a shuffle: lets ptxas keep warp-derived addresses in uniform registers)
@@ -1073,6 +1118,14 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
     // segmented backward pass (checkpointed alpha): beta-hat, colsum_b and absum carry over in global memory, the
     // log-scale books through runlog_b
     if (P.t_hi < P.Tmax && cta == 0 && tid < P.N) runlog = P.runlog_b[tid];
+    if (own_smem) {
+        // the rows the first frame reads: frame t_hi + 1 as the previous segment launch left it, or zeros at Tmax + 1 (read
+        // only for utterances of length Tmax, whose first backward frame takes the final weights and discards the sums)
+        const float *src = P.bh + (size_t)((P.t_hi + 1) & 1) * frame_elems;
+        for (int q = sb; q < se; ++q)
+            for (int n = lane; n < Npad; n += 32)
+                s_own[(size_t)(q - tile_s0) * Npad + n] = P.t_hi < P.Tmax ? __ldcg(src + (size_t)q * Npad + n) : 0.f;
+    }
     __syncthreads();
 
     for (int tau = P.t_hi; tau > P.t_lo; --tau) {
@@ -1129,13 +1182,17 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
             // wrote them one frame ago) and their coefficients, fetched one group ahead like the alpha rows
             const bool own = P.own != 0;
             const char *const b_base = reinterpret_cast<const char *>(bh_next + n0);
+            const uint32_t own_base = own_smem ? own_lane_base(s_own, n0, tile_s0, row_bytes) : 0u;
             Vec<U> xa = vec_zero<U>(), xb = vec_zero<U>();
             float2 c01 = make_float2(0.f, 0.f), c23 = make_float2(0.f, 0.f);
             auto own_prefetch = [&](uint32_t row) {
                 if (!own || (int)row >= se) return;
                 c01 = __ldg(reinterpret_cast<const float2 *>(P.own_c) + row);
                 c23 = __ldg(reinterpret_cast<const float2 *>(P.own_c) + row + 1);
-                if (TMA || lane_act) {
+                if (own_smem && lane_act) {
+                    xa = lds_row<U>(own_base + row * row_bytes);
+                    if ((int)row + 1 < se) xb = lds_row<U>(own_base + (row + 1u) * row_bytes);
+                } else if (TMA || lane_act) {
                     xa = gather_row<U>(b_base, row * row_bytes);
                     if ((int)row + 1 < se) xb = gather_row<U>(b_base, (row + 1u) * row_bytes);
                 }
@@ -1181,7 +1238,10 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
                     sum_b[u] += out.v[u];
                     acc[u] = 0.f;
                 }
-                if ((TMA || lane_act) && sub == 0) out.stcg(row_ptr<U>(out_base, out_row, row_bytes));   // (TMA: every lane reads the row later)
+                if ((TMA || lane_act) && sub == 0) {   // (TMA: every lane reads the row later)
+                    out.stcg(row_ptr<U>(out_base, out_row, row_bytes));
+                    if (own_smem) sts_row<U>(own_base + out_row * row_bytes, out);
+                }
                 ++out_row;
                 ++ql;
             };
@@ -1395,14 +1455,22 @@ bool EncodeRowTensorMap(CUtensorMap *tm, const float *base, size_t rows, int Npa
 template <int U>
 const void *ForwardKernel(const DenLaunch &L, bool hubs) {
     constexpr int B = FwdBatch(U);
+    if (L.own_smem)   // (plans with own-row terms have no hub rows)
+        return L.tier == kTierShared ? (const void *)den_forward_kernel<U, B, true, false, false, true>
+                                     : (const void *)den_forward_kernel<U, B, false, false, false, true>;
     if (L.tier == kTierShared) return hubs ? (const void *)den_forward_kernel<U, B, true, true> : (const void *)den_forward_kernel<U, B, true, false>;
     return hubs ? (const void *)den_forward_kernel<U, B, false, true> : (const void *)den_forward_kernel<U, B, false, false>;
+}
+template <int U, bool OWN_SMEM>
+const void *RegisterBackwardKernel(const DenLaunch &L) {
+    if (L.tier == kTierGlobal) return (const void *)den_backward_kernel<U, kBwdBatch, false, false, false, false, OWN_SMEM>;
+    return L.w1_smem ? (const void *)den_backward_kernel<U, kBwdBatch, true, true, false, false, OWN_SMEM>
+                     : (const void *)den_backward_kernel<U, kBwdBatch, true, false, false, false, OWN_SMEM>;
 }
 template <int U>
 const void *BackwardKernel(const DenLaunch &L) {
     if (L.tier == kTierStreamed) return (const void *)den_backward_kernel<U, kStreamRows, false, true, false, true>;
-    if (L.tier == kTierGlobal) return (const void *)den_backward_kernel<U, kBwdBatch, false>;
-    return L.w1_smem ? (const void *)den_backward_kernel<U, kBwdBatch, true, true> : (const void *)den_backward_kernel<U, kBwdBatch, true, false>;
+    return L.own_smem ? RegisterBackwardKernel<U, true>(L) : RegisterBackwardKernel<U, false>(L);
 }
 const void *DenKernel(bool backward, const DenLaunch &L, bool hubs) {
     if (L.tier == kTierSmall)
@@ -1486,6 +1554,7 @@ int LaunchDen(bool backward, const DeviceGraph &g, DenParams &p, cudaStream_t st
     p.tq = L.tier == kTierStreamed ? pass.tq : nullptr;
     p.tile_rows = L.tile_rows; p.gacc_rows = L.gacc_rows;
     p.ring_off = (int)L.ring_off; p.bar_off = (int)L.bar_off; p.abar_off = (int)L.abar_off; p.aring_off = (int)L.aring_off;
+    p.own_off = L.own_smem ? (int)L.own_off : 0;
     return LaunchCoop(DenKernel(backward, L, g.shape.n_hubs > 0), p, g.n_ctas, L.total, stream, err);
 }
 

@@ -39,10 +39,11 @@ CCB_HD inline size_t BwdArcsOff(int Npad, int gacc_rows, int tile_rows) {
 CCB_HD inline uint32_t SmallW1Off(uint32_t bar_off, int n_warps) { return bar_off + (uint32_t)n_warps * kSmallBarWarpBytes; }
 
 struct DenPassShape { int max_tile_arcs = 0, max_tile_rows = 0, max_tile_labels = 0; };
-// streamed_quads: the backward quads also exist in the streamed-arc form (DevicePass::tq)
-struct DenGraphShape { DenPassShape fwd, bwd; int n_hubs = 0, n_warps = 0; bool streamed_quads = false; };
-// test hooks CCB_ARCS_IN_GLOBAL, CCB_W1_IN_GLOBAL (force the large-graph tiers) and CCB_NO_TMA (register gathers everywhere)
-struct DenHooks { bool arcs_in_global = false, w1_in_global = false, no_tma = false; };
+// streamed_quads: the backward quads also exist in the streamed-arc form (DevicePass::tq); own_rows: DenPlan::own_rows
+struct DenGraphShape { DenPassShape fwd, bwd; int n_hubs = 0, n_warps = 0; bool streamed_quads = false, own_rows = false; };
+// test hooks CCB_ARCS_IN_GLOBAL, CCB_W1_IN_GLOBAL (force the large-graph tiers), CCB_NO_TMA (register gathers everywhere) and
+// CCB_OWN_IN_L2 (own rows re-read from L2, not kept on chip)
+struct DenHooks { bool arcs_in_global = false, w1_in_global = false, no_tma = false, own_in_l2 = false; };
 
 // Arcs resident in shared memory or read from L2 with rows gathered into registers; backward only, arcs streamed through
 // bulk-copy rings with rows staged by TMA; Npad = 16, arcs resident and 16-float rows staged by bulk copies.
@@ -51,8 +52,11 @@ struct DenLaunch {
     int tier = kTierShared, lanes_per_row = 32, U = 1, batch = 0;   // U: utterances per lane; batch: gathers (rows) per batch
     bool w1_smem = false;   // backward: second weights resident with the arc tile (12 bytes per slot, else 8)
     int tile_rows = 0, gacc_rows = 0;
+    // register tiers of a plan with own-row terms: the CTA tile's own rows of the last frame, [tile_rows][Npad] floats at
+    // own_off, so that a warp reads back the rows it wrote itself from shared memory instead of L2
+    bool own_smem = false;
     // dynamic shared memory in bytes from its base (0: a region the tier does not have)
-    size_t arcs_off = 0, ring_off = 0, bar_off = 0, w1_off = 0, abar_off = 0, aring_off = 0, total = 0;
+    size_t arcs_off = 0, ring_off = 0, bar_off = 0, w1_off = 0, abar_off = 0, aring_off = 0, own_off = 0, total = 0;
 };
 
 // The launch of one pass at lane padding Npad with smem_optin bytes of shared memory per block; false, why, if none runs it.

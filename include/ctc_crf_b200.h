@@ -261,10 +261,13 @@ int ccb_plan_info(void *plan, long *info);
  *        13 fwd_cta_labels[n_ctas*4] i32, 14 bwd_cta_labels, 15 bwd second weights f32[A_bwd], 16 hub_states[n_hubs] i32 */
 int ccb_plan_copy(void *plan, int which, void *dst, size_t dst_bytes);
 /* The den kernel launch chosen for one pass (backward 0 / 1) of N utterances at smem_optin bytes of shared memory per block;
- * hooks: bit 0 CCB_ARCS_IN_GLOBAL, 1 CCB_W1_IN_GLOBAL, 2 CCB_NO_TMA.  out[0..14] = tier (0 arcs in shared memory, 1 from L2,
- * 2 streamed, 3 small batch), lanes per row, U, batch, w1_smem, Npad, tile_rows, gacc_rows and the shared-memory offsets
- * arcs, ring, bar, w1, abar, aring, total (den_launch.h DenLaunch).  Non-zero: no kernel runs the pass. */
+ * hooks: bit 0 CCB_ARCS_IN_GLOBAL, 1 CCB_W1_IN_GLOBAL, 2 CCB_NO_TMA, 3 CCB_OWN_IN_L2.  out[0..14] = tier (0 arcs in shared
+ * memory, 1 from L2, 2 streamed, 3 small batch), lanes per row, U, batch, w1_smem, Npad, tile_rows, gacc_rows and the
+ * shared-memory offsets arcs, ring, bar, w1, abar, aring, total (den_launch.h DenLaunch).  Non-zero: no kernel runs the pass. */
 int ccb_plan_launch(void *plan, int N, int backward, int smem_optin, int hooks, long *out);
+/* The same launch's own rows: out[0] = 1 if the pass keeps each warp's own rows of the last frame in shared memory (0: it
+ * re-reads them from L2), out[1] = their byte offset in dynamic shared memory ([tile_rows][Npad] floats, up to total). */
+int ccb_plan_launch_own(void *plan, int N, int backward, int smem_optin, int hooks, long *out);
 
 #ifdef __cplusplus
 }
