@@ -10,7 +10,9 @@ ignored (binding.cpp:105,111) or exiting the process (den_calculate.cu:16-25).
 Addition: ``ctc_crf_loss_fwd`` -- the fused, synchronisation-free entry used by ``CTC_CRF_LOSS``; ``ctc_crf_loss_fwd_only``
 and ``ctc_loss_fwd_only`` -- the losses without a gradient, used when grad mode is off.  Every loss function takes
 ``reduction`` (None: the scalar of ``size_average``; 'none': one cost per utterance) and ``zero_infinity``;
-``grad_rows_scale`` is the backward of the per-utterance costs.
+``grad_rows_scale`` is the backward of the per-utterance costs.  ``ctc_crf_loss_seqs``, ``ctc_crf_loss_seqs_fwd_only``,
+``ctc_loss_seqs`` and ``ctc_align_seqs`` take several label sequences per utterance (``utt``: the logits row of each), with the
+den passes run once per utterance; ``seqs_backward`` is the backward of their per-sequence costs.
 """
 from __future__ import annotations
 
@@ -225,18 +227,30 @@ def ckpt_interval(tmax: int) -> int:
     return max(1, math.isqrt(max(1, tmax) - 1) + 1)
 
 
-def _slice_need(L, n, tmax, maxl, k):
+def _slice_need(L, n, tmax, maxl, k, m=None):
+    """Scratch bytes of a slice of n utterances; m: its label sequences when they are not one per utterance."""
     alpha = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
-    return int(alpha) * 4 + int(L.ccb_den_aux_bytes(n, tmax)) + int(L.ccb_ctc_workspace_bytes(n, tmax, maxl))
+    return (int(alpha) * 4 + int(L.ccb_den_aux_bytes(n, tmax))
+            + int(L.ccb_ctc_workspace_bytes(n if m is None else m, tmax, maxl)))
 
 
-def _plan_slices(L, lx, ly, N, V, dev):
+def _slice_seqs(ly, n0, n1, seq_off):
+    """(label sequences, longest one) of utterances [n0, n1): one per utterance (seq_off None), or those of a grouping."""
+    if seq_off is None:
+        return n1 - n0, int(ly[n0:n1].max())
+    s0, s1 = int(seq_off[n0]), int(seq_off[n1])
+    return s1 - s0, int(ly[s0:s1].max()) if s1 > s0 else 0
+
+
+def _plan_slices(L, lx, ly, N, V, dev, seq_off=None):
     """Split the batch into contiguous slices whose scratch (alpha spill etc.) fits the free device memory.
     Each slice walks only max(lx[slice]) frames.  Returns (n0, n1, tmax, maxl, K) per slice; K = 0 keeps every alpha
     frame, K > 0 keeps every K-th and recomputes the rest in the backward pass.
     A slice whose full alpha spill does not fit is halved while it is wider than CKPT_WIDTH and halving shrinks its lane
     padding (the spill is proportional to the padding); otherwise it runs checkpointed with K = ceil(sqrt(tmax)), and is
-    halved further only if that does not fit either."""
+    halved further only if that does not fit either.
+    seq_off (N+1,): several label sequences per utterance -- ly holds their lengths grouped by utterance, those of utterance
+    n at seq_off[n] .. seq_off[n+1]-1, and a slice's numerator workspace is sized by its sequences."""
     budget = _scratch_budget(dev)
     slices, n0 = [], 0
     while n0 < N:
@@ -245,9 +259,9 @@ def _plan_slices(L, lx, ly, N, V, dev):
             n = n1 - n0
             half = max(1, n // 2)
             tmax = max(1, int(lx[n0:n1].max()))
-            maxl = int(ly[n0:n1].max())
+            m, maxl = _slice_seqs(ly, n0, n1, seq_off)
             k = 0 if _ckpt_k_override is None else int(_ckpt_k_override)
-            need = _slice_need(L, n, tmax, maxl, k)
+            need = _slice_need(L, n, tmax, maxl, k, m)
             if need > budget:
                 budget = _scratch_budget(dev, need)     # a stale (cached) figure must not split a batch needlessly
             if need <= budget:
@@ -258,7 +272,7 @@ def _plan_slices(L, lx, ly, N, V, dev):
                 continue
             if k == 0:
                 k = ckpt_interval(tmax)
-                need = _slice_need(L, n, tmax, maxl, k)
+                need = _slice_need(L, n, tmax, maxl, k, m)
                 if need > budget:
                     budget = _scratch_budget(dev, need)
                 if need <= budget:
@@ -350,28 +364,30 @@ def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tenso
     return (costs if per_utt else loss), grad, parts
 
 
-def _fwd_only_need(L, n, tmax):
+def _fwd_only_need(L, n, tmax, m=None):
     return (int(L.ccb_den_fwd_alpha_floats(n)) * 4 + int(L.ccb_den_aux_bytes(n, tmax))
-            + int(L.ccb_num_fwd_only_bytes(n)))
+            + int(L.ccb_num_fwd_only_bytes(n if m is None else m)))
 
 
-def _plan_fwd_only_slices(L, lx, ly, N, dev):
+def _plan_fwd_only_slices(L, lx, ly, N, dev, seq_off=None):
     """Slices of the forward-only loss: contiguous runs of at most MAX_UTTS_PER_CALL utterances, each walking its own
     max(lx).  Its alpha is a ring of a few frames whose size does not depend on the length, so a slice is never halved or
-    checkpointed; one whose scratch does not fit the free device memory is an error.  Returns (n0, n1, tmax, maxl)."""
+    checkpointed; one whose scratch does not fit the free device memory is an error.  Returns (n0, n1, tmax, maxl).
+    seq_off: as for _plan_slices."""
     budget = _scratch_budget(dev)
     slices = []
     for n0 in range(0, N, MAX_UTTS_PER_CALL):
         n1 = min(N, n0 + MAX_UTTS_PER_CALL)
         tmax = max(1, int(lx[n0:n1].max()))
-        need = _fwd_only_need(L, n1 - n0, tmax)
+        m, maxl = _slice_seqs(ly, n0, n1, seq_off)
+        need = _fwd_only_need(L, n1 - n0, tmax, m)
         if need > budget:
             budget = _scratch_budget(dev, need)
         if need > budget:
             raise RuntimeError(f"forward-only CTC-CRF scratch for {n1 - n0} utterances of up to {tmax} frames needs "
                                f"{need >> 20} MiB (alpha ring {int(L.ccb_den_fwd_alpha_floats(n1 - n0)) * 4 >> 20} MiB), "
                                f"only {budget >> 20} MiB free")
-        slices.append((n0, n1, tmax, int(ly[n0:n1].max())))
+        slices.append((n0, n1, tmax, maxl))
     return slices
 
 
@@ -554,6 +570,287 @@ def grad_rows_scale(grad: torch.Tensor, w: torch.Tensor, lx: torch.Tensor, dtype
         _check(rc, "grad_rows_scale")
         lens.record_stream(torch.cuda.current_stream(dev))
     return out
+
+
+# ---------------------------------------------------------------------------------------------------
+# several label sequences per utterance (utt=)
+# ---------------------------------------------------------------------------------------------------
+class SeqGroups:
+    """M label sequences grouped by the logits row they are scored against, in the caller's order within a row.
+    pos[j]: the caller's index of grouped sequence j; row[j]: its logits row; labels / ly: the grouped sequences;
+    off (N+1,) int64: the sequences of row n are off[n] .. off[n+1]-1."""
+
+    def __init__(self, pos, row, labels, ly, off):
+        self.pos, self.row, self.labels, self.ly, self.off = pos, row, labels, ly, off
+        self.M = int(pos.numel())
+
+
+def group_seqs(utt: torch.Tensor, labels: torch.Tensor, ly: torch.Tensor, N: int) -> SeqGroups:
+    """Check `utt` ((M,) int32 CPU, entries in [0, N), one per label sequence of `ly`) and group the sequences by row with a
+    stable sort.  Host work only: the labels are on the CPU already."""
+    if not isinstance(utt, torch.Tensor) or utt.dtype != torch.int32 or utt.is_cuda or utt.dim() != 1:
+        what = f"{utt.dtype} {utt.device} of shape {tuple(utt.shape)}" if isinstance(utt, torch.Tensor) else type(utt).__name__
+        raise RuntimeError(f"utt must be a 1-D int32 CPU tensor (the logits row of each label sequence), not {what}")
+    M = int(utt.numel())
+    if int(ly.numel()) != M:
+        raise RuntimeError(f"utt has {M} entries but ly has {int(ly.numel())}: both need one entry per label sequence")
+    if M == 0:
+        raise RuntimeError("utt names no label sequence")
+    if int(utt.min()) < 0 or int(utt.max()) >= N:
+        raise RuntimeError(f"utt entries must lie in [0, N) = [0, {N}): they name logits rows")
+    if int(ly.min()) < 0:
+        raise RuntimeError("label lengths must be non-negative")
+    u = utt.to(torch.int64)
+    pos = torch.sort(u, stable=True).indices
+    ly64 = ly.to(torch.int64)
+    total = int(ly64.sum())
+    if total != int(labels.numel()):
+        raise RuntimeError(f"labels has {labels.numel()} entries but label lengths sum to {total}")
+    gly = ly64[pos]
+    src = (torch.cumsum(ly64, 0) - ly64)[pos]          # where each grouped sequence starts in the caller's labels
+    dst = torch.cumsum(gly, 0) - gly                   # ... and in the grouped labels
+    idx = torch.repeat_interleave(src - dst, gly, output_size=total) + torch.arange(total)
+    off = torch.zeros(N + 1, dtype=torch.int64)
+    off[1:] = torch.cumsum(torch.bincount(u, minlength=N), 0)
+    return SeqGroups(pos.to(torch.int32), u[pos].to(torch.int32), labels.reshape(-1)[idx].to(torch.int32),
+                     gly.to(torch.int32), off)
+
+
+def _check_seq_args(logits, labels, lx, ly, utt):
+    assert logits.is_cuda and logits.dim() == 3 and logits.is_contiguous()
+    if logits.dtype not in _DTYPES:
+        raise RuntimeError(f"unsupported logits dtype {logits.dtype}")
+    N, T, V = logits.shape
+    if N == 0:
+        raise RuntimeError("empty batch")
+    if int(lx.numel()) != N:
+        raise RuntimeError("lx must have one entry per utterance (logits row)")
+    if int(lx.max()) > T or int(lx.min()) < 0:
+        raise RuntimeError("input lengths must lie in [0, T]")
+    if labels.numel() and (int(labels.min()) < 0 or int(labels.max()) >= V):
+        raise RuntimeError("label out of range")
+    return N, T, V, group_seqs(utt, labels, ly, N)
+
+
+class _SeqMeta:
+    """Device addresses of the int32 meta block of a grouped call:
+    [labels | label_off (M+1) | ly (M) | lx (N) | row (M) | pos (M) | seq_off, (n1-n0+1) entries per slice]
+    row and seq_off are relative to the slice that holds the sequence (its logits pointer and first sequence); pos is the
+    caller's index.  Slice i of utterances [n0, n1) finds its offsets at seq_off + n0 + i."""
+
+    def __init__(self, grp: SeqGroups, lx: torch.Tensor, bounds, device):
+        N = int(lx.numel())
+        M = grp.M
+        label_off = torch.zeros(M + 1, dtype=torch.int32)
+        label_off[1:].copy_(torch.cumsum(grp.ly.to(torch.int64), 0))
+        first = torch.empty(N, dtype=torch.int64)            # first utterance of the slice of each utterance
+        offs = []
+        for n0, n1 in bounds:
+            first[n0:n1] = n0
+            offs.append(grp.off[n0:n1 + 1] - grp.off[n0])
+        row = (grp.row.to(torch.int64) - first[grp.row.to(torch.int64)]).to(torch.int32)
+        parts = [grp.labels, label_off, grp.ly, lx.to(torch.int32), row, grp.pos, torch.cat(offs).to(torch.int32)]
+        ring = _rings.setdefault(torch.device(device).index, _PinnedRing())
+        self.buf = ring.stage(parts, device)
+        base = self.buf.data_ptr()
+        sizes = [int(p.numel()) for p in parts]
+        ptrs = [base]
+        for s in sizes[:-1]:
+            ptrs.append(ptrs[-1] + 4 * s)
+        self.labels, self.label_off, self.ly, self.lx, self.row, self.pos, self.seq_off = ptrs
+
+    def slice_args(self, i, n0, s0):
+        """(labels, label_off, label_len, len, row, pos, seq_off) of slice i, utterances from n0, sequences from s0."""
+        return (self.labels, self.label_off + 4 * s0, self.ly + 4 * s0, self.lx + 4 * n0, self.row + 4 * s0,
+                self.pos + 4 * s0, self.seq_off + 4 * (n0 + i))
+
+
+class SeqsGradState:
+    """What the backward of a grouped call with reduction 'none' needs: the logits, the meta block, and per slice the numerator
+    cells (and the den aux block) of the forward call, plus the unscaled den occupancies `den` (None for CTC)."""
+
+    def __init__(self, logits, meta, slices, den, from_logits, zero_infinity, num_coef, blank, M):
+        self.logits, self.meta, self.slices, self.den = logits, meta, slices, den
+        self.from_logits, self.zero_infinity, self.num_coef, self.blank, self.M = from_logits, zero_infinity, num_coef, blank, M
+
+
+def ctc_crf_loss_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, utt: torch.Tensor,
+                      lamb: float, size_average: bool, from_logits: bool = False, reduction: Optional[str] = None,
+                      zero_infinity: bool = False) -> Tuple[torch.Tensor, torch.Tensor, Optional[SeqsGradState]]:
+    """``ctc_crf_loss_fwd`` for M label sequences, sequence m scored against logits row utt[m]: labels / ly describe the M
+    sequences, lx stays (N,).  The den passes run once per utterance, every numerator of a slice in one launch.
+    cost[m] = logZ_den[utt[m]] - (1+lamb) log p_ctc[m]; reduction None: the sum over the sequences (/ M with size_average) and
+    grad = its gradient.  reduction 'none': the (M,) costs in the caller's order; grad then holds the unscaled den occupancies
+    and the third result is the state ``seqs_backward`` turns into the gradient for given per-sequence weights."""
+    check_reduction(reduction)
+    per_seq = reduction == "none"
+    L = _lib.lib()
+    N, T, V, grp = _check_seq_args(logits, labels, lx, ly, utt)
+    M = grp.M
+    dev = logits.device
+    esz = logits.element_size()
+    scale = 1.0 if per_seq else 1.0 / M if size_average else 1.0
+    with torch.cuda.device(dev):
+        grad = torch.empty((N, T, V), dtype=torch.float32, device=dev)
+        costs = torch.empty(M, dtype=torch.float32, device=dev) if per_seq else None
+        stream = _stream(dev)
+
+        def run_slices():
+            slices = _plan_slices(L, lx, grp.ly, N, V, dev, seq_off=grp.off)
+            meta = _SeqMeta(grp, lx, [(s[0], s[1]) for s in slices], dev)
+            losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
+            kept = []
+            for i, (n0, n1, tmax, maxl, k) in enumerate(slices):
+                n = n1 - n0
+                s0, m = int(grp.off[n0]), int(grp.off[n1] - grp.off[n0])
+                alpha_floats = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
+                alpha_ws = torch.empty(int(alpha_floats), dtype=torch.float32, device=dev)
+                aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
+                ctc_ws = torch.empty(int(L.ccb_ctc_workspace_bytes(m, tmax, maxl)), dtype=torch.uint8, device=dev)
+                lab, loff, lly, llx, row, pos, soff = meta.slice_args(i, n0, s0)
+                rc = L.ccb_ctc_crf_loss_seqs(logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype], int(from_logits),
+                                             n, T, V, tmax, k, lab, loff, lly, llx, m, row, pos, soff, maxl, float(lamb),
+                                             float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(), ctc_ws.data_ptr(),
+                                             grad.data_ptr() + n0 * T * V * 4, losses.data_ptr() + 4 * i,
+                                             costs.data_ptr() if per_seq else None, int(zero_infinity), int(per_seq), stream)
+                _check(rc, "ctc_crf_loss_seqs")
+                if per_seq:    # the backward reads this slice's numerator cells and den aux block (logZ, normalisers)
+                    kept.append((n0, n1, tmax, maxl, s0, m, i, aux_ws, ctc_ws))
+                del alpha_ws, aux_ws, ctc_ws
+            return slices, losses, meta, kept
+
+        try:
+            slices, losses, meta, kept = run_slices()
+        except torch.cuda.OutOfMemoryError:       # as in ctc_crf_loss_fwd
+            _budget_cache.pop(torch.device(dev).index, None)
+            torch.cuda.empty_cache()
+            slices, losses, meta, kept = run_slices()
+        loss = losses.sum().reshape(1) if len(slices) > 1 else losses
+        meta.buf.record_stream(torch.cuda.current_stream(dev))
+    state = (SeqsGradState(logits, meta, kept, grad, from_logits, zero_infinity, -(1.0 + float(lamb)), 0, M)
+             if per_seq else None)
+    return (costs if per_seq else loss), grad, state
+
+
+def ctc_crf_loss_seqs_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
+                               utt: torch.Tensor, lamb: float, size_average: bool, from_logits: bool = False,
+                               reduction: Optional[str] = None, zero_infinity: bool = False) -> torch.Tensor:
+    """The loss of ``ctc_crf_loss_seqs`` without a gradient (the passes of ``ctc_crf_loss_fwd_only``): the scalar, or the (M,)
+    costs with reduction 'none'."""
+    check_reduction(reduction)
+    per_seq = reduction == "none"
+    L = _lib.lib()
+    N, T, V, grp = _check_seq_args(logits, labels, lx, ly, utt)
+    M = grp.M
+    dev = logits.device
+    esz = logits.element_size()
+    scale = 1.0 if per_seq else 1.0 / M if size_average else 1.0
+    with torch.cuda.device(dev):
+        costs = torch.empty(M, dtype=torch.float32, device=dev) if per_seq else None
+        stream = _stream(dev)
+        slices = _plan_fwd_only_slices(L, lx, grp.ly, N, dev, seq_off=grp.off)
+        meta = _SeqMeta(grp, lx, [(s[0], s[1]) for s in slices], dev)
+        losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
+        for i, (n0, n1, tmax, maxl) in enumerate(slices):
+            n = n1 - n0
+            s0, m = int(grp.off[n0]), int(grp.off[n1] - grp.off[n0])
+            alpha_ws = torch.empty(int(L.ccb_den_fwd_alpha_floats(n)), dtype=torch.float32, device=dev)
+            aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
+            num_ws = torch.empty(max(4, int(L.ccb_num_fwd_only_bytes(m))), dtype=torch.uint8, device=dev)
+            lab, loff, lly, llx, row, pos, _ = meta.slice_args(i, n0, s0)
+            rc = L.ccb_ctc_crf_loss_seqs_fwd_only(logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype],
+                                                  int(from_logits), n, T, V, tmax, lab, loff, lly, llx, m, row, pos, maxl,
+                                                  float(lamb), float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(),
+                                                  num_ws.data_ptr(), losses.data_ptr() + 4 * i,
+                                                  costs.data_ptr() if per_seq else None, int(zero_infinity), stream)
+            _check(rc, "ctc_crf_loss_seqs_fwd_only")
+            del alpha_ws, aux_ws, num_ws
+        loss = losses.sum().reshape(1) if len(slices) > 1 else losses
+        meta.buf.record_stream(torch.cuda.current_stream(dev))
+    return costs if per_seq else loss
+
+
+def ctc_loss_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, utt: torch.Tensor,
+                  size_average: bool, blank: int = 0, reduction: Optional[str] = None, zero_infinity: bool = False,
+                  with_grad: bool = True) -> Tuple[torch.Tensor, Optional[torch.Tensor], Optional[SeqsGradState]]:
+    """``ctc_loss_fwd`` for M label sequences (sequence m on logits row utt[m]), every numerator in one launch: the loss
+    (reduction None: the sum over the sequences, / M with size_average; 'none': the (M,) costs -log p[m] in the caller's
+    order), then grad = d loss / d logits (None without with_grad, or with reduction 'none', whose gradient comes from
+    ``seqs_backward`` on the returned state)."""
+    check_reduction(reduction)
+    per_seq = reduction == "none"
+    defer = per_seq and with_grad
+    L = _lib.lib()
+    N, T, V, grp = _check_seq_args(logits, labels, lx, ly, utt)
+    M = grp.M
+    dev = logits.device
+    scale = 1.0 if per_seq else 1.0 / M if size_average else 1.0
+    with torch.cuda.device(dev):
+        meta = _SeqMeta(grp, lx, [(0, N)], dev)
+        tmax = max(1, int(lx.max()))
+        maxl = int(grp.ly.max())
+        grad = torch.empty((N, T, V), dtype=torch.float32, device=dev) if with_grad and not defer else None
+        ws = torch.empty(int(L.ccb_ctc_workspace_bytes(M, tmax, maxl)), dtype=torch.uint8, device=dev) if with_grad else None
+        loss = torch.empty(1, dtype=torch.float32, device=dev)
+        logp = torch.empty(M, dtype=torch.float32, device=dev)
+        costs = torch.empty(M, dtype=torch.float32, device=dev) if per_seq else None
+        lab, loff, lly, llx, row, pos, soff = meta.slice_args(0, 0, 0)
+        rc = L.ccb_ctc_loss_seqs(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, lab, loff, lly, llx, M, row, pos,
+                                 soff, maxl, int(blank), float(scale), ws.data_ptr() if ws is not None else None,
+                                 grad.data_ptr() if grad is not None else None, loss.data_ptr(), logp.data_ptr(),
+                                 costs.data_ptr() if per_seq else None, int(zero_infinity), int(defer), _stream(dev))
+        _check(rc, "ctc_loss_seqs")
+        meta.buf.record_stream(torch.cuda.current_stream(dev))
+    state = (SeqsGradState(logits, meta, [(0, N, tmax, maxl, 0, M, 0, None, ws)], None, False, zero_infinity, -1.0,
+                           int(blank), M) if defer else None)
+    return (costs if per_seq else loss), grad, state
+
+
+def seqs_backward(state: SeqsGradState, w: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """Backward of a grouped call with reduction 'none': the gradient of sum_m w[m] cost[m] with respect to the logits, in
+    `dtype`.  One pass per slice over the rows of its utterances: W_n * den + num_coef * sum_m w[m] gamma_m (then the
+    log_softmax Jacobian for from_logits); w (M,) in the caller's order."""
+    L = _lib.lib()
+    y = state.logits
+    N, T, V = y.shape
+    dev, esz = y.device, y.element_size()
+    meta = state.meta
+    with torch.cuda.device(dev):
+        w = w.to(device=dev, dtype=torch.float32).reshape(state.M).contiguous()
+        out = torch.empty((N, T, V), dtype=torch.float32, device=dev)
+        stream = _stream(dev)
+        for n0, n1, tmax, maxl, s0, m, i, aux_ws, ctc_ws in state.slices:
+            lab, loff, lly, llx, _, pos, soff = meta.slice_args(i, n0, s0)
+            rc = L.ccb_seqs_grad(y.data_ptr() + n0 * T * V * esz, _DTYPES[y.dtype], int(state.from_logits), n1 - n0, T, V,
+                                 tmax, lab, loff, lly, llx, m, pos, soff, maxl, state.blank, float(state.num_coef),
+                                 w.data_ptr(), state.den.data_ptr() + n0 * T * V * 4 if state.den is not None else None,
+                                 aux_ws.data_ptr() if aux_ws is not None else None, ctc_ws.data_ptr(),
+                                 int(state.zero_infinity), out.data_ptr() + n0 * T * V * 4, stream)
+            _check(rc, "seqs_backward")
+        meta.buf.record_stream(torch.cuda.current_stream(dev))
+    return out if dtype == torch.float32 else out.to(dtype)
+
+
+def ctc_align_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, utt: torch.Tensor,
+                   blank: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``ctc_align`` of M label sequences, sequence m aligned to logits row utt[m]: (align (M,T) int32, score (M,) fp32) in
+    the caller's order."""
+    L = _lib.lib()
+    N, T, V, grp = _check_seq_args(logits, labels, lx, ly, utt)
+    M = grp.M
+    dev = logits.device
+    with torch.cuda.device(dev):
+        meta = _SeqMeta(grp, lx, [(0, N)], dev)
+        maxl = int(grp.ly.max())
+        align = torch.empty((M, T), dtype=torch.int32, device=dev)
+        score = torch.empty(M, dtype=torch.float32, device=dev)
+        ws = torch.empty(int(L.ccb_ctc_align_workspace_bytes(M, T, maxl)), dtype=torch.uint8, device=dev)
+        lab, loff, lly, llx, row, pos, _ = meta.slice_args(0, 0, 0)
+        rc = L.ccb_ctc_align_seqs(logits.data_ptr(), _DTYPES[logits.dtype], T * V, V, N, T, V, lab, loff, lly, llx, M, row,
+                                  pos, maxl, int(blank), ws.data_ptr(), align.data_ptr(), score.data_ptr(), _stream(dev))
+        _check(rc, "ctc_align_seqs")
+        meta.buf.record_stream(torch.cuda.current_stream(dev))
+    return align, score
 
 
 def launch_count() -> int:

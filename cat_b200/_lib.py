@@ -28,6 +28,7 @@ SYMBOLS = [
     "ccb_den_ckpt_alpha_floats", "ccb_ctc_crf_loss_ckpt_fwd", "ccb_ctc_crf_loss_logits_ckpt_fwd",
     "ccb_den_fwd_alpha_floats", "ccb_num_fwd_only_bytes", "ccb_ctc_crf_loss_fwd_only", "ccb_ctc_loss_fwd_only",
     "ccb_ctc_crf_loss_costs", "ccb_ctc_crf_loss_costs_fwd_only", "ccb_ctc_loss_costs", "ccb_grad_rows_scale",
+    "ccb_ctc_crf_loss_seqs", "ccb_ctc_crf_loss_seqs_fwd_only", "ccb_ctc_loss_seqs", "ccb_seqs_grad", "ccb_ctc_align_seqs",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -103,6 +104,19 @@ def lib() -> C.CDLL:
     L.ccb_ctc_align.argtypes = [vp, C.c_int, C.c_long, C.c_long, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int,
                                 vp, vp, vp, vp]
     L.ccb_ctc_align.restype = C.c_int
+    i, f, l = C.c_int, C.c_float, C.c_long
+    L.ccb_ctc_crf_loss_seqs.argtypes = [vp, i, i, i, i, i, i, i, vp, vp, vp, vp, i, vp, vp, vp, i, f, f, vp, vp, vp, vp, vp,
+                                        vp, i, i, vp]
+    L.ccb_ctc_crf_loss_seqs.restype = C.c_int
+    L.ccb_ctc_crf_loss_seqs_fwd_only.argtypes = [vp, i, i, i, i, i, i, vp, vp, vp, vp, i, vp, vp, i, f, f, vp, vp, vp, vp,
+                                                 vp, i, vp]
+    L.ccb_ctc_crf_loss_seqs_fwd_only.restype = C.c_int
+    L.ccb_ctc_loss_seqs.argtypes = [vp, i, i, i, i, i, vp, vp, vp, vp, i, vp, vp, vp, i, i, f, vp, vp, vp, vp, vp, i, i, vp]
+    L.ccb_ctc_loss_seqs.restype = C.c_int
+    L.ccb_seqs_grad.argtypes = [vp, i, i, i, i, i, i, vp, vp, vp, vp, i, vp, vp, i, i, f, vp, vp, vp, vp, i, vp, vp]
+    L.ccb_seqs_grad.restype = C.c_int
+    L.ccb_ctc_align_seqs.argtypes = [vp, i, l, l, i, i, i, vp, vp, vp, vp, i, vp, vp, i, i, vp, vp, vp, vp]
+    L.ccb_ctc_align_seqs.restype = C.c_int
     L.ccb_launch_count.argtypes = []; L.ccb_launch_count.restype = C.c_long
     L.ccb_debug_timeline.argtypes = [vp, C.c_int, C.c_int]; L.ccb_debug_timeline.restype = None
     L.ccb_plan_create.argtypes = [C.c_char_p, C.c_int, C.c_int]; L.ccb_plan_create.restype = vp

@@ -735,6 +735,173 @@ int ccb_ctc_loss_fwd_only(const void *logits, int dtype, int N, int T, int V, in
                        max_label_len, blank, scale, nullptr, nullptr, loss, logp, nullptr, 0, stream);
 }
 
+/* ---- several label sequences per utterance ------------------------------------------------------ */
+static int CheckSeqMap(const char *what, int M, const int *seq_row, const int *seq_pos) {
+    // M = 0 is a slice of utterances without sequences: their gradient rows are zeros, their share of the loss 0
+    if (M < 0 || (M > 0 && (!seq_row || !seq_pos))) return Fail(std::string(what) + ": bad sequence map");
+    return 0;
+}
+
+// the numerator's log-likelihoods of M sequences, behind their cells in the numerator workspace (as in LossFwdImpl)
+static float *SeqLogp(void *ctc_ws, int M, int Tmax, int max_label_len) {
+    return reinterpret_cast<float *>(reinterpret_cast<double *>(ctc_ws) +
+                                     (size_t)M * (2 * (size_t)Tmax * (2 * (size_t)max_label_len + 1) + 1) + 32);
+}
+
+int ccb_ctc_crf_loss_seqs(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax, int ckpt_k,
+                          const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                          int M, const int *seq_row_dev, const int *seq_pos_dev, const int *seq_off_dev, int max_label_len,
+                          float lamb, float scale, float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss,
+                          float *costs, int zero_inf, int defer_num, void *stream) {
+    g_err.clear();
+    const bool raw = from_logits != 0;
+    DeviceGraph *g;
+    if (CurrentGraph(&g)) return 1;
+    if (Tmax <= 0 || Tmax > T) return Fail("ctc_crf_loss_seqs: Tmax must lie in [1, T]");
+    if (ckpt_k < 0) return Fail("ctc_crf_loss_seqs: checkpoint interval must be >= 0");
+    if (CheckSeqMap("ctc_crf_loss_seqs", M, seq_row_dev, seq_pos_dev) || CheckDen(*g, dtype, N, Tmax, V)) return 1;
+    if (!alpha_ws || !aux_ws || !ctc_ws || !grad || !loss || !seq_off_dev) return Fail("ctc_crf_loss_seqs: missing buffer");
+    cudaStream_t s = (cudaStream_t)stream;
+    const long sn = (long)T * V, st = V;
+    const DenAuxLayout L = MakeDenAuxLayout(g->S, N, Tmax, g->small_ok);
+    float *logz = reinterpret_cast<float *>((char *)aux_ws + L.logz_a);
+    float *logp = SeqLogp(ctc_ws, M, Tmax, max_label_len);
+    const double *lnorm = raw ? reinterpret_cast<const double *>((char *)aux_ws + L.lnorm) : nullptr;
+    // the den passes run once per utterance and leave its occupancies UNSCALED in grad; the gamma pass scales them by the
+    // weight of the utterance's sequences
+    CCB_CUDA(cudaMemsetAsync(grad, 0, sizeof(float) * (size_t)N * T * V, s));
+    if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw, ckpt_k)) return 1;
+    if (DenBackward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, grad, sn, st, 1.f, s, raw, ckpt_k)) return 1;
+    std::string err;
+    int rc = LaunchCtcSeqs(logits, dtype, sn, st, M, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev, seq_row_dev,
+                           max_label_len, 0, reinterpret_cast<float *>(ctc_ws), true, logp, lnorm, s, &err);
+    if (rc) return Fail(err);
+    if (!defer_num) {
+        rc = LaunchCtcGammaSeqs(logits, dtype, sn, st, N, Tmax, T, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+                                seq_off_dev, seq_pos_dev, max_label_len, 0, reinterpret_cast<float *>(ctc_ws), nullptr, scale,
+                                -(1.f + lamb), grad, logz, zero_inf, grad, sn, st, s, &err);
+        if (rc) return Fail(err);
+        if (raw) {
+            rc = LaunchLogitGrad(logits, dtype, sn, st, N, Tmax, V, len_dev,
+                                 reinterpret_cast<const float *>((char *)aux_ws + L.lz), L.Npad, grad, sn, st, s);
+            if (rc) return FailCuda("logit_grad", (cudaError_t)rc);
+        }
+    }
+    rc = LaunchSeqCosts(logz, logp, seq_row_dev, seq_pos_dev, M, lamb, scale, loss, costs, zero_inf, s);
+    if (rc) return FailCuda("seq_costs", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_ctc_crf_loss_seqs_fwd_only(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax,
+                                   const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                                   const int *len_dev, int M, const int *seq_row_dev, const int *seq_pos_dev,
+                                   int max_label_len, float lamb, float scale, float *alpha_ws, void *aux_ws, void *num_ws,
+                                   float *loss, float *costs, int zero_inf, void *stream) {
+    g_err.clear();
+    const bool raw = from_logits != 0;
+    DeviceGraph *g;
+    if (CurrentGraph(&g)) return 1;
+    if (Tmax <= 0 || Tmax > T) return Fail("ctc_crf_loss_seqs_fwd_only: Tmax must lie in [1, T]");
+    if (CheckSeqMap("ctc_crf_loss_seqs_fwd_only", M, seq_row_dev, seq_pos_dev) || CheckDen(*g, dtype, N, Tmax, V)) return 1;
+    if (!alpha_ws || !aux_ws || !num_ws || !loss) return Fail("ctc_crf_loss_seqs_fwd_only: missing buffer");
+    cudaStream_t s = (cudaStream_t)stream;
+    const long sn = (long)T * V, st = V;
+    const DenAuxLayout L = MakeDenAuxLayout(g->S, N, Tmax, g->small_ok);
+    float *logz = reinterpret_cast<float *>((char *)aux_ws + L.logz_a);
+    float *logp = reinterpret_cast<float *>(num_ws);
+    const double *lnorm = raw ? reinterpret_cast<const double *>((char *)aux_ws + L.lnorm) : nullptr;
+    if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, raw, 0, /*fwd_only=*/true)) return 1;
+    std::string err;
+    int rc = LaunchCtcSeqs(logits, dtype, sn, st, M, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev, seq_row_dev,
+                           max_label_len, 0, nullptr, false, logp, lnorm, s, &err);
+    if (rc) return Fail(err);
+    rc = LaunchSeqCosts(logz, logp, seq_row_dev, seq_pos_dev, M, lamb, scale, loss, costs, zero_inf, s);
+    if (rc) return FailCuda("seq_costs", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_ctc_loss_seqs(const void *logits, int dtype, int N, int T, int V, int Tmax,
+                      const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                      int M, const int *seq_row_dev, const int *seq_pos_dev, const int *seq_off_dev, int max_label_len,
+                      int blank, float scale, void *ctc_ws, float *grad, float *loss, float *logp, float *costs,
+                      int zero_inf, int defer_num, void *stream) {
+    g_err.clear();
+    if (N <= 0 || T <= 0 || V <= 0 || !logits || !loss || !logp || (ctc_ws && !defer_num && !grad))
+        return Fail("ctc_loss_seqs: bad arguments");
+    if (Tmax <= 0 || Tmax > T) return Fail("ctc_loss_seqs: Tmax must lie in [1, T]");
+    if (!KnownDtype(dtype)) return FailDtype("ctc_loss_seqs", dtype);
+    if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
+    if (CheckSeqMap("ctc_loss_seqs", M, seq_row_dev, seq_pos_dev)) return 1;
+    if (ctc_ws && !defer_num && !seq_off_dev) return Fail("ctc_loss_seqs: missing sequence offsets");
+    cudaStream_t s = (cudaStream_t)stream;
+    const long sn = (long)T * V, st = V;
+    std::string err;
+    int rc = LaunchCtcSeqs(logits, dtype, sn, st, M, Tmax, V, labels_dev, label_off_dev, label_len_dev, len_dev, seq_row_dev,
+                           max_label_len, blank, reinterpret_cast<float *>(ctc_ws), ctc_ws != nullptr, logp, nullptr, s, &err);
+    if (rc) return Fail(err);
+    if (ctc_ws && !defer_num) {   // every row of the (N,T,V) gradient is written
+        rc = LaunchCtcGammaSeqs(logits, dtype, sn, st, N, Tmax, T, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+                                seq_off_dev, seq_pos_dev, max_label_len, blank, reinterpret_cast<float *>(ctc_ws), nullptr,
+                                scale, -1.f, nullptr, nullptr, zero_inf, grad, sn, st, s, &err);
+        if (rc) return Fail(err);
+    }
+    rc = LaunchSeqCosts(nullptr, logp, seq_row_dev, seq_pos_dev, M, 0.f, scale, loss, costs, zero_inf, s);
+    if (rc) return FailCuda("seq_costs", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_seqs_grad(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax,
+                  const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                  int M, const int *seq_pos_dev, const int *seq_off_dev, int max_label_len, int blank, float num_coef,
+                  const float *w, const float *den, void *aux_ws, void *ctc_ws, int zero_inf, float *out, void *stream) {
+    g_err.clear();
+    const bool raw = from_logits != 0;
+    if (N <= 0 || T <= 0 || V <= 0 || M < 0 || !logits || !w || !ctc_ws || !out || !seq_off_dev || (M > 0 && !seq_pos_dev))
+        return Fail("seqs_grad: bad arguments");
+    if (Tmax <= 0 || Tmax > T) return Fail("seqs_grad: Tmax must lie in [1, T]");
+    if (!KnownDtype(dtype)) return FailDtype("seqs_grad", dtype);
+    if ((den || raw) && !aux_ws) return Fail("seqs_grad: the den part needs the forward call's aux workspace");
+    if (raw && !den) return Fail("seqs_grad: from_logits needs the den part");
+    cudaStream_t s = (cudaStream_t)stream;
+    const long sn = (long)T * V, st = V;
+    const float *logz = nullptr;
+    DenAuxLayout L;
+    if (den) {
+        DeviceGraph *g;
+        if (CurrentGraph(&g)) return 1;
+        L = MakeDenAuxLayout(g->S, N, Tmax, g->small_ok);
+        logz = reinterpret_cast<const float *>((char *)aux_ws + L.logz_a);
+    }
+    std::string err;
+    int rc = LaunchCtcGammaSeqs(logits, dtype, sn, st, N, Tmax, T, V, labels_dev, label_off_dev, label_len_dev, len_dev,
+                                seq_off_dev, seq_pos_dev, max_label_len, blank, reinterpret_cast<float *>(ctc_ws), w, 1.f,
+                                num_coef, den, logz, zero_inf, out, sn, st, s, &err);
+    if (rc) return Fail(err);
+    if (raw) {
+        rc = LaunchLogitGrad(logits, dtype, sn, st, N, Tmax, V, len_dev,
+                             reinterpret_cast<const float *>((char *)aux_ws + L.lz), L.Npad, out, sn, st, s);
+        if (rc) return FailCuda("logit_grad", (cudaError_t)rc);
+    }
+    return 0;
+}
+
+int ccb_ctc_align_seqs(const void *logits, int dtype, long sn, long st, int N, int T, int V,
+                       const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                       int M, const int *seq_row_dev, const int *seq_pos_dev, int max_label_len, int blank, void *workspace,
+                       int *align, float *score, void *stream) {
+    g_err.clear();
+    if (N <= 0 || T <= 0 || V <= 0 || !logits || !workspace || !align) return Fail("ctc_align_seqs: bad arguments");
+    if (!KnownDtype(dtype)) return FailDtype("ctc_align_seqs", dtype);
+    if (blank < 0 || blank >= V) return Fail("ctc: blank label out of range");
+    if (CheckSeqMap("ctc_align_seqs", M, seq_row_dev, seq_pos_dev)) return 1;
+    std::string err;
+    int rc = LaunchCtcViterbiSeqs(logits, dtype, sn, st, M, T, V, labels_dev, label_off_dev, label_len_dev, len_dev, seq_row_dev,
+                                  seq_pos_dev, max_label_len, blank, reinterpret_cast<unsigned char *>(workspace), align, score,
+                                  (cudaStream_t)stream, &err);
+    if (rc) return Fail(err);
+    return 0;
+}
+
 /* ---- gpu_ctc/ctc.h surface ------------------------------------------------------------------- */
 const char *ctcGetStatusString(ctcStatus_t status) {
     switch (status) {

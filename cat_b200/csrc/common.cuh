@@ -179,6 +179,27 @@ int LaunchCtcViterbi(const void *y, int y_dtype, long sn, long st, int N, int T,
                      unsigned char *bp_ws, int *align, float *score, cudaStream_t stream, std::string *err);
 int LaunchAssembleLoss(const float *logz, const float *logp, int N, float lamb, float scale, float *loss,
                        cudaStream_t stream, float *costs = nullptr, int zero_inf = 0);
+// Several label sequences per utterance.  Sequence m (of M, grouped by utterance) is scored against logits row seq_row[m];
+// seq_pos[m] is its index in the caller's order; the sequences of utterance n are seq_off[n] .. seq_off[n+1]-1.
+// The numerator's alpha (|| beta) chains over the M sequences: logp[m], and the cells of sequence m in alpha_ws (null: none).
+int LaunchCtcSeqs(const void *y, int y_dtype, long sn, long st, int M, int T, int V, const int *labels,
+                  const int *label_off, const int *label_len, const int *len, const int *seq_row, int max_label_len,
+                  int blank, float *alpha_ws, bool want_beta, float *logp, const double *lnorm, cudaStream_t stream,
+                  std::string *err);
+// The occupancies of every sequence of an utterance summed into its rows, once: out = W_n den + num_coef sum_m w_m gamma_m
+// (ctc_kernels.cu ctc_gamma_seqs_kernel); every row t < Tfull of the N utterances is written.
+int LaunchCtcGammaSeqs(const void *y, int y_dtype, long sn, long st, int N, int T, int Tfull, int V, const int *labels,
+                       const int *label_off, const int *label_len, const int *len, const int *seq_off, const int *seq_pos,
+                       int max_label_len, int blank, float *alpha_ws, const float *w, float w_scale, float num_coef,
+                       const float *den, const float *logz, int zero_inf, float *out, long gsn, long gst, cudaStream_t stream,
+                       std::string *err);
+// costs[seq_pos[m]] = logz[seq_row[m]] - (1+lamb) logp[m] (logz = null: -logp[m]); loss[0] = scale * sum_m cost
+int LaunchSeqCosts(const float *logz, const float *logp, const int *seq_row, const int *seq_pos, int M, float lamb, float scale,
+                   float *loss, float *costs, int zero_inf, cudaStream_t stream);
+int LaunchCtcViterbiSeqs(const void *y, int y_dtype, long sn, long st, int M, int T, int V, const int *labels,
+                         const int *label_off, const int *label_len, const int *len, const int *seq_row, const int *seq_pos,
+                         int max_label_len, int blank, unsigned char *bp_ws, int *align, float *score, cudaStream_t stream,
+                         std::string *err);
 // out[n][t][:] = w[n] * grad[n][t][:] for t < len[n], 0 beyond (grad not read there); out in the CCB_DTYPE_* out_dtype
 int LaunchGradRowsScale(const float *grad, const float *w, const int *len, int N, int T, int V, void *out, int out_dtype,
                         cudaStream_t stream);

@@ -71,16 +71,20 @@ struct CtcWorkspace {
 // shared memory carve-up: a[2][ScMax] doubles | lab[Lmax+1] ints | yrow[2][V] floats
 // SPILL = false (forward-only loss): one CTA per utterance walks the alpha chain and writes only logp_out; no cell, no
 // workspace.  The arithmetic is the same, so logp_out is bit-identical to the spilling launch's.
-template <bool SPILL>
+// MAP = true (several label sequences per utterance): n is a label sequence, scored against logits row seq_row[n] with that
+// row's length and log-normaliser; labels, workspace and logp_out are indexed by the sequence.  MAP = false: row = n, and
+// seq_row is not read.
+template <bool SPILL, bool MAP = false>
 __global__ void ctc_alpha_beta_kernel(const void *y, int y_dtype, long sn, long st, int T, int V,
                                       const int *labels, const int *label_off, const int *label_len, const int *len,
                                       int max_label_len, int blank, float *alpha_ws, bool want_beta, float *logp_out,
-                                      const double *lnorm) {
+                                      const double *lnorm, const int *seq_row) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int n = SPILL ? blockIdx.x >> 1 : blockIdx.x;
+    const int row = MAP ? seq_row[n] : n;
     const unsigned role = SPILL ? blockIdx.x & 1 : 0;   // 0: alpha pass, 1: beta pass
     const int tid = threadIdx.x, NT = blockDim.x;
-    const int L = label_len[n], Tn = len[n];
+    const int L = label_len[n], Tn = len[row];
     const int Sc = 2 * L + 1, L1 = L + 1;
     const int ScMax = 2 * max_label_len + 1;
     double *s_a = reinterpret_cast<double *>(smem_raw);                        // [2][ScMax]
@@ -104,7 +108,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_dtype, long sn, long 
     if (!want_beta && role == 1) return;   // likelihood only
     for (int i = tid; i < L; i += NT) s_lab[i] = lab[i];
     double *ws = W.a, *wsb = W.b;
-    const long ybase = n * sn;
+    const long ybase = row * sn;
     constexpr int kRowRegs = 4;
     const bool row_in_regs = V <= kRowRegs * NT;
     float yreg[kRowRegs];
@@ -169,7 +173,7 @@ __global__ void ctc_alpha_beta_kernel(const void *y, int y_dtype, long sn, long 
         double lp = last[Sc - 1];
         if (Sc > 1) lp = log_add_d(lp, last[Sc - 2]);
         // raw-logit entry: the reported log-likelihood is normalised; everything else stays in the raw domain
-        logp_out[n] = (float)(lp - (lnorm ? lnorm[n] : 0.0));
+        logp_out[n] = (float)(lp - (lnorm ? lnorm[row] : 0.0));
         if (SPILL) *W.logp = lp;
     }
     } else if (SPILL) {
@@ -287,6 +291,88 @@ __global__ void ctc_gamma_kernel(const void *y, int y_dtype, long sn, long st, i
     }
 }
 
+// Occupancies of several label sequences per utterance.  The sequences of utterance n are seq_off[n] .. seq_off[n+1]-1 of the
+// grouped workspace; one warp per (utterance, frame) walks them in order, so the sum over them is deterministic and needs no
+// global atomics.  Every row t < Tfull of out is written once:
+//   out[n][t][:] = W_n * den[n][t][:] + num_coef * sum_m w_m gamma_m,t[:]      (t < len[n], n has an unmasked sequence)
+//   out[n][t][:] = 0                                                            (otherwise)
+// w_m = w_scale * (w ? w[seq_pos[m]] : 1), W_n = sum of w_m over the unmasked sequences of n; a sequence is masked when zero_inf
+// is set and its log p or logz[n] is not finite.  den = null (CTC-only loss): no den part.  out may alias den: a warp reads its
+// row before it writes it.
+__global__ void ctc_gamma_seqs_kernel(const void *y, int y_dtype, long sn, long st, int N, int T, int Tfull, int V,
+                                      const int *labels, const int *label_off, const int *label_len, const int *len,
+                                      const int *seq_off, const int *seq_pos, int max_label_len, int blank, float *alpha_ws,
+                                      const float *w, float w_scale, float num_coef, const float *den, const float *logz,
+                                      int zero_inf, float *out, long gsn, long gst) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+    const long row = (long)blockIdx.x * wpb + warp;
+    if (row >= (long)N * Tfull) return;
+    const int n = (int)(row / Tfull), t = (int)(row % Tfull);
+    const int m0 = seq_off[n], m1 = seq_off[n + 1], ScMax = 2 * max_label_len + 1;
+    float *orow = out + n * gsn + (long)t * gst;
+    const bool logz_bad = logz != nullptr && !isfinite(logz[n]);
+    float wsum = 0.f;
+    int live = 0;
+    if (t < len[n]) {
+        for (int m = m0; m < m1; ++m) {
+            const double lp = *CtcWorkspace(alpha_ws, m, T, ScMax).logp;
+            if (zero_inf && (logz_bad || !isfinite(lp))) continue;
+            wsum += w_scale * (w ? __ldg(w + seq_pos[m]) : 1.f);
+            ++live;
+        }
+    }
+    if (live == 0) {      // padding frame, an utterance without sequences, or every sequence masked
+        for (int k = lane; k < V; k += 32) orow[k] = 0.f;
+        return;
+    }
+    float *g = reinterpret_cast<float *>(smem_raw) + (size_t)warp * V;
+    for (int k = lane; k < V; k += 32) g[k] = 0.f;
+    __syncwarp();
+    const long yrow = n * sn + (long)t * st;
+    float occ_blank = 0.f;
+    for (int m = m0; m < m1; ++m) {
+        const CtcWorkspace W(alpha_ws, m, T, ScMax);
+        const double logp_d = *W.logp;
+        if (!(logp_d > -INFINITY) || (zero_inf && (logz_bad || !isfinite(logp_d)))) continue;   // infeasible or masked
+        const float wm = w_scale * (w ? __ldg(w + seq_pos[m]) : 1.f);
+        const int Sc = 2 * label_len[m] + 1;
+        const double *al = W.a + (size_t)t * ScMax, *bl = W.b + (size_t)t * ScMax;
+        const int *lab = labels + label_off[m];
+        for (int s = lane; s < Sc; s += 32) {   // lane parity == cell parity: even lanes take blanks, odd lanes labels
+            const int li = (s & 1) ? __ldg(lab + (s >> 1)) : blank;
+            const float o = (float)(al[s] + bl[s] - (double)load_y(y, y_dtype, yrow + li) - logp_d);
+            const float e = (o == -INFINITY || o != o) ? 0.f : wm * expf(o);
+            if (s & 1) { if (e != 0.f) atomicAdd(&g[li], e); }
+            else occ_blank += e;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) occ_blank += __shfl_xor_sync(kFull, occ_blank, o);
+    __syncwarp();
+    if (lane == 0 && occ_blank != 0.f) g[blank] += occ_blank;
+    __syncwarp();
+    const float *drow = den ? den + n * gsn + (long)t * gst : nullptr;
+    for (int k = lane; k < V; k += 32) orow[k] = (drow ? wsum * drow[k] : 0.f) + num_coef * g[k];
+}
+
+// The costs of M label sequences, in the caller's order: cost = logz[seq_row[m]] - (1+lamb) logp[m] (CTC-CRF) or -logp[m]
+// (logz = null, CTC), written to costs[seq_pos[m]] (optional); loss[0] = scale * sum_m cost.  zero_inf as in
+// assemble_loss_kernel.
+__global__ void seq_costs_kernel(const float *logz, const float *logp, const int *seq_row, const int *seq_pos, int M,
+                                 float lamb, float scale, float *loss, float *costs, int zero_inf) {
+    double acc = 0.0;
+    for (int m = threadIdx.x; m < M; m += 32) {
+        double c = logz ? (double)logz[seq_row[m]] - (1.0 + (double)lamb) * (double)logp[m] : -(double)logp[m];
+        if (zero_inf && !isfinite(c)) c = 0.0;
+        if (costs) costs[seq_pos[m]] = (float)c;
+        acc += c;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
+    if (threadIdx.x == 0) loss[0] = (float)(acc * (double)scale);
+}
+
 // cost[n] = -logp[n];  loss[0] = scale * sum_n cost[n]   (CTC-only loss, ctc_crf/__init__.py:41-47: costs = -sum log p, / batch
 // when averaging).  costs (optional) receives each cost; zero_inf sets a cost that is not finite to 0 first.
 __global__ void sum_scale_kernel(const float *logp, int N, float scale, float *loss, float *costs, int zero_inf) {
@@ -326,18 +412,22 @@ __global__ void grad_rows_scale_kernel(const float *grad, const float *w, const 
 // path of finite score (too few frames for its labels, or every path through a -inf emission).
 // Ties are broken towards the smaller predecessor index (stay < s-1 < s-2).
 // shared memory: lab[Lmax] ints | v[2][ScMax] floats
+// MAP = true: n is a label sequence aligned to logits row seq_row[n]; its alignment and score go to index seq_pos[n].
+template <bool MAP = false>
 __global__ void ctc_viterbi_kernel(const void *y, int y_dtype, long sn, long st, int T, int V,
                                    const int *labels, const int *label_off, const int *label_len, const int *len,
-                                   int max_label_len, int blank, unsigned char *bp_ws, int *align, float *score) {
+                                   int max_label_len, int blank, unsigned char *bp_ws, int *align, float *score,
+                                   const int *seq_row, const int *seq_pos) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int n = blockIdx.x, tid = threadIdx.x, NT = blockDim.x;
-    const int L = label_len[n], Tn = len[n];
+    const int row = MAP ? seq_row[n] : n, out_n = MAP ? seq_pos[n] : n;
+    const int L = label_len[n], Tn = len[row];
     const int Sc = 2 * L + 1, L1 = L + 1, ScMax = 2 * max_label_len + 1;
     int *s_lab = reinterpret_cast<int *>(smem_raw);
     float *s_v = reinterpret_cast<float *>(s_lab + max_label_len + 1);
     unsigned char *bp = bp_ws + (size_t)n * T * ScMax;
     const int *lab = labels + label_off[n];
-    int *arow = align + (size_t)n * T;
+    int *arow = align + (size_t)out_n * T;
     for (int t = tid; t < T; t += NT) arow[t] = -1;
     int rep = 0;
     for (int i = tid + 1; i < L; i += NT) rep += (lab[i] == lab[i - 1]);
@@ -346,10 +436,10 @@ __global__ void ctc_viterbi_kernel(const void *y, int y_dtype, long sn, long st,
     __syncthreads();
     if (rep) atomicAdd(&s_rep, rep);
     __syncthreads();
-    if (Tn <= 0 || L + s_rep > Tn) { if (tid == 0 && score) score[n] = -INFINITY; return; }
+    if (Tn <= 0 || L + s_rep > Tn) { if (tid == 0 && score) score[out_n] = -INFINITY; return; }
     for (int i = tid; i < L; i += NT) s_lab[i] = lab[i];
     __syncthreads();
-    const long ybase = n * sn;
+    const long ybase = row * sn;
     for (int s = tid; s < Sc; s += NT) {
         float v = -INFINITY;
         if (s == 0) v = load_y(y, y_dtype, ybase + blank);
@@ -386,7 +476,7 @@ __global__ void ctc_viterbi_kernel(const void *y, int y_dtype, long sn, long st,
         const float *last = s_v + ((Tn - 1) & 1) * ScMax;
         int s = Sc - 1;
         if (Sc > 1 && last[Sc - 2] > last[Sc - 1]) s = Sc - 2;
-        if (score) score[n] = last[s];
+        if (score) score[out_n] = last[s];
         // every path killed by -inf emissions: the back-pointers lead nowhere, so the row keeps its -1s
         if (last[s] == -INFINITY) return;
         for (int t = Tn - 1; t >= 0; --t) {
@@ -417,7 +507,7 @@ __global__ void assemble_loss_kernel(const float *logz, const float *logp, int N
 int LaunchCtcAlphaBeta(const void *y, int y_dtype, long sn, long st, int N, int T, int V, const int *labels,
                        const int *label_off, const int *label_len, const int *len, int max_label_len, int blank,
                        float *alpha_ws, bool want_beta, float *logp, const double *lnorm, cudaStream_t stream,
-                       std::string *err) {
+                       std::string *err, const int *seq_row = nullptr) {
     if (N == 0) return 0;
     const int ScMax = 2 * max_label_len + 1;
     int threads = ((max_label_len + 1 + 31) / 32) * 32;
@@ -436,15 +526,26 @@ int LaunchCtcAlphaBeta(const void *y, int y_dtype, long sn, long st, int N, int 
         return 1;
     }
     const bool spill = alpha_ws != nullptr;
-    const void *kernel = spill ? (const void *)ctc_alpha_beta_kernel<true> : (const void *)ctc_alpha_beta_kernel<false>;
+    // seq_row != null: N counts label sequences, each scored against its own logits row (the MAP instances)
+    const void *kernel = seq_row ? (spill ? (const void *)ctc_alpha_beta_kernel<true, true> : (const void *)ctc_alpha_beta_kernel<false, true>)
+                                 : (spill ? (const void *)ctc_alpha_beta_kernel<true> : (const void *)ctc_alpha_beta_kernel<false>);
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc): ") + cudaGetErrorString(e); return (int)e; }
-    if (spill)
+    if (seq_row && spill)
+        ctc_alpha_beta_kernel<true, true><<<2 * N, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len,
+                                                                            len, max_label_len, blank, alpha_ws, want_beta, logp,
+                                                                            lnorm, seq_row);
+    else if (seq_row)
+        ctc_alpha_beta_kernel<false, true><<<N, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len,
+                                                                         len, max_label_len, blank, nullptr, false, logp, lnorm,
+                                                                         seq_row);
+    else if (spill)
         ctc_alpha_beta_kernel<true><<<2 * N, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len, len,
-                                                                      max_label_len, blank, alpha_ws, want_beta, logp, lnorm);
+                                                                      max_label_len, blank, alpha_ws, want_beta, logp, lnorm,
+                                                                      nullptr);
     else
         ctc_alpha_beta_kernel<false><<<N, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len, len,
-                                                                   max_label_len, blank, nullptr, false, logp, lnorm);
+                                                                   max_label_len, blank, nullptr, false, logp, lnorm, nullptr);
     CountLaunch();
     e = cudaGetLastError();
     if (e != cudaSuccess) { *err = std::string("ctc launch: ") + cudaGetErrorString(e); return (int)e; }
@@ -517,14 +618,72 @@ int LaunchCtcViterbi(const void *y, int y_dtype, long sn, long st, int N, int T,
     threads = threads < 64 ? 64 : (threads > 1024 ? 1024 : threads);
     const size_t smem = (size_t)(max_label_len + 1) * 4 + (size_t)2 * ScMax * 4;
     if (smem > 200 * 1024) { *err = "label sequence too long for the alignment kernel's shared memory"; return 1; }
-    cudaError_t e = cudaFuncSetAttribute(ctc_viterbi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute((const void *)ctc_viterbi_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
     if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc viterbi): ") + cudaGetErrorString(e); return (int)e; }
     ctc_viterbi_kernel<<<N, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len, len, max_label_len,
-                                                     blank, bp_ws, align, score);
+                                                     blank, bp_ws, align, score, nullptr, nullptr);
     CountLaunch();
     e = cudaGetLastError();
     if (e != cudaSuccess) { *err = std::string("ctc viterbi launch: ") + cudaGetErrorString(e); return (int)e; }
     return 0;
+}
+
+int LaunchCtcViterbiSeqs(const void *y, int y_dtype, long sn, long st, int M, int T, int V, const int *labels,
+                         const int *label_off, const int *label_len, const int *len, const int *seq_row, const int *seq_pos,
+                         int max_label_len, int blank, unsigned char *bp_ws, int *align, float *score, cudaStream_t stream,
+                         std::string *err) {
+    if (M == 0) return 0;
+    const int ScMax = 2 * max_label_len + 1;
+    int threads = ((max_label_len + 1 + 31) / 32) * 32;
+    threads = threads < 64 ? 64 : (threads > 1024 ? 1024 : threads);
+    const size_t smem = (size_t)(max_label_len + 1) * 4 + (size_t)2 * ScMax * 4;
+    if (smem > 200 * 1024) { *err = "label sequence too long for the alignment kernel's shared memory"; return 1; }
+    cudaError_t e = cudaFuncSetAttribute((const void *)ctc_viterbi_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
+    if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc viterbi): ") + cudaGetErrorString(e); return (int)e; }
+    ctc_viterbi_kernel<true><<<M, threads, smem, stream>>>(y, y_dtype, sn, st, T, V, labels, label_off, label_len, len,
+                                                           max_label_len, blank, bp_ws, align, score, seq_row, seq_pos);
+    CountLaunch();
+    e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = std::string("ctc viterbi launch: ") + cudaGetErrorString(e); return (int)e; }
+    return 0;
+}
+
+int LaunchCtcSeqs(const void *y, int y_dtype, long sn, long st, int M, int T, int V, const int *labels,
+                  const int *label_off, const int *label_len, const int *len, const int *seq_row, int max_label_len,
+                  int blank, float *alpha_ws, bool want_beta, float *logp, const double *lnorm, cudaStream_t stream,
+                  std::string *err) {
+    return LaunchCtcAlphaBeta(y, y_dtype, sn, st, M, T, V, labels, label_off, label_len, len, max_label_len, blank, alpha_ws,
+                              want_beta, logp, lnorm, stream, err, seq_row);
+}
+
+int LaunchCtcGammaSeqs(const void *y, int y_dtype, long sn, long st, int N, int T, int Tfull, int V, const int *labels,
+                       const int *label_off, const int *label_len, const int *len, const int *seq_off, const int *seq_pos,
+                       int max_label_len, int blank, float *alpha_ws, const float *w, float w_scale, float num_coef,
+                       const float *den, const float *logz, int zero_inf, float *out, long gsn, long gst, cudaStream_t stream,
+                       std::string *err) {
+    if (N == 0) return 0;
+    int wpb = 8;   // as LaunchCtcGamma
+    while (wpb > 1 && (size_t)wpb * V * 4 > 48 * 1024) wpb >>= 1;
+    const size_t gsm = (size_t)wpb * V * 4;
+    cudaError_t e = cudaFuncSetAttribute(ctc_gamma_seqs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gsm);
+    if (e != cudaSuccess) { *err = std::string("cudaFuncSetAttribute(ctc gamma seqs): ") + cudaGetErrorString(e); return (int)e; }
+    const long rows = (long)N * Tfull;
+    ctc_gamma_seqs_kernel<<<(unsigned)((rows + wpb - 1) / wpb), wpb * 32, gsm, stream>>>(
+        y, y_dtype, sn, st, N, T, Tfull, V, labels, label_off, label_len, len, seq_off, seq_pos, max_label_len, blank, alpha_ws,
+        w, w_scale, num_coef, den, logz, zero_inf, out, gsn, gst);
+    CountLaunch();
+    e = cudaGetLastError();
+    if (e != cudaSuccess) { *err = std::string("ctc gamma seqs launch: ") + cudaGetErrorString(e); return (int)e; }
+    return 0;
+}
+
+int LaunchSeqCosts(const float *logz, const float *logp, const int *seq_row, const int *seq_pos, int M, float lamb, float scale,
+                   float *loss, float *costs, int zero_inf, cudaStream_t stream) {
+    seq_costs_kernel<<<1, 32, 0, stream>>>(logz, logp, seq_row, seq_pos, M, lamb, scale, loss, costs, zero_inf);
+    CountLaunch();
+    return (int)cudaGetLastError();
 }
 
 int LaunchAssembleLoss(const float *logz, const float *logp, int N, float lamb, float scale, float *loss,

@@ -121,6 +121,53 @@ def _costs_backward(ctx, grad_output):
     return (ctx.grads * grad_output.to(ctx.grads.device)).to(ctx.in_dtype)
 
 
+class _CTC_CRF_SEQS(Function):
+    """CTC_CRF_LOSS with several label sequences per utterance (``utt``): cost[m] = logZ_den[utt[m]] - (1+lamb) log p_ctc[m],
+    one den pass per utterance.  reduction None: the forward writes the final gradient; 'none': the forward keeps the den
+    occupancies unscaled and the numerator's cells, and the backward weights them by grad_output (``_C.seqs_backward``)."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, lx, ly, utt, lamb, size_average, from_logits, reduction, zero_infinity):
+        logits = logits.contiguous()
+        out, grads, state = core.ctc_crf_loss_seqs(logits, labels, lx, ly, utt, lamb, size_average, from_logits=from_logits,
+                                                   reduction=reduction, zero_infinity=zero_infinity)
+        ctx.grads, ctx.state, ctx.in_dtype = grads, state, logits.dtype
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        return (_seqs_backward(ctx, grad_output),) + (None,) * 9
+
+
+class _WARP_CTC_SEQS(Function):
+    """WARP_CTC_LOSS with several label sequences per utterance (``utt``): cost[m] = -log p[m], every numerator in one
+    launch; backward as in ``_CTC_CRF_SEQS``."""
+
+    @staticmethod
+    def forward(ctx, logits, labels, lx, ly, utt, size_average, reduction, zero_infinity):
+        logits = logits.contiguous()
+        out, grads, state = core.ctc_loss_seqs(logits, labels, lx, ly, utt, size_average, reduction=reduction,
+                                               zero_infinity=zero_infinity)
+        ctx.grads, ctx.state, ctx.in_dtype = grads, state, logits.dtype
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_output):
+        return (_seqs_backward(ctx, grad_output),) + (None,) * 7
+
+
+def _seqs_backward(ctx, grad_output):
+    if ctx.state is not None:       # reduction 'none': sum_m grad_output[m] * d cost[m] / d logits, in the logits' dtype
+        return core.seqs_backward(ctx.state, grad_output, ctx.in_dtype)
+    return (ctx.grads * grad_output.to(ctx.grads.device)).to(ctx.in_dtype)
+
+
+def _check_utt(utt):
+    """`utt` is placed and asserted as lx / ly are; `_C.group_seqs` checks its values."""
+    assert utt.dtype == torch.int, f"expect utt to be torch.int object, instead: {utt.dtype}"
+    _assert_no_grad(utt)
+
+
 def _loss_options(reduction, zero_infinity) -> dict:
     """The keyword arguments the `_C` loss functions get for these settings: none at the defaults, so that the default
     path calls exactly what it called before the two options existed."""
@@ -154,7 +201,7 @@ class CTC_CRF_LOSS(Module):
         self.reduction = reduction
         self.zero_infinity = zero_infinity
 
-    def forward(self, logits, labels, lx, ly) -> torch.FloatTensor:
+    def forward(self, logits, labels, lx, ly, utt=None) -> torch.FloatTensor:
         """
         logits (torch.FloatTensor): size (N, T, V), log-probabilities, on GPU device.
             (torch.bfloat16 and torch.float16 are accepted too, read in place with fp32 arithmetic -- the reference asserts
@@ -162,7 +209,15 @@ class CTC_CRF_LOSS(Module):
         labels (torch.IntTensor)  : size (sum {Ui}, ) flattened without paddings, on CPU.
         lx (torch.IntTensor) : size (N, ), on CPU
         ly (torch.IntTensor) : size (N, ), on CPU
+        utt (torch.IntTensor, optional): addition -- size (M, ), on CPU: several label sequences per utterance (samples,
+            N-best lists, alternative pronunciations).  labels / ly then describe M sequences, sequence m scored against
+            logits row utt[m] (any order); lx stays (N, ).  cost[m] = logZ_den[utt[m]] - (1+lamb) log p_ctc(l_m | x_utt[m]),
+            with the den computed once per utterance.  The scalar is the sum over the M sequences (/ M with size_average);
+            reduction='none' returns the (M,) costs in the caller's order; zero_infinity masks per sequence.  An utterance
+            without a sequence contributes nothing and gets a zero gradient.
         """
+        if utt is not None:
+            return self._forward_seqs(logits, labels, lx, ly, utt)
         assert len(labels.size()) == 1
         assert logits.dtype in (torch.float, torch.bfloat16, torch.float16), \
             f"expect logits to be torch.float (or torch.bfloat16 / torch.float16) object, instead: {logits.dtype}"
@@ -183,6 +238,25 @@ class CTC_CRF_LOSS(Module):
                                         self.reduction, bool(self.zero_infinity))
         return self.ctc_crf(logits, labels, lx, ly, self.lamb, self.size_average)
 
+    def _forward_seqs(self, logits, labels, lx, ly, utt):
+        assert len(labels.size()) == 1
+        assert logits.dtype in (torch.float, torch.bfloat16, torch.float16), \
+            f"expect logits to be torch.float (or torch.bfloat16 / torch.float16) object, instead: {logits.dtype}"
+        assert labels.dtype == torch.int, f"expect labels to be torch.int object, instead: {labels.dtype}"
+        assert lx.dtype == torch.int, f"expect lx to be torch.int object, instead: {lx.dtype}"
+        assert ly.dtype == torch.int, f"expect ly to be torch.int object, instead: {ly.dtype}"
+        _check_utt(utt)
+        _assert_no_grad(labels)
+        _assert_no_grad(lx)
+        _assert_no_grad(ly)
+        core.check_reduction(self.reduction)
+        if not torch.is_grad_enabled():
+            return core.ctc_crf_loss_seqs_fwd_only(logits.contiguous(), labels, lx, ly, utt, self.lamb, self.size_average,
+                                                   from_logits=self.from_logits, reduction=self.reduction,
+                                                   zero_infinity=bool(self.zero_infinity))
+        return _CTC_CRF_SEQS.apply(logits, labels, lx, ly, utt, self.lamb, self.size_average, self.from_logits,
+                                   self.reduction, bool(self.zero_infinity))
+
 
 class WARP_CTC_LOSS(Module):
     """__init__.py:128-144.  reduction and zero_infinity (additions) as for CTC_CRF_LOSS, with cost[n] = -log p[n]."""
@@ -195,11 +269,22 @@ class WARP_CTC_LOSS(Module):
         self.reduction = reduction
         self.zero_infinity = zero_infinity
 
-    def forward(self, logits, labels, input_lengths, label_lengths):
+    def forward(self, logits, labels, input_lengths, label_lengths, utt=None):
+        """utt (addition): (M,) int32 on CPU, sequence m of labels / label_lengths scored against logits row utt[m], as for
+        CTC_CRF_LOSS; cost[m] = -log p[m], all M numerators in one launch."""
         assert len(labels.size()) == 1
         _assert_no_grad(labels)
         _assert_no_grad(input_lengths)
         _assert_no_grad(label_lengths)
+        if utt is not None:
+            _check_utt(utt)
+            core.check_reduction(self.reduction)
+            if not torch.is_grad_enabled():
+                return core.ctc_loss_seqs(logits.contiguous(), labels, input_lengths, label_lengths, utt, self.size_average,
+                                          reduction=self.reduction, zero_infinity=bool(self.zero_infinity),
+                                          with_grad=False)[0]
+            return _WARP_CTC_SEQS.apply(logits, labels, input_lengths, label_lengths, utt, self.size_average, self.reduction,
+                                        bool(self.zero_infinity))
         opts = _loss_options(self.reduction, self.zero_infinity)
         if not torch.is_grad_enabled():   # evaluation: the loss alone (see CTC_CRF_LOSS.forward)
             return core.ctc_loss_fwd_only(logits.contiguous(), labels, input_lengths, label_lengths, self.size_average,
@@ -210,11 +295,15 @@ class WARP_CTC_LOSS(Module):
         return self.ctc(logits, labels, input_lengths, label_lengths, self.size_average)
 
 
-def ctc_align(logits, labels, input_lengths, label_lengths):
+def ctc_align(logits, labels, input_lengths, label_lengths, utt=None):
     """Best-path forced alignment of every utterance to its label sequence over the CTC lattice -- the alignment that comes
     with the numerator (SURVEY 8f-4; cat/ctc/train_jsa.py consumes frame-level paths).  Arguments as for WARP_CTC_LOSS.
-    Returns (align (N,T) int32 on the GPU, token per frame incl. blank 0, -1 past each length; score (N,) fp32)."""
+    Returns (align (N,T) int32 on the GPU, token per frame incl. blank 0, -1 past each length; score (N,) fp32).
+    utt (addition, (M,) int32 CPU): align each of M label sequences to its logits row utt[m]; align (M,T), score (M,)."""
     assert len(labels.size()) == 1
+    if utt is not None:
+        _check_utt(utt)
+        return core.ctc_align_seqs(logits.contiguous(), labels, input_lengths, label_lengths, utt)
     return core.ctc_align(logits.contiguous(), labels, input_lengths, label_lengths)
 
 

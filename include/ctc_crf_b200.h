@@ -228,6 +228,55 @@ int ccb_ctc_loss_costs(const void *logits, int dtype, int N, int T, int V, int T
 int ccb_grad_rows_scale(const float *grad, const float *w, const int *len_dev, int N, int T, int V, void *out, int out_dtype,
                         void *stream);
 
+/* Several label sequences per utterance (sampled sequences, N-best lists, alternative pronunciations), with the den passes run
+ * once per utterance.  M sequences, grouped by utterance (the sequences of utterance n are seq_off[n] .. seq_off[n+1]-1):
+ *   labels_dev / label_off_dev / label_len_dev describe the M sequences in that order (label_off: M entries);
+ *   len_dev      (N,) frames per utterance;
+ *   seq_row_dev  (M,) the logits row, in [0, N), sequence m is scored against;
+ *   seq_pos_dev  (M,) the index of sequence m in the caller's order: costs[seq_pos[m]] (and w[seq_pos[m]]) belong to it;
+ *   seq_off_dev  (N+1,) offsets of each utterance's sequences; seq_off[0] is the first sequence of this call.
+ *   cost[m] = logZ_den[seq_row[m]] - (1+lamb) logp_ctc[m] (CTC-CRF) or -logp[m] (CTC); loss[0] = scale * sum_m cost[m];
+ *   grad[n] = sum_{m of n} w_m (gamma_den[n] - (1+lamb) gamma_ctc[m]), w_m = scale (CTC-CRF; CTC: -scale gamma_ctc[m] alone).
+ * The den occupancies are computed once per utterance and scaled by W_n = sum of w_m over its unmasked sequences; an utterance
+ * without an unmasked sequence (or without any) gets zero rows.  zero_inf masks per sequence.  logp_ctc[m] is bit-identical to
+ * a single-sequence call on row seq_row[m].  ctc_ws: ccb_ctc_workspace_bytes(M, Tmax, max_label_len); alpha_ws / aux_ws as
+ * for N utterances.  M = 0 is allowed (zero rows, loss 0).
+ * defer_num != 0 (reduction 'none' with a gradient): grad receives the UNSCALED den occupancies only (CTC: grad is not used),
+ * and the numerator's cells stay in ctc_ws for ccb_seqs_grad, which the caller runs later with its per-sequence weights. */
+int ccb_ctc_crf_loss_seqs(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax, int ckpt_k,
+                          const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                          int M, const int *seq_row_dev, const int *seq_pos_dev, const int *seq_off_dev, int max_label_len,
+                          float lamb, float scale, float *alpha_ws, void *aux_ws, void *ctc_ws, float *grad, float *loss,
+                          float *costs, int zero_inf, int defer_num, void *stream);
+/* Its forward-only counterpart (ccb_ctc_crf_loss_fwd_only's passes); num_ws: ccb_num_fwd_only_bytes(M). */
+int ccb_ctc_crf_loss_seqs_fwd_only(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax,
+                                   const int *labels_dev, const int *label_off_dev, const int *label_len_dev,
+                                   const int *len_dev, int M, const int *seq_row_dev, const int *seq_pos_dev,
+                                   int max_label_len, float lamb, float scale, float *alpha_ws, void *aux_ws, void *num_ws,
+                                   float *loss, float *costs, int zero_inf, void *stream);
+/* CTC-only loss over M sequences: logp (M,) out in the grouped order.  ctc_ws = NULL: forward only (no cells, grad unused);
+ * otherwise every row of the (N,T,V) grad is written (unless defer_num). */
+int ccb_ctc_loss_seqs(const void *logits, int dtype, int N, int T, int V, int Tmax,
+                      const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                      int M, const int *seq_row_dev, const int *seq_pos_dev, const int *seq_off_dev, int max_label_len,
+                      int blank, float scale, void *ctc_ws, float *grad, float *loss, float *logp, float *costs,
+                      int zero_inf, int defer_num, void *stream);
+/* The deferred gradient of a defer_num call, with per-sequence weights w (M,) in the caller's order:
+ *   out[n] = W_n den[n] + num_coef * sum_{m of n} w[seq_pos[m]] gamma_ctc[m],  W_n = sum of w over the unmasked sequences of n
+ * written to every row of the (N,T,V) fp32 `out` (zeros for t >= len); den = NULL for the CTC-only loss.  from_logits != 0
+ * chains it through log_softmax as the fused entry does.  aux_ws / ctc_ws: the forward call's, untouched since; out may not
+ * alias den.  num_coef: -(1+lamb) for CTC-CRF, -1 for CTC. */
+int ccb_seqs_grad(const void *logits, int dtype, int from_logits, int N, int T, int V, int Tmax,
+                  const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                  int M, const int *seq_pos_dev, const int *seq_off_dev, int max_label_len, int blank, float num_coef,
+                  const float *w, const float *den, void *aux_ws, void *ctc_ws, int zero_inf, float *out, void *stream);
+/* ccb_ctc_align over M sequences: align (M,T) and score (M,) in the caller's order (row seq_pos[m]); workspace:
+ * ccb_ctc_align_workspace_bytes(M, T, max_label_len). */
+int ccb_ctc_align_seqs(const void *logits, int dtype, long sn, long st, int N, int T, int V,
+                       const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
+                       int M, const int *seq_row_dev, const int *seq_pos_dev, int max_label_len, int blank, void *workspace,
+                       int *align, float *score, void *stream);
+
 /* Best-path (Viterbi) alignment over the numerator lattice -- the forced alignment that comes with the CTC numerator
  * (SURVEY.md 8f-4).  align: (N,T) int32 device out, the token emitted at every frame t < len (blank included), -1 beyond
  * the length and for infeasible utterances; score (optional, may be NULL): (N,) log-probability of the best path.
