@@ -12,7 +12,8 @@ and ``ctc_loss_fwd_only`` -- the losses without a gradient, used when grad mode 
 ``reduction`` (None: the scalar of ``size_average``; 'none': one cost per utterance) and ``zero_infinity``;
 ``grad_rows_scale`` is the backward of the per-utterance costs.  ``ctc_crf_loss_seqs``, ``ctc_crf_loss_seqs_fwd_only``,
 ``ctc_loss_seqs`` and ``ctc_align_seqs`` take several label sequences per utterance (``utt``: the logits row of each), with the
-den passes run once per utterance; ``seqs_backward`` is the backward of their per-sequence costs.
+den passes run once per utterance; ``seqs_backward`` is the backward of their per-sequence costs.  ``crf_sample`` draws paths
+from the CTC-CRF posterior and ``samples_to_labels`` packs them for the ``utt=`` loss.
 """
 from __future__ import annotations
 
@@ -227,11 +228,12 @@ def ckpt_interval(tmax: int) -> int:
     return max(1, math.isqrt(max(1, tmax) - 1) + 1)
 
 
-def _slice_need(L, n, tmax, maxl, k, m=None):
-    """Scratch bytes of a slice of n utterances; m: its label sequences when they are not one per utterance."""
+def _slice_need(L, n, tmax, maxl, k, m=None, ws_bytes=None):
+    """Scratch bytes of a slice of n utterances; m: its label sequences when they are not one per utterance; ws_bytes(n, tmax):
+    the workspace that takes the numerator's place (the sampler's)."""
     alpha = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
-    return (int(alpha) * 4 + int(L.ccb_den_aux_bytes(n, tmax))
-            + int(L.ccb_ctc_workspace_bytes(n if m is None else m, tmax, maxl)))
+    ws = ws_bytes(n, tmax) if ws_bytes is not None else L.ccb_ctc_workspace_bytes(n if m is None else m, tmax, maxl)
+    return int(alpha) * 4 + int(L.ccb_den_aux_bytes(n, tmax)) + int(ws)
 
 
 def _slice_seqs(ly, n0, n1, seq_off):
@@ -242,7 +244,7 @@ def _slice_seqs(ly, n0, n1, seq_off):
     return s1 - s0, int(ly[s0:s1].max()) if s1 > s0 else 0
 
 
-def _plan_slices(L, lx, ly, N, V, dev, seq_off=None):
+def _plan_slices(L, lx, ly, N, V, dev, seq_off=None, ws_bytes=None):
     """Split the batch into contiguous slices whose scratch (alpha spill etc.) fits the free device memory.
     Each slice walks only max(lx[slice]) frames.  Returns (n0, n1, tmax, maxl, K) per slice; K = 0 keeps every alpha
     frame, K > 0 keeps every K-th and recomputes the rest in the backward pass.
@@ -250,7 +252,8 @@ def _plan_slices(L, lx, ly, N, V, dev, seq_off=None):
     padding (the spill is proportional to the padding); otherwise it runs checkpointed with K = ceil(sqrt(tmax)), and is
     halved further only if that does not fit either.
     seq_off (N+1,): several label sequences per utterance -- ly holds their lengths grouped by utterance, those of utterance
-    n at seq_off[n] .. seq_off[n+1]-1, and a slice's numerator workspace is sized by its sequences."""
+    n at seq_off[n] .. seq_off[n+1]-1, and a slice's numerator workspace is sized by its sequences.
+    ws_bytes(n, tmax): the bytes of the workspace a slice needs in place of the numerator's (the posterior sampler: ly unused)."""
     budget = _scratch_budget(dev)
     slices, n0 = [], 0
     while n0 < N:
@@ -259,9 +262,9 @@ def _plan_slices(L, lx, ly, N, V, dev, seq_off=None):
             n = n1 - n0
             half = max(1, n // 2)
             tmax = max(1, int(lx[n0:n1].max()))
-            m, maxl = _slice_seqs(ly, n0, n1, seq_off)
+            m, maxl = _slice_seqs(ly, n0, n1, seq_off) if ws_bytes is None else (n, 0)
             k = 0 if _ckpt_k_override is None else int(_ckpt_k_override)
-            need = _slice_need(L, n, tmax, maxl, k, m)
+            need = _slice_need(L, n, tmax, maxl, k, m, ws_bytes)
             if need > budget:
                 budget = _scratch_budget(dev, need)     # a stale (cached) figure must not split a batch needlessly
             if need <= budget:
@@ -272,7 +275,7 @@ def _plan_slices(L, lx, ly, N, V, dev, seq_off=None):
                 continue
             if k == 0:
                 k = ckpt_interval(tmax)
-                need = _slice_need(L, n, tmax, maxl, k, m)
+                need = _slice_need(L, n, tmax, maxl, k, m, ws_bytes)
                 if need > budget:
                     budget = _scratch_budget(dev, need)
                 if need <= budget:
@@ -851,6 +854,99 @@ def ctc_align_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor,
         _check(rc, "ctc_align_seqs")
         meta.buf.record_stream(torch.cuda.current_stream(dev))
     return align, score
+
+
+# ---------------------------------------------------------------------------------------------------
+# samples from the CTC-CRF posterior
+# ---------------------------------------------------------------------------------------------------
+def draw_seed(generator: Optional[torch.Generator] = None) -> int:
+    """The call's 64-bit Philox key: two 32-bit draws from `generator` (a CPU torch.Generator; None: torch's default one)."""
+    gen = torch.default_generator if generator is None else generator
+    if not isinstance(gen, torch.Generator) or gen.device.type != "cpu":
+        raise RuntimeError(f"generator must be a CPU torch.Generator, not {gen!r}")
+    hi, lo = (int(x) for x in torch.randint(0, 1 << 32, (2,), generator=gen, dtype=torch.int64))
+    return (hi << 32) | lo
+
+
+def _check_sample_args(logits, lx, num_samples):
+    if not isinstance(logits, torch.Tensor) or not logits.is_cuda or logits.dim() != 3:
+        raise RuntimeError("logits must be an (N,T,V) CUDA tensor")
+    if logits.dtype not in _DTYPES:
+        raise RuntimeError(f"unsupported logits dtype {logits.dtype}: fp32, bf16 or fp16")
+    N, T, V = logits.shape
+    if N == 0 or T == 0 or V == 0:
+        raise RuntimeError(f"empty logits of shape {tuple(logits.shape)}")
+    if not isinstance(lx, torch.Tensor) or lx.dtype != torch.int32 or lx.is_cuda or lx.dim() != 1 or int(lx.numel()) != N:
+        raise RuntimeError("lx must be an (N,) int32 CPU tensor, one input length per utterance")
+    if int(lx.max()) > T or int(lx.min()) < 0:
+        raise RuntimeError("input lengths must lie in [0, T]")
+    if isinstance(num_samples, bool) or not isinstance(num_samples, int) or num_samples < 1:
+        raise RuntimeError(f"num_samples must be an int >= 1, not {num_samples!r}")
+    return N, T, V
+
+
+def crf_sample(logits: torch.Tensor, lx: torch.Tensor, num_samples: int = 1, generator: Optional[torch.Generator] = None
+               ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """K = num_samples paths per utterance drawn exactly from the CTC-CRF posterior over the loaded den graph.  Returns device
+    tensors (tokens (N,K,T) int32, lengths (N,K) int32, align (N,K,T) int32, path_logp (N,K) fp32); see
+    ``ctc_crf.crf_sample``.  Batches are sliced as for the loss, the sampler's workspace in the numerator's place; never
+    synchronises the host."""
+    N, T, V = _check_sample_args(logits, lx, num_samples)
+    K = num_samples
+    seed = draw_seed(generator)
+    L = _lib.lib()
+    dev = logits.device
+    with torch.no_grad(), torch.cuda.device(dev):
+        y = logits.detach().contiguous()
+        esz = y.element_size()
+        lens = _rings.setdefault(torch.device(dev).index, _PinnedRing()).stage([lx], dev)
+        tokens = torch.empty((N, K, T), dtype=torch.int32, device=dev)
+        lengths = torch.empty((N, K), dtype=torch.int32, device=dev)
+        align = torch.empty((N, K, T), dtype=torch.int32, device=dev)
+        path_logp = torch.empty((N, K), dtype=torch.float32, device=dev)
+        stream = _stream(dev)
+
+        def run_slices():
+            slices = _plan_slices(L, lx, None, N, V, dev, ws_bytes=lambda n, tmax: L.ccb_crf_sample_ws_bytes(n, K, tmax))
+            for n0, n1, tmax, _, k in slices:
+                n = n1 - n0
+                alpha_floats = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
+                alpha_ws = torch.empty(int(alpha_floats), dtype=torch.float32, device=dev)
+                aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
+                sample_ws = torch.empty(int(L.ccb_crf_sample_ws_bytes(n, K, tmax)), dtype=torch.uint8, device=dev)
+                rc = L.ccb_crf_sample(y.data_ptr() + n0 * T * V * esz, _DTYPES[y.dtype], n, T, V, tmax, k,
+                                      lens.data_ptr() + 4 * n0, K, seed, n0, alpha_ws.data_ptr(), aux_ws.data_ptr(),
+                                      sample_ws.data_ptr(), tokens.data_ptr() + n0 * K * T * 4,
+                                      lengths.data_ptr() + n0 * K * 4, align.data_ptr() + n0 * K * T * 4,
+                                      path_logp.data_ptr() + n0 * K * 4, stream)
+                _check(rc, "crf_sample")
+                del alpha_ws, aux_ws, sample_ws
+
+        try:
+            run_slices()
+        except torch.cuda.OutOfMemoryError:       # as in ctc_crf_loss_fwd
+            _budget_cache.pop(torch.device(dev).index, None)
+            torch.cuda.empty_cache()
+            run_slices()
+        lens.record_stream(torch.cuda.current_stream(dev))
+    return tokens, lengths, align, path_logp
+
+
+def samples_to_labels(tokens: torch.Tensor, lengths: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(labels, ly, utt) int32 CPU tensors of the feasible samples (lengths >= 0), utterance by utterance, sample by sample:
+    the arguments ``CTC_CRF_LOSS(...)(logits, labels, lx, ly, utt=utt)`` takes.  One device-to-host copy (lengths and tokens
+    together), which waits for the sampler to finish."""
+    if tokens.dim() != 3 or lengths.shape != tokens.shape[:2]:
+        raise RuntimeError(f"tokens must be (N,K,T) and lengths (N,K), not {tuple(tokens.shape)} and {tuple(lengths.shape)}")
+    N, K, T = tokens.shape
+    host = torch.cat([lengths.reshape(N * K, 1).to(torch.int32), tokens.reshape(N * K, T).to(torch.int32)], 1).cpu()
+    ly = host[:, 0]
+    keep = ly >= 0
+    rows = host[keep, 1:]
+    ly = ly[keep]
+    labels = rows[torch.arange(T).unsqueeze(0) < ly.unsqueeze(1)]
+    utt = torch.arange(N, dtype=torch.int32).repeat_interleave(K)[keep]
+    return labels.to(torch.int32).contiguous(), ly.to(torch.int32).contiguous(), utt.contiguous()
 
 
 def launch_count() -> int:

@@ -73,6 +73,7 @@ void FreeDevice(DeviceGraph &d) {
     if (!d.loaded) return;
     cudaFree(d.state_label); cudaFree(d.state_pos); cudaFree(d.final_lin); cudaFree(d.start_arcs); cudaFree(d.hub_states);
     for (DevicePass *p : {&d.fwd, &d.bwd}) { cudaFree(p->arcs); cudaFree(p->chunk_state); cudaFree(p->chunk_arc); cudaFree(p->chunk_pair); cudaFree(p->cta_labels); cudaFree(p->w1); cudaFree(p->tq); cudaFree(p->own_c); }
+    cudaFree(d.in_off); cudaFree(d.in_src); cudaFree(d.in_w);
     d = DeviceGraph();
 }
 
@@ -139,6 +140,9 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
     g_plan_valid = true;
     DEN_NUM_STATES = g_plan.num_states + g_plan.num_pairs;   // rows per alpha frame (what binding.cpp sizes scratch with)
     DEN_NUM_ARCS = (int)g_plan.fwd.arcs.size();
+    // the sampler's in-arc CSR stays on the host until a sampling call needs it on a device (UploadSampleCsr)
+    auto csr = std::make_shared<DenPlan>();
+    csr->in_off = g_plan.in_off; csr->in_src = g_plan.in_src; csr->in_w = g_plan.in_w;
     int rc = 0;
     for (int i = 0; i < n_gpus && rc == 0; ++i) {
         DeviceGraph &d = g_dev[gpus[i]];
@@ -168,6 +172,7 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
         d.small_ok = SmallBatchOk(d.shape, d.max_smem_optin, d.hooks);
         d.n_start_arcs = (int)g_plan.start_arcs.size();
         d.start_final = g_plan.final_lin[(size_t)g_plan.start];
+        d.host_plan = csr;
         d.loaded = (rc == 0);
         if (rc == 0) ++g_refs[gpus[i]];
     }
@@ -275,6 +280,25 @@ int DenForward(const DeviceGraph &g, const void *y, int dtype, long sn, long st,
     return 0;
 }
 
+// Checkpointed alpha: recompute the frames (lo, hi] of segment j from its checkpoint into the segment positions (frame t at
+// position t - lo), as a forward launch that writes neither column sums nor logZ.  Returns lo and hi.
+int DenRecompute(const DeviceGraph &g, const void *y, int dtype, long sn, long st, int N, int T, int V, const int *len,
+                 float *alpha, void *aux, const DenAuxLayout &L, int ckpt_k, int j, int *lo_out, int *hi_out,
+                 cudaStream_t stream) {
+    char *a = reinterpret_cast<char *>(aux);
+    DenParams f = BaseParams(g, y, dtype, sn, st, N, T, V, len, alpha, aux, L);
+    SetCkpt(f, g, T, ckpt_k);
+    const int lo = j * f.ckpt_k, hi = std::min(lo + f.ckpt_k, T);
+    f.ckpt_mode = 2; f.a_base = lo; f.a_frames = CkptSegFrames(T, ckpt_k);
+    f.t_lo = lo; f.t_hi = hi;
+    f.barrier = reinterpret_cast<unsigned *>(a + L.barrier);
+    CCB_CUDA(cudaMemsetAsync(a + L.barrier, 0, 128, stream));
+    std::string err;
+    if (LaunchDen(false, g, f, stream, &err)) return Fail(err);
+    *lo_out = lo; *hi_out = hi;
+    return 0;
+}
+
 // backward part (beta recursion, occupancies, logz_b).  ckpt_k > 0: one segment of ckpt_k frames at a time, from the last
 // to the first, each first recomputed from its checkpoint into the segment positions by a forward launch.
 int DenBackward(const DeviceGraph &g, const void *y, int dtype, long sn, long st, int N, int T, int V, const int *len,
@@ -299,17 +323,9 @@ int DenBackward(const DeviceGraph &g, const void *y, int dtype, long sn, long st
         if (rc) return Fail(err);
     } else {
         SetCkpt(p, g, T, ckpt_k);
-        const int K = p.ckpt_k;
         for (int j = CkptCount(T, ckpt_k) - 1; j >= 0; --j) {
-            const int lo = j * K, hi = std::min(lo + K, T);
-            DenParams f = BaseParams(g, y, dtype, sn, st, N, T, V, len, alpha, aux, L);   // recompute frames (lo, hi]
-            SetCkpt(f, g, T, ckpt_k);
-            f.ckpt_mode = 2; f.a_base = lo; f.a_frames = CkptSegFrames(T, ckpt_k);
-            f.t_lo = lo; f.t_hi = hi;
-            f.barrier = reinterpret_cast<unsigned *>(a + L.barrier);
-            CCB_CUDA(cudaMemsetAsync(a + L.barrier, 0, 128, stream));
-            rc = LaunchDen(false, g, f, stream, &err);
-            if (rc) return Fail(err);
+            int lo = 0, hi = 0;
+            if (DenRecompute(g, y, dtype, sn, st, N, T, V, len, alpha, aux, L, ckpt_k, j, &lo, &hi, stream)) return 1;
             p.a_base = lo; p.t_lo = lo; p.t_hi = hi;   // tau = hi .. lo + 1 (tau = 0 epilogue with the first segment)
             CCB_CUDA(cudaMemsetAsync(a + L.barrier + 128, 0, 128, stream));
             rc = LaunchDen(true, g, p, stream, &err);
@@ -902,6 +918,70 @@ int ccb_ctc_align_seqs(const void *logits, int dtype, long sn, long st, int N, i
     return 0;
 }
 
+/* ---- samples from the CTC-CRF posterior ------------------------------------------------------ */
+// The in-arc CSR of the device's graph, uploaded by the first sampling call on the device (Release frees it with the graph)
+static int UploadSampleCsr(DeviceGraph *g) {
+    std::lock_guard<std::mutex> lk(g_mu);
+    if (g->in_off) return 0;
+    if (!g->host_plan) return Fail("crf_sample: the den graph's in-arc table is missing");
+    const DenPlan &h = *g->host_plan;
+    int *off = nullptr, *src = nullptr;
+    float *w = nullptr;
+    if (Upload(&off, h.in_off) || Upload(&src, h.in_src) || Upload(&w, h.in_w)) {
+        cudaFree(off); cudaFree(src); cudaFree(w);
+        return 1;
+    }
+    g->in_src = src; g->in_w = w; g->in_off = off;
+    return 0;
+}
+
+size_t ccb_crf_sample_ws_bytes(int N, int K, int T) {
+    (void)T;   // the records carry the walk across segments; nothing in the workspace grows with the frames
+    int S, P;
+    bool small_ok;
+    CurrentSizes(&S, &P, &small_ok);
+    return N > 0 && K > 0 ? SampleWsBytes(N, K, S) : 0;
+}
+
+int ccb_crf_sample(const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k, const int *len_dev, int K,
+                   unsigned long long seed, int n_base, float *alpha_ws, void *aux_ws, void *sample_ws, int *tokens,
+                   int *lengths, int *align, float *path_logp, void *stream) {
+    g_err.clear();
+    DeviceGraph *g;
+    if (CurrentGraph(&g)) return 1;
+    if (Tmax <= 0 || Tmax > T) return Fail("crf_sample: Tmax must lie in [1, T]");
+    if (ckpt_k < 0) return Fail("crf_sample: checkpoint interval must be >= 0");
+    if (K <= 0 || n_base < 0) return Fail("crf_sample: bad sample count or utterance offset");
+    if (CheckDen(*g, dtype, N, Tmax, V)) return 1;
+    if (!logits || !len_dev || !alpha_ws || !aux_ws || !sample_ws || !tokens || !lengths || !align || !path_logp)
+        return Fail("crf_sample: missing buffer");
+    if (UploadSampleCsr(g)) return 1;
+    cudaStream_t s = (cudaStream_t)stream;
+    const long sn = (long)T * V, st = V;
+    const DenAuxLayout L = MakeDenAuxLayout(g->S, N, Tmax, g->small_ok);
+    const float *logz = reinterpret_cast<const float *>((char *)aux_ws + L.logz_a);
+    // log-probs or raw logits alike: every path emits one label per frame, so a per-frame shift cancels in p(path | x)
+    if (DenForward(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, s, false, ckpt_k)) return 1;
+    // frames (lo, hi] of alpha at positions t - lo: the full spill is the one segment (0, Tmax]
+    auto walk = [&](int lo, int hi, bool first) -> int {
+        int rc = LaunchSampleFinalPrefix(alpha_ws, lo, g->S, L.Npad, g->final_lin, len_dev, N, lo, hi, sample_ws,
+                                         K, s);
+        if (rc) return FailCuda("sample_final_prefix", (cudaError_t)rc);
+        rc = LaunchSampleWalk(*g, logits, dtype, sn, st, N, T, Tmax, L.Npad, len_dev, alpha_ws, lo, lo, hi, first,
+                              K, seed, n_base, logz, sample_ws, tokens, lengths, align, path_logp, s);
+        if (rc) return FailCuda("sample_walk", (cudaError_t)rc);
+        return 0;
+    };
+    if (ckpt_k <= 0) return walk(0, Tmax, true);
+    // checkpointed: each segment is recomputed from its checkpoint and walked, the last one first
+    for (int j = CkptCount(Tmax, ckpt_k) - 1; j >= 0; --j) {
+        int lo = 0, hi = 0;
+        if (DenRecompute(*g, logits, dtype, sn, st, N, Tmax, V, len_dev, alpha_ws, aux_ws, L, ckpt_k, j, &lo, &hi, s)) return 1;
+        if (walk(lo, hi, j == CkptCount(Tmax, ckpt_k) - 1)) return 1;
+    }
+    return 0;
+}
+
 /* ---- gpu_ctc/ctc.h surface ------------------------------------------------------------------- */
 const char *ctcGetStatusString(ctcStatus_t status) {
     switch (status) {
@@ -1019,6 +1099,9 @@ int ccb_plan_copy(void *plan, int which, void *dst, size_t dst_bytes) {
         case 16: src = p->hub_states.data(); bytes = p->hub_states.size() * 4; break;
         case 17: src = p->own_fwd.data(); bytes = (size_t)p->num_states * 2 * 4; break;   // (without the 4 floats of padding)
         case 18: src = p->own_bwd.data(); bytes = (size_t)p->num_states * 2 * 4; break;
+        case 19: src = p->in_off.data(); bytes = p->in_off.size() * 4; break;
+        case 20: src = p->in_src.data(); bytes = p->in_src.size() * 4; break;
+        case 21: src = p->in_w.data(); bytes = p->in_w.size() * 4; break;
         default: return 1;
     }
     if (bytes > dst_bytes) return 2;

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <memory>
 #include <string>
 
 #include "../../include/ctc_crf_b200.h"
@@ -51,6 +52,11 @@ struct DeviceGraph {
     // batches of <= 16 utterances run the small-batch kernels (rows of 16 floats): SmallBatchOk, decided once at Init
     bool small_ok = false;
     bool own_rows = false;     // DenPlan::own_rows: own-row coefficients instead of own-row arcs (DevicePass::own_c)
+    // the posterior sampler's in-arc CSR (DenPlan::in_off / in_src / in_w): uploaded by the first sampling call on the device,
+    // from the host copy Init keeps, so that callers who never sample do not hold it in device memory
+    std::shared_ptr<const DenPlan> host_plan;
+    int *in_off = nullptr, *in_src = nullptr;
+    float *in_w = nullptr;
 };
 
 // Kernel parameter block shared by the two persistent den kernels (passed as a __grid_constant__ kernel parameter: the TMA
@@ -204,6 +210,27 @@ int LaunchCtcViterbiSeqs(const void *y, int y_dtype, long sn, long st, int M, in
 int LaunchGradRowsScale(const float *grad, const float *w, const int *len, int N, int T, int V, void *out, int out_dtype,
                         cudaStream_t stream);
 void CountLaunch(int n = 1);
+// Posterior sampler (den_sample.cu) over alpha frames held at positions t - a_base of `alpha` ([pos][S][Npad]).
+// Workspace: a SampleRec per (utterance, sample), then per utterance S doubles of the final-state prefix sum.
+struct SampleRec {
+    int q;          // state at the frame the walk has reached
+    int last_lab;   // label of that frame (-1 before the first), for the collapse
+    int ntok;       // tokens written so far, last one first
+    int status;     // kSamplePending / kSampleWalking / kSampleDead
+    double score;   // sum of y + log w (+ log final) of the frames walked so far
+    double pad;
+};
+constexpr int kSamplePending = 0, kSampleWalking = 1, kSampleDead = 2;
+size_t SampleWsBytes(int N, int K, int S);
+// Final-state prefix sums of the utterances whose length lies in (t_lo, t_hi]
+int LaunchSampleFinalPrefix(const float *alpha, int a_base, int S, int Npad, const float *final_lin, const int *len, int N,
+                            int t_lo, int t_hi, void *sample_ws, int K, cudaStream_t stream);
+// The backward walk over frames (t_lo, t_hi] for all K samples of the N utterances; first: this is the first launch of the
+// call (initialise the records), t_lo == 0: the last (write the outputs)
+int LaunchSampleWalk(const DeviceGraph &g, const void *y, int y_dtype, long sn, long st, int N, int T, int Tmax, int Npad,
+                     const int *len, const float *alpha, int a_base, int t_lo, int t_hi, bool first, int K,
+                     unsigned long long seed, int n_base, const float *logz, void *sample_ws, int *tokens, int *lengths,
+                     int *align, float *path_logp, cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------------
 // device helpers

@@ -753,6 +753,16 @@ static bool BuildDenPlanImpl(const HostFst &fst, int n_ctas, int n_warps, bool a
     build(order);
     Layout(fgroups, (int)S, plan->state_label, plan->state_pos, n_ctas, n_warps, chunk_group, false, &plan->fwd);
     Layout(bgroups, (int)S, plan->state_label, plan->state_pos, n_ctas, n_warps, chunk_group, true, &plan->bwd);
+    // the sampler's in-arc CSR, rows in the final numbering, each row's arcs in file order
+    std::vector<int> sid_of_fid(S);
+    for (size_t s = 0; s < S; ++s) sid_of_fid[(size_t)fid[s]] = (int)s;
+    plan->in_off.assign(S + 1, 0);
+    plan->in_src.clear(); plan->in_w.clear();
+    plan->in_src.reserve(A); plan->in_w.reserve(A);
+    for (size_t f = 0; f < S; ++f) {
+        for (auto &a : in_s[(size_t)sid_of_fid[f]]) { plan->in_src.push_back(fid[(size_t)a.peer]); plan->in_w.push_back(a.w); }
+        plan->in_off[f + 1] = (int)plan->in_src.size();
+    }
     return true;
 }
 

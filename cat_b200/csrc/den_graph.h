@@ -101,6 +101,11 @@ struct DenPlan {
     //      two members share are gathered once.  Event kEvRow = one-row group, kEvRowPos1 = two-row group; the
     //      label-changed flags of the two rows are sign(w[0]) and sign(w[1]) of the last quad.
     PassPlan fwd, bwd;
+    // Plain in-arc CSR of the split graph in this renumbering, for the posterior sampler (den_sample.cu): the in-arcs of
+    // state q are in_off[q] .. in_off[q+1]-1, each with its source state in_src and its LINEAR weight in_w.  Every arc once:
+    // no pairs, no own-row coefficients, no padding, no event bits.
+    std::vector<int> in_off, in_src;
+    std::vector<float> in_w;
 };
 
 // Build the plan:

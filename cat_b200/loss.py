@@ -307,6 +307,36 @@ def ctc_align(logits, labels, input_lengths, label_lengths, utt=None):
     return core.ctc_align(logits.contiguous(), labels, input_lengths, label_lengths)
 
 
+def crf_sample(logits, lx, num_samples=1, generator=None):
+    """Draw label sequences from the CTC-CRF posterior of the den graph loaded by ``CRFContext``, exactly: forward filtering
+    (the den forward pass) and backward sampling, for sampling-based objectives (JSA, minimum-risk training with sampled
+    hypotheses, REINFORCE-style estimators).  A path is drawn with probability w(path) prod_t exp(y[t][label]) final / Z, so
+    for a T-compose-LM den graph the label sequence follows p_LM(l) p_ctc(l|x) / Z, the sequence posterior the loss
+    normalises by.  A per-frame multinomial on the softmax is exact only for a CTC model.
+
+    logits (N,T,V) fp32, bf16 or fp16 on the GPU: log-probs or raw logits, which give the same distribution (every path
+    emits one label per frame, so the log-softmax shift cancels); frames t >= lx[n] are never read.  lx (N,) int32 on the CPU.
+    num_samples K >= 1.  generator: a CPU torch.Generator (default: torch's), from which ONE 64-bit seed is drawn per call;
+    ``torch.manual_seed`` reproduces a call and successive calls differ.  The samples of an utterance depend on the seed, its
+    index in the batch and its own inputs only.
+
+    Returns device tensors, without synchronising the host and without recording autograd:
+      tokens (N,K,T) int32: the CTC collapse of each path (repeats merged, blank 0 dropped), padded with -1;
+      lengths (N,K) int32: tokens per sample;
+      align (N,K,T) int32: the label of every frame t < lx[n] (blank included), -1 beyond, as ``ctc_align``;
+      path_logp (N,K) fp32: log p(path | x), accumulated in fp64.
+    An utterance with no path of finite score (lx = 0, -inf frames, no reachable final state) gets lengths -1, rows of -1
+    and path_logp -inf.  ``samples_to_labels`` turns the result into the ``utt=`` arguments of ``CTC_CRF_LOSS``."""
+    return core.crf_sample(logits, lx, num_samples, generator)
+
+
+def samples_to_labels(tokens, lengths):
+    """(labels, ly, utt) CPU int32 tensors for ``CTC_CRF_LOSS(...)(logits, labels, lx, ly, utt=utt)`` from the
+    ``crf_sample`` outputs: every feasible sample (lengths >= 0), utterance by utterance, samples in order; infeasible samples
+    are dropped.  It performs ONE device-to-host copy, which waits for the sampler."""
+    return core.samples_to_labels(tokens, lengths)
+
+
 class CRFContext:
     def __init__(self, den_lm: str, gpus: Union[int, List[int]]) -> None:
         """

@@ -286,6 +286,27 @@ int ccb_ctc_align(const void *logits, int dtype, long sn, long st, int N, int T,
                   const int *labels_dev, const int *label_off_dev, const int *label_len_dev, const int *len_dev,
                   int max_label_len, int blank, void *workspace, int *align, float *score, void *stream);
 
+/* Exact samples from the CTC-CRF posterior p(path | x) over the den graph loaded by Init (forward filtering, backward
+ * sampling): K paths per utterance, each drawn with probability w(path) prod_t exp(y[t][lab]) final / Z.  The den forward
+ * pass runs once per utterance; then one warp per (utterance, sample) walks back from a final state drawn with probability
+ * ~ alpha_len(q) final(q), drawing at every frame a predecessor p with probability ~ alpha_{t-1}(p) w_pq.
+ *   logits   (N,T,V) log-probs or raw logits in the CCB_DTYPE_* code dtype (the same distribution: the per-frame log-softmax
+ *            shift cancels); only frames t < len are read.
+ *   Tmax     the longest length (<= T); ckpt_k 0: the full alpha spill, > 0: checkpointed alpha (ccb_ctc_crf_loss_ckpt_fwd),
+ *            each segment recomputed and walked, the last one first.  alpha_ws / aux_ws as for the loss entries.
+ *   seed     64-bit Philox4x32-10 key; the uniform that picks the state of frame t of sample k of utterance n is counter
+ *            (t, k, n_base + n, 0), so an utterance's samples do not depend on the rest of the batch.
+ *   sample_ws  ccb_crf_sample_ws_bytes(N, K, Tmax) bytes.
+ *   tokens (N,K,T) int32 out: the CTC collapse of each path (repeats merged, blank 0 dropped), -1 after the last token;
+ *   lengths (N,K) int32 out: token count; align (N,K,T) int32 out: the label of every frame t < len (blank included), -1
+ *   beyond; path_logp (N,K) fp32 out: log p(path | x), accumulated in fp64.  An utterance with no path of finite score (length
+ *   0, -inf frames, no final state reachable) gets length -1, rows of -1 and -inf.  Everything is enqueued on `stream`; the
+ *   first call on a device uploads the graph's in-arc table (about 8 bytes per arc) synchronously. */
+size_t ccb_crf_sample_ws_bytes(int N, int K, int T);
+int ccb_crf_sample(const void *logits, int dtype, int N, int T, int V, int Tmax, int ckpt_k, const int *len_dev, int K,
+                   unsigned long long seed, int n_base, float *alpha_ws, void *aux_ws, void *sample_ws, int *tokens,
+                   int *lengths, int *align, float *path_logp, void *stream);
+
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 long ccb_launch_count(void);
 
@@ -307,7 +328,10 @@ int ccb_plan_info(void *plan, long *info);
  *        3 fwd_arcs[A_fwd] {u32 peer, f32 w (sign bits = segment events)}, 4 fwd_chunk_state[n_ctas*n_warps+1] i32,
  *        5 fwd_chunk_arc[n_ctas*n_warps+1] i32, 6 bwd_arcs[A_bwd], 7 bwd_chunk_state, 8 bwd_chunk_arc,
  *        9 state_pos[S] i32, 10 fwd_chunk_pair, 11 bwd_chunk_pair, 12 start_arcs[n_start_arcs],
- *        13 fwd_cta_labels[n_ctas*4] i32, 14 bwd_cta_labels, 15 bwd second weights f32[A_bwd], 16 hub_states[n_hubs] i32 */
+ *        13 fwd_cta_labels[n_ctas*4] i32, 14 bwd_cta_labels, 15 bwd second weights f32[A_bwd], 16 hub_states[n_hubs] i32,
+ *        17 / 18 own-row coefficients f32[2S] of the forward / backward pass,
+ *        19 in_off[S+1] i32, 20 in_src[A] i32, 21 in_w[A] f32: the in-arc CSR of the split graph the sampler walks (every arc
+ *        once, A = in_off[S], linear weights) */
 int ccb_plan_copy(void *plan, int which, void *dst, size_t dst_bytes);
 /* The den kernel launch chosen for one pass (backward 0 / 1) of N utterances at smem_optin bytes of shared memory per block;
  * hooks: bit 0 CCB_ARCS_IN_GLOBAL, 1 CCB_W1_IN_GLOBAL, 2 CCB_NO_TMA, 3 CCB_OWN_IN_L2.  out[0..14] = tier (0 arcs in shared
