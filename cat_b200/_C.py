@@ -13,7 +13,8 @@ and ``ctc_loss_fwd_only`` -- the losses without a gradient, used when grad mode 
 ``grad_rows_scale`` is the backward of the per-utterance costs.  ``ctc_crf_loss_seqs``, ``ctc_crf_loss_seqs_fwd_only``,
 ``ctc_loss_seqs`` and ``ctc_align_seqs`` take several label sequences per utterance (``utt``: the logits row of each), with the
 den passes run once per utterance; ``seqs_backward`` is the backward of their per-sequence costs.  ``crf_sample`` draws paths
-from the CTC-CRF posterior and ``samples_to_labels`` packs them for the ``utt=`` loss.
+from the CTC-CRF posterior and ``samples_to_labels`` packs them for the ``utt=`` loss.  ``ctc_beam_search`` returns N-best
+lists by CTC prefix beam search, over the logits or over the den graph.
 """
 from __future__ import annotations
 
@@ -947,6 +948,46 @@ def samples_to_labels(tokens: torch.Tensor, lengths: torch.Tensor) -> Tuple[torc
     labels = rows[torch.arange(T).unsqueeze(0) < ly.unsqueeze(1)]
     utt = torch.arange(N, dtype=torch.int32).repeat_interleave(K)[keep]
     return labels.to(torch.int32).contiguous(), ly.to(torch.int32).contiguous(), utt.contiguous()
+
+
+# ---------------------------------------------------------------------------------------------------
+# prefix beam search
+# ---------------------------------------------------------------------------------------------------
+MAX_BEAM = 128
+
+
+def _check_beam_args(logits, lx, beam_size, cutoff_top_n):
+    N, T, V = _check_sample_args(logits, lx, 1)
+    for name, v, hi in (("beam_size", beam_size, MAX_BEAM), ("cutoff_top_n", cutoff_top_n, V)):
+        if isinstance(v, bool) or not isinstance(v, int) or not 1 <= v <= hi:
+            raise RuntimeError(f"{name} must be an int in [1, {hi}], not {v!r}")
+    return N, T, V
+
+
+def ctc_beam_search(logits: torch.Tensor, lx: torch.Tensor, beam_size: int, cutoff_top_n: int, crf: bool
+                    ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """The beam_size best label sequences per utterance by CTC prefix beam search, over the logits alone (crf False) or over
+    the loaded den graph (crf True).  Returns device tensors (tokens (N,B,T) int32, lengths (N,B) int32, timesteps (N,B,T)
+    int32, scores (N,B) fp32); see ``ctc_crf.ctc_beam_search``.  One native call for the batch; never synchronises the
+    host."""
+    N, T, V = _check_beam_args(logits, lx, beam_size, cutoff_top_n)
+    B = beam_size
+    L = _lib.lib()
+    dev = logits.device
+    with torch.no_grad(), torch.cuda.device(dev):
+        y = logits.detach().contiguous()
+        lens = _rings.setdefault(torch.device(dev).index, _PinnedRing()).stage([lx], dev)
+        tokens = torch.empty((N, B, T), dtype=torch.int32, device=dev)
+        lengths = torch.empty((N, B), dtype=torch.int32, device=dev)
+        timesteps = torch.empty((N, B, T), dtype=torch.int32, device=dev)
+        scores = torch.empty((N, B), dtype=torch.float32, device=dev)
+        ws = torch.empty(int(L.ccb_ctc_beam_search_ws_bytes(N, T, B)), dtype=torch.uint8, device=dev)
+        rc = L.ccb_ctc_beam_search(y.data_ptr(), _DTYPES[y.dtype], N, T, V, lens.data_ptr(), B, int(cutoff_top_n), int(bool(crf)),
+                                   ws.data_ptr(), tokens.data_ptr(), lengths.data_ptr(), timesteps.data_ptr(),
+                                   scores.data_ptr(), _stream(dev))
+        _check(rc, "ctc_beam_search")
+        lens.record_stream(torch.cuda.current_stream(dev))
+    return tokens, lengths, timesteps, scores
 
 
 def launch_count() -> int:

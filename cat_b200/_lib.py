@@ -29,7 +29,7 @@ SYMBOLS = [
     "ccb_den_fwd_alpha_floats", "ccb_num_fwd_only_bytes", "ccb_ctc_crf_loss_fwd_only", "ccb_ctc_loss_fwd_only",
     "ccb_ctc_crf_loss_costs", "ccb_ctc_crf_loss_costs_fwd_only", "ccb_ctc_loss_costs", "ccb_grad_rows_scale",
     "ccb_ctc_crf_loss_seqs", "ccb_ctc_crf_loss_seqs_fwd_only", "ccb_ctc_loss_seqs", "ccb_seqs_grad", "ccb_ctc_align_seqs",
-    "ccb_crf_sample_ws_bytes", "ccb_crf_sample",
+    "ccb_crf_sample_ws_bytes", "ccb_crf_sample", "ccb_ctc_beam_search_ws_bytes", "ccb_ctc_beam_search", "ccb_plan_ctc_shape",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -121,6 +121,10 @@ def lib() -> C.CDLL:
     L.ccb_crf_sample_ws_bytes.argtypes = [i, i, i]; L.ccb_crf_sample_ws_bytes.restype = C.c_size_t
     L.ccb_crf_sample.argtypes = [vp, i, i, i, i, i, i, vp, i, C.c_uint64, i, vp, vp, vp, vp, vp, vp, vp, vp]
     L.ccb_crf_sample.restype = C.c_int
+    L.ccb_ctc_beam_search_ws_bytes.argtypes = [i, i, i]; L.ccb_ctc_beam_search_ws_bytes.restype = C.c_size_t
+    L.ccb_ctc_beam_search.argtypes = [vp, i, i, i, i, vp, i, i, i, vp, vp, vp, vp, vp, vp]
+    L.ccb_ctc_beam_search.restype = C.c_int
+    L.ccb_plan_ctc_shape.argtypes = [vp]; L.ccb_plan_ctc_shape.restype = C.c_int
     L.ccb_launch_count.argtypes = []; L.ccb_launch_count.restype = C.c_long
     L.ccb_debug_timeline.argtypes = [vp, C.c_int, C.c_int]; L.ccb_debug_timeline.restype = None
     L.ccb_plan_create.argtypes = [C.c_char_p, C.c_int, C.c_int]; L.ccb_plan_create.restype = vp

@@ -74,6 +74,7 @@ void FreeDevice(DeviceGraph &d) {
     cudaFree(d.state_label); cudaFree(d.state_pos); cudaFree(d.final_lin); cudaFree(d.start_arcs); cudaFree(d.hub_states);
     for (DevicePass *p : {&d.fwd, &d.bwd}) { cudaFree(p->arcs); cudaFree(p->chunk_state); cudaFree(p->chunk_arc); cudaFree(p->chunk_pair); cudaFree(p->cta_labels); cudaFree(p->w1); cudaFree(p->tq); cudaFree(p->own_c); }
     cudaFree(d.in_off); cudaFree(d.in_src); cudaFree(d.in_w);
+    cudaFree(d.out_off); cudaFree(d.out_dst); cudaFree(d.out_w);
     d = DeviceGraph();
 }
 
@@ -140,9 +141,13 @@ int InitImpl(const char *fst_name, int n_gpus, const int *gpus) {
     g_plan_valid = true;
     DEN_NUM_STATES = g_plan.num_states + g_plan.num_pairs;   // rows per alpha frame (what binding.cpp sizes scratch with)
     DEN_NUM_ARCS = (int)g_plan.fwd.arcs.size();
-    // the sampler's in-arc CSR stays on the host until a sampling call needs it on a device (UploadSampleCsr)
+    // the sampler's in-arc CSR and the beam search's out-arc CSR stay on the host until a call needs them on a device
+    // (UploadSampleCsr, EnsureBeamGraph)
     auto csr = std::make_shared<DenPlan>();
     csr->in_off = g_plan.in_off; csr->in_src = g_plan.in_src; csr->in_w = g_plan.in_w;
+    csr->out_off = g_plan.out_off; csr->out_dst = g_plan.out_dst; csr->out_w = g_plan.out_w;
+    csr->num_states = g_plan.num_states; csr->start = g_plan.start;
+    csr->state_label = g_plan.state_label; csr->orig_state = g_plan.orig_state;
     int rc = 0;
     for (int i = 0; i < n_gpus && rc == 0; ++i) {
         DeviceGraph &d = g_dev[gpus[i]];
@@ -982,6 +987,60 @@ int ccb_crf_sample(const void *logits, int dtype, int N, int T, int V, int Tmax,
     return 0;
 }
 
+/* ---- CTC prefix beam search ------------------------------------------------------------------ */
+// crf mode: the CTC-shape check of the device's graph (once; the result is kept) and its out-arc CSR on the device
+static int EnsureBeamGraph(DeviceGraph *g) {
+    std::lock_guard<std::mutex> lk(g_mu);
+    if (g->ctc_shape < 0) {
+        if (!g->host_plan) return Fail("ctc_beam_search: the den graph's out-arc table is missing");
+        std::string err;
+        g->ctc_shape = CheckCtcShape(*g->host_plan, &err) ? 0 : 1;
+        g->ctc_shape_err = err;
+    }
+    if (g->ctc_shape != 0) return Fail("ctc_beam_search(crf=1): " + g->ctc_shape_err);
+    if (g->out_off) return 0;
+    const DenPlan &h = *g->host_plan;
+    int *off = nullptr, *dst = nullptr;
+    float *w = nullptr;
+    if (Upload(&off, h.out_off) || Upload(&dst, h.out_dst) || Upload(&w, h.out_w)) {
+        cudaFree(off); cudaFree(dst); cudaFree(w);
+        return 1;
+    }
+    g->out_dst = dst; g->out_w = w; g->out_off = off;
+    return 0;
+}
+
+size_t ccb_ctc_beam_search_ws_bytes(int N, int T, int beam) {
+    return N > 0 && T > 0 && beam >= 1 && beam <= kBeamMax ? BeamWsBytes(N, T, beam) : 0;
+}
+
+int ccb_ctc_beam_search(const void *logits, int dtype, int N, int T, int V, const int *len_dev, int beam, int cutoff_top_n,
+                        int crf, void *workspace, int *tokens, int *lengths, int *timesteps, float *scores, void *stream) {
+    g_err.clear();
+    if (N <= 0 || T <= 0 || V <= 0) return Fail("ctc_beam_search: N, T and V must be positive");
+    if (!KnownDtype(dtype)) return FailDtype("ctc_beam_search", dtype);
+    if (beam < 1 || beam > kBeamMax)
+        return Fail("ctc_beam_search: beam must lie in [1, " + std::to_string(kBeamMax) + "], not " + std::to_string(beam));
+    if (cutoff_top_n < 1 || cutoff_top_n > V)
+        return Fail("ctc_beam_search: cutoff_top_n must lie in [1, V] = [1, " + std::to_string(V) + "], not " +
+                    std::to_string(cutoff_top_n));
+    if (V > kBeamMaxV) return Fail("ctc_beam_search: at most " + std::to_string(kBeamMaxV) + " labels, not " + std::to_string(V));
+    if (!logits || !len_dev || !workspace || !tokens || !lengths || !timesteps || !scores)
+        return Fail("ctc_beam_search: missing buffer");
+    DeviceGraph *g = nullptr;
+    if (crf) {
+        if (CurrentGraph(&g)) return 1;
+        if (g->num_labels > V)
+            return Fail("ctc_beam_search: the den graph has labels up to " + std::to_string(g->num_labels - 1) + ", V is " +
+                        std::to_string(V));
+        if (EnsureBeamGraph(g)) return 1;
+    }
+    const int rc = LaunchBeamSearch(g, logits, dtype, N, T, V, len_dev, beam, cutoff_top_n, workspace, tokens, lengths,
+                                    timesteps, scores, (cudaStream_t)stream);
+    if (rc) return FailCuda("beam_search", (cudaError_t)rc);
+    return 0;
+}
+
 /* ---- gpu_ctc/ctc.h surface ------------------------------------------------------------------- */
 const char *ctcGetStatusString(ctcStatus_t status) {
     switch (status) {
@@ -1102,11 +1161,21 @@ int ccb_plan_copy(void *plan, int which, void *dst, size_t dst_bytes) {
         case 19: src = p->in_off.data(); bytes = p->in_off.size() * 4; break;
         case 20: src = p->in_src.data(); bytes = p->in_src.size() * 4; break;
         case 21: src = p->in_w.data(); bytes = p->in_w.size() * 4; break;
+        case 22: src = p->out_off.data(); bytes = p->out_off.size() * 4; break;
+        case 23: src = p->out_dst.data(); bytes = p->out_dst.size() * 4; break;
+        case 24: src = p->out_w.data(); bytes = p->out_w.size() * 4; break;
         default: return 1;
     }
     if (bytes > dst_bytes) return 2;
     memcpy(dst, src, bytes);
     return 0;
+}
+
+int ccb_plan_ctc_shape(void *plan) {
+    g_err.clear();
+    if (!plan) return Fail("ccb_plan_ctc_shape: null plan");
+    std::string err;
+    return CheckCtcShape(*reinterpret_cast<const DenPlan *>(plan), &err) ? 0 : Fail(err);
 }
 
 static int PlanLaunch(void *plan, int N, int backward, int smem_optin, int hooks, DenLaunch *L, int *Npad) {

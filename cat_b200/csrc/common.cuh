@@ -57,6 +57,12 @@ struct DeviceGraph {
     std::shared_ptr<const DenPlan> host_plan;
     int *in_off = nullptr, *in_src = nullptr;
     float *in_w = nullptr;
+    // the beam search's out-arc CSR (DenPlan::out_off / out_dst / out_w), likewise uploaded by the first crf=1 beam search on
+    // the device, after CheckCtcShape has passed; ctc_shape caches that check (-1 not run yet, 0 passed, 1 failed: ctc_shape_err)
+    int *out_off = nullptr, *out_dst = nullptr;
+    float *out_w = nullptr;
+    int ctc_shape = -1;
+    std::string ctc_shape_err;
 };
 
 // Kernel parameter block shared by the two persistent den kernels (passed as a __grid_constant__ kernel parameter: the TMA
@@ -231,6 +237,13 @@ int LaunchSampleWalk(const DeviceGraph &g, const void *y, int y_dtype, long sn, 
                      const int *len, const float *alpha, int a_base, int t_lo, int t_hi, bool first, int K,
                      unsigned long long seed, int n_base, const float *logz, void *sample_ws, int *tokens, int *lengths,
                      int *align, float *path_logp, cudaStream_t stream);
+// CTC prefix beam search (beam_search.cu): one CTA per utterance, one launch for the batch.  g: the den graph for crf mode,
+// null for plain CTC.  Workspace: per utterance the trie (B*T + 1 nodes) and its hash table.
+constexpr int kBeamMax = 128;
+constexpr int kBeamMaxV = 8192;
+size_t BeamWsBytes(int N, int T, int B);
+int LaunchBeamSearch(const DeviceGraph *g, const void *y, int y_dtype, int N, int T, int V, const int *len, int B, int topn,
+                     void *ws, int *tokens, int *lengths, int *timesteps, float *scores, cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------------
 // device helpers

@@ -9,6 +9,7 @@
 #include <cstring>
 #include <limits>
 #include <numeric>
+#include <unordered_set>
 
 namespace ccb {
 
@@ -762,6 +763,112 @@ static bool BuildDenPlanImpl(const HostFst &fst, int n_ctas, int n_warps, bool a
     for (size_t f = 0; f < S; ++f) {
         for (auto &a : in_s[(size_t)sid_of_fid[f]]) { plan->in_src.push_back(fid[(size_t)a.peer]); plan->in_w.push_back(a.w); }
         plan->in_off[f + 1] = (int)plan->in_src.size();
+    }
+    // the beam search's out-arc CSR: the same arcs by source, sorted by destination label, then destination
+    plan->out_off.assign(S + 1, 0);
+    for (int q : plan->in_src) ++plan->out_off[(size_t)q + 1];
+    for (size_t s = 0; s < S; ++s) plan->out_off[s + 1] += plan->out_off[s];
+    plan->out_dst.assign(plan->in_src.size(), 0);
+    plan->out_w.assign(plan->in_src.size(), 0.f);
+    {
+        std::vector<int> fill(plan->out_off.begin(), plan->out_off.end() - 1);
+        for (size_t f = 0; f < S; ++f)
+            for (int i = plan->in_off[f]; i < plan->in_off[f + 1]; ++i) {
+                const int k = fill[(size_t)plan->in_src[(size_t)i]]++;
+                plan->out_dst[(size_t)k] = (int)f;
+                plan->out_w[(size_t)k] = plan->in_w[(size_t)i];
+            }
+        std::vector<std::pair<int, int>> row;
+        std::vector<float> roww;
+        for (size_t s = 0; s < S; ++s) {
+            const int b = plan->out_off[s], e = plan->out_off[s + 1];
+            row.clear();
+            for (int i = b; i < e; ++i) row.emplace_back(i, plan->out_dst[(size_t)i]);
+            std::sort(row.begin(), row.end(), [&](const std::pair<int, int> &x, const std::pair<int, int> &y) {
+                const int lx = plan->state_label[(size_t)x.second], ly = plan->state_label[(size_t)y.second];
+                return lx != ly ? lx < ly : (x.second != y.second ? x.second < y.second : x.first < y.first);
+            });
+            roww.clear();
+            for (auto &r : row) roww.push_back(plan->out_w[(size_t)r.first]);
+            for (int i = b; i < e; ++i) {
+                plan->out_dst[(size_t)i] = row[(size_t)(i - b)].second;
+                plan->out_w[(size_t)i] = roww[(size_t)(i - b)];
+            }
+        }
+    }
+    return true;
+}
+
+namespace {
+// the out-arc of p into a state of label c (-1: none); the labels of a state's out-arcs are sorted
+int OutArcTo(const DenPlan &g, int p, int c) {
+    if (p < 0) return -1;
+    int lo = g.out_off[(size_t)p], hi = g.out_off[(size_t)p + 1];
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (g.state_label[(size_t)g.out_dst[(size_t)mid]] < c) lo = mid + 1; else hi = mid;
+    }
+    return lo < g.out_off[(size_t)p + 1] && g.state_label[(size_t)g.out_dst[(size_t)lo]] == c ? g.out_dst[(size_t)lo] : -1;
+}
+
+std::string StateName(const DenPlan &g, int q) {
+    return std::to_string(q) + " (file state " + std::to_string(g.orig_state[(size_t)q]) + ", label " +
+           std::to_string(g.state_label[(size_t)q]) + ")";
+}
+}  // namespace
+
+bool CheckCtcShape(const DenPlan &g, std::string *err) {
+    const int S = g.num_states;
+    for (int p = 0; p < S; ++p)
+        for (int i = g.out_off[(size_t)p] + 1; i < g.out_off[(size_t)p + 1]; ++i) {
+            const int a = g.out_dst[(size_t)i - 1], b = g.out_dst[(size_t)i];
+            if (g.state_label[(size_t)a] == g.state_label[(size_t)b]) {
+                *err = "den graph is not CTC-shaped: state " + StateName(g, p) + " has out-arcs into two states of label " +
+                       std::to_string(g.state_label[(size_t)a]) + ": " + StateName(g, a) + " and " + StateName(g, b);
+                return false;
+            }
+        }
+    // a slot in state q that reads label c again (the blank slot: blank; the token slot: its token) must stay in q
+    auto stays = [&](int q, int c, const char *slot) {
+        const int d = OutArcTo(g, q, c);
+        if (d < 0 || d == q) return true;
+        *err = std::string("den graph is not CTC-shaped: the ") + slot + " slot in state " + StateName(g, q) +
+               " moves to state " + StateName(g, d) + " on label " + std::to_string(c) + " instead of staying";
+        return false;
+    };
+    // signature of a prefix: (blank-slot state, token-slot state), -1 = empty; the last token is the token-slot state's label
+    auto key = [](int b, int t) { return ((uint64_t)(uint32_t)(b + 1) << 32) | (uint32_t)(t + 1); };
+    std::unordered_set<uint64_t> seen;
+    std::vector<std::pair<int, int>> queue;
+    if (!stays(g.start, 0, "blank")) return false;
+    queue.emplace_back(g.start, -1);
+    seen.insert(key(g.start, -1));
+    std::vector<int> labels;
+    for (size_t head = 0; head < queue.size(); ++head) {
+        const int b = queue[head].first, t = queue[head].second;
+        const int last = t >= 0 ? g.state_label[(size_t)t] : -1;
+        labels.clear();
+        for (int q : {b, t})
+            if (q >= 0)
+                for (int i = g.out_off[(size_t)q]; i < g.out_off[(size_t)q + 1]; ++i) labels.push_back(g.state_label[(size_t)g.out_dst[(size_t)i]]);
+        std::sort(labels.begin(), labels.end());
+        labels.erase(std::unique(labels.begin(), labels.end()), labels.end());
+        for (int c : labels) {
+            if (c == 0) continue;
+            const int d1 = OutArcTo(g, b, c), d2 = c != last ? OutArcTo(g, t, c) : -1;
+            if (d1 >= 0 && d2 >= 0 && d1 != d2) {
+                *err = "den graph is not CTC-shaped: the blank slot in state " + StateName(g, b) + " and the token slot in state " +
+                       StateName(g, t) + " of one prefix step into different states " + StateName(g, d1) + " and " +
+                       StateName(g, d2) + " on token " + std::to_string(c);
+                return false;
+            }
+            const int nt = d1 >= 0 ? d1 : d2;
+            if (nt < 0) continue;
+            if (!stays(nt, c, "token")) return false;
+            const int nb = OutArcTo(g, nt, 0);
+            if (nb >= 0 && !stays(nb, 0, "blank")) return false;
+            if (seen.insert(key(nb, nt)).second) queue.emplace_back(nb, nt);
+        }
     }
     return true;
 }

@@ -106,7 +106,19 @@ struct DenPlan {
     // no pairs, no own-row coefficients, no padding, no event bits.
     std::vector<int> in_off, in_src;
     std::vector<float> in_w;
+    // The same arcs as an out-arc CSR, for the prefix beam search (beam_search.cu): the out-arcs of state p are
+    // out_off[p] .. out_off[p+1]-1, sorted by the label of their destination out_dst (then by out_dst), with LINEAR weights
+    // out_w, so that the arc of p into a state of label c is found by binary search.
+    std::vector<int> out_off, out_dst;
+    std::vector<float> out_w;
 };
+
+// The condition under which a CTC prefix beam search over the plan's split graph is exact with two slots per prefix
+// (DESIGN.md §7 "Prefix beam search"): no state has two out-arcs into states of one label, and every prefix reachable from
+// the start state keeps ONE state in its blank slot and ONE in its token slot -- both slots step into the same state on a
+// new token, the token slot repeats in place, the blank slot stays in place.  Breadth-first search over the signatures
+// (blank-slot state, token-slot state) of the prefixes.  Returns false and names the states in *err when it does not hold.
+bool CheckCtcShape(const DenPlan &plan, std::string *err);
 
 // Build the plan:
 //  1. split every state by the label of its incoming arcs so that each state has exactly one in-label

@@ -337,6 +337,63 @@ def samples_to_labels(tokens, lengths):
     return core.samples_to_labels(tokens, lengths)
 
 
+def ctc_beam_search(logits, lx, beam_size=16, cutoff_top_n=40, crf=False):
+    """N-best label sequences by CTC prefix beam search on the GPU (DESIGN.md §7 "Prefix beam search").
+
+    crf False: plain CTC, as ``ctcdecode`` computes it without a word LM -- a hypothesis collects the paths whose CTC
+    collapse it is, each path scored sum_t y[t][label].  crf True: the paths run over the den graph loaded by ``CRFContext``
+    and carry its arc and final weights, so for a T-compose-LM graph a sequence's total is log p_LM(l) + log p_ctc(l|x),
+    the CTC-CRF posterior up to log Z.  The graph must be CTC-shaped (both slots of a prefix step into one state on a token;
+    checked at the first crf call per graph and device, RuntimeError naming the states otherwise).
+
+    logits (N,T,V) fp32, bf16 or fp16 on the GPU, log-probs or raw logits: every path has lx[n] frames, so raw logits give the
+    same hypotheses, each score shifted by sum_t logsumexp(logits[n,t]).  Frames t >= lx[n] are never read.  lx (N,) int32
+    on the CPU.  beam_size B in 1..128; cutoff_top_n in 1..V: a frame extends hypotheses by its cutoff_top_n most likely
+    tokens (ties: lower id), plus blank and each hypothesis's own last token.
+
+    Returns device tensors, best first, without synchronising the host and without recording autograd:
+      tokens (N,B,T) int32, padded with -1; lengths (N,B) int32;
+      timesteps (N,B,T) int32: the frame at which each token's prefix first entered the beam, -1 padded;
+      scores (N,B) fp32: the log-sum of the kept paths (fp64 inside), a lower bound on the sequence's log mass, exact when
+      nothing was pruned.
+    Rows past the hypotheses of finite score have length -1, tokens -1 and score -inf; lx = 0 gives the empty sequence.
+    ``samples_to_labels(tokens, lengths)`` turns the lists into the ``utt=`` arguments of the losses."""
+    return core.ctc_beam_search(logits, lx, beam_size, cutoff_top_n, crf)
+
+
+class CTCBeamDecoder:
+    """Drop-in for ``ctcdecode.CTCBeamDecoder`` without a word LM, on the GPU (``ctc_beam_search``, plain CTC).
+    ``decode(probs, seq_lens)`` returns (beam_results (N,B,T), beam_scores (N,B) = -log score, timesteps (N,B,T),
+    out_lens (N,B)) as ``ctcdecode`` does, on the device of the input (CPU inputs run on the current CUDA device).
+    model_path, blank_id != 0 and cutoff_prob != 1.0 are not supported (NotImplementedError); alpha, beta and
+    num_processes are accepted and unused."""
+
+    def __init__(self, labels, model_path=None, alpha=0, beta=0, cutoff_top_n=40, cutoff_prob=1.0, beam_width=100,
+                 num_processes=4, blank_id=0, log_probs_input=False):
+        if model_path is not None:
+            raise NotImplementedError("CTCBeamDecoder: word-level LMs (model_path) are not supported")
+        if blank_id != 0:
+            raise NotImplementedError("CTCBeamDecoder: the blank must be label 0")
+        if cutoff_prob != 1.0:
+            raise NotImplementedError("CTCBeamDecoder: cutoff_prob must be 1.0 (use cutoff_top_n)")
+        self._labels = list(labels)
+        self._cutoff_top_n = min(int(cutoff_top_n), len(self._labels))
+        self._beam_width = int(beam_width)
+        self._log_probs_input = bool(log_probs_input)
+
+    def decode(self, probs, seq_lens=None):
+        """probs (N,T,V): probabilities, or log-probabilities with log_probs_input=True.  seq_lens (N,): frames per utterance
+        (default: all T)."""
+        x = probs if probs.is_cuda else probs.to(torch.device("cuda", torch.cuda.current_device()))
+        if not self._log_probs_input:
+            x = x.float().log()
+        N, T, _ = x.shape
+        lx = torch.full((N,), T, dtype=torch.int32) if seq_lens is None else torch.as_tensor(seq_lens).to("cpu", torch.int32)
+        tokens, lengths, timesteps, scores = core.ctc_beam_search(x, lx, self._beam_width,
+                                                                  min(self._cutoff_top_n, int(x.shape[2])), False)
+        return tokens, -scores, timesteps, lengths
+
+
 class CRFContext:
     def __init__(self, den_lm: str, gpus: Union[int, List[int]]) -> None:
         """

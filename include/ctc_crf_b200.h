@@ -307,6 +307,27 @@ int ccb_crf_sample(const void *logits, int dtype, int N, int T, int V, int Tmax,
                    unsigned long long seed, int n_base, float *alpha_ws, void *aux_ws, void *sample_ws, int *tokens,
                    int *lengths, int *align, float *path_logp, void *stream);
 
+/* CTC prefix beam search: the `beam` best label sequences of every utterance, one CTA per utterance, one launch.
+ *   crf 0: plain CTC -- a path is any frame-label sequence, scored sum_t y[t][lab_t];
+ *   crf 1: over the split den graph loaded by Init -- a path is a state sequence from the start state, scored
+ *          sum log w(arcs) + sum_t y[t][lab(q_t)] + log final(q_len): for a T-compose-LM graph, a label sequence's total is
+ *          log p_LM(l) + log p_ctc(l|x).  The graph must pass the CTC-shape check (ccb_plan_ctc_shape), run once per graph
+ *          and device at the first crf=1 call, which also uploads the out-arc table (about 12 bytes per arc) synchronously.
+ * A hypothesis's score is the log-sum of the scores of its paths the beam kept (fp64 inside): a lower bound on the exact
+ * log mass of the sequence, equal to it when nothing was pruned.  Raw logits give the same hypotheses as their log-softmax,
+ * with every score shifted by sum_t logsumexp(y[t]).
+ *   logits   (N,T,V) contiguous in the CCB_DTYPE_* code dtype; only frames t < len are read.  V <= 8192.
+ *   beam     1 .. 128; cutoff_top_n 1 .. V: the tokens of a frame are its cutoff_top_n largest entries (ties: lower id),
+ *            plus blank and each hypothesis's own last token.  Ties between candidates break on (parent rank, token).
+ *   workspace  ccb_ctc_beam_search_ws_bytes(N, T, beam) bytes; nothing needs to be initialised.
+ *   tokens (N,beam,T) int32 out, -1 padded; lengths (N,beam) int32 out; timesteps (N,beam,T) int32 out: the frame at
+ *   which the trie node of each token was created, -1 padded; scores (N,beam) fp32 out, best first.  Rows beyond the
+ *   hypotheses of finite score get length -1, tokens and timesteps -1 and score -inf.  len = 0 gives the empty sequence,
+ *   scored 0 (crf 0) or log final(start) (crf 1). */
+size_t ccb_ctc_beam_search_ws_bytes(int N, int T, int beam);
+int ccb_ctc_beam_search(const void *logits, int dtype, int N, int T, int V, const int *len_dev, int beam, int cutoff_top_n,
+                        int crf, void *workspace, int *tokens, int *lengths, int *timesteps, float *scores, void *stream);
+
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 long ccb_launch_count(void);
 
@@ -331,8 +352,12 @@ int ccb_plan_info(void *plan, long *info);
  *        13 fwd_cta_labels[n_ctas*4] i32, 14 bwd_cta_labels, 15 bwd second weights f32[A_bwd], 16 hub_states[n_hubs] i32,
  *        17 / 18 own-row coefficients f32[2S] of the forward / backward pass,
  *        19 in_off[S+1] i32, 20 in_src[A] i32, 21 in_w[A] f32: the in-arc CSR of the split graph the sampler walks (every arc
- *        once, A = in_off[S], linear weights) */
+ *        once, A = in_off[S], linear weights),
+ *        22 out_off[S+1] i32, 23 out_dst[A] i32, 24 out_w[A] f32: the same arcs as an out-arc CSR, each state's arcs sorted
+ *        by the label of their destination (the beam search's table) */
 int ccb_plan_copy(void *plan, int which, void *dst, size_t dst_bytes);
+/* The CTC-shape check of ccb_ctc_beam_search(crf=1) on a plan: 0 if it holds, 1 if not (ccb_last_error names the states) */
+int ccb_plan_ctc_shape(void *plan);
 /* The den kernel launch chosen for one pass (backward 0 / 1) of N utterances at smem_optin bytes of shared memory per block;
  * hooks: bit 0 CCB_ARCS_IN_GLOBAL, 1 CCB_W1_IN_GLOBAL, 2 CCB_NO_TMA, 3 CCB_OWN_IN_L2.  out[0..14] = tier (0 arcs in shared
  * memory, 1 from L2, 2 streamed, 3 small batch), lanes per row, U, batch, w1_smem, Npad, tile_rows, gacc_rows and the
