@@ -14,7 +14,7 @@ and ``ctc_loss_fwd_only`` -- the losses without a gradient, used when grad mode 
 ``ctc_loss_seqs`` and ``ctc_align_seqs`` take several label sequences per utterance (``utt``: the logits row of each), with the
 den passes run once per utterance; ``seqs_backward`` is the backward of their per-sequence costs.  ``crf_sample`` draws paths
 from the CTC-CRF posterior and ``samples_to_labels`` packs them for the ``utt=`` loss.  ``ctc_beam_search`` returns N-best
-lists by CTC prefix beam search, over the logits or over the den graph.
+lists by CTC prefix beam search, over the logits or over the den graph, optionally with a token n-gram LM fused in.
 """
 from __future__ import annotations
 
@@ -964,13 +964,31 @@ def _check_beam_args(logits, lx, beam_size, cutoff_top_n):
     return N, T, V
 
 
-def ctc_beam_search(logits: torch.Tensor, lx: torch.Tensor, beam_size: int, cutoff_top_n: int, crf: bool
-                    ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+def _check_lm_args(lm, alpha, beta, crf, V):
+    """The LM arguments of ``ctc_beam_search`` (ValueError), checked before anything touches a device."""
+    if lm is None:
+        return
+    if crf:
+        raise ValueError("ctc_beam_search: an n-gram LM cannot be combined with crf=True (the den graph has its own LM, "
+                         "and two LMs would count twice)")
+    for name, v in (("alpha", alpha), ("beta", beta)):
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+            raise ValueError(f"ctc_beam_search: {name} must be a finite number, not {v!r}")
+    if alpha < 0:
+        raise ValueError(f"ctc_beam_search: alpha must be >= 0, not {alpha!r}")
+    if lm.V != V:
+        raise ValueError(f"ctc_beam_search: the LM was loaded for {lm.V} labels, the logits have V = {V}")
+
+
+def ctc_beam_search(logits: torch.Tensor, lx: torch.Tensor, beam_size: int, cutoff_top_n: int, crf: bool, lm=None,
+                    alpha: float = 1.0, beta: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
     """The beam_size best label sequences per utterance by CTC prefix beam search, over the logits alone (crf False) or over
-    the loaded den graph (crf True).  Returns device tensors (tokens (N,B,T) int32, lengths (N,B) int32, timesteps (N,B,T)
+    the loaded den graph (crf True), with the token n-gram LM ``lm`` (an ``ngram.NGramLM``) fused in at weight alpha and
+    token bonus beta when given.  Returns device tensors (tokens (N,B,T) int32, lengths (N,B) int32, timesteps (N,B,T)
     int32, scores (N,B) fp32); see ``ctc_crf.ctc_beam_search``.  One native call for the batch; never synchronises the
     host."""
     N, T, V = _check_beam_args(logits, lx, beam_size, cutoff_top_n)
+    _check_lm_args(lm, alpha, beta, crf, V)
     B = beam_size
     L = _lib.lib()
     dev = logits.device
@@ -982,9 +1000,14 @@ def ctc_beam_search(logits: torch.Tensor, lx: torch.Tensor, beam_size: int, cuto
         timesteps = torch.empty((N, B, T), dtype=torch.int32, device=dev)
         scores = torch.empty((N, B), dtype=torch.float32, device=dev)
         ws = torch.empty(int(L.ccb_ctc_beam_search_ws_bytes(N, T, B)), dtype=torch.uint8, device=dev)
-        rc = L.ccb_ctc_beam_search(y.data_ptr(), _DTYPES[y.dtype], N, T, V, lens.data_ptr(), B, int(cutoff_top_n), int(bool(crf)),
-                                   ws.data_ptr(), tokens.data_ptr(), lengths.data_ptr(), timesteps.data_ptr(),
-                                   scores.data_ptr(), _stream(dev))
+        if lm is None:
+            rc = L.ccb_ctc_beam_search(y.data_ptr(), _DTYPES[y.dtype], N, T, V, lens.data_ptr(), B, int(cutoff_top_n),
+                                       int(bool(crf)), ws.data_ptr(), tokens.data_ptr(), lengths.data_ptr(),
+                                       timesteps.data_ptr(), scores.data_ptr(), _stream(dev))
+        else:
+            rc = L.ccb_ctc_beam_search_lm(y.data_ptr(), _DTYPES[y.dtype], N, T, V, lens.data_ptr(), B, int(cutoff_top_n), 0,
+                                          ws.data_ptr(), tokens.data_ptr(), lengths.data_ptr(), timesteps.data_ptr(),
+                                          scores.data_ptr(), lm.handle, float(alpha), float(beta), _stream(dev))
         _check(rc, "ctc_beam_search")
         lens.record_stream(torch.cuda.current_stream(dev))
     return tokens, lengths, timesteps, scores

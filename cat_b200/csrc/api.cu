@@ -12,6 +12,7 @@
 
 #include "../../include/ctc_crf_b200.h"
 #include "common.cuh"
+#include "ngram.h"
 
 using namespace ccb;
 
@@ -988,6 +989,44 @@ int ccb_crf_sample(const void *logits, int dtype, int N, int T, int V, int Tmax,
 }
 
 /* ---- CTC prefix beam search ------------------------------------------------------------------ */
+// A token n-gram LM handle (ccb_ngram_create): the host tables, and their device copies, uploaded by the first search that
+// uses the LM on a device and freed by ccb_ngram_destroy
+struct NGram {
+    NGramHost host;
+    bool uploaded[kMaxDevices] = {};
+    NGramDev dev[kMaxDevices];
+    std::vector<void *> blocks[kMaxDevices];
+};
+
+static int EnsureNGram(NGram *m, const NGramDev **out) {
+    std::lock_guard<std::mutex> lk(g_mu);
+    int d = 0;
+    CCB_CUDA(cudaGetDevice(&d));
+    if (d < 0 || d >= kMaxDevices) return Fail("ctc_beam_search: CUDA device " + std::to_string(d) + " is out of range");
+    if (!m->uploaded[d]) {
+        const NGramHost &h = m->host;
+        NGramDev t;
+        int *tok2word = nullptr, *root_dst = nullptr, *arc_off = nullptr, *arc_word = nullptr, *arc_dst = nullptr, *back = nullptr;
+        float *root_p = nullptr, *arc_p = nullptr, *bow = nullptr;
+        const int rc = Upload(&tok2word, h.tok2word) || Upload(&root_dst, h.root_dst) || Upload(&arc_off, h.arc_off) ||
+                       Upload(&arc_word, h.arc_word) || Upload(&arc_dst, h.arc_dst) || Upload(&back, h.back) ||
+                       Upload(&root_p, h.root_p) || Upload(&arc_p, h.arc_p) || Upload(&bow, h.bow);
+        m->blocks[d] = {tok2word, root_dst, arc_off, arc_word, arc_dst, back, root_p, arc_p, bow};
+        if (rc) {
+            for (void *p : m->blocks[d]) cudaFree(p);
+            m->blocks[d].clear();
+            return 1;
+        }
+        t.tok2word = tok2word; t.root_dst = root_dst; t.arc_off = arc_off; t.arc_word = arc_word; t.arc_dst = arc_dst;
+        t.back = back; t.root_p = root_p; t.arc_p = arc_p; t.bow = bow; t.bos = h.bos; t.eos = h.eos;
+        m->dev[d] = t;
+        m->uploaded[d] = true;
+    }
+    *out = &m->dev[d];
+    return 0;
+}
+
+
 // crf mode: the CTC-shape check of the device's graph (once; the result is kept) and its out-arc CSR on the device
 static int EnsureBeamGraph(DeviceGraph *g) {
     std::lock_guard<std::mutex> lk(g_mu);
@@ -1016,6 +1055,13 @@ size_t ccb_ctc_beam_search_ws_bytes(int N, int T, int beam) {
 
 int ccb_ctc_beam_search(const void *logits, int dtype, int N, int T, int V, const int *len_dev, int beam, int cutoff_top_n,
                         int crf, void *workspace, int *tokens, int *lengths, int *timesteps, float *scores, void *stream) {
+    return ccb_ctc_beam_search_lm(logits, dtype, N, T, V, len_dev, beam, cutoff_top_n, crf, workspace, tokens, lengths,
+                                  timesteps, scores, nullptr, 0.0, 0.0, stream);
+}
+
+int ccb_ctc_beam_search_lm(const void *logits, int dtype, int N, int T, int V, const int *len_dev, int beam, int cutoff_top_n,
+                           int crf, void *workspace, int *tokens, int *lengths, int *timesteps, float *scores, const void *lm,
+                           double alpha, double beta, void *stream) {
     g_err.clear();
     if (N <= 0 || T <= 0 || V <= 0) return Fail("ctc_beam_search: N, T and V must be positive");
     if (!KnownDtype(dtype)) return FailDtype("ctc_beam_search", dtype);
@@ -1027,6 +1073,16 @@ int ccb_ctc_beam_search(const void *logits, int dtype, int N, int T, int V, cons
     if (V > kBeamMaxV) return Fail("ctc_beam_search: at most " + std::to_string(kBeamMaxV) + " labels, not " + std::to_string(V));
     if (!logits || !len_dev || !workspace || !tokens || !lengths || !timesteps || !scores)
         return Fail("ctc_beam_search: missing buffer");
+    const NGramDev *lmd = nullptr;
+    if (lm) {
+        NGram *m = reinterpret_cast<NGram *>(const_cast<void *>(lm));
+        if (crf) return Fail("ctc_beam_search: an n-gram LM cannot be combined with crf=1 (the den graph has its own LM)");
+        if (!(std::isfinite(alpha) && alpha >= 0.0)) return Fail("ctc_beam_search: alpha must be finite and >= 0");
+        if (!std::isfinite(beta)) return Fail("ctc_beam_search: beta must be finite");
+        if (m->host.V != V)
+            return Fail("ctc_beam_search: the LM was loaded for " + std::to_string(m->host.V) + " labels, V is " + std::to_string(V));
+        if (EnsureNGram(m, &lmd)) return 1;
+    }
     DeviceGraph *g = nullptr;
     if (crf) {
         if (CurrentGraph(&g)) return 1;
@@ -1036,8 +1092,65 @@ int ccb_ctc_beam_search(const void *logits, int dtype, int N, int T, int V, cons
         if (EnsureBeamGraph(g)) return 1;
     }
     const int rc = LaunchBeamSearch(g, logits, dtype, N, T, V, len_dev, beam, cutoff_top_n, workspace, tokens, lengths,
-                                    timesteps, scores, (cudaStream_t)stream);
+                                    timesteps, scores, (cudaStream_t)stream, lmd, alpha, beta);
     if (rc) return FailCuda("beam_search", (cudaError_t)rc);
+    return 0;
+}
+
+/* ---- token n-gram LM ------------------------------------------------------------------------ */
+void *ccb_ngram_create(const char *path, const char *const *labels, int V) {
+    g_err.clear();
+    NGram *m = new NGram();
+    std::string err;
+    if (!LoadArpa(path, labels, V, &m->host, &err)) { g_err = err; delete m; return nullptr; }
+    return m;
+}
+
+void ccb_ngram_destroy(void *lm) {
+    if (!lm) return;
+    NGram *m = reinterpret_cast<NGram *>(lm);
+    {
+        std::lock_guard<std::mutex> lk(g_mu);
+        int prev = -1;
+        for (int d = 0; d < kMaxDevices; ++d) {
+            if (!m->uploaded[d]) continue;
+            if (prev < 0) cudaGetDevice(&prev);
+            if (cudaSetDevice(d) != cudaSuccess) continue;
+            for (void *p : m->blocks[d]) cudaFree(p);
+        }
+        if (prev >= 0) cudaSetDevice(prev);
+    }
+    delete m;
+}
+
+int ccb_ngram_info(void *lm, long *info) {
+    if (!lm || !info) return 1;
+    const NGramHost &h = reinterpret_cast<const NGram *>(lm)->host;
+    const long v[] = {h.order, h.num_states(), h.num_arcs(), h.unk_substituted ? 1 : 0, h.W, h.V, h.bos, h.eos};
+    memcpy(info, v, sizeof(v));
+    for (int k = 0; k < kNgramMaxOrder; ++k) info[8 + k] = h.counts[k];
+    return 0;
+}
+
+int ccb_ngram_copy(void *lm, int which, void *dst, size_t dst_bytes) {
+    if (!lm || !dst) return 1;
+    const NGramHost &h = reinterpret_cast<const NGram *>(lm)->host;
+    const void *src = nullptr;
+    size_t bytes = 0;
+    switch (which) {
+        case 0: src = h.tok2word.data(); bytes = h.tok2word.size() * 4; break;
+        case 1: src = h.root_p.data(); bytes = h.root_p.size() * 4; break;
+        case 2: src = h.root_dst.data(); bytes = h.root_dst.size() * 4; break;
+        case 3: src = h.arc_off.data(); bytes = h.arc_off.size() * 4; break;
+        case 4: src = h.arc_word.data(); bytes = h.arc_word.size() * 4; break;
+        case 5: src = h.arc_p.data(); bytes = h.arc_p.size() * 4; break;
+        case 6: src = h.arc_dst.data(); bytes = h.arc_dst.size() * 4; break;
+        case 7: src = h.bow.data(); bytes = h.bow.size() * 4; break;
+        case 8: src = h.back.data(); bytes = h.back.size() * 4; break;
+        default: return 1;
+    }
+    if (bytes > dst_bytes) return 2;
+    if (bytes) memcpy(dst, src, bytes);
     return 0;
 }
 

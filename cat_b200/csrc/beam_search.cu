@@ -15,6 +15,9 @@
 //      and created if missing, new node ids in rank order.
 // After the last frame every entry gets its final score (crf: plus log final of each slot's state), the entries are ranked
 // by it, and the trie is walked back to write tokens, the frame at which each token's node was created, lengths and scores.
+// With a token n-gram LM (plain mode, the LM template flag; DESIGN.md §7 "N-gram LM fusion") each entry also carries an LM
+// state and LM part, an extension's rank adds alpha ln P(c | state) + beta (a back-off walk over the LM's tables), and the
+// final score adds alpha ln P(</s> | state).
 #include <cmath>
 
 #include "common.cuh"
@@ -163,8 +166,55 @@ struct Params {
     char *ws;
     int *tokens, *lengths, *timesteps;
     float *scores;
+    // the LM instantiation only (kept last: the fields above keep their offsets in both instantiations)
+    NGramDev lm;
+    double alpha, beta;
 };
 
+constexpr double kLn10 = 2.302585092994045684;
+
+// log10 P(word w | LM state s) by the back-off walk (ngram.h); *dst the state after w.  An arc whose probability is NaN
+// was inserted by the loader's prefix closure: it gives the destination, the probability is the back-off value.
+__device__ __forceinline__ double LmLog10(const NGramDev &lm, int s, int w, int *dst) {
+    double acc = 0.0;
+    int d = -1;
+    for (;;) {
+        if (s == 0) {
+            acc += (double)lm.root_p[w];
+            if (d < 0) d = lm.root_dst[w];
+            break;
+        }
+        int lo = lm.arc_off[s];
+        const int end = lm.arc_off[s + 1];
+        int hi = end;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (lm.arc_word[mid] < w) lo = mid + 1; else hi = mid;
+        }
+        if (lo < end && lm.arc_word[lo] == w) {
+            if (d < 0) d = lm.arc_dst[lo];
+            const float p = lm.arc_p[lo];
+            if (p == p) { acc += (double)p; break; }
+        }
+        acc += (double)lm.bow[s];
+        s = lm.back[s];
+    }
+    *dst = d;
+    return acc;
+}
+
+// What an extension by token c from LM state s adds to a prefix's LM part: alpha ln P(c | s) + beta; *dst the state after
+// c.  alpha = 0 does not consult the LM.
+__device__ __forceinline__ double LmTerm(const Params &P, int s, int c, int *dst) {
+    if (P.alpha == 0.0) { *dst = s; return P.beta; }
+    // (rounded operation by operation, not fused, so that a restatement in numpy reproduces it)
+    return __dadd_rn(__dmul_rn(P.alpha, __dmul_rn(LmLog10(P.lm, s, P.lm.tok2word[c], dst), kLn10)), P.beta);
+}
+
+// LM: the token n-gram LM fused in (plain mode only).  Each entry then also carries its LM state and LM part (the sum of
+// its extensions' LmTerm); a candidate ranks by its acoustic mass plus its prefix's LM part, and after the last frame each
+// entry adds alpha ln P(</s> | state).  The instantiation without it is the search without an LM.
+template <bool LM>
 __global__ void __launch_bounds__(kThreads) beam_search_kernel(const Params P) {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int s_nb, s_next, s_count;
@@ -188,6 +238,9 @@ __global__ void __launch_bounds__(kThreads) beam_search_kernel(const Params P) {
     }
     int *map = bi + 10 * B;
     int *wnode = map + kMapSlots;
+    // LM: the LM part (fp64) and LM state of the entries of both beams
+    double *lmd = reinterpret_cast<double *>(wnode + B + (B & 1));
+    int *lsd = reinterpret_cast<int *>(lmd + 2 * B);
 
     // the utterance's trie: node 0 is the root (the empty prefix)
     const size_t cap = NodeCap(T, B), hslots = HashSlots(T, B);
@@ -203,12 +256,15 @@ __global__ void __launch_bounds__(kThreads) beam_search_kernel(const Params P) {
         bm[0].mb[0] = 0.0; bm[0].sb[0] = crf ? g.start : -1;
         bm[0].mt[0] = kNegInf; bm[0].st[0] = -1;
         s_nb = 1; s_next = 1;
+        if constexpr (LM) { lmd[0] = 0.0; lsd[0] = P.lm.bos; }
     }
     __syncthreads();
     int cur = 0;
     const int per = topn + 2;   // candidates per entry: stay, the frame tokens, its own last token
     for (int t = 0; t < ln; ++t) {
         Beam &o = bm[cur], &w = bm[cur ^ 1];
+        const double *lmo = lmd + cur * B;
+        const int *lso = lsd + cur * B;
         const int nb = s_nb;
         // 1. the y row and the frame's tokens
         const long yb = ((long)n * T + t) * V;
@@ -256,6 +312,7 @@ __global__ void __launch_bounds__(kThreads) beam_search_kernel(const Params P) {
                     if (j == 0) {
                         const Slots s = Stay(crf, g, o, r, yrow);
                         m = lse(s.mb, s.mt);
+                        if constexpr (LM) m += lmo[r];
                         key = r * (V + 1);
                     } else {
                         const int c = j <= topn ? toks[j - 1] : o.last[r];
@@ -270,6 +327,10 @@ __global__ void __launch_bounds__(kThreads) beam_search_kernel(const Params P) {
                             int d;
                             const double ein = ExtIn(crf, g, o, r, c, &d);
                             m = ein > kNegInf ? ein + (double)yrow[c] : kNegInf;
+                            if constexpr (LM) {
+                                int ls;
+                                if (m > kNegInf) m += lmo[r] + LmTerm(P, lso[r], c, &ls);
+                            }
                             key = r * (V + 1) + c + 1;
                         }
                     }
@@ -296,12 +357,18 @@ __global__ void __launch_bounds__(kThreads) beam_search_kernel(const Params P) {
                 w.node[k] = o.node[r]; w.last[k] = o.last[r];
                 w.mb[k] = s.mb; w.sb[k] = s.sb; w.mt[k] = s.mt; w.st[k] = s.st;
                 wnode[k] = -2;
+                if constexpr (LM) { lmd[(cur ^ 1) * B + k] = lmo[r]; lsd[(cur ^ 1) * B + k] = lso[r]; }
             } else {
                 int d;
                 const double ein = ExtIn(crf, g, o, r, c, &d);
                 const int parent = o.node[r];
                 w.last[k] = c;
                 w.mb[k] = kNegInf; w.sb[k] = -1; w.mt[k] = ein + (double)yrow[c]; w.st[k] = d;
+                if constexpr (LM) {
+                    int ls;
+                    lmd[(cur ^ 1) * B + k] = lmo[r] + LmTerm(P, lso[r], c, &ls);
+                    lsd[(cur ^ 1) * B + k] = ls;
+                }
                 int found = -1;
                 for (unsigned h = TrieHash(parent, c, hslots);; h = (h + 1) & (unsigned)(hslots - 1)) {
                     const int x = hash[h];
@@ -348,6 +415,14 @@ __global__ void __launch_bounds__(kThreads) beam_search_kernel(const Params P) {
             } else {
                 s = lse(o.mb[k], o.mt[k]);
             }
+            if constexpr (LM) {
+                if (s > kNegInf) {
+                    int d;
+                    const double *lmf = lmd + cur * B;
+                    const int *lsf = lsd + cur * B;
+                    s += lmf[k] + (P.alpha != 0.0 ? __dmul_rn(P.alpha, __dmul_rn(LmLog10(P.lm, lsf[k], P.lm.eos, &d), kLn10)) : 0.0);
+                }
+            }
         }
         fs[k] = s > kNegInf ? s : kNegInf;
     }
@@ -391,8 +466,11 @@ __global__ void __launch_bounds__(kThreads) beam_search_kernel(const Params P) {
 size_t BeamWsBytes(int N, int T, int B) { return (size_t)N * UttBytes(T, B); }
 
 int LaunchBeamSearch(const DeviceGraph *dg, const void *y, int y_dtype, int N, int T, int V, const int *len, int B, int topn,
-                     void *ws, int *tokens, int *lengths, int *timesteps, float *scores, cudaStream_t stream) {
+                     void *ws, int *tokens, int *lengths, int *timesteps, float *scores, cudaStream_t stream,
+                     const NGramDev *lm, double alpha, double beta) {
     Params p;
+    p.lm = lm ? *lm : NGramDev{};
+    p.alpha = alpha; p.beta = beta;
     p.crf = dg != nullptr;
     p.g = Graph{};
     if (dg) {
@@ -403,11 +481,14 @@ int LaunchBeamSearch(const DeviceGraph *dg, const void *y, int y_dtype, int N, i
     p.psort = Pow2Ceil(V) > kChunkSort ? Pow2Ceil(V) : kChunkSort;
     p.ws = reinterpret_cast<char *>(ws);
     p.tokens = tokens; p.lengths = lengths; p.timesteps = timesteps; p.scores = scores;
+    // (the LM instantiation: + the LM part and state of the entries of both beams, 24 B bytes)
     const size_t smem = (size_t)p.psort * (sizeof(double) + sizeof(int)) + (size_t)V * 3 * sizeof(int) + sizeof(int) * (V & 1) +
-                        (size_t)B * 4 * sizeof(double) + ((size_t)B * 11 + kMapSlots) * sizeof(int);
-    cudaError_t e = cudaFuncSetAttribute(beam_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+                        (size_t)B * 4 * sizeof(double) + ((size_t)B * 11 + kMapSlots) * sizeof(int) +
+                        (lm ? sizeof(int) * (B & 1) + (size_t)B * 2 * (sizeof(double) + sizeof(int)) : 0);
+    auto kernel = lm ? beam_search_kernel<true> : beam_search_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
-    beam_search_kernel<<<N, kThreads, smem, stream>>>(p);
+    kernel<<<N, kThreads, smem, stream>>>(p);
     CountLaunch();
     return (int)cudaGetLastError();
 }

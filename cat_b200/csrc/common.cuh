@@ -242,8 +242,17 @@ int LaunchSampleWalk(const DeviceGraph &g, const void *y, int y_dtype, long sn, 
 constexpr int kBeamMax = 128;
 constexpr int kBeamMaxV = 8192;
 size_t BeamWsBytes(int N, int T, int B);
+// A token n-gram LM's tables on one device (ngram.h NGramHost), for shallow fusion into the plain-mode search
+struct NGramDev {
+    const int *tok2word = nullptr, *root_dst = nullptr, *arc_off = nullptr, *arc_word = nullptr, *arc_dst = nullptr,
+              *back = nullptr;
+    const float *root_p = nullptr, *arc_p = nullptr, *bow = nullptr;
+    int bos = 0, eos = 0;
+};
+// lm null: the search without an LM; else every extension p -> p+c adds alpha ln P(c | p) + beta to the candidate's rank
 int LaunchBeamSearch(const DeviceGraph *g, const void *y, int y_dtype, int N, int T, int V, const int *len, int B, int topn,
-                     void *ws, int *tokens, int *lengths, int *timesteps, float *scores, cudaStream_t stream);
+                     void *ws, int *tokens, int *lengths, int *timesteps, float *scores, cudaStream_t stream,
+                     const NGramDev *lm = nullptr, double alpha = 0.0, double beta = 0.0);
 
 // ------------------------------------------------------------------------------------------------
 // device helpers

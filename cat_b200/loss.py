@@ -337,7 +337,7 @@ def samples_to_labels(tokens, lengths):
     return core.samples_to_labels(tokens, lengths)
 
 
-def ctc_beam_search(logits, lx, beam_size=16, cutoff_top_n=40, crf=False):
+def ctc_beam_search(logits, lx, beam_size=16, cutoff_top_n=40, crf=False, lm=None, alpha=1.0, beta=0.0):
     """N-best label sequences by CTC prefix beam search on the GPU (DESIGN.md §7 "Prefix beam search").
 
     crf False: plain CTC, as ``ctcdecode`` computes it without a word LM -- a hypothesis collects the paths whose CTC
@@ -357,21 +357,28 @@ def ctc_beam_search(logits, lx, beam_size=16, cutoff_top_n=40, crf=False):
       scores (N,B) fp32: the log-sum of the kept paths (fp64 inside), a lower bound on the sequence's log mass, exact when
       nothing was pruned.
     Rows past the hypotheses of finite score have length -1, tokens -1 and score -inf; lx = 0 gives the empty sequence.
-    ``samples_to_labels(tokens, lengths)`` turns the lists into the ``utt=`` arguments of the losses."""
-    return core.ctc_beam_search(logits, lx, beam_size, cutoff_top_n, crf)
+    ``samples_to_labels(tokens, lengths)`` turns the lists into the ``utt=`` arguments of the losses.
+
+    lm: an ``NGramLM`` (a token n-gram LM read from ARPA text) fused into the plain search (DESIGN.md §7 "N-gram LM
+    fusion").  A hypothesis l_1..l_k then scores  A + alpha sum_{i=1..k+1} ln P(w_i | history) + beta k,  A the score above,
+    w_i the LM word of token l_i and w_{k+1} = </s>; an extension adds its term to the candidate's rank during the search,
+    and the </s> term is added after the last frame, where the hypotheses are re-ranked.  alpha = 0 does not consult the
+    LM.  alpha must be finite and >= 0, beta finite, ``len(labels)`` of the LM equal to V, and crf False (ValueError)."""
+    return core.ctc_beam_search(logits, lx, beam_size, cutoff_top_n, crf, lm, alpha, beta)
 
 
 class CTCBeamDecoder:
-    """Drop-in for ``ctcdecode.CTCBeamDecoder`` without a word LM, on the GPU (``ctc_beam_search``, plain CTC).
-    ``decode(probs, seq_lens)`` returns (beam_results (N,B,T), beam_scores (N,B) = -log score, timesteps (N,B,T),
-    out_lens (N,B)) as ``ctcdecode`` does, on the device of the input (CPU inputs run on the current CUDA device).
-    model_path, blank_id != 0 and cutoff_prob != 1.0 are not supported (NotImplementedError); alpha, beta and
-    num_processes are accepted and unused."""
+    """Drop-in for ``ctcdecode.CTCBeamDecoder`` on the GPU (``ctc_beam_search``, plain CTC).  ``decode(probs, seq_lens)``
+    returns (beam_results (N,B,T), beam_scores (N,B) = -log score, timesteps (N,B,T), out_lens (N,B)) as ``ctcdecode`` does,
+    on the device of the input (CPU inputs run on the current CUDA device).
+    model_path: a token-level n-gram LM in ARPA text (``is_token_based=True``, as CAT's ``decode.py`` passes it), loaded as
+    ``NGramLM(model_path, labels)`` and fused in with ``alpha`` and ``beta``; without it alpha and beta are unused.  Word-level
+    LMs (``is_token_based=False``), KenLM binaries and a missing file raise NotImplementedError, a malformed ARPA file
+    RuntimeError.  blank_id != 0 and cutoff_prob != 1.0 are not supported (NotImplementedError); num_processes is accepted
+    and unused."""
 
     def __init__(self, labels, model_path=None, alpha=0, beta=0, cutoff_top_n=40, cutoff_prob=1.0, beam_width=100,
-                 num_processes=4, blank_id=0, log_probs_input=False):
-        if model_path is not None:
-            raise NotImplementedError("CTCBeamDecoder: word-level LMs (model_path) are not supported")
+                 num_processes=4, blank_id=0, log_probs_input=False, is_token_based=False):
         if blank_id != 0:
             raise NotImplementedError("CTCBeamDecoder: the blank must be label 0")
         if cutoff_prob != 1.0:
@@ -380,6 +387,16 @@ class CTCBeamDecoder:
         self._cutoff_top_n = min(int(cutoff_top_n), len(self._labels))
         self._beam_width = int(beam_width)
         self._log_probs_input = bool(log_probs_input)
+        self._lm, self._alpha, self._beta = None, float(alpha), float(beta)
+        if model_path is not None:
+            if not is_token_based:
+                raise NotImplementedError("CTCBeamDecoder: word-level LMs scored on spaces are not supported; pass "
+                                          "is_token_based=True with a token n-gram LM")
+            if not _is_arpa_text(model_path):
+                raise NotImplementedError(f"CTCBeamDecoder: only ARPA text LMs are supported (`ngram.sh --arpa`), and "
+                                          f"{model_path!r} is missing or is not ARPA text (a KenLM binary?)")
+            from .ngram import NGramLM
+            self._lm = NGramLM(model_path, self._labels)
 
     def decode(self, probs, seq_lens=None):
         """probs (N,T,V): probabilities, or log-probabilities with log_probs_input=True.  seq_lens (N,): frames per utterance
@@ -390,8 +407,19 @@ class CTCBeamDecoder:
         N, T, _ = x.shape
         lx = torch.full((N,), T, dtype=torch.int32) if seq_lens is None else torch.as_tensor(seq_lens).to("cpu", torch.int32)
         tokens, lengths, timesteps, scores = core.ctc_beam_search(x, lx, self._beam_width,
-                                                                  min(self._cutoff_top_n, int(x.shape[2])), False)
+                                                                  min(self._cutoff_top_n, int(x.shape[2])), False,
+                                                                  self._lm, self._alpha, self._beta)
         return tokens, -scores, timesteps, lengths
+
+
+def _is_arpa_text(path) -> bool:
+    """False for a missing file, a KenLM binary, a gzip file or one with NUL bytes near its start: files the ARPA loader
+    does not read.  Anything else goes to the loader, which names the line of what it cannot parse."""
+    if not os.path.isfile(path):
+        return False
+    with open(path, "rb") as f:
+        head = f.read(4096)
+    return not (head.startswith(b"mmap lm ") or head.startswith(b"\x1f\x8b") or b"\0" in head)
 
 
 class CRFContext:

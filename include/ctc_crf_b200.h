@@ -328,6 +328,31 @@ size_t ccb_ctc_beam_search_ws_bytes(int N, int T, int beam);
 int ccb_ctc_beam_search(const void *logits, int dtype, int N, int T, int V, const int *len_dev, int beam, int cutoff_top_n,
                         int crf, void *workspace, int *tokens, int *lengths, int *timesteps, float *scores, void *stream);
 
+/* Token-level shallow fusion of a back-off n-gram LM into the plain (crf 0) prefix beam search.  A hypothesis l = l_1..l_k
+ * scores  A(l) + alpha sum_{i=1..k+1} ln P(w_i | w_{i-n+1} .. w_{i-1}) + beta k,  where A(l) is ccb_ctc_beam_search's score,
+ * w_i = labels[l_i] (w_0 = <s> when the LM lists it, w_{k+1} = </s>) and P is ARPA back-off (log10 values, fp32 as parsed,
+ * turned into natural log in fp64).  An extension p -> p+c adds alpha ln P(c | p) + beta to the candidate's rank during the
+ * search; the </s> term is added after the last frame and the hypotheses re-ranked.  alpha = 0 does not consult the LM.
+ *   ccb_ngram_create: parse the ARPA text at `path` for the token labels labels[0..V) (labels[0], the blank, is never scored;
+ *     a label the LM does not list, or an empty one, scores as <unk>; <s> or </s> as a label is an error).  Host only, no CUDA.
+ *     NULL on failure, with ccb_last_error naming the line.  KenLM binaries and compressed files are not read.
+ *   ccb_ngram_destroy: frees the host tables and the device copies; it calls cudaFree, which waits for the device.
+ *   ccb_ngram_info: info[0..7] = order, states, arcs, <unk> substituted (0/1), words, V, state after <s>, word id of </s>;
+ *     info[8..17] = n-gram counts of orders 1..10 as \data\ declares them (0 past the order).
+ *   ccb_ngram_copy (tests): which 0 tok2word[V] i32, 1 root_p[W] f32, 2 root_dst[W] i32, 3 arc_off[S+1] i32, 4 arc_word[A]
+ *     i32, 5 arc_p[A] f32 (NaN: a prefix inserted by the closure, whose value is the back-off value), 6 arc_dst[A] i32,
+ *     7 bow[S] f32, 8 back[S] i32 (ngram.h NGramHost).
+ *   ccb_ctc_beam_search_lm: ccb_ctc_beam_search with the LM fused in; lm = NULL is ccb_ctc_beam_search.  crf must be 0, alpha
+ *     finite and >= 0, beta finite, V the LM's label count.  The first search with an LM on a device uploads its tables
+ *     (about 12 bytes per arc) synchronously; the workspace is the same. */
+void *ccb_ngram_create(const char *path, const char *const *labels, int V);
+void ccb_ngram_destroy(void *lm);
+int ccb_ngram_info(void *lm, long *info);
+int ccb_ngram_copy(void *lm, int which, void *dst, size_t dst_bytes);
+int ccb_ctc_beam_search_lm(const void *logits, int dtype, int N, int T, int V, const int *len_dev, int beam, int cutoff_top_n,
+                           int crf, void *workspace, int *tokens, int *lengths, int *timesteps, float *scores, const void *lm,
+                           double alpha, double beta, void *stream);
+
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 long ccb_launch_count(void);
 
