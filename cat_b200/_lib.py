@@ -31,6 +31,7 @@ SYMBOLS = [
     "ccb_ctc_crf_loss_seqs", "ccb_ctc_crf_loss_seqs_fwd_only", "ccb_ctc_loss_seqs", "ccb_seqs_grad", "ccb_ctc_align_seqs",
     "ccb_crf_sample_ws_bytes", "ccb_crf_sample", "ccb_ctc_beam_search_ws_bytes", "ccb_ctc_beam_search", "ccb_plan_ctc_shape",
     "ccb_ngram_create", "ccb_ngram_destroy", "ccb_ngram_info", "ccb_ngram_copy", "ccb_ctc_beam_search_lm",
+    "ccb_wfst_create", "ccb_wfst_destroy", "ccb_wfst_info", "ccb_wfst_copy", "ccb_wfst_decode_ws_bytes", "ccb_wfst_decode",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -132,6 +133,13 @@ def lib() -> C.CDLL:
     L.ccb_ngram_copy.argtypes = [vp, i, vp, C.c_size_t]; L.ccb_ngram_copy.restype = C.c_int
     L.ccb_ctc_beam_search_lm.argtypes = [vp, i, i, i, i, vp, i, i, i, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, vp]
     L.ccb_ctc_beam_search_lm.restype = C.c_int
+    L.ccb_wfst_create.argtypes = [C.c_char_p]; L.ccb_wfst_create.restype = vp
+    L.ccb_wfst_destroy.argtypes = [vp]; L.ccb_wfst_destroy.restype = None
+    L.ccb_wfst_info.argtypes = [vp, C.POINTER(C.c_long)]; L.ccb_wfst_info.restype = C.c_int
+    L.ccb_wfst_copy.argtypes = [vp, i, vp, C.c_size_t]; L.ccb_wfst_copy.restype = C.c_int
+    L.ccb_wfst_decode_ws_bytes.argtypes = [vp, i, i, i]; L.ccb_wfst_decode_ws_bytes.restype = C.c_size_t
+    L.ccb_wfst_decode.argtypes = [vp, i, i, i, i, vp, vp, f, f, f, f, i, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.ccb_wfst_decode.restype = C.c_int
     L.ccb_launch_count.argtypes = []; L.ccb_launch_count.restype = C.c_long
     L.ccb_debug_timeline.argtypes = [vp, C.c_int, C.c_int]; L.ccb_debug_timeline.restype = None
     L.ccb_plan_create.argtypes = [C.c_char_p, C.c_int, C.c_int]; L.ccb_plan_create.restype = vp

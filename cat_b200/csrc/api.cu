@@ -13,6 +13,7 @@
 #include "../../include/ctc_crf_b200.h"
 #include "common.cuh"
 #include "ngram.h"
+#include "wfst.h"
 
 using namespace ccb;
 
@@ -1151,6 +1152,140 @@ int ccb_ngram_copy(void *lm, int which, void *dst, size_t dst_bytes) {
     }
     if (bytes > dst_bytes) return 2;
     if (bytes) memcpy(dst, src, bytes);
+    return 0;
+}
+
+/* ---- TLG decoding graph and its Viterbi beam search ------------------------------------------- */
+// A decoding graph handle (ccb_wfst_create): the host tables, and their device copies, uploaded by the first search that
+// uses the graph on a device and freed by ccb_wfst_destroy
+struct Wfst {
+    WfstHost host;
+    bool uploaded[kMaxDevices] = {};
+    WfstDev dev[kMaxDevices];
+    std::vector<void *> blocks[kMaxDevices];
+};
+
+static WfstDev WfstShape(const WfstHost &h) {
+    WfstDev t;
+    t.S = h.S; t.start = h.start; t.L = h.L; t.E = h.E; t.max_out = h.max_out;
+    return t;
+}
+
+static int EnsureWfst(Wfst *m, const WfstDev **out) {
+    std::lock_guard<std::mutex> lk(g_mu);
+    int d = 0;
+    CCB_CUDA(cudaGetDevice(&d));
+    if (d < 0 || d >= kMaxDevices) return Fail("wfst_decode: CUDA device " + std::to_string(d) + " is out of range");
+    if (!m->uploaded[d]) {
+        const WfstHost &h = m->host;
+        WfstDev t = WfstShape(h);
+        int *arc_off = nullptr, *eps_off = nullptr, *dst = nullptr, *tok = nullptr, *olabel = nullptr, *fid = nullptr,
+            *src = nullptr, *lay = nullptr, *level = nullptr;
+        float *w = nullptr, *fin = nullptr;
+        const int rc = Upload(&arc_off, h.arc_off) || Upload(&eps_off, h.eps_off) || Upload(&dst, h.dst) ||
+                       Upload(&tok, h.tok) || Upload(&olabel, h.olabel) || Upload(&fid, h.fid) || Upload(&src, h.src) ||
+                       Upload(&lay, h.lay) || Upload(&level, h.level) || Upload(&w, h.w) || Upload(&fin, h.final_cost);
+        m->blocks[d] = {arc_off, eps_off, dst, tok, olabel, fid, src, lay, level, w, fin};
+        if (rc) {
+            for (void *p : m->blocks[d]) cudaFree(p);
+            m->blocks[d].clear();
+            return 1;
+        }
+        t.arc_off = arc_off; t.eps_off = eps_off; t.dst = dst; t.tok = tok; t.olabel = olabel; t.fid = fid; t.src = src;
+        t.lay = lay; t.level = level; t.w = w; t.final_cost = fin;
+        m->dev[d] = t;
+        m->uploaded[d] = true;
+    }
+    *out = &m->dev[d];
+    return 0;
+}
+
+void *ccb_wfst_create(const char *path) {
+    g_err.clear();
+    Wfst *m = new Wfst();
+    std::string err;
+    if (!LoadWfst(path, &m->host, &err)) { g_err = err; delete m; return nullptr; }
+    return m;
+}
+
+void ccb_wfst_destroy(void *graph) {
+    if (!graph) return;
+    Wfst *m = reinterpret_cast<Wfst *>(graph);
+    {
+        std::lock_guard<std::mutex> lk(g_mu);
+        int prev = -1;
+        for (int d = 0; d < kMaxDevices; ++d) {
+            if (!m->uploaded[d]) continue;
+            if (prev < 0) cudaGetDevice(&prev);
+            if (cudaSetDevice(d) != cudaSuccess) continue;
+            for (void *p : m->blocks[d]) cudaFree(p);
+        }
+        if (prev >= 0) cudaSetDevice(prev);
+    }
+    delete m;
+}
+
+int ccb_wfst_info(void *graph, long *info) {
+    if (!graph || !info) return 1;
+    const WfstHost &h = reinterpret_cast<const Wfst *>(graph)->host;
+    const long v[] = {h.S, h.A, h.start, h.L, h.E, h.max_out, h.max_ilabel, h.eps_arcs};
+    memcpy(info, v, sizeof(v));
+    return 0;
+}
+
+int ccb_wfst_copy(void *graph, int which, void *dst, size_t dst_bytes) {
+    if (!graph || !dst) return 1;
+    const WfstHost &h = reinterpret_cast<const Wfst *>(graph)->host;
+    const void *src = nullptr;
+    size_t bytes = 0;
+    switch (which) {
+        case 0: src = h.arc_off.data(); bytes = h.arc_off.size() * 4; break;
+        case 1: src = h.eps_off.data(); bytes = h.eps_off.size() * 4; break;
+        case 2: src = h.dst.data(); bytes = h.dst.size() * 4; break;
+        case 3: src = h.tok.data(); bytes = h.tok.size() * 4; break;
+        case 4: src = h.olabel.data(); bytes = h.olabel.size() * 4; break;
+        case 5: src = h.w.data(); bytes = h.w.size() * 4; break;
+        case 6: src = h.fid.data(); bytes = h.fid.size() * 4; break;
+        case 7: src = h.final_cost.data(); bytes = h.final_cost.size() * 4; break;
+        case 8: src = h.level.data(); bytes = h.level.size() * 4; break;
+        default: return 1;
+    }
+    if (bytes > dst_bytes) return 2;
+    if (bytes) memcpy(dst, src, bytes);
+    return 0;
+}
+
+size_t ccb_wfst_decode_ws_bytes(void *graph, int N, int T, int max_active) {
+    if (!graph || N <= 0 || T <= 0 || max_active < 1 || max_active > kWfstMaxActive) return 0;
+    return WfstWsBytes(WfstShape(reinterpret_cast<const Wfst *>(graph)->host), N, T, max_active);
+}
+
+int ccb_wfst_decode(const void *logits, int dtype, int N, int T, int V, const int *len_dev, void *graph, float acwt,
+                    float lmwt, float wip, float beam, int max_active, void *workspace, int *words, int *num_words,
+                    int *align, float *ac_logp, float *graph_cost, float *cost, int *reached_final, void *stream) {
+    g_err.clear();
+    if (!graph) return Fail("wfst_decode: null graph");
+    if (N <= 0 || T <= 0 || V <= 0) return Fail("wfst_decode: N, T and V must be positive");
+    if (!KnownDtype(dtype)) return FailDtype("wfst_decode", dtype);
+    if (V > kWfstMaxV) return Fail("wfst_decode: at most " + std::to_string(kWfstMaxV) + " labels, not " + std::to_string(V));
+    if (max_active < 1 || max_active > kWfstMaxActive)
+        return Fail("wfst_decode: max_active must lie in [1, " + std::to_string(kWfstMaxActive) + "], not " +
+                    std::to_string(max_active));
+    if (!(beam > 0.f)) return Fail("wfst_decode: beam must be > 0 (inf is allowed)");
+    if (!(std::isfinite(acwt) && acwt >= 0.f)) return Fail("wfst_decode: acwt must be finite and >= 0");
+    if (!(std::isfinite(lmwt) && lmwt > 0.f)) return Fail("wfst_decode: lmwt must be finite and > 0");
+    if (!std::isfinite(wip)) return Fail("wfst_decode: wip must be finite");
+    Wfst *m = reinterpret_cast<Wfst *>(graph);
+    if (m->host.max_ilabel > V)
+        return Fail("wfst_decode: the graph has ilabels up to " + std::to_string(m->host.max_ilabel) + " (tokens up to " +
+                    std::to_string(m->host.max_ilabel - 1) + "), V is " + std::to_string(V));
+    if (!logits || !len_dev || !workspace || !words || !num_words || !align || !ac_logp || !graph_cost || !cost || !reached_final)
+        return Fail("wfst_decode: missing buffer");
+    const WfstDev *g = nullptr;
+    if (EnsureWfst(m, &g)) return 1;
+    const int rc = LaunchWfstDecode(*g, logits, dtype, N, T, V, len_dev, acwt, lmwt, wip, beam, max_active, workspace, words,
+                                    num_words, align, ac_logp, graph_cost, cost, reached_final, (cudaStream_t)stream);
+    if (rc) return FailCuda("wfst_decode", (cudaError_t)rc);
     return 0;
 }
 

@@ -253,6 +253,21 @@ struct NGramDev {
 int LaunchBeamSearch(const DeviceGraph *g, const void *y, int y_dtype, int N, int T, int V, const int *len, int B, int topn,
                      void *ws, int *tokens, int *lengths, int *timesteps, float *scores, cudaStream_t stream,
                      const NGramDev *lm = nullptr, double alpha = 0.0, double beta = 0.0);
+// A decoding graph's tables on one device (wfst.h WfstHost), for the TLG Viterbi beam search (wfst_decode.cu)
+struct WfstDev {
+    const int *arc_off = nullptr, *eps_off = nullptr, *dst = nullptr, *tok = nullptr, *olabel = nullptr, *fid = nullptr,
+              *src = nullptr, *lay = nullptr, *level = nullptr;
+    const float *w = nullptr, *final_cost = nullptr;
+    int S = 0, start = 0, L = 0, E = 0, max_out = 0;
+};
+constexpr int kWfstMaxActive = 1 << 20;
+constexpr int kWfstMaxV = 8192;
+// Workspace of N utterances of T frames at max_active K: per utterance two state hashes sized from K, the largest emitting
+// out-degree and the largest epsilon closure (never more states than the graph has), and the (T+1) x K records of L+1 arcs
+size_t WfstWsBytes(const WfstDev &g, int N, int T, int K);
+int LaunchWfstDecode(const WfstDev &g, const void *y, int y_dtype, int N, int T, int V, const int *len, float acwt, float lmwt,
+                     float wip, float beam, int K, void *ws, int *words, int *num_words, int *align, float *ac_logp,
+                     float *graph_cost, float *cost, int *reached_final, cudaStream_t stream);
 
 // ------------------------------------------------------------------------------------------------
 // device helpers

@@ -39,9 +39,12 @@ struct ByteReader {
 
 // OpenFst binary container, "vector" fst of "standard" (tropical) arcs.  Layout: SURVEY.md 8c.
 // Semantics: fst_read.cc:40-59 (weight negated, ilabel shifted by one, -inf for Zero finals).
-bool ReadFstFile(const char *path, HostFst *out, std::string *err) {
+// decoding: a decoding graph (wfst.h) -- olabels are kept and ilabel 0 (epsilon, label -1) is accepted; the refusals name
+// the conversion that makes a file readable.
+bool ReadFstFile(const char *path, HostFst *out, std::string *err, bool decoding) {
+    const std::string what = decoding ? "decoding graph" : "den graph";
     FILE *f = fopen(path, "rb");
-    if (!f) { *err = std::string("cannot open den graph: ") + path; return false; }
+    if (!f) { *err = "cannot open " + what + ": " + path; return false; }
     fseek(f, 0, SEEK_END);
     long sz = ftell(f);
     fseek(f, 0, SEEK_SET);
@@ -53,6 +56,10 @@ bool ReadFstFile(const char *path, HostFst *out, std::string *err) {
     ByteReader r{buf.data(), buf.size()};
     if ((uint32_t)r.get<int32_t>() != 0x7EB2FDD6u) { *err = std::string("not an OpenFst binary file: ") + path; return false; }
     std::string fst_type = r.str(), arc_type = r.str();
+    if (decoding && r.ok && fst_type == "const") {
+        *err = what + " " + path + " is a const FST; convert it with `fstconvert --fst_type=vector`";
+        return false;
+    }
     if (!r.ok || fst_type != "vector" || arc_type != "standard") {
         *err = "unsupported fst/arc type '" + fst_type + "'/'" + arc_type + "' (need vector/standard)";
         return false;
@@ -60,39 +67,52 @@ bool ReadFstFile(const char *path, HostFst *out, std::string *err) {
     const int32_t version = r.get<int32_t>();
     const int32_t flags = r.get<int32_t>();
     if (r.ok && version != 2) { *err = "unsupported VectorFst file version " + std::to_string(version) + " (need 2)"; return false; }
-    if (flags & 0x3) { *err = "den graph carries embedded symbol tables; strip them (fstsymbols --clear_*)"; return false; }
-    if (flags & 0x4) { *err = "den graph was written with aligned fields (FstHeader::IS_ALIGNED); rewrite it with --fst_align=false"; return false; }
+    if (flags & 0x3) {
+        *err = decoding ? what + " carries embedded symbol tables; strip them with `fstsymbols --clear_isymbols --clear_osymbols`"
+                        : "den graph carries embedded symbol tables; strip them (fstsymbols --clear_*)";
+        return false;
+    }
+    if (flags & 0x4) {
+        *err = decoding ? what + " was written with aligned fields; rewrite it with `fstconvert --fst_align=false`"
+                        : "den graph was written with aligned fields (FstHeader::IS_ALIGNED); rewrite it with --fst_align=false";
+        return false;
+    }
     (void)r.get<uint64_t>();  // properties
     int64_t start = r.get<int64_t>();
     int64_t ns = r.get<int64_t>();
     (void)r.get<int64_t>();   // header arc count: 0 in files written by fstcompile pipelines, not trusted
     if (!r.ok || ns <= 0 || ns > (int64_t)0x7fffffff || start < 0 || start >= ns) {
-        *err = "corrupt den graph header";
+        *err = "corrupt " + what + " header";
         return false;
     }
     out->num_states = (int)ns;
     out->start = (int)start;
     out->final_logw.assign((size_t)ns, -std::numeric_limits<float>::infinity());
-    out->src.clear(); out->dst.clear(); out->label.clear(); out->logw.clear();
+    out->src.clear(); out->dst.clear(); out->label.clear(); out->logw.clear(); out->olabel.clear();
     for (int64_t s = 0; s < ns; ++s) {
         float fin = r.get<float>();
         int64_t na = r.get<int64_t>();
-        if (!r.ok || na < 0 || r.off + (size_t)na * 16 > r.n) { *err = "truncated den graph"; return false; }
+        if (!r.ok || na < 0 || r.off + (size_t)na * 16 > r.n) { *err = "truncated " + what; return false; }
         if (!std::isinf(fin)) out->final_logw[(size_t)s] = -fin;
         for (int64_t a = 0; a < na; ++a) {
             int32_t il = r.get<int32_t>();
-            (void)r.get<int32_t>();  // olabel
+            const int32_t ol = r.get<int32_t>();
             float w = r.get<float>();
             int32_t nx = r.get<int32_t>();
-            if (nx < 0 || nx >= ns || il < 1) { *err = "den graph arc out of range (epsilon input labels are not allowed)"; return false; }
+            if (!decoding && (nx < 0 || nx >= ns || il < 1)) { *err = "den graph arc out of range (epsilon input labels are not allowed)"; return false; }
+            if (decoding && (nx < 0 || nx >= ns || il < 0 || ol < 0)) {
+                *err = what + " arc " + std::to_string(out->src.size()) + " out of range (state " + std::to_string(s) + ")";
+                return false;
+            }
             out->src.push_back((int)s);
             out->dst.push_back(nx);
             out->label.push_back(il - 1);
             out->logw.push_back(-w);
+            if (decoding) out->olabel.push_back(ol);
         }
     }
-    if (r.off != r.n) { *err = "trailing bytes in den graph"; return false; }
-    if (out->src.size() > (size_t)0x3fffffff) { *err = "den graph too large"; return false; }
+    if (r.off != r.n) { *err = "trailing bytes in " + what; return false; }
+    if (out->src.size() > (size_t)0x3fffffff) { *err = what + " too large"; return false; }
     return true;
 }
 

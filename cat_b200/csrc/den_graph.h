@@ -43,10 +43,13 @@ struct HostFst {
     std::vector<int> src, dst, label;   // label = ilabel-1
     std::vector<float> logw;            // -tropical
     std::vector<float> final_logw;      // -Final, -inf for non-final states
+    std::vector<int> olabel;            // decoding graphs only (ReadFstFile decoding = true): the output label of every arc
 };
 
-// Returns false and fills err on failure (never exits, unlike den_calculate.cu:16-25,331-334).
-bool ReadFstFile(const char *path, HostFst *out, std::string *err);
+// Returns false and fills err on failure (never exits, unlike den_calculate.cu:16-25,331-334).  decoding = false reads a den
+// graph (epsilon input labels refused, olabels dropped); true reads a decoding graph (wfst.h): epsilon input labels are kept
+// as label -1, olabels are kept, and const FSTs, symbol tables and aligned files are refused with the conversion to run.
+bool ReadFstFile(const char *path, HostFst *out, std::string *err, bool decoding = false);
 
 // Pass-specific half of the plan: a chunk-major stream of arc segments.  chunk_* cut the states (whole groups)
 // into n_ctas*n_warps contiguous chunks of near-equal cost; CTA c owns chunks [c*n_warps, (c+1)*n_warps).

@@ -308,3 +308,163 @@ def make_random_lm(H: int, V: int, d: int, seed: int = 0, p_final: float = 0.2) 
             final[h] = -np.log(p_final)
     return PhoneLm(H, 0, np.asarray(src, np.int32), np.asarray(dst, np.int32), np.asarray(ph, np.int32),
                    np.asarray(w, np.float32), final)
+
+
+# ---------------------------------------------------------------------------------------------------
+# Decoding graphs without Kaldi/OpenFst: a TLG-shaped graph for the word decoder (csrc/wfst_decode.cu)
+# ---------------------------------------------------------------------------------------------------
+_LN10 = 2.302585092994045684
+
+
+def read_arpa(path: str):
+    """The n-grams of an ARPA file: {tuple of words: (log10 p, log10 bow)} (bow 0 when the line has none), and the order."""
+    grams, order, k = {}, 0, 0
+    with open(path) as f:
+        for line in f:
+            p = line.split()
+            if not p:
+                continue
+            if p[0].startswith("\\"):
+                k = int(p[0][1:].split("-")[0]) if p[0].endswith("-grams:") else 0
+                continue
+            if p[0] == "ngram" and k == 0:
+                order = max(order, int(p[1].split("=")[0]))
+                continue
+            if k:
+                words = tuple(p[1:1 + k])
+                grams.setdefault(words, (float(p[0]), float(p[1 + k]) if len(p) > k + 1 else 0.0))
+    return grams, order
+
+
+def make_tlg(V: int, lexicon, arpa_path: str):
+    """A TLG-shaped decoding graph built without OpenFst: T o L o G in CAT's conventions (ilabel = token + 1, blank = token 0,
+    ilabel 0 = epsilon, olabel = word id).  Returns (DenGraph, words) with words[i] the word of id i (words[0] = "<eps>").
+
+    lexicon: (word, tokens) or (word, tokens, cost) entries, tokens in 1..V-1; a word may have several pronunciations.  Word
+    ids follow the lexicon's order from 1.  ARPA words the lexicon does not list are left out of G.
+    G follows arpa2fst: a state per history (the root, every n-gram below the top order that does not end in </s>), an arc
+    per n-gram into the longest suffix of its words that is a state, a back-off arc (epsilon, the `#0` arc once T o is
+    applied) into the longest proper suffix, </s> as the final cost, costs in natural log (-ln 10 log10).  The start state is
+    <s>'s (the root when the file lists none).
+    L is a token trie of pronunciations per G state over the words that state has arcs for, as det(L o G) shares prefixes:
+    the arc completing a word carries it (into the G destination) when nothing else ends or continues at its node; else the
+    node has an epsilon arc per word ending there.  This keeps the out-degree near V.
+    T is CAT's CTC topology (cat/utils/tool/build_ctc_topo.py): every state of LG becomes a blank state and one state per
+    token entering it (through an emitting arc, or carried along epsilon arcs); a token state repeats its token in place,
+    goes to the blank state on blank, and takes LG's arcs of other tokens; the blank state takes every LG arc.
+    The graph is not minimised."""
+    grams, order = read_arpa(arpa_path)
+    words = ["<eps>"]
+    wid, prons = {}, {}
+    for e in lexicon:
+        w, toks, c = (e[0], e[1], e[2]) if len(e) == 3 else (e[0], e[1], 0.0)
+        toks = tuple(int(x) for x in toks)
+        if not toks or min(toks) < 1 or max(toks) >= V:
+            raise ValueError(f"make_tlg: the pronunciation {toks} of {w!r} must be non-empty tokens in 1..{V - 1}")
+        if w not in wid:
+            wid[w] = len(words)
+            words.append(w)
+        prons.setdefault(w, []).append((toks, float(c)))
+    # G
+    hist = sorted({g for g in grams if len(g) < order and g[-1] != "</s>"} | {()}, key=lambda g: (len(g), g))
+    gid = {h: i for i, h in enumerate(hist)}
+
+    def state_of(ws):            # the longest suffix of ws that is a state
+        for j in range(len(ws) + 1):
+            if ws[j:] in gid:
+                return gid[ws[j:]]
+
+    g_arcs = [[] for _ in hist]  # per G state: (word, dst, cost)
+    g_final = np.full(len(hist), np.inf)
+    for ng, (p, _) in grams.items():
+        h, w = ng[:-1], ng[-1]
+        if h not in gid:
+            if len(h) > 0 and any(x not in wid and x not in ("<s>", "</s>") for x in h):
+                continue
+            raise ValueError(f"make_tlg: the history {h} of an n-gram is not listed in {arpa_path}")
+        if w == "</s>":
+            g_final[gid[h]] = -p * _LN10
+        elif w in wid:
+            g_arcs[gid[h]].append((w, state_of(ng), -p * _LN10))
+    start_g = gid.get(("<s>",), 0)
+    # LG: G states first, then trie nodes; arcs (src, dst, token (-1: epsilon), word id, cost)
+    src, dst, tok, olab, cost = [], [], [], [], []
+    n_lg = len(hist)
+    for g, arcs in enumerate(g_arcs):
+        child = {}               # (node, token) -> node
+        ends = {}                # node -> [(word id, dst, cost)]
+        for w, d, c in arcs:
+            for toks, pc in prons[w]:
+                node = g
+                for x in toks:
+                    nx = child.get((node, x))
+                    if nx is None:
+                        nx = child[(node, x)] = n_lg
+                        n_lg += 1
+                    node = nx
+                ends.setdefault(node, []).append((wid[w], d, c + pc))
+        has_child = {node for node, _ in child}
+        for (node, x), nx in child.items():
+            e = ends.get(nx, [])
+            if len(e) == 1 and nx not in has_child:      # the arc completes one word: it carries the word
+                src.append(node); dst.append(e[0][1]); tok.append(x); olab.append(e[0][0]); cost.append(e[0][2])
+            else:
+                src.append(node); dst.append(nx); tok.append(x); olab.append(0); cost.append(0.0)
+                for w, d, c in e:
+                    src.append(nx); dst.append(d); tok.append(-1); olab.append(w); cost.append(c)
+        if len(hist[g]) > 0:     # back-off
+            h = hist[g]
+            src.append(g); dst.append(state_of(h[1:])); tok.append(-1); olab.append(0)
+            cost.append(-grams.get(h, (0.0, 0.0))[1] * _LN10)
+    src, dst, tok, olab = (np.asarray(a, np.int64) for a in (src, dst, tok, olab))
+    cost = np.asarray(cost, np.float64)
+    lg_final = np.concatenate([g_final, np.full(n_lg - len(hist), np.inf)])
+    # T o LG: the tokens of each LG state (entering through emitting arcs, carried along epsilon arcs; LG's epsilon arcs go
+    # from trie nodes to G states and from G states to shorter histories, so that order is topological)
+    toks_of = [set() for _ in range(n_lg)]
+    em = tok >= 0
+    for d, x in zip(dst[em].tolist(), tok[em].tolist()):
+        toks_of[d].add(x)
+    eps = np.nonzero(~em)[0]
+    rank = np.array([-len(h) for h in hist] + [-order - 1] * (n_lg - len(hist)))
+    for a in eps[np.argsort(rank[src[eps]], kind="stable")].tolist():
+        toks_of[dst[a]] |= toks_of[src[a]]
+    # CTC states grouped by LG state: blank first (key 0), then tokens ascending (key token + 1)
+    cnt = np.array([1 + len(t) for t in toks_of], np.int64)
+    off = np.concatenate([[0], np.cumsum(cnt)])
+    ckey = np.concatenate([np.array([0] + sorted(x + 1 for x in t), np.int64) for t in toks_of])
+    cstate = np.repeat(np.arange(n_lg), cnt)
+    glob = cstate * (V + 1) + ckey        # sorted
+    S = int(off[-1])
+
+    def cid(x, k):
+        return np.searchsorted(glob, x * (V + 1) + k)
+
+    ar = np.arange(S)
+    out_s, out_d, out_i, out_o, out_w = [], [], [], [], []
+    # blank self loop on blank states, token self loop and token -> blank on token states
+    isb = ckey == 0
+    out_s += [ar[isb], ar[~isb], ar[~isb]]
+    out_d += [ar[isb], ar[~isb], off[cstate[~isb]]]
+    out_i += [np.ones(int(isb.sum()), np.int64), ckey[~isb], np.ones(int((~isb).sum()), np.int64)]
+    out_o += [np.zeros(S, np.int64)]
+    out_w += [np.zeros(S + int((~isb).sum()))]
+    out_o += [np.zeros(int((~isb).sum()), np.int64)]
+    # LG arcs from every CTC state of their source: emitting ones skip the token state of their own token
+    rep = cnt[src]
+    a_idx = np.repeat(np.arange(len(src)), rep)
+    c_idx = off[src[a_idx]] + (np.arange(int(rep.sum())) - np.repeat(np.cumsum(rep) - rep, rep))
+    keep = ~((tok[a_idx] >= 0) & (ckey[c_idx] == tok[a_idx] + 1))
+    a_idx, c_idx = a_idx[keep], c_idx[keep]
+    e = tok[a_idx] >= 0
+    d_em = cid(dst[a_idx], tok[a_idx] + 1)
+    d_ep = cid(dst[a_idx], ckey[c_idx])
+    out_s.append(c_idx); out_d.append(np.where(e, d_em, d_ep)); out_i.append(np.where(e, tok[a_idx] + 1, 0))
+    out_o.append(olab[a_idx]); out_w.append(cost[a_idx])
+    s_ = np.concatenate(out_s); d_ = np.concatenate(out_d)
+    order_ = np.argsort(s_, kind="stable")
+    final = lg_final[cstate].astype(np.float32)
+    g = DenGraph(num_states=S, start=int(off[start_g]), src=s_[order_].astype(np.int32), dst=d_[order_].astype(np.int32),
+                 ilabel=np.concatenate(out_i)[order_].astype(np.int32), olabel=np.concatenate(out_o)[order_].astype(np.int32),
+                 weight=np.concatenate(out_w)[order_].astype(np.float32), final=final)
+    return g, words

@@ -353,6 +353,44 @@ int ccb_ctc_beam_search_lm(const void *logits, int dtype, int N, int T, int V, c
                            int crf, void *workspace, int *tokens, int *lengths, int *timesteps, float *scores, const void *lm,
                            double alpha, double beta, void *stream);
 
+/* 1-best word decoding through a TLG decoding graph: a frame-synchronous Viterbi beam search on the GPU, the 1-best step of
+ * Kaldi's latgen-faster + lattice-best-path without the lattice (DESIGN.md §7 "TLG decoding").  The graph is an OpenFst
+ * vector/standard file in CAT's conventions: ilabel = token + 1 (blank = token 0), ilabel 0 = epsilon, olabel = word id
+ * (0 = no word), tropical weights.  With acs = acwt / lmwt and wps = wip / lmwt (fp32), the search cost of an emitting arc
+ * from a token of cost c is ((c + w) + (-acs * y[t][token])) + (word ? wps : 0), of an epsilon arc (c + w) + (word ? wps : 0),
+ * each operation rounded in fp32.  Each frame keeps the tokens within best + beam (best: the cheapest emitting candidate),
+ * recombines per state on the smallest (cost, arc position in the file), runs the epsilon closure by increasing epsilon
+ * level, and keeps the max_active cheapest by (cost, state).  The result is the kept token with the smallest
+ * (cost + final, state), or without a final state among them the smallest (cost, state) with reached_final = 0.
+ *   ccb_wfst_create: read the file and derive the arc layout, the epsilon levels and the sizes below.  Host only, no CUDA.
+ *     NULL on failure, with ccb_last_error saying what is wrong: an epsilon cycle (naming a state on it), a const FST, an
+ *     embedded symbol table or an aligned file (each with the conversion to run).  Several graphs may coexist, and none
+ *     depends on the den graph of Init.
+ *   ccb_wfst_destroy: frees the host tables and the device copies; it calls cudaFree, which waits for the device.
+ *   ccb_wfst_info: info[0..7] = states, arcs, start, L (the longest epsilon path), E (the most states one state reaches
+ *     through epsilon arcs), the largest emitting out-degree, the largest ilabel, epsilon arcs.
+ *   ccb_wfst_copy (tests): which 0 arc_off[S+1], 1 eps_off[S] (each state's arcs: emitting ones, in file order, up to
+ *     eps_off, then epsilon ones), 2 dst[A], 3 token[A] (-1: epsilon), 4 olabel[A], 5 weight[A] f32, 6 file position[A],
+ *     7 final[S] f32 (+inf: not final), 8 epsilon level[S]; i32 unless stated.
+ *   ccb_wfst_decode_ws_bytes: the workspace of N utterances of T frames; 0 for bad arguments.
+ *   ccb_wfst_decode: logits (N,T,V) log-probs or raw logits in dtype, frames t >= len_dev[n] never read; max_active in
+ *     [1, 2^20], beam > 0 (inf allowed), acwt finite >= 0, lmwt finite > 0, wip finite, V <= 8192 and at least the graph's
+ *     largest ilabel.  Outputs, written on `stream` without a host synchronisation, in one launch:
+ *       words (N, Wcap) i32 padded with -1, Wcap = (T+1)(1+L); num_words (N) i32; align (N,T) i32: the token of each frame's
+ *       emitting arc, -1 for t >= len; ac_logp (N) = sum_t y[t][align[t]] and graph_cost (N) = the path's weights plus its
+ *       final cost, both summed in fp64; cost (N) = lmwt graph_cost - acwt ac_logp + wip num_words (lattice-best-path's
+ *       objective); reached_final (N) i32.  An utterance whose candidates all cost +inf gets num_words -1, rows of -1,
+ *       ac_logp -inf and graph_cost and cost +inf.  The first search with a graph on a device uploads its tables (about 36
+ *       bytes per arc) synchronously. */
+void *ccb_wfst_create(const char *path);
+void ccb_wfst_destroy(void *graph);
+int ccb_wfst_info(void *graph, long *info);
+int ccb_wfst_copy(void *graph, int which, void *dst, size_t dst_bytes);
+size_t ccb_wfst_decode_ws_bytes(void *graph, int N, int T, int max_active);
+int ccb_wfst_decode(const void *logits, int dtype, int N, int T, int V, const int *len_dev, void *graph, float acwt,
+                    float lmwt, float wip, float beam, int max_active, void *workspace, int *words, int *num_words,
+                    int *align, float *ac_logp, float *graph_cost, float *cost, int *reached_final, void *stream);
+
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 long ccb_launch_count(void);
 
