@@ -32,12 +32,13 @@ from ._lib import ctcOptions
 _DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
 
 
-def check_reduction(reduction) -> None:
+def check_reduction(reduction) -> bool:
     """reduction None keeps the scalar loss of ``size_average`` (the sum, or the mean over the batch); 'none' returns the
-    (N,) costs.  There is no second spelling of the sum or the mean."""
+    (N,) costs.  There is no second spelling of the sum or the mean.  Returns whether the costs are returned ('none')."""
     if reduction is not None and reduction != "none":
         raise ValueError(f"reduction must be None or 'none', not {reduction!r}: for the batch sum or mean leave it None and "
                          f"choose with size_average (False: sum, True: mean over the batch)")
+    return reduction == "none"
 
 
 def _check(rc: int, what: str) -> None:
@@ -57,6 +58,11 @@ def _stream(device: torch.device) -> C.c_void_p:
 
 def _iptr(t: torch.Tensor):
     return C.cast(t.data_ptr(), C.POINTER(C.c_int))
+
+
+def _ptr(t: Optional[torch.Tensor]):
+    """The device address of an optional buffer: NULL for None."""
+    return None if t is None else t.data_ptr()
 
 
 def init_env(fst_name: str, gpus: torch.Tensor) -> None:
@@ -177,19 +183,32 @@ class _PinnedRing:
 _rings = {}
 
 
-def upload_meta(labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, device) -> Tuple[torch.Tensor, int, int]:
-    """Pack [labels | label_off(N+1) | ly | lx] into one pinned buffer and upload it asynchronously.
-    Returns (device int32 tensor, sum(ly), max(ly))."""
-    N = int(lx.numel())
-    ly64 = ly.to(torch.int64)
-    off = torch.zeros(N + 1, dtype=torch.int32)
-    off[1:].copy_(torch.cumsum(ly64, 0))
+class _Meta:
+    """An int32 meta block: its named parts packed into one pinned buffer of the device's staging ring and uploaded with one
+    asynchronous copy.  `buf` is the device tensor; each part's device address is the attribute of its name."""
+
+    def __init__(self, device, **parts):
+        self.buf = _rings.setdefault(torch.device(device).index, _PinnedRing()).stage(list(parts.values()), device)
+        addr = self.buf.data_ptr()
+        for name, p in parts.items():
+            setattr(self, name, addr)
+            addr += 4 * int(p.numel())
+
+
+def _label_off(ly: torch.Tensor) -> torch.Tensor:
+    """Where each label sequence starts in the flat labels, and their total at the end: (len(ly) + 1,) int32."""
+    off = torch.zeros(int(ly.numel()) + 1, dtype=torch.int32)
+    off[1:].copy_(torch.cumsum(ly.to(torch.int64), 0))
+    return off
+
+
+def upload_meta(labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, device) -> Tuple[_Meta, int]:
+    """Stage [labels | label_off (N+1) | ly | lx] as one meta block.  Returns (the block, max(ly))."""
+    off = _label_off(ly)
     sum_l = int(off[-1])
     if sum_l != int(labels.numel()):
         raise RuntimeError(f"labels has {labels.numel()} entries but label lengths sum to {sum_l}")
-    ring = _rings.setdefault(torch.device(device).index, _PinnedRing())
-    meta = ring.stage([labels, off, ly, lx], device)
-    return meta, sum_l, int(ly.max()) if N else 0
+    return _Meta(device, labels=labels, label_off=off, ly=ly, lx=lx), int(ly.max()) if ly.numel() else 0
 
 
 MAX_UTTS_PER_CALL = 64           # utterances per native call: the den kernels are fastest per utterance at two utterances
@@ -291,83 +310,6 @@ def _plan_slices(L, lx, ly, N, V, dev, seq_off=None, ws_bytes=None):
     return slices
 
 
-def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
-                     lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False,
-                     reduction: Optional[str] = None, zero_infinity: bool = False
-                     ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
-    """Fused CTC-CRF loss.  logits (N,T,V) fp32, bf16 or fp16 CUDA contiguous log-probs; labels/lx/ly int32 CPU.
-    Returns (loss[1] fp32 CUDA, grad (N,T,V) fp32 CUDA, parts[2N] or None).  Never synchronises the host.
-    Batches whose scratch does not fit the free memory (or > 512 utterances) are processed in slices.
-    from_logits: `logits` are the RAW encoder outputs; log_softmax and its Jacobian are applied inside
-    (grad = d loss / d raw logits), replacing cat/ctc/train.py:173-174.
-    reduction 'none': the first result is costs (N,) fp32 CUDA, cost[n] = logZ_den[n] - (1+lamb) log p_ctc[n], and grad is
-    unscaled (grad[n] = d cost[n] / d logits[n]); size_average is then ignored.
-    zero_infinity: an utterance whose cost is not finite gets cost 0 and zero gradient rows (the divisor of size_average
-    stays N)."""
-    check_reduction(reduction)
-    per_utt = reduction == "none"
-    with_costs = per_utt or zero_infinity
-    L = _lib.lib()
-    entry = L.ccb_ctc_crf_loss_logits_fwd if from_logits else L.ccb_ctc_crf_loss_fwd
-    ckpt_entry = L.ccb_ctc_crf_loss_logits_ckpt_fwd if from_logits else L.ccb_ctc_crf_loss_ckpt_fwd
-    assert logits.is_cuda and logits.dim() == 3 and logits.is_contiguous()
-    if logits.dtype not in _DTYPES:
-        raise RuntimeError(f"unsupported logits dtype {logits.dtype}")
-    N, T, V = _check_batch_args(logits, labels, lx, ly)
-    dev = logits.device
-    esz = logits.element_size()
-    scale = 1.0 if per_utt else 1.0 / N if size_average else 1.0
-    with torch.cuda.device(dev):
-        meta, sum_l, _ = upload_meta(labels, lx, ly, dev)
-        base = meta.data_ptr()
-        p_labels, p_off = base, base + 4 * sum_l
-        p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
-        grad = torch.empty((N, T, V), dtype=torch.float32, device=dev)
-        costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
-        parts = torch.empty(2 * N, dtype=torch.float32, device=dev) if want_parts else None
-        stream = _stream(dev)
-
-        def run_slices():
-            slices = _plan_slices(L, lx, ly, N, V, dev)
-            losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
-            for i, (n0, n1, tmax, maxl, k) in enumerate(slices):
-                n = n1 - n0
-                alpha_floats = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
-                alpha_ws = torch.empty(int(alpha_floats), dtype=torch.float32, device=dev)
-                aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
-                ctc_ws = torch.empty(int(L.ccb_ctc_workspace_bytes(n, tmax, maxl)), dtype=torch.uint8, device=dev)
-                sub_parts = torch.empty(2 * n, dtype=torch.float32, device=dev) if want_parts else None
-                args = (p_labels, p_off + 4 * n0, p_ly + 4 * n0, p_lx + 4 * n0, maxl, float(lamb),
-                        float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(), ctc_ws.data_ptr(),
-                        grad.data_ptr() + n0 * T * V * 4, losses.data_ptr() + 4 * i,
-                        sub_parts.data_ptr() if want_parts else None)
-                y_ptr = logits.data_ptr() + n0 * T * V * esz
-                if with_costs:      # each slice writes its own costs[n0:n1] in place
-                    rc = L.ccb_ctc_crf_loss_costs(y_ptr, _DTYPES[logits.dtype], int(from_logits), n, T, V, tmax, k, *args,
-                                                  costs.data_ptr() + 4 * n0 if per_utt else None, int(zero_infinity),
-                                                  stream)
-                elif k:
-                    rc = ckpt_entry(y_ptr, _DTYPES[logits.dtype], n, T, V, tmax, k, *args, stream)
-                else:
-                    rc = entry(y_ptr, _DTYPES[logits.dtype], n, T, V, tmax, *args, stream)
-                _check(rc, "ctc_crf_loss_fwd")
-                if want_parts:
-                    parts[n0:n1] = sub_parts[:n]
-                    parts[N + n0:N + n1] = sub_parts[n:]
-                del alpha_ws, aux_ws, ctc_ws      # stream-ordered reuse by the caching allocator for the next slice
-            return slices, losses
-
-        try:
-            slices, losses = run_slices()
-        except torch.cuda.OutOfMemoryError:       # the cached memory figure was stale: measure again, slice finer, redo
-            _budget_cache.pop(torch.device(dev).index, None)
-            torch.cuda.empty_cache()
-            slices, losses = run_slices()
-        loss = losses.sum().reshape(1) if len(slices) > 1 else losses
-        meta.record_stream(torch.cuda.current_stream(dev))
-    return (costs if per_utt else loss), grad, parts
-
-
 def _fwd_only_need(L, n, tmax, m=None):
     return (int(L.ccb_den_fwd_alpha_floats(n)) * 4 + int(L.ccb_den_aux_bytes(n, tmax))
             + int(L.ccb_num_fwd_only_bytes(n if m is None else m)))
@@ -395,6 +337,56 @@ def _plan_fwd_only_slices(L, lx, ly, N, dev, seq_off=None):
     return slices
 
 
+def _den_slices(L, dev, slices, fwd_only=False):
+    """The den scratch of each slice, allocated when its turn comes: yields (i, slice, alpha_ws, aux_ws).  alpha is the
+    frame ring of the forward-only loss (fwd_only; slices of _plan_fwd_only_slices), or else the full or the checkpointed
+    spill by the slice's K (slices of _plan_slices).  The caller drops its references to a slice's scratch before asking for
+    the next one, so that the caching allocator reuses the blocks in stream order."""
+    for i, s in enumerate(slices):
+        n, tmax = s[1] - s[0], s[2]
+        if fwd_only:
+            alpha_floats = L.ccb_den_fwd_alpha_floats(n)
+        else:
+            k = s[4]
+            alpha_floats = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
+        alpha_ws = torch.empty(int(alpha_floats), dtype=torch.float32, device=dev)
+        aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
+        yield i, s, alpha_ws, aux_ws
+        del alpha_ws, aux_ws
+
+
+def _retry_oom(dev, run):
+    """run(), and once more if it runs out of device memory: the cached memory figure was stale, so it is measured again
+    and run() plans finer slices.  The retry starts after the failed attempt's buffers have been released."""
+    try:
+        return run()
+    except torch.cuda.OutOfMemoryError:
+        _budget_cache.pop(torch.device(dev).index, None)
+    torch.cuda.empty_cache()
+    return run()
+
+
+def _batch_loss(losses: torch.Tensor) -> torch.Tensor:
+    """The (1,) loss of a call from the loss of each of its slices (a single slice's is the call's)."""
+    return losses.sum().reshape(1) if losses.numel() > 1 else losses
+
+
+def ctc_crf_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
+                     lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False,
+                     reduction: Optional[str] = None, zero_infinity: bool = False
+                     ) -> Tuple[torch.Tensor, torch.Tensor, Optional[torch.Tensor]]:
+    """Fused CTC-CRF loss.  logits (N,T,V) fp32, bf16 or fp16 CUDA contiguous log-probs; labels/lx/ly int32 CPU.
+    Returns (loss[1] fp32 CUDA, grad (N,T,V) fp32 CUDA, parts[2N] or None).  Never synchronises the host.
+    Batches whose scratch does not fit the free memory (or > 512 utterances) are processed in slices.
+    from_logits: `logits` are the RAW encoder outputs; log_softmax and its Jacobian are applied inside
+    (grad = d loss / d raw logits), replacing cat/ctc/train.py:173-174.
+    reduction 'none': the first result is costs (N,) fp32 CUDA, cost[n] = logZ_den[n] - (1+lamb) log p_ctc[n], and grad is
+    unscaled (grad[n] = d cost[n] / d logits[n]); size_average is then ignored.
+    zero_infinity: an utterance whose cost is not finite gets cost 0 and zero gradient rows (the divisor of size_average
+    stays N)."""
+    return _ctc_crf_loss(logits, labels, lx, ly, lamb, size_average, want_parts, from_logits, reduction, zero_infinity, True)
+
+
 def ctc_crf_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
                           lamb: float, size_average: bool, want_parts: bool = False, from_logits: bool = False,
                           reduction: Optional[str] = None, zero_infinity: bool = False
@@ -403,46 +395,59 @@ def ctc_crf_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.
     The den forward pass keeps alpha on a ring of frames, the numerator writes no cells, and no (N,T,V) buffer is
     allocated, so the scratch is a few frames of the den graph per slice whatever the lengths.  Never synchronises the
     host.  Arguments as for ``ctc_crf_loss_fwd`` (reduction 'none': the first result is the (N,) costs)."""
-    check_reduction(reduction)
-    per_utt = reduction == "none"
+    loss, _, parts = _ctc_crf_loss(logits, labels, lx, ly, lamb, size_average, want_parts, from_logits, reduction,
+                                   zero_infinity, False)
+    return loss, parts
+
+
+def _ctc_crf_loss(logits, labels, lx, ly, lamb, size_average, want_parts, from_logits, reduction, zero_infinity, with_grad):
+    """ctc_crf_loss_fwd (with_grad) or ctc_crf_loss_fwd_only: (loss or costs, grad or None, parts or None).  The two differ
+    in the slice planner, the alpha and numerator workspaces and the native entry only."""
+    per_utt = check_reduction(reduction)
     L = _lib.lib()
     N, T, V = _check_batch_args(logits, labels, lx, ly)
     dev = logits.device
     esz = logits.element_size()
     scale = 1.0 if per_utt else 1.0 / N if size_average else 1.0
     with torch.cuda.device(dev):
-        meta, sum_l, _ = upload_meta(labels, lx, ly, dev)
-        base = meta.data_ptr()
-        p_labels, p_off = base, base + 4 * sum_l
-        p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
-        parts = torch.empty(2 * N, dtype=torch.float32, device=dev) if want_parts else None
+        meta, _ = upload_meta(labels, lx, ly, dev)
+        grad = torch.empty((N, T, V), dtype=torch.float32, device=dev) if with_grad else None
         costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
+        parts = torch.empty(2 * N, dtype=torch.float32, device=dev) if want_parts else None
         stream = _stream(dev)
-        slices = _plan_fwd_only_slices(L, lx, ly, N, dev)
-        losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
-        for i, (n0, n1, tmax, maxl) in enumerate(slices):
-            n = n1 - n0
-            alpha_ws = torch.empty(int(L.ccb_den_fwd_alpha_floats(n)), dtype=torch.float32, device=dev)
-            aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
-            num_ws = torch.empty(int(L.ccb_num_fwd_only_bytes(n)), dtype=torch.uint8, device=dev)
-            sub_parts = torch.empty(2 * n, dtype=torch.float32, device=dev) if want_parts else None
-            args = (logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype], int(from_logits),
-                    n, T, V, tmax, p_labels, p_off + 4 * n0, p_ly + 4 * n0, p_lx + 4 * n0, maxl,
-                    float(lamb), float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(),
-                    num_ws.data_ptr(), losses.data_ptr() + 4 * i, sub_parts.data_ptr() if want_parts else None)
-            if per_utt or zero_infinity:
-                rc = L.ccb_ctc_crf_loss_costs_fwd_only(*args, costs.data_ptr() + 4 * n0 if per_utt else None,
-                                                       int(zero_infinity), stream)
-            else:
-                rc = L.ccb_ctc_crf_loss_fwd_only(*args, stream)
-            _check(rc, "ctc_crf_loss_fwd_only")
-            if want_parts:
-                parts[n0:n1] = sub_parts[:n]
-                parts[N + n0:N + n1] = sub_parts[n:]
-            del alpha_ws, aux_ws, num_ws      # stream-ordered reuse by the caching allocator for the next slice
-        loss = losses.sum().reshape(1) if len(slices) > 1 else losses
-        meta.record_stream(torch.cuda.current_stream(dev))
-    return (costs if per_utt else loss), parts
+
+        def run_slices():
+            slices = _plan_slices(L, lx, ly, N, V, dev) if with_grad else _plan_fwd_only_slices(L, lx, ly, N, dev)
+            losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
+            for i, s, alpha_ws, aux_ws in _den_slices(L, dev, slices, fwd_only=not with_grad):
+                n0, n1, tmax, maxl = s[:4]
+                n = n1 - n0
+                # the numerator's cells and log-likelihoods, or its log-likelihoods alone
+                num_bytes = L.ccb_ctc_workspace_bytes(n, tmax, maxl) if with_grad else L.ccb_num_fwd_only_bytes(n)
+                num_ws = torch.empty(int(num_bytes), dtype=torch.uint8, device=dev)
+                sub_parts = torch.empty(2 * n, dtype=torch.float32, device=dev) if want_parts else None
+                y = (logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype], int(from_logits), n, T, V, tmax)
+                ins = (meta.labels, meta.label_off + 4 * n0, meta.ly + 4 * n0, meta.lx + 4 * n0, maxl, float(lamb),
+                       float(scale), alpha_ws.data_ptr(), aux_ws.data_ptr(), num_ws.data_ptr())
+                # each slice writes its own costs[n0:n1] (and grad[n0:n1]) in place
+                outs = (losses.data_ptr() + 4 * i, _ptr(sub_parts), costs.data_ptr() + 4 * n0 if per_utt else None,
+                        int(zero_infinity), stream)
+                if with_grad:
+                    rc = L.ccb_ctc_crf_loss_costs(*y, s[4], *ins, grad.data_ptr() + n0 * T * V * 4, *outs)
+                else:
+                    rc = L.ccb_ctc_crf_loss_costs_fwd_only(*y, *ins, *outs)
+                _check(rc, "ctc_crf_loss_fwd" if with_grad else "ctc_crf_loss_fwd_only")
+                if want_parts:
+                    parts[n0:n1] = sub_parts[:n]
+                    parts[N + n0:N + n1] = sub_parts[n:]
+                del alpha_ws, aux_ws, num_ws      # stream-ordered reuse by the caching allocator for the next slice
+            return losses
+
+        # the forward-only planner never reslices: there is nothing to retry
+        losses = _retry_oom(dev, run_slices) if with_grad else run_slices()
+        loss = _batch_loss(losses)
+        meta.buf.record_stream(torch.cuda.current_stream(dev))
+    return (costs if per_utt else loss), grad, parts
 
 
 def _check_batch_args(logits, labels, lx, ly):
@@ -471,32 +476,7 @@ def ctc_loss_fwd(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, l
     Returns (loss[1], grad (N,T,V) fp32 = d loss / d logits, logp[N]) on the device; never synchronises the host.
     reduction 'none': the first result is costs (N,), cost[n] = -log p[n], and grad is unscaled; zero_infinity: a cost
     that is not finite becomes 0 and its gradient rows zeros (as in ``ctc_crf_loss_fwd``)."""
-    check_reduction(reduction)
-    per_utt = reduction == "none"
-    L = _lib.lib()
-    N, T, V = _check_batch_args(logits, labels, lx, ly)
-    dev = logits.device
-    scale = 1.0 if per_utt else 1.0 / N if size_average else 1.0
-    with torch.cuda.device(dev):
-        meta, sum_l, maxl = upload_meta(labels, lx, ly, dev)
-        base = meta.data_ptr()
-        p_labels, p_off = base, base + 4 * sum_l
-        p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
-        tmax = max(1, int(lx.max()))
-        grad = torch.empty((N, T, V), dtype=torch.float32, device=dev)
-        loss = torch.empty(1, dtype=torch.float32, device=dev)
-        logp = torch.empty(N, dtype=torch.float32, device=dev)
-        ws = torch.empty(int(L.ccb_ctc_workspace_bytes(N, tmax, maxl)), dtype=torch.uint8, device=dev)
-        args = (logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx, maxl,
-                int(blank), float(scale), ws.data_ptr(), grad.data_ptr(), loss.data_ptr(), logp.data_ptr())
-        if per_utt or zero_infinity:
-            costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
-            rc = L.ccb_ctc_loss_costs(*args, costs.data_ptr() if per_utt else None, int(zero_infinity), _stream(dev))
-        else:
-            rc = L.ccb_ctc_loss_fwd(*args, _stream(dev))
-        _check(rc, "ctc_loss_fwd")
-        meta.record_stream(torch.cuda.current_stream(dev))
-    return (costs if per_utt else loss), grad, logp
+    return _ctc_loss(logits, labels, lx, ly, size_average, blank, reduction, zero_infinity, True)
 
 
 def ctc_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor,
@@ -505,31 +485,31 @@ def ctc_loss_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tens
     """The loss of ``ctc_loss_fwd`` without its gradient: (loss[1], logp[N]) on the device, the same values, from one alpha
     chain per utterance that writes no cells.  No workspace, no (N,T,V) buffer, no host synchronisation.
     reduction and zero_infinity as for ``ctc_loss_fwd``."""
-    check_reduction(reduction)
-    per_utt = reduction == "none"
+    loss, _, logp = _ctc_loss(logits, labels, lx, ly, size_average, blank, reduction, zero_infinity, False)
+    return loss, logp
+
+
+def _ctc_loss(logits, labels, lx, ly, size_average, blank, reduction, zero_infinity, with_grad):
+    """ctc_loss_fwd (with_grad) or ctc_loss_fwd_only: (loss or costs, grad or None, logp)."""
+    per_utt = check_reduction(reduction)
     L = _lib.lib()
     N, T, V = _check_batch_args(logits, labels, lx, ly)
     dev = logits.device
     scale = 1.0 if per_utt else 1.0 / N if size_average else 1.0
     with torch.cuda.device(dev):
-        meta, sum_l, maxl = upload_meta(labels, lx, ly, dev)
-        base = meta.data_ptr()
-        p_labels, p_off = base, base + 4 * sum_l
-        p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
+        meta, maxl = upload_meta(labels, lx, ly, dev)
         tmax = max(1, int(lx.max()))
+        grad = torch.empty((N, T, V), dtype=torch.float32, device=dev) if with_grad else None
         loss = torch.empty(1, dtype=torch.float32, device=dev)
         logp = torch.empty(N, dtype=torch.float32, device=dev)
-        if per_utt or zero_infinity:
-            costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
-            rc = L.ccb_ctc_loss_costs(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx,
-                                      maxl, int(blank), float(scale), None, None, loss.data_ptr(), logp.data_ptr(),
-                                      costs.data_ptr() if per_utt else None, int(zero_infinity), _stream(dev))
-        else:
-            rc = L.ccb_ctc_loss_fwd_only(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, p_labels, p_off, p_ly, p_lx,
-                                         maxl, int(blank), float(scale), loss.data_ptr(), logp.data_ptr(), _stream(dev))
-        _check(rc, "ctc_loss_fwd_only")
-        meta.record_stream(torch.cuda.current_stream(dev))
-    return (costs if per_utt else loss), logp
+        ws = torch.empty(int(L.ccb_ctc_workspace_bytes(N, tmax, maxl)), dtype=torch.uint8, device=dev) if with_grad else None
+        costs = torch.empty(N, dtype=torch.float32, device=dev) if per_utt else None
+        rc = L.ccb_ctc_loss_costs(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, meta.labels, meta.label_off,
+                                  meta.ly, meta.lx, maxl, int(blank), float(scale), _ptr(ws), _ptr(grad), loss.data_ptr(),
+                                  logp.data_ptr(), _ptr(costs), int(zero_infinity), _stream(dev))
+        _check(rc, "ctc_loss_fwd" if with_grad else "ctc_loss_fwd_only")
+        meta.buf.record_stream(torch.cuda.current_stream(dev))
+    return (costs if per_utt else loss), grad, logp
 
 
 def ctc_align(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: torch.Tensor, blank: int = 0
@@ -541,17 +521,14 @@ def ctc_align(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, ly: 
     N, T, V = _check_batch_args(logits, labels, lx, ly)
     dev = logits.device
     with torch.cuda.device(dev):
-        meta, sum_l, maxl = upload_meta(labels, lx, ly, dev)
-        base = meta.data_ptr()
-        p_labels, p_off = base, base + 4 * sum_l
-        p_ly, p_lx = p_off + 4 * (N + 1), p_off + 4 * (2 * N + 1)
+        meta, maxl = upload_meta(labels, lx, ly, dev)
         align = torch.empty((N, T), dtype=torch.int32, device=dev)
         score = torch.empty(N, dtype=torch.float32, device=dev)
         ws = torch.empty(int(L.ccb_ctc_align_workspace_bytes(N, T, maxl)), dtype=torch.uint8, device=dev)
-        rc = L.ccb_ctc_align(logits.data_ptr(), _DTYPES[logits.dtype], T * V, V, N, T, V, p_labels, p_off, p_ly, p_lx, maxl,
-                             int(blank), ws.data_ptr(), align.data_ptr(), score.data_ptr(), _stream(dev))
+        rc = L.ccb_ctc_align(logits.data_ptr(), _DTYPES[logits.dtype], T * V, V, N, T, V, meta.labels, meta.label_off, meta.ly,
+                             meta.lx, maxl, int(blank), ws.data_ptr(), align.data_ptr(), score.data_ptr(), _stream(dev))
         _check(rc, "ctc_align")
-        meta.record_stream(torch.cuda.current_stream(dev))
+        meta.buf.record_stream(torch.cuda.current_stream(dev))
     return align, score
 
 
@@ -636,32 +613,22 @@ def _check_seq_args(logits, labels, lx, ly, utt):
     return N, T, V, group_seqs(utt, labels, ly, N)
 
 
-class _SeqMeta:
-    """Device addresses of the int32 meta block of a grouped call:
+class _SeqMeta(_Meta):
+    """The meta block of a grouped call:
     [labels | label_off (M+1) | ly (M) | lx (N) | row (M) | pos (M) | seq_off, (n1-n0+1) entries per slice]
     row and seq_off are relative to the slice that holds the sequence (its logits pointer and first sequence); pos is the
     caller's index.  Slice i of utterances [n0, n1) finds its offsets at seq_off + n0 + i."""
 
     def __init__(self, grp: SeqGroups, lx: torch.Tensor, bounds, device):
         N = int(lx.numel())
-        M = grp.M
-        label_off = torch.zeros(M + 1, dtype=torch.int32)
-        label_off[1:].copy_(torch.cumsum(grp.ly.to(torch.int64), 0))
         first = torch.empty(N, dtype=torch.int64)            # first utterance of the slice of each utterance
         offs = []
         for n0, n1 in bounds:
             first[n0:n1] = n0
             offs.append(grp.off[n0:n1 + 1] - grp.off[n0])
         row = (grp.row.to(torch.int64) - first[grp.row.to(torch.int64)]).to(torch.int32)
-        parts = [grp.labels, label_off, grp.ly, lx.to(torch.int32), row, grp.pos, torch.cat(offs).to(torch.int32)]
-        ring = _rings.setdefault(torch.device(device).index, _PinnedRing())
-        self.buf = ring.stage(parts, device)
-        base = self.buf.data_ptr()
-        sizes = [int(p.numel()) for p in parts]
-        ptrs = [base]
-        for s in sizes[:-1]:
-            ptrs.append(ptrs[-1] + 4 * s)
-        self.labels, self.label_off, self.ly, self.lx, self.row, self.pos, self.seq_off = ptrs
+        super().__init__(device, labels=grp.labels, label_off=_label_off(grp.ly), ly=grp.ly, lx=lx.to(torch.int32),
+                         row=row, pos=grp.pos, seq_off=torch.cat(offs).to(torch.int32))
 
     def slice_args(self, i, n0, s0):
         """(labels, label_off, label_len, len, row, pos, seq_off) of slice i, utterances from n0, sequences from s0."""
@@ -686,8 +653,7 @@ def ctc_crf_loss_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tens
     cost[m] = logZ_den[utt[m]] - (1+lamb) log p_ctc[m]; reduction None: the sum over the sequences (/ M with size_average) and
     grad = its gradient.  reduction 'none': the (M,) costs in the caller's order; grad then holds the unscaled den occupancies
     and the third result is the state ``seqs_backward`` turns into the gradient for given per-sequence weights."""
-    check_reduction(reduction)
-    per_seq = reduction == "none"
+    per_seq = check_reduction(reduction)
     L = _lib.lib()
     N, T, V, grp = _check_seq_args(logits, labels, lx, ly, utt)
     M = grp.M
@@ -704,12 +670,9 @@ def ctc_crf_loss_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tens
             meta = _SeqMeta(grp, lx, [(s[0], s[1]) for s in slices], dev)
             losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
             kept = []
-            for i, (n0, n1, tmax, maxl, k) in enumerate(slices):
+            for i, (n0, n1, tmax, maxl, k), alpha_ws, aux_ws in _den_slices(L, dev, slices):
                 n = n1 - n0
                 s0, m = int(grp.off[n0]), int(grp.off[n1] - grp.off[n0])
-                alpha_floats = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
-                alpha_ws = torch.empty(int(alpha_floats), dtype=torch.float32, device=dev)
-                aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
                 ctc_ws = torch.empty(int(L.ccb_ctc_workspace_bytes(m, tmax, maxl)), dtype=torch.uint8, device=dev)
                 lab, loff, lly, llx, row, pos, soff = meta.slice_args(i, n0, s0)
                 rc = L.ccb_ctc_crf_loss_seqs(logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype], int(from_logits),
@@ -721,15 +684,10 @@ def ctc_crf_loss_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tens
                 if per_seq:    # the backward reads this slice's numerator cells and den aux block (logZ, normalisers)
                     kept.append((n0, n1, tmax, maxl, s0, m, i, aux_ws, ctc_ws))
                 del alpha_ws, aux_ws, ctc_ws
-            return slices, losses, meta, kept
+            return losses, meta, kept
 
-        try:
-            slices, losses, meta, kept = run_slices()
-        except torch.cuda.OutOfMemoryError:       # as in ctc_crf_loss_fwd
-            _budget_cache.pop(torch.device(dev).index, None)
-            torch.cuda.empty_cache()
-            slices, losses, meta, kept = run_slices()
-        loss = losses.sum().reshape(1) if len(slices) > 1 else losses
+        losses, meta, kept = _retry_oom(dev, run_slices)
+        loss = _batch_loss(losses)
         meta.buf.record_stream(torch.cuda.current_stream(dev))
     state = (SeqsGradState(logits, meta, kept, grad, from_logits, zero_infinity, -(1.0 + float(lamb)), 0, M)
              if per_seq else None)
@@ -741,8 +699,7 @@ def ctc_crf_loss_seqs_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: t
                                reduction: Optional[str] = None, zero_infinity: bool = False) -> torch.Tensor:
     """The loss of ``ctc_crf_loss_seqs`` without a gradient (the passes of ``ctc_crf_loss_fwd_only``): the scalar, or the (M,)
     costs with reduction 'none'."""
-    check_reduction(reduction)
-    per_seq = reduction == "none"
+    per_seq = check_reduction(reduction)
     L = _lib.lib()
     N, T, V, grp = _check_seq_args(logits, labels, lx, ly, utt)
     M = grp.M
@@ -755,11 +712,9 @@ def ctc_crf_loss_seqs_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: t
         slices = _plan_fwd_only_slices(L, lx, grp.ly, N, dev, seq_off=grp.off)
         meta = _SeqMeta(grp, lx, [(s[0], s[1]) for s in slices], dev)
         losses = torch.empty(len(slices), dtype=torch.float32, device=dev)
-        for i, (n0, n1, tmax, maxl) in enumerate(slices):
+        for i, (n0, n1, tmax, maxl), alpha_ws, aux_ws in _den_slices(L, dev, slices, fwd_only=True):
             n = n1 - n0
             s0, m = int(grp.off[n0]), int(grp.off[n1] - grp.off[n0])
-            alpha_ws = torch.empty(int(L.ccb_den_fwd_alpha_floats(n)), dtype=torch.float32, device=dev)
-            aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
             num_ws = torch.empty(max(4, int(L.ccb_num_fwd_only_bytes(m))), dtype=torch.uint8, device=dev)
             lab, loff, lly, llx, row, pos, _ = meta.slice_args(i, n0, s0)
             rc = L.ccb_ctc_crf_loss_seqs_fwd_only(logits.data_ptr() + n0 * T * V * esz, _DTYPES[logits.dtype],
@@ -769,7 +724,7 @@ def ctc_crf_loss_seqs_fwd_only(logits: torch.Tensor, labels: torch.Tensor, lx: t
                                                   costs.data_ptr() if per_seq else None, int(zero_infinity), stream)
             _check(rc, "ctc_crf_loss_seqs_fwd_only")
             del alpha_ws, aux_ws, num_ws
-        loss = losses.sum().reshape(1) if len(slices) > 1 else losses
+        loss = _batch_loss(losses)
         meta.buf.record_stream(torch.cuda.current_stream(dev))
     return costs if per_seq else loss
 
@@ -781,8 +736,7 @@ def ctc_loss_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, 
     (reduction None: the sum over the sequences, / M with size_average; 'none': the (M,) costs -log p[m] in the caller's
     order), then grad = d loss / d logits (None without with_grad, or with reduction 'none', whose gradient comes from
     ``seqs_backward`` on the returned state)."""
-    check_reduction(reduction)
-    per_seq = reduction == "none"
+    per_seq = check_reduction(reduction)
     defer = per_seq and with_grad
     L = _lib.lib()
     N, T, V, grp = _check_seq_args(logits, labels, lx, ly, utt)
@@ -800,9 +754,8 @@ def ctc_loss_seqs(logits: torch.Tensor, labels: torch.Tensor, lx: torch.Tensor, 
         costs = torch.empty(M, dtype=torch.float32, device=dev) if per_seq else None
         lab, loff, lly, llx, row, pos, soff = meta.slice_args(0, 0, 0)
         rc = L.ccb_ctc_loss_seqs(logits.data_ptr(), _DTYPES[logits.dtype], N, T, V, tmax, lab, loff, lly, llx, M, row, pos,
-                                 soff, maxl, int(blank), float(scale), ws.data_ptr() if ws is not None else None,
-                                 grad.data_ptr() if grad is not None else None, loss.data_ptr(), logp.data_ptr(),
-                                 costs.data_ptr() if per_seq else None, int(zero_infinity), int(defer), _stream(dev))
+                                 soff, maxl, int(blank), float(scale), _ptr(ws), _ptr(grad), loss.data_ptr(),
+                                 logp.data_ptr(), _ptr(costs), int(zero_infinity), int(defer), _stream(dev))
         _check(rc, "ctc_loss_seqs")
         meta.buf.record_stream(torch.cuda.current_stream(dev))
     state = (SeqsGradState(logits, meta, [(0, N, tmax, maxl, 0, M, 0, None, ws)], None, False, zero_infinity, -1.0,
@@ -909,11 +862,8 @@ def crf_sample(logits: torch.Tensor, lx: torch.Tensor, num_samples: int = 1, gen
 
         def run_slices():
             slices = _plan_slices(L, lx, None, N, V, dev, ws_bytes=lambda n, tmax: L.ccb_crf_sample_ws_bytes(n, K, tmax))
-            for n0, n1, tmax, _, k in slices:
+            for _, (n0, n1, tmax, _, k), alpha_ws, aux_ws in _den_slices(L, dev, slices):
                 n = n1 - n0
-                alpha_floats = L.ccb_den_ckpt_alpha_floats(n, tmax, k) if k else L.ccb_den_alpha_floats(n, tmax)
-                alpha_ws = torch.empty(int(alpha_floats), dtype=torch.float32, device=dev)
-                aux_ws = torch.empty(int(L.ccb_den_aux_bytes(n, tmax)), dtype=torch.uint8, device=dev)
                 sample_ws = torch.empty(int(L.ccb_crf_sample_ws_bytes(n, K, tmax)), dtype=torch.uint8, device=dev)
                 rc = L.ccb_crf_sample(y.data_ptr() + n0 * T * V * esz, _DTYPES[y.dtype], n, T, V, tmax, k,
                                       lens.data_ptr() + 4 * n0, K, seed, n0, alpha_ws.data_ptr(), aux_ws.data_ptr(),
@@ -923,12 +873,7 @@ def crf_sample(logits: torch.Tensor, lx: torch.Tensor, num_samples: int = 1, gen
                 _check(rc, "crf_sample")
                 del alpha_ws, aux_ws, sample_ws
 
-        try:
-            run_slices()
-        except torch.cuda.OutOfMemoryError:       # as in ctc_crf_loss_fwd
-            _budget_cache.pop(torch.device(dev).index, None)
-            torch.cuda.empty_cache()
-            run_slices()
+        _retry_oom(dev, run_slices)
         lens.record_stream(torch.cuda.current_stream(dev))
     return tokens, lengths, align, path_logp
 

@@ -28,94 +28,60 @@ class _WARP_CTC_GPU(Function):
     """__init__.py:25-56: CTC loss on log-softmax inputs.  Same arguments, result and gradient as the reference's
     Function; underneath it is ONE native call on the (N,T,V) tensor in place -- no (T,N,V) transpose copy (:31), no
     zero-filled gradient (:32), no host round trip for the per-utterance costs (:33-35) -- see ``_C.ctc_loss_fwd``.
-    (``_C.gpu_ctc`` keeps the reference's pybind signature for callers that use it directly.)"""
+    (``_C.gpu_ctc`` keeps the reference's pybind signature for callers that use it directly.)
+    reduction and zero_infinity (additions, after the reference's arguments) as for ``_CTC_CRF``, cost[n] = -log p[n]."""
 
     @staticmethod
-    def forward(ctx, logits, labels, input_lengths, label_lengths, size_average=True):
+    def forward(ctx, logits, labels, input_lengths, label_lengths, size_average=True, reduction=None, zero_infinity=False):
         logits = logits.contiguous()
-        costs, grads, _ = core.ctc_loss_fwd(logits, labels, input_lengths, label_lengths, size_average)
-        ctx.grads = grads
-        return costs
+        out, grads, _ = core.ctc_loss_fwd(logits, labels, input_lengths, label_lengths, size_average,
+                                          **_loss_options(reduction, zero_infinity))
+        ctx.grads, ctx.lx, ctx.in_dtype, ctx.reduction = grads, input_lengths, logits.dtype, reduction
+        return out
 
     @staticmethod
     def backward(ctx, grad_output):
-        return ctx.grads * grad_output.to(ctx.grads.device), None, None, None, None, None, None
+        return (_loss_backward(ctx, grad_output),) + (None,) * 6
 
 
 class _CTC_CRF(Function):
     """__init__.py:58-94.  loss = sum_n [logZ_den(n) - (1+lamb) log p_ctc(n)] (/N),
-    grad = [gamma_den - (1+lamb) gamma_ctc] (/N); backward = grads * grad_output."""
+    grad = [gamma_den - (1+lamb) gamma_ctc] (/N); backward = grads * grad_output.
+    Additions, after the reference's arguments: ``reduction='none'`` returns the (N,) costs
+    cost[n] = logZ_den[n] - (1+lamb) log p_ctc[n], with the gradient kept unscaled, G[n] = d cost[n] / d logits[n], so that the
+    backward is one pass that writes grad_output[n] * G[n] in the logits' dtype (``_C.grad_rows_scale``); ``zero_infinity``
+    as for ``CTC_CRF_LOSS``; ``from_logits=True`` is the loss of ``_CTC_CRF_LOGITS``."""
 
     @staticmethod
-    def forward(ctx, logits, labels, input_lengths, label_lengths, lamb=0.1, size_average=True):
+    def forward(ctx, logits, labels, input_lengths, label_lengths, lamb=0.1, size_average=True, reduction=None,
+                zero_infinity=False, from_logits=False):
         logits = logits.contiguous()
-        costs, grads, _ = core.ctc_crf_loss_fwd(logits, labels, input_lengths, label_lengths, lamb, size_average)
-        ctx.grads = grads
-        return costs
+        opts = _loss_options(reduction, zero_infinity)
+        if from_logits:
+            opts["from_logits"] = True
+        out, grads, _ = core.ctc_crf_loss_fwd(logits, labels, input_lengths, label_lengths, lamb, size_average, **opts)
+        ctx.grads, ctx.lx, ctx.in_dtype, ctx.reduction = grads, input_lengths, logits.dtype, reduction
+        return out
 
     @staticmethod
     def backward(ctx, grad_output):
-        return ctx.grads * grad_output.to(ctx.grads.device), None, None, None, None, None, None
+        return (_loss_backward(ctx, grad_output),) + (None,) * 8
 
 
-class _CTC_CRF_LOGITS(Function):
+class _CTC_CRF_LOGITS(_CTC_CRF):
     """SURVEY 8f-1: the same loss taken on the RAW encoder outputs.  Replaces, in one native call,
     ``logits = net_out.float().log_softmax(-1); loss = _CTC_CRF(logits, ...)`` and the autograd backward of the cast
     and of log_softmax (cat/ctc/train.py:173-174,184-190): no normalised fp32 copy is materialised and the gradient
     comes back already chained through the softmax Jacobian, in the dtype of the input."""
 
     @staticmethod
-    def forward(ctx, logits, labels, input_lengths, label_lengths, lamb=0.1, size_average=True):
-        logits = logits.contiguous()
-        costs, grads, _ = core.ctc_crf_loss_fwd(logits, labels, input_lengths, label_lengths, lamb, size_average,
-                                                from_logits=True)
-        ctx.grads = grads
-        ctx.in_dtype = logits.dtype
-        return costs
-
-    @staticmethod
-    def backward(ctx, grad_output):
-        g = ctx.grads * grad_output.to(ctx.grads.device)
-        return g.to(ctx.in_dtype), None, None, None, None, None, None
+    def forward(ctx, logits, labels, input_lengths, label_lengths, lamb=0.1, size_average=True, reduction=None,
+                zero_infinity=False):
+        return _CTC_CRF.forward(ctx, logits, labels, input_lengths, label_lengths, lamb, size_average, reduction,
+                                zero_infinity, True)
 
 
-class _CTC_CRF_COSTS(Function):
-    """The loss of ``_CTC_CRF`` / ``_CTC_CRF_LOGITS`` with ``reduction='none'`` (the (N,) costs
-    cost[n] = logZ_den[n] - (1+lamb) log p_ctc[n]) and / or ``zero_infinity``.  With 'none' the native call keeps the gradient
-    unscaled, G[n] = d cost[n] / d logits[n], and the backward is one pass that writes grad_output[n] * G[n] in the logits'
-    dtype (``_C.grad_rows_scale``)."""
-
-    @staticmethod
-    def forward(ctx, logits, labels, input_lengths, label_lengths, lamb, size_average, from_logits, reduction, zero_infinity):
-        logits = logits.contiguous()
-        out, grads, _ = core.ctc_crf_loss_fwd(logits, labels, input_lengths, label_lengths, lamb, size_average,
-                                              from_logits=from_logits, reduction=reduction, zero_infinity=zero_infinity)
-        ctx.grads, ctx.lx, ctx.in_dtype, ctx.reduction = grads, input_lengths, logits.dtype, reduction
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_output):
-        return (_costs_backward(ctx, grad_output),) + (None,) * 8
-
-
-class _WARP_CTC_COSTS(Function):
-    """``_WARP_CTC_GPU`` with ``reduction='none'`` (cost[n] = -log p[n]) and / or ``zero_infinity``; backward as in
-    ``_CTC_CRF_COSTS``."""
-
-    @staticmethod
-    def forward(ctx, logits, labels, input_lengths, label_lengths, size_average, reduction, zero_infinity):
-        logits = logits.contiguous()
-        out, grads, _ = core.ctc_loss_fwd(logits, labels, input_lengths, label_lengths, size_average,
-                                          reduction=reduction, zero_infinity=zero_infinity)
-        ctx.grads, ctx.lx, ctx.in_dtype, ctx.reduction = grads, input_lengths, logits.dtype, reduction
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_output):
-        return (_costs_backward(ctx, grad_output),) + (None,) * 6
-
-
-def _costs_backward(ctx, grad_output):
+def _loss_backward(ctx, grad_output):
     if ctx.reduction == "none":     # grad_logits[n] = grad_output[n] * G[n], in one pass, in the logits' dtype
         return core.grad_rows_scale(ctx.grads, grad_output, ctx.lx, ctx.in_dtype)
     return (ctx.grads * grad_output.to(ctx.grads.device)).to(ctx.in_dtype)
@@ -168,6 +134,23 @@ def _check_utt(utt):
     _assert_no_grad(utt)
 
 
+def _check_loss_args(logits, labels, lx, ly, utt, dtypes=True):
+    """The reference's argument asserts (ctc_crf/__init__.py:115-124): flat labels, with `dtypes` the logits and int32
+    labels and lengths (WARP_CTC_LOSS asserts no dtypes, as the reference's does not), and no gradient on any of them."""
+    assert len(labels.size()) == 1
+    if dtypes:
+        assert logits.dtype in (torch.float, torch.bfloat16, torch.float16), \
+            f"expect logits to be torch.float (or torch.bfloat16 / torch.float16) object, instead: {logits.dtype}"
+        assert labels.dtype == torch.int, f"expect labels to be torch.int object, instead: {labels.dtype}"
+        assert lx.dtype == torch.int, f"expect lx to be torch.int object, instead: {lx.dtype}"
+        assert ly.dtype == torch.int, f"expect ly to be torch.int object, instead: {ly.dtype}"
+    if utt is not None:
+        _check_utt(utt)
+    _assert_no_grad(labels)
+    _assert_no_grad(lx)
+    _assert_no_grad(ly)
+
+
 def _loss_options(reduction, zero_infinity) -> dict:
     """The keyword arguments the `_C` loss functions get for these settings: none at the defaults, so that the default
     path calls exactly what it called before the two options existed."""
@@ -216,17 +199,9 @@ class CTC_CRF_LOSS(Module):
             reduction='none' returns the (M,) costs in the caller's order; zero_infinity masks per sequence.  An utterance
             without a sequence contributes nothing and gets a zero gradient.
         """
+        _check_loss_args(logits, labels, lx, ly, utt)
         if utt is not None:
             return self._forward_seqs(logits, labels, lx, ly, utt)
-        assert len(labels.size()) == 1
-        assert logits.dtype in (torch.float, torch.bfloat16, torch.float16), \
-            f"expect logits to be torch.float (or torch.bfloat16 / torch.float16) object, instead: {logits.dtype}"
-        assert labels.dtype == torch.int, f"expect labels to be torch.int object, instead: {labels.dtype}"
-        assert lx.dtype == torch.int, f"expect lx to be torch.int object, instead: {lx.dtype}"
-        assert ly.dtype == torch.int, f"expect ly to be torch.int object, instead: {ly.dtype}"
-        _assert_no_grad(labels)
-        _assert_no_grad(lx)
-        _assert_no_grad(ly)
         opts = _loss_options(self.reduction, self.zero_infinity)    # read on every call: the attributes may be reassigned
         if not torch.is_grad_enabled():
             # evaluation (torch.no_grad / inference_mode): the loss alone, with the den alpha on a ring of frames and no
@@ -234,21 +209,11 @@ class CTC_CRF_LOSS(Module):
             return core.ctc_crf_loss_fwd_only(logits.contiguous(), labels, lx, ly, self.lamb, self.size_average,
                                               from_logits=self.from_logits, **opts)[0]
         if opts:
-            return _CTC_CRF_COSTS.apply(logits, labels, lx, ly, self.lamb, self.size_average, self.from_logits,
-                                        self.reduction, bool(self.zero_infinity))
+            return _CTC_CRF.apply(logits, labels, lx, ly, self.lamb, self.size_average, self.reduction,
+                                  bool(self.zero_infinity), self.from_logits)
         return self.ctc_crf(logits, labels, lx, ly, self.lamb, self.size_average)
 
     def _forward_seqs(self, logits, labels, lx, ly, utt):
-        assert len(labels.size()) == 1
-        assert logits.dtype in (torch.float, torch.bfloat16, torch.float16), \
-            f"expect logits to be torch.float (or torch.bfloat16 / torch.float16) object, instead: {logits.dtype}"
-        assert labels.dtype == torch.int, f"expect labels to be torch.int object, instead: {labels.dtype}"
-        assert lx.dtype == torch.int, f"expect lx to be torch.int object, instead: {lx.dtype}"
-        assert ly.dtype == torch.int, f"expect ly to be torch.int object, instead: {ly.dtype}"
-        _check_utt(utt)
-        _assert_no_grad(labels)
-        _assert_no_grad(lx)
-        _assert_no_grad(ly)
         core.check_reduction(self.reduction)
         if not torch.is_grad_enabled():
             return core.ctc_crf_loss_seqs_fwd_only(logits.contiguous(), labels, lx, ly, utt, self.lamb, self.size_average,
@@ -272,12 +237,8 @@ class WARP_CTC_LOSS(Module):
     def forward(self, logits, labels, input_lengths, label_lengths, utt=None):
         """utt (addition): (M,) int32 on CPU, sequence m of labels / label_lengths scored against logits row utt[m], as for
         CTC_CRF_LOSS; cost[m] = -log p[m], all M numerators in one launch."""
-        assert len(labels.size()) == 1
-        _assert_no_grad(labels)
-        _assert_no_grad(input_lengths)
-        _assert_no_grad(label_lengths)
+        _check_loss_args(logits, labels, input_lengths, label_lengths, utt, dtypes=False)
         if utt is not None:
-            _check_utt(utt)
             core.check_reduction(self.reduction)
             if not torch.is_grad_enabled():
                 return core.ctc_loss_seqs(logits.contiguous(), labels, input_lengths, label_lengths, utt, self.size_average,
@@ -289,10 +250,8 @@ class WARP_CTC_LOSS(Module):
         if not torch.is_grad_enabled():   # evaluation: the loss alone (see CTC_CRF_LOSS.forward)
             return core.ctc_loss_fwd_only(logits.contiguous(), labels, input_lengths, label_lengths, self.size_average,
                                           **opts)[0]
-        if opts:
-            return _WARP_CTC_COSTS.apply(logits, labels, input_lengths, label_lengths, self.size_average, self.reduction,
-                                         bool(self.zero_infinity))
-        return self.ctc(logits, labels, input_lengths, label_lengths, self.size_average)
+        return self.ctc(logits, labels, input_lengths, label_lengths, self.size_average, self.reduction,
+                        bool(self.zero_infinity))
 
 
 def ctc_align(logits, labels, input_lengths, label_lengths, utt=None):
