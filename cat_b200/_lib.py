@@ -32,6 +32,8 @@ SYMBOLS = [
     "ccb_crf_sample_ws_bytes", "ccb_crf_sample", "ccb_ctc_beam_search_ws_bytes", "ccb_ctc_beam_search", "ccb_plan_ctc_shape",
     "ccb_ngram_create", "ccb_ngram_destroy", "ccb_ngram_info", "ccb_ngram_copy", "ccb_ctc_beam_search_lm",
     "ccb_wfst_create", "ccb_wfst_destroy", "ccb_wfst_info", "ccb_wfst_copy", "ccb_wfst_decode_ws_bytes", "ccb_wfst_decode",
+    "ccb_rnnt_workspace_bytes", "ccb_rnnt_forward", "ccb_rnnt_backward", "ccb_gather_ws_bytes", "ccb_gather_sum",
+    "ccb_gather_sum_backward",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -140,6 +142,15 @@ def lib() -> C.CDLL:
     L.ccb_wfst_decode_ws_bytes.argtypes = [vp, i, i, i]; L.ccb_wfst_decode_ws_bytes.restype = C.c_size_t
     L.ccb_wfst_decode.argtypes = [vp, i, i, i, i, vp, vp, f, f, f, f, i, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.ccb_wfst_decode.restype = C.c_int
+    L.ccb_rnnt_workspace_bytes.argtypes = [i, l]; L.ccb_rnnt_workspace_bytes.restype = C.c_size_t
+    L.ccb_rnnt_forward.argtypes = [vp, i, i, i, i, l, i, i, i, vp, l, vp, vp, i, i, vp, vp, vp, vp]
+    L.ccb_rnnt_forward.restype = C.c_int
+    L.ccb_rnnt_backward.argtypes = [vp, i, i, i, l, i, vp, i, vp, vp, vp, vp]
+    L.ccb_rnnt_backward.restype = C.c_int
+    L.ccb_gather_ws_bytes.argtypes = [i]; L.ccb_gather_ws_bytes.restype = C.c_size_t
+    L.ccb_gather_sum.argtypes = [vp, vp, i, i, l, i, vp, vp, vp, vp, vp]; L.ccb_gather_sum.restype = C.c_int
+    L.ccb_gather_sum_backward.argtypes = [vp, i, i, l, l, i, vp, vp, vp, vp, vp, vp]
+    L.ccb_gather_sum_backward.restype = C.c_int
     L.ccb_launch_count.argtypes = []; L.ccb_launch_count.restype = C.c_long
     L.ccb_debug_timeline.argtypes = [vp, C.c_int, C.c_int]; L.ccb_debug_timeline.restype = None
     L.ccb_plan_create.argtypes = [C.c_char_p, C.c_int, C.c_int]; L.ccb_plan_create.restype = vp

@@ -1289,6 +1289,63 @@ int ccb_wfst_decode(const void *logits, int dtype, int N, int T, int V, const in
     return 0;
 }
 
+size_t ccb_rnnt_workspace_bytes(int N, long rows) { return N > 0 && rows >= 0 ? RnntWsBytes(N, rows) : 0; }
+
+int ccb_rnnt_forward(const void *x, int dtype, int from_logits, int compact, int N, long rows, int V, int Tmax, int Umax,
+                     const int *labels_dev, long n_labels, const int *lx_dev, const int *ly_dev, int blank, int want_beta,
+                     void *workspace, float *costs, float *costs_beta, void *stream) {
+    g_err.clear();
+    if (N <= 0 || rows < 0 || V <= 0 || n_labels < 0) return Fail("rnnt_forward: N and V must be positive, rows and n_labels >= 0");
+    if (!KnownDtype(dtype)) return FailDtype("rnnt_forward", dtype);
+    if (blank < 0 || blank >= V) return Fail("rnnt_forward: blank must lie in [0, V)");
+    if (!compact && (Tmax < 1 || Umax < 0 || rows != (long)N * Tmax * (Umax + 1) || n_labels != (long)N * Umax))
+        return Fail("rnnt_forward: the padded layout needs rows = N Tmax (Umax+1) and n_labels = N Umax");
+    if (!x || (n_labels && !labels_dev) || !lx_dev || !ly_dev || !workspace || !costs)
+        return Fail("rnnt_forward: missing buffer");
+    const int rc = LaunchRnntForward(x, dtype, from_logits, compact, N, rows, V, Tmax, Umax, labels_dev, n_labels, lx_dev,
+                                     ly_dev, blank, want_beta, workspace, costs, costs_beta, (cudaStream_t)stream);
+    if (rc) return FailCuda("rnnt_forward", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_rnnt_backward(const void *x, int dtype, int from_logits, int N, long rows, int V, const int *labels_dev, int blank,
+                      void *workspace, const float *w, void *grad, void *stream) {
+    g_err.clear();
+    if (N <= 0 || rows < 0 || V <= 0) return Fail("rnnt_backward: N and V must be positive, rows >= 0");
+    if (!KnownDtype(dtype)) return FailDtype("rnnt_backward", dtype);
+    if (blank < 0 || blank >= V) return Fail("rnnt_backward: blank must lie in [0, V)");
+    if ((from_logits && !x) || !workspace || !w || !grad) return Fail("rnnt_backward: missing buffer");
+    const int rc = LaunchRnntBackward(x, dtype, from_logits, N, rows, V, labels_dev, blank, workspace, w, grad,
+                                      (cudaStream_t)stream);
+    if (rc) return FailCuda("rnnt_backward", (cudaError_t)rc);
+    return 0;
+}
+
+size_t ccb_gather_ws_bytes(int N) { return N > 0 ? GatherWsBytes(N) : 0; }
+
+int ccb_gather_sum(const void *a, const void *b, int dtype, int N, long rows_out, int H, const int *la_dev, const int *lb_dev,
+                   void *workspace, void *out, void *stream) {
+    g_err.clear();
+    if (N <= 0 || rows_out < 0 || H <= 0) return Fail("gather_sum: N and H must be positive, rows_out >= 0");
+    if (!KnownDtype(dtype)) return FailDtype("gather_sum", dtype);
+    if (!a || !b || !la_dev || !lb_dev || !workspace || (rows_out && !out)) return Fail("gather_sum: missing buffer");
+    const int rc = LaunchGatherSum(a, b, dtype, N, rows_out, H, la_dev, lb_dev, workspace, out, (cudaStream_t)stream);
+    if (rc) return FailCuda("gather_sum", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_gather_sum_backward(const void *grad_out, int dtype, int N, long rows_a, long rows_b, int H, const int *la_dev,
+                            const int *lb_dev, void *workspace, void *grad_a, void *grad_b, void *stream) {
+    g_err.clear();
+    if (N <= 0 || rows_a < 0 || rows_b < 0 || H <= 0) return Fail("gather_sum_backward: N and H must be positive");
+    if (!KnownDtype(dtype)) return FailDtype("gather_sum_backward", dtype);
+    if (!grad_out || !la_dev || !lb_dev || !workspace || !grad_a || !grad_b) return Fail("gather_sum_backward: missing buffer");
+    const int rc = LaunchGatherSumBackward(grad_out, dtype, N, rows_a, rows_b, H, la_dev, lb_dev, workspace, grad_a, grad_b,
+                                           (cudaStream_t)stream);
+    if (rc) return FailCuda("gather_sum_backward", (cudaError_t)rc);
+    return 0;
+}
+
 /* ---- gpu_ctc/ctc.h surface ------------------------------------------------------------------- */
 const char *ctcGetStatusString(ctcStatus_t status) {
     switch (status) {

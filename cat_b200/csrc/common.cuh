@@ -268,6 +268,20 @@ size_t WfstWsBytes(const WfstDev &g, int N, int T, int K);
 int LaunchWfstDecode(const WfstDev &g, const void *y, int y_dtype, int N, int T, int V, const int *len, float acwt, float lmwt,
                      float wip, float beam, int K, void *ws, int *words, int *num_words, int *align, float *ac_logp,
                      float *graph_cost, float *cost, int *reached_final, cudaStream_t stream);
+// RNN-T loss (rnnt_kernels.cu): the forward runs the prep, row and alpha (|| beta when want_beta) passes; the backward the
+// gradient pass over the same workspace of RnntWsBytes(N, rows) bytes.  Lengths and labels are device pointers.
+size_t RnntWsBytes(int N, long long rows);
+int LaunchRnntForward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
+                      const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
+                      float *costs, float *costs_beta, cudaStream_t s);
+int LaunchRnntBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
+                       void *ws, const float *w, void *grad, cudaStream_t s);
+// gather.sum of the joiner and its backward; ws: GatherWsBytes(N) bytes of per-utterance offsets
+size_t GatherWsBytes(int N);
+int LaunchGatherSum(const void *a, const void *b, int dtype, int N, long long rows_out, int H, const int *la, const int *lb,
+                    void *ws, void *out, cudaStream_t s);
+int LaunchGatherSumBackward(const void *g, int dtype, int N, long long rows_a, long long rows_b, int H, const int *la,
+                            const int *lb, void *ws, void *grad_a, void *grad_b, cudaStream_t s);
 
 // ------------------------------------------------------------------------------------------------
 // device helpers

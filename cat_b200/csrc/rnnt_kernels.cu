@@ -1,0 +1,524 @@
+// RNN-T loss over the joint tensor in CAT's compact layout or the padded one, and the joiner's gather.sum (DESIGN.md §7
+// "RNN-T loss").  Row pass -> alpha/beta pass (forward); gradient pass (backward).  No atomics anywhere: every output
+// element has one writer and every sum a fixed order, so two identical calls give identical bits.
+#include <algorithm>
+#include <type_traits>
+
+#include "common.cuh"
+
+namespace ccb {
+namespace {
+
+constexpr int kRowThreads = 256;    // row and gradient passes: 8 warps per CTA
+constexpr int kAbThreads = 256;     // alpha/beta pass: one CTA per (utterance, direction), threads over u
+constexpr int kPrepThreads = 256;
+
+size_t Align256(size_t b) { return (b + 255) / 256 * 256; }
+
+// per utterance, in the workspace (rnnt_prep_kernel)
+struct RnntMeta {
+    long long roff;   // first row of the utterance's block
+    long long loff;   // first label
+    long long span;   // rows of the block, clamped to the tensor: what the gradient pass writes
+    int T, U;         // lengths as given
+    int ts;           // rows per frame: U + 1 (compact) or Umax + 1 (padded)
+    int bad;          // lengths or labels invalid: NaN cost, zero gradient, rows never read
+};
+
+struct RnntLayout {
+    size_t meta, tail, logp, alpha, beta, lpb, lpl, lse, total;
+};
+
+RnntLayout MakeRnntLayout(int N, long long rows) {
+    RnntLayout L;
+    size_t o = 0;
+    L.meta = o;  o += Align256(sizeof(RnntMeta) * (size_t)N);
+    L.tail = o;  o += 256;
+    L.logp = o;  o += Align256(2 * sizeof(double) * (size_t)N);   // from alpha, then from beta
+    L.alpha = o; o += Align256(sizeof(double) * (size_t)rows);
+    L.beta = o;  o += Align256(sizeof(double) * (size_t)rows);
+    L.lpb = o;   o += Align256(sizeof(float) * (size_t)rows);
+    L.lpl = o;   o += Align256(sizeof(float) * (size_t)rows);
+    L.lse = o;   o += Align256(sizeof(float) * (size_t)rows);
+    L.total = o;
+    return L;
+}
+
+template <typename T> T *At(void *ws, size_t off) { return reinterpret_cast<T *>(reinterpret_cast<char *>(ws) + off); }
+
+// ------------------------------------------------------------------------------------------------
+// 16-byte row chunks in a compile-time dtype (VEC) or single elements through load_y (rows whose byte length or base is not
+// a multiple of 16)
+// ------------------------------------------------------------------------------------------------
+template <int DT> __host__ __device__ constexpr int EltBytes() { return DT == CCB_DTYPE_F32 ? 4 : 2; }
+template <int DT, bool VEC> __host__ __device__ constexpr int ChunkElems() { return VEC ? 16 / EltBytes<DT>() : 1; }
+
+template <int DT> __device__ __forceinline__ float From16(unsigned h) {
+    return DT == CCB_DTYPE_BF16 ? __bfloat162float(__ushort_as_bfloat16((unsigned short)h))
+                                : __half2float(__ushort_as_half((unsigned short)h));
+}
+template <int DT> __device__ __forceinline__ unsigned To16(float v) {
+    return DT == CCB_DTYPE_BF16 ? __bfloat16_as_ushort(__float2bfloat16_rn(v)) : __half_as_ushort(__float2half_rn(v));
+}
+
+// chunk c of the row whose first element is `base`, read once (streaming)
+template <int DT, bool VEC>
+__device__ __forceinline__ void LoadChunk(const void *p, long long base, long long c, float *v) {
+    if constexpr (!VEC) {
+        v[0] = load_y(p, DT, base + c);
+    } else if constexpr (DT == CCB_DTYPE_F32) {
+        const float4 q = __ldcs(reinterpret_cast<const float4 *>(reinterpret_cast<const float *>(p) + base) + c);
+        v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+    } else {
+        const uint4 q = __ldcs(reinterpret_cast<const uint4 *>(reinterpret_cast<const unsigned short *>(p) + base) + c);
+        const unsigned w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { v[2 * i] = From16<DT>(w[i] & 0xffffu); v[2 * i + 1] = From16<DT>(w[i] >> 16); }
+    }
+}
+
+template <int DT, bool VEC>
+__device__ __forceinline__ void StoreChunk(void *p, long long base, long long c, const float *v) {
+    if constexpr (!VEC) {
+        store_y(p, DT, base + c, v[0]);
+    } else if constexpr (DT == CCB_DTYPE_F32) {
+        __stcs(reinterpret_cast<float4 *>(reinterpret_cast<float *>(p) + base) + c, make_float4(v[0], v[1], v[2], v[3]));
+    } else {
+        uint4 q;
+        q.x = To16<DT>(v[0]) | (To16<DT>(v[1]) << 16); q.y = To16<DT>(v[2]) | (To16<DT>(v[3]) << 16);
+        q.z = To16<DT>(v[4]) | (To16<DT>(v[5]) << 16); q.w = To16<DT>(v[6]) | (To16<DT>(v[7]) << 16);
+        __stcs(reinterpret_cast<uint4 *>(reinterpret_cast<unsigned short *>(p) + base) + c, q);
+    }
+}
+
+// (max, sum of exp(x - max)) pairs: the online logsumexp state; -inf max means "nothing finite seen"
+__device__ __forceinline__ void LseMerge(float &m, float &s, float mo, float so) {
+    const float mm = fmaxf(m, mo);
+    if (mm == -INFINITY) return;
+    s = s * __expf(m - mm) + so * __expf(mo - mm);
+    m = mm;
+}
+
+__device__ __forceinline__ double LogAddD(double a, double b) {
+    const double m = fmax(a, b);
+    if (m == -INFINITY) return m;
+    return m + log1p(exp(-fabs(a - b)));
+}
+
+// ------------------------------------------------------------------------------------------------
+// Exclusive int64 prefix sums over the N utterances, one CTA, in chunks of kPrepThreads (fixed order: deterministic).  f(n) returns the two inputs of
+// utterance n; g(n, ex0, ex1) receives their exclusive sums.  Returns the totals (on every thread).
+// ------------------------------------------------------------------------------------------------
+template <typename F, typename G>
+__device__ void ScanUtts(int N, F f, G g, long long *tot0, long long *tot1) {
+    constexpr int kWarps = kPrepThreads / 32;
+    __shared__ longlong2 part[kWarps];
+    __shared__ long long carry[2];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) { carry[0] = 0; carry[1] = 0; }
+    __syncthreads();
+    for (int base = 0; base < N; base += kPrepThreads) {
+        const int n = base + (int)threadIdx.x;
+        const longlong2 in = n < N ? f(n) : make_longlong2(0, 0);
+        longlong2 inc = in;   // inclusive sums within the warp, then across warps
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const long long x = __shfl_up_sync(0xffffffffu, inc.x, o), y = __shfl_up_sync(0xffffffffu, inc.y, o);
+            if (lane >= o) { inc.x += x; inc.y += y; }
+        }
+        if (lane == 31) part[warp] = inc;
+        __syncthreads();
+        long long wx = 0, wy = 0;
+        for (int i = 0; i < warp; ++i) { wx += part[i].x; wy += part[i].y; }
+        if (n < N) g(n, carry[0] + wx + inc.x - in.x, carry[1] + wy + inc.y - in.y);
+        __syncthreads();
+        if (threadIdx.x == kPrepThreads - 1) { carry[0] += wx + inc.x; carry[1] += wy + inc.y; }
+        __syncthreads();
+    }
+    *tot0 = carry[0];
+    *tot1 = carry[1];
+}
+
+// Per-utterance metadata from the device lengths.  Compact: rows (and labels) of utterance n follow those of n-1; padded:
+// block n of Tmax (Umax+1) rows and row n of the (N, Umax) labels.  Negative lengths count as 0 in the offsets, so that
+// the utterances' row ranges never overlap whatever the lengths are.
+__global__ void __launch_bounds__(kPrepThreads) rnnt_prep_kernel(const int *lx, const int *ly, int N, long long rows,
+                                                                 long long n_labels, int compact, int Tmax, int Umax,
+                                                                 RnntMeta *meta, long long *tail) {
+    auto in = [=](int n) {
+        const long long T = max(lx[n], 0), U = max(ly[n], 0);
+        return compact ? make_longlong2(T * (U + 1), U) : make_longlong2(0, 0);
+    };
+    auto out = [=](int n, long long roff, long long loff) {
+        const int T = lx[n], U = ly[n];
+        RnntMeta m;
+        m.T = T; m.U = U;
+        bool bad = T < 1 || U < 0;
+        if (compact) {
+            const long long own = (long long)max(T, 0) * (max(U, 0) + 1);
+            m.roff = roff; m.loff = loff; m.ts = max(U, 0) + 1;
+            m.span = min(own, max(rows - roff, 0LL));
+            bad = bad || roff + own > rows;
+        } else {
+            m.ts = Umax + 1;
+            m.span = (long long)Tmax * m.ts;
+            m.roff = (long long)n * m.span; m.loff = (long long)n * Umax;
+            bad = bad || T > Tmax || U > Umax;
+        }
+        bad = bad || m.loff + max(U, 0) > n_labels;
+        m.bad = bad ? 1 : 0;
+        meta[n] = m;
+    };
+    long long r_tot, l_tot;
+    ScanUtts(N, in, out, &r_tot, &l_tot);
+    if (threadIdx.x == 0) *tail = compact ? min(r_tot, rows) : rows;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Row pass.  Grid (row chunk, utterance): CTA (x, n) walks the rows t < T_n, u <= U_n of utterance n with stride gridDim.x.
+// lpb = log p(blank), lpl = log p(y_{u+1}) (u < U_n); raw logits: minus the row's logsumexp, which is kept in lse.
+// A label outside [0, V) or equal to blank marks the utterance bad (every writer writes 1; no atomics needed).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kRowThreads) rnnt_lp_rows_kernel(const void *x, int dtype, long long V, const int *labels,
+                                                                   int blank, RnntMeta *meta, float *lpb, float *lpl) {
+    const int n = blockIdx.y;
+    const RnntMeta m = meta[n];
+    if (m.bad) return;
+    const long long live = (long long)m.T * m.ts;
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < live; r += (long long)gridDim.x * blockDim.x) {
+        const long long t = r / m.ts;
+        const int u = (int)(r - t * m.ts);
+        if (u > m.U) continue;
+        const long long row = m.roff + r;
+        lpb[row] = load_y(x, dtype, row * V + blank);
+        if (u < m.U) {
+            const int y = labels[m.loff + u];
+            if (y < 0 || y >= V || y == blank) { meta[n].bad = 1; lpl[row] = NAN; }
+            else lpl[row] = load_y(x, dtype, row * V + y);
+        }
+    }
+}
+
+template <int DT, bool VEC>
+__global__ void __launch_bounds__(kRowThreads) rnnt_logit_rows_kernel(const void *x, long long V, const int *labels, int blank,
+                                                                      RnntMeta *meta, float *lpb, float *lpl, float *lse) {
+    constexpr int K = ChunkElems<DT, VEC>();
+    const int n = blockIdx.y;
+    const RnntMeta m = meta[n];
+    if (m.bad) return;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const long long live = (long long)m.T * m.ts, chunks = V / K;
+    for (long long r = (long long)blockIdx.x * W + warp; r < live; r += (long long)gridDim.x * W) {
+        const long long t = r / m.ts;
+        const int u = (int)(r - t * m.ts);
+        if (u > m.U) continue;
+        const long long row = m.roff + r, base = row * V;
+        float mx = -INFINITY, s = 0.f;
+        for (long long c = lane; c < chunks; c += 32) {
+            float v[K];
+            LoadChunk<DT, VEC>(x, base, c, v);
+            float cm = v[0];
+#pragma unroll
+            for (int i = 1; i < K; ++i) cm = fmaxf(cm, v[i]);
+            if (cm == -INFINITY) continue;
+            if (cm > mx) { s *= __expf(mx - cm); mx = cm; }
+#pragma unroll
+            for (int i = 0; i < K; ++i) s += __expf(v[i] - mx);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float mo = __shfl_xor_sync(0xffffffffu, mx, o), so = __shfl_xor_sync(0xffffffffu, s, o);
+            LseMerge(mx, s, mo, so);
+        }
+        if (lane == 0) {
+            const float l = mx == -INFINITY ? -INFINITY : mx + __logf(s);
+            lse[row] = l;
+            lpb[row] = load_y(x, DT, base + blank) - l;
+            if (u < m.U) {
+                const int y = labels[m.loff + u];
+                if (y < 0 || y >= V || y == blank) { meta[n].bad = 1; lpl[row] = NAN; }
+                else lpl[row] = load_y(x, DT, base + y) - l;
+            }
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// alpha / beta pass: CTA (n, 0) runs alpha, CTA (n, 1) beta, over anti-diagonals, threads over u; cells in fp64, kept per row
+// in the workspace and read back by the next diagonal after the CTA barrier.
+//   alpha(t,u) = logaddexp(alpha(t-1,u) + lpb(t-1,u), alpha(t,u-1) + lpl(t,u-1)),  log P = alpha(T-1,U) + lpb(T-1,U)
+//   beta(t,u)  = logaddexp(beta(t+1,u) + lpb(t,u),   beta(t,u+1) + lpl(t,u)),     beta(T-1,U) = lpb(T-1,U), log P = beta(0,0)
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kAbThreads) rnnt_alpha_beta_kernel(const RnntMeta *meta, const float *lpb, const float *lpl,
+                                                                     double *alpha, double *beta, double *logp, int N,
+                                                                     float *costs, float *costs_beta) {
+    const int n = blockIdx.x;
+    const bool bwd = blockIdx.y == 1;
+    const RnntMeta m = meta[n];
+    if (m.bad) {
+        if (threadIdx.x == 0) {
+            logp[bwd ? N + n : n] = NAN;
+            if (bwd) { if (costs_beta) costs_beta[n] = NAN; }
+            else costs[n] = NAN;
+        }
+        return;
+    }
+    const int T = m.T, U = m.U;
+    const long long ts = m.ts, off = m.roff;
+    double *cell = bwd ? beta : alpha;
+    for (int d = 0; d < T + U; ++d) {
+        const int k_lo = max(0, d - (T - 1)), k_hi = min(U, d);
+        for (int k = k_lo + (int)threadIdx.x; k <= k_hi; k += blockDim.x) {
+            if (!bwd) {
+                const int u = k, t = d - k;
+                const long long r = off + t * ts + u;
+                double a = 0.0;
+                if (d > 0) {
+                    const double x1 = t > 0 ? cell[r - ts] + (double)lpb[r - ts] : -INFINITY;
+                    const double x2 = u > 0 ? cell[r - 1] + (double)lpl[r - 1] : -INFINITY;
+                    a = LogAddD(x1, x2);
+                }
+                cell[r] = a;
+            } else {
+                const int u = U - k, t = (T - 1) - (d - k);
+                const long long r = off + t * ts + u;
+                double b = (double)lpb[r];
+                if (d > 0) {
+                    const double x1 = t < T - 1 ? cell[r + ts] + (double)lpb[r] : -INFINITY;
+                    const double x2 = u < U ? cell[r + 1] + (double)lpl[r] : -INFINITY;
+                    b = LogAddD(x1, x2);
+                }
+                cell[r] = b;
+            }
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        if (!bwd) {
+            const long long last = off + (T - 1) * ts + U;
+            const double lp = cell[last] + (double)lpb[last];
+            logp[n] = lp;
+            costs[n] = (float)-lp;
+        } else {
+            logp[N + n] = cell[off];
+            if (costs_beta) costs_beta[n] = (float)-cell[off];
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Gradient pass: one warp per row, every row of the tensor written once.  Grid (row chunk, N + 1): CTA (x, n < N) walks
+// utterance n's span (rows outside t < T_n, u <= U_n, and every row of a bad utterance, get zeros and are not read);
+// CTA (x, N) zeroes the compact tail behind the last utterance.  With w = w_n,
+//   pb = w exp(alpha + lpb + beta(t+1,u) - log P)   (at t = T-1 only for u = U, as exp(alpha + lpb - log P))
+//   pl = w exp(alpha + lpl + beta(t,u+1) - log P)   (u < U)
+//   grad[k] = [raw: exp(z_k - lse) (pb + pl)] - pb [k == blank] - pl [k == y_{u+1}]
+// ------------------------------------------------------------------------------------------------
+template <int DT, bool VEC, bool RAW>
+__global__ void __launch_bounds__(kRowThreads) rnnt_grad_kernel(const void *x, long long V, const int *labels, int blank, int N,
+                                                                const RnntMeta *meta, const long long *tail, long long rows,
+                                                                const double *alpha, const double *beta, const double *logp,
+                                                                const float *lpb, const float *lpl, const float *lse,
+                                                                const float *w, void *grad) {
+    constexpr int K = ChunkElems<DT, VEC>();
+    const int n = blockIdx.y;
+    const bool utt = n < N;
+    RnntMeta m{};
+    long long first, count;
+    if (utt) { m = meta[n]; first = m.roff; count = m.span; }
+    else { first = *tail; count = rows - first; }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const long long chunks = V / K;
+    const float wn = utt && !m.bad ? w[n] : 0.f;
+    const double lP = utt && !m.bad ? logp[n] : 0.0;
+    for (long long r = (long long)blockIdx.x * W + warp; r < count; r += (long long)gridDim.x * W) {
+        const long long row = first + r, base = row * V;
+        float pb = 0.f, pl = 0.f, l = 0.f;
+        int y = -1;
+        bool live = false;
+        if (utt && !m.bad) {
+            const long long t = r / m.ts;
+            const int u = (int)(r - t * m.ts);
+            if (t < m.T && u <= m.U) {
+                live = true;
+                const double a = alpha[row];
+                if (t < m.T - 1) pb = (float)exp(a + (double)lpb[row] + beta[row + m.ts] - lP);
+                else if (u == m.U) pb = (float)exp(a + (double)lpb[row] - lP);
+                if (u < m.U) { pl = (float)exp(a + (double)lpl[row] + beta[row + 1] - lP); y = labels[m.loff + u]; }
+                pb *= wn; pl *= wn;
+                if constexpr (RAW) l = lse[row];
+            }
+        }
+        const float occ = pb + pl;
+        for (long long c = lane; c < chunks; c += 32) {
+            float v[K];
+            if (RAW && live) {
+                LoadChunk<DT, VEC>(x, base, c, v);
+#pragma unroll
+                for (int i = 0; i < K; ++i) v[i] = __expf(v[i] - l) * occ;
+            } else {
+#pragma unroll
+                for (int i = 0; i < K; ++i) v[i] = 0.f;
+            }
+            if (live) {
+#pragma unroll
+                for (int i = 0; i < K; ++i) {
+                    const long long k = c * K + i;
+                    if (k == blank) v[i] -= pb;
+                    if (k == y) v[i] -= pl;
+                }
+            }
+            StoreChunk<DT, VEC>(grad, base, c, v);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// gather.sum: out[off_n + t lb_n + u][h] = a[ta_n + t][h] + b[ub_n + u][h]; one warp per output row.  Backward: grad_a by a
+// sum over u (contiguous rows), grad_b by a sum over t (rows at stride lb_n), each a fixed-order fp32 sum per (row, h).
+// ------------------------------------------------------------------------------------------------
+struct GatherMeta {
+    long long off, ta, ub;
+    int la, lb;
+};
+
+__global__ void __launch_bounds__(kPrepThreads) gather_prep_kernel(const int *la, const int *lb, int N, GatherMeta *meta) {
+    // the scan carries (a rows, b rows); the output offset is a second pass of the same scan
+    auto in = [=](int n) { return make_longlong2(max(la[n], 0), max(lb[n], 0)); };
+    auto out = [=](int n, long long ta, long long ub) {
+        meta[n].ta = ta; meta[n].ub = ub; meta[n].la = max(la[n], 0); meta[n].lb = max(lb[n], 0);
+    };
+    long long t0, t1;
+    ScanUtts(N, in, out, &t0, &t1);
+    auto in2 = [=](int n) { return make_longlong2((long long)max(la[n], 0) * max(lb[n], 0), 0); };
+    auto out2 = [=](int n, long long off, long long) { meta[n].off = off; };
+    __syncthreads();
+    ScanUtts(N, in2, out2, &t0, &t1);
+}
+
+template <int DT>
+__global__ void __launch_bounds__(kRowThreads) gather_sum_kernel(const void *a, const void *b, int H, const GatherMeta *meta,
+                                                                 void *out) {
+    const GatherMeta m = meta[blockIdx.y];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const long long count = (long long)m.la * m.lb;
+    for (long long r = (long long)blockIdx.x * W + warp; r < count; r += (long long)gridDim.x * W) {
+        const long long t = r / m.lb, u = r - t * m.lb;
+        const long long ra = (m.ta + t) * H, rb = (m.ub + u) * H, ro = (m.off + r) * H;
+        for (int h = lane; h < H; h += 32) store_y(out, DT, ro + h, load_y(a, DT, ra + h) + load_y(b, DT, rb + h));
+    }
+}
+
+// grad_a (by_t = true: rows ta_n + t, summing over u) or grad_b (rows ub_n + u, summing over t); threads over h
+template <int DT>
+__global__ void __launch_bounds__(kRowThreads) gather_sum_bwd_kernel(const void *g, int H, const GatherMeta *meta, bool by_t,
+                                                                     void *grad) {
+    const GatherMeta m = meta[blockIdx.y];
+    const int outer = by_t ? m.la : m.lb, inner = by_t ? m.lb : m.la;
+    const long long step = by_t ? 1 : m.lb;
+    for (int i = blockIdx.x; i < outer; i += gridDim.x) {
+        const long long r0 = m.off + (by_t ? (long long)i * m.lb : i), dst = (by_t ? m.ta : m.ub) + i;
+        for (int h = threadIdx.x; h < H; h += blockDim.x) {
+            float acc = 0.f;
+            for (int j = 0; j < inner; ++j) acc += load_y(g, DT, (r0 + j * step) * H + h);
+            store_y(grad, DT, dst * H + h, acc);
+        }
+    }
+}
+
+int GridX(long long rows_per_utt, int per_cta) {
+    long long g = (rows_per_utt + per_cta - 1) / per_cta;
+    return (int)std::max(1LL, std::min(g, 65535LL));
+}
+
+template <typename F>
+void DispatchDtype(int dtype, F f) {
+    if (dtype == CCB_DTYPE_F32) f(std::integral_constant<int, CCB_DTYPE_F32>{});
+    else if (dtype == CCB_DTYPE_BF16) f(std::integral_constant<int, CCB_DTYPE_BF16>{});
+    else f(std::integral_constant<int, CCB_DTYPE_F16>{});
+}
+
+bool RowsVectorisable(const void *p, long long V, int dtype) {
+    const long long bytes = V * (dtype == CCB_DTYPE_F32 ? 4 : 2);
+    return bytes % 16 == 0 && reinterpret_cast<uintptr_t>(p) % 16 == 0;
+}
+
+}  // namespace
+
+size_t RnntWsBytes(int N, long long rows) { return MakeRnntLayout(N, rows).total; }
+
+int LaunchRnntForward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
+                      const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
+                      float *costs, float *costs_beta, cudaStream_t s) {
+    const RnntLayout L = MakeRnntLayout(N, rows);
+    RnntMeta *meta = At<RnntMeta>(ws, L.meta);
+    rnnt_prep_kernel<<<1, kPrepThreads, 0, s>>>(lx, ly, N, rows, n_labels, compact, Tmax, Umax, meta, At<long long>(ws, L.tail));
+    const long long per_utt = (rows + N - 1) / N;
+    if (from_logits) {
+        const int gx = GridX(per_utt, kRowThreads / 32 * 4);
+        const bool vec = RowsVectorisable(x, V, dtype);
+        DispatchDtype(dtype, [&](auto dt) {
+            constexpr int DT = decltype(dt)::value;
+            auto k = vec ? rnnt_logit_rows_kernel<DT, true> : rnnt_logit_rows_kernel<DT, false>;
+            k<<<dim3(gx, N), kRowThreads, 0, s>>>(x, V, labels, blank, meta, At<float>(ws, L.lpb), At<float>(ws, L.lpl),
+                                                  At<float>(ws, L.lse));
+        });
+    } else {
+        rnnt_lp_rows_kernel<<<dim3(GridX(per_utt, kRowThreads * 4), N), kRowThreads, 0, s>>>(
+            x, dtype, V, labels, blank, meta, At<float>(ws, L.lpb), At<float>(ws, L.lpl));
+    }
+    rnnt_alpha_beta_kernel<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(
+        meta, At<float>(ws, L.lpb), At<float>(ws, L.lpl), At<double>(ws, L.alpha), At<double>(ws, L.beta),
+        At<double>(ws, L.logp), N, costs, want_beta ? costs_beta : nullptr);
+    CountLaunch(3);
+    return (int)cudaGetLastError();
+}
+
+int LaunchRnntBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
+                       void *ws, const float *w, void *grad, cudaStream_t s) {
+    const RnntLayout L = MakeRnntLayout(N, rows);
+    const long long per_utt = (rows + N - 1) / N;
+    const int gx = GridX(per_utt, kRowThreads / 32 * 4);
+    const bool vec = RowsVectorisable(grad, V, dtype) && (!from_logits || RowsVectorisable(x, V, dtype));
+    DispatchDtype(dtype, [&](auto dt) {
+        constexpr int DT = decltype(dt)::value;
+        auto k = from_logits ? (vec ? rnnt_grad_kernel<DT, true, true> : rnnt_grad_kernel<DT, false, true>)
+                             : (vec ? rnnt_grad_kernel<DT, true, false> : rnnt_grad_kernel<DT, false, false>);
+        k<<<dim3(gx, N + 1), kRowThreads, 0, s>>>(x, V, labels, blank, N, At<RnntMeta>(ws, L.meta), At<long long>(ws, L.tail),
+                                                  rows, At<double>(ws, L.alpha), At<double>(ws, L.beta),
+                                                  At<double>(ws, L.logp), At<float>(ws, L.lpb), At<float>(ws, L.lpl),
+                                                  At<float>(ws, L.lse), w, grad);
+    });
+    CountLaunch(1);
+    return (int)cudaGetLastError();
+}
+
+size_t GatherWsBytes(int N) { return Align256(sizeof(GatherMeta) * (size_t)N); }
+
+int LaunchGatherSum(const void *a, const void *b, int dtype, int N, long long rows_out, int H, const int *la, const int *lb,
+                    void *ws, void *out, cudaStream_t s) {
+    GatherMeta *meta = reinterpret_cast<GatherMeta *>(ws);
+    gather_prep_kernel<<<1, kPrepThreads, 0, s>>>(la, lb, N, meta);
+    const int gx = GridX((rows_out + N - 1) / N, kRowThreads / 32 * 4);
+    DispatchDtype(dtype, [&](auto dt) {
+        gather_sum_kernel<decltype(dt)::value><<<dim3(gx, N), kRowThreads, 0, s>>>(a, b, H, meta, out);
+    });
+    CountLaunch(2);
+    return (int)cudaGetLastError();
+}
+
+int LaunchGatherSumBackward(const void *g, int dtype, int N, long long rows_a, long long rows_b, int H, const int *la,
+                            const int *lb, void *ws, void *grad_a, void *grad_b, cudaStream_t s) {
+    GatherMeta *meta = reinterpret_cast<GatherMeta *>(ws);
+    gather_prep_kernel<<<1, kPrepThreads, 0, s>>>(la, lb, N, meta);
+    DispatchDtype(dtype, [&](auto dt) {
+        constexpr int DT = decltype(dt)::value;
+        const int ga = GridX((rows_a + N - 1) / N, 1), gb = GridX((rows_b + N - 1) / N, 1);
+        gather_sum_bwd_kernel<DT><<<dim3(ga, N), kRowThreads, 0, s>>>(g, H, meta, true, grad_a);
+        gather_sum_bwd_kernel<DT><<<dim3(gb, N), kRowThreads, 0, s>>>(g, H, meta, false, grad_b);
+    });
+    CountLaunch(3);
+    return (int)cudaGetLastError();
+}
+
+}  // namespace ccb

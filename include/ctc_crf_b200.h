@@ -391,6 +391,49 @@ int ccb_wfst_decode(const void *logits, int dtype, int N, int T, int V, const in
                     float lmwt, float wip, float beam, int max_active, void *workspace, int *words, int *num_words,
                     int *align, float *ac_logp, float *graph_cost, float *cost, int *reached_final, void *stream);
 
+/* RNN-T loss (DESIGN.md §7 "RNN-T loss"), the textbook transducer loss over a joint tensor x of log-probs (from_logits = 0)
+ * or raw joiner outputs (from_logits = 1: the log-softmax is taken inside, no normalised copy is written).  Utterance n has
+ * T_n = lx[n] >= 1 frames and U_n = ly[n] >= 0 labels y_1..y_U; with lp(t,u,k) the log-prob of token k at row (t,u),
+ *   alpha(0,0) = 0,  alpha(t,u) = logaddexp(alpha(t-1,u) + lp(t-1,u,blank), alpha(t,u-1) + lp(t,u-1,y_u)),
+ *   cost[n] = -(alpha(T-1,U) + lp(T-1,U,blank)).
+ * Layouts (x is read in place in the CCB_DTYPE_* code dtype; all arithmetic in fp32, the lattice cells in fp64):
+ *   compact != 0: x (rows, V), utterance n at rows off_n + t (U_n+1) + u, off_n = sum_{m<n} T_m (U_m+1), computed on the
+ *     device in int64; labels (n_labels,) the label sequences concatenated.  Rows behind the last utterance are not read.
+ *   compact == 0: x (N, Tmax, Umax+1, V) = rows of N Tmax (Umax+1); labels (N, Umax) = n_labels of N Umax.  Rows outside
+ *     t < T_n, u <= U_n are never read.
+ * An utterance whose lengths overrun the tensor or the labels (or T_n < 1, U_n < 0, or T_n > Tmax, U_n > Umax when padded), or
+ * with a label outside [0, V) or equal to blank, gets cost NaN and zero gradient rows; nothing outside the tensors is read.
+ * No atomics: two identical calls give identical bits.
+ *   ccb_rnnt_workspace_bytes: the workspace of a call, about 28 bytes per row (lp of blank and label, the row's logsumexp,
+ *     alpha and beta in fp64) plus 56 bytes per utterance.  Nothing needs to be initialised.
+ *   ccb_rnnt_forward: costs (N,) fp32 out, from alpha.  want_beta != 0 also runs beta (concurrently with alpha, one CTA per
+ *     utterance and direction), which ccb_rnnt_backward needs; costs_beta (N,) (optional, may be NULL) then gets
+ *     -beta(0,0), the same cost from the other direction.  Lengths and labels are device pointers; no host synchronisation.
+ *   ccb_rnnt_backward: after a want_beta forward on the same workspace (untouched since) and the same x, labels and
+ *     lengths: grad (the shape of x, in dtype) = w[n] d cost[n] / d x for every row of utterance n, and zeros in every other
+ *     row (not read), in one pass.  With pb / pl the posteriors of the blank / label transition out of row (t,u):
+ *     log-prob input: -pb at blank, -pl at y_{u+1}, 0 elsewhere; raw logits: softmax(x) (pb + pl) minus the same two terms.
+ *     w (N,) fp32 device: the caller's weight of each cost (1/N for a batch mean).  x is read only when from_logits. */
+size_t ccb_rnnt_workspace_bytes(int N, long rows);
+int ccb_rnnt_forward(const void *x, int dtype, int from_logits, int compact, int N, long rows, int V, int Tmax, int Umax,
+                     const int *labels_dev, long n_labels, const int *lx_dev, const int *ly_dev, int blank, int want_beta,
+                     void *workspace, float *costs, float *costs_beta, void *stream);
+int ccb_rnnt_backward(const void *x, int dtype, int from_logits, int N, long rows, int V, const int *labels_dev, int blank,
+                      void *workspace, const float *w, void *grad, void *stream);
+
+/* The compact joiner's broadcast sum (CAT's gather.sum): for N utterances with la[n] rows of a and lb[n] rows of b, laid out
+ * one utterance after the other in each (offsets ta_n, ub_n and off_n = sum_{m<n} la_m lb_m computed on the device),
+ *   out[off_n + t lb_n + u][h] = a[ta_n + t][h] + b[ub_n + u][h]   (fp32 sum, rounded to dtype),
+ * a (sum la, H), b (sum lb, H), out (rows_out = sum la lb, H), all in the CCB_DTYPE_* code dtype; la / lb (N,) int32 device,
+ * >= 0 and consistent with the row counts (the caller checks; the kernels trust them).  The backward writes
+ * grad_a[ta_n + t] = sum_u grad_out[off_n + t lb_n + u] and grad_b[ub_n + u] = sum_t grad_out[...], each accumulated in fp32
+ * in a fixed order, without atomics.  workspace: ccb_gather_ws_bytes(N) bytes. */
+size_t ccb_gather_ws_bytes(int N);
+int ccb_gather_sum(const void *a, const void *b, int dtype, int N, long rows_out, int H, const int *la_dev, const int *lb_dev,
+                   void *workspace, void *out, void *stream);
+int ccb_gather_sum_backward(const void *grad_out, int dtype, int N, long rows_a, long rows_b, int H, const int *la_dev,
+                            const int *lb_dev, void *workspace, void *grad_a, void *grad_b, void *stream);
+
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 long ccb_launch_count(void);
 

@@ -1,0 +1,5 @@
+"""Drop-in for the ``warp_rnnt`` package CAT's transducer trainers import (cat/rnnt/train.py:22,217): ``rnnt_loss`` with
+``compact=True`` over the joiner's compact output, or the padded (N, T, U+1, V) layout."""
+from cat_b200.rnnt import rnnt_loss  # noqa: F401
+
+__all__ = ["rnnt_loss"]
