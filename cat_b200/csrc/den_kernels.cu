@@ -135,8 +135,30 @@ template <> __device__ __forceinline__ void sts_row<4>(uint32_t addr, const Vec<
     asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(r.v[0]), "f"(r.v[1]), "f"(r.v[2]), "f"(r.v[3]) : "memory");
 }
 
-__device__ __forceinline__ void prefetch_l2(const void *p) {
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+// A row read once, as the backward pass reads its alpha rows: not allocated in L1, and first in line for eviction from L2
+// (a per-instruction .L2::cache_hint policy, no device or context setting), so the alpha stream -- 10 MB per frame from
+// HBM -- does not push the beta-hat rows, each gathered ~24 times per frame, out of L2.
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+template <int U> __device__ __forceinline__ Vec<U> ld_row_once(const char *p, uint64_t pol);
+template <> __device__ __forceinline__ Vec<1> ld_row_once<1>(const char *p, uint64_t pol) {
+    Vec<1> r;
+    asm volatile("ld.global.L1::no_allocate.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(r.v[0]) : "l"(p), "l"(pol));
+    return r;
+}
+template <> __device__ __forceinline__ Vec<2> ld_row_once<2>(const char *p, uint64_t pol) {
+    Vec<2> r;
+    asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;" : "=f"(r.v[0]), "=f"(r.v[1]) : "l"(p), "l"(pol));
+    return r;
+}
+template <> __device__ __forceinline__ Vec<4> ld_row_once<4>(const char *p, uint64_t pol) {
+    Vec<4> r;
+    asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+                 : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]) : "l"(p), "l"(pol));
+    return r;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1067,6 +1089,7 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
         s_final[i] = __ldg(P.final_lin + tile_s0 + i);
     }
     const uint32_t row_bytes = (uint32_t)Npad * 4u;
+    const uint64_t pol_once = l2_policy_evict_first();
     if (SMEM_ARCS) {   // stage the tile once, quad-wise transposed: {byte offset 0..3}{w0 0..3}[{w1 0..3}]
         uint4 *sq = reinterpret_cast<uint4 *>(s_arcs);
         const uint4 *src = reinterpret_cast<const uint4 *>(P.arcs + tile_a0);
@@ -1135,11 +1158,6 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
         float *bh_cur = P.bh + (size_t)(tau & 1) * frame_elems;
         // alpha_pos without the ring (a_ring = 0 for every backward launch): frame tau - 1 is the position before frame tau
         const float *a_row = P.alpha + (size_t)(tau - P.a_base) * alpha_frame;
-        if (tau > 1 && se > sb) {   // pull next step's alpha rows of this chunk towards L2
-            const char *nb = reinterpret_cast<const char *>(a_row - alpha_frame + (size_t)sb * Npad);
-            const size_t bytes = (size_t)(se - sb) * Npad * 4;
-            for (size_t off = (size_t)lane * 128; off < bytes; off += 32 * 128) prefetch_l2(nb + off);
-        }
         for (int gc = 0; gc < (LPR == 32 ? Npad / (32 * U) : 1); ++gc) {
             const int n0 = gc * 32 * U + ul * U;
             bool act[U], gat[U];
@@ -1175,9 +1193,12 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
             uint32_t out_row = (uint32_t)sb;
             float *const out_base = bh_cur + n0;
             const char *const a_base = reinterpret_cast<const char *>(a_row + n0);
-            // alpha rows of the next group (one or two states) are fetched one group ahead
-            Vec<U> a_q = (se > sb && lane_act) ? gather_row<U>(a_base, out_row * row_bytes) : vec_zero<U>();
-            Vec<U> a_q1 = (se > sb + 1 && lane_act) ? gather_row<U>(a_base, (out_row + 1) * row_bytes) : vec_zero<U>();
+            // alpha rows of the next group (one or two states) are fetched one group ahead.  That alone hides their HBM
+            // latency: a prefetch of the next frame's rows into L2 only kept another 10 MB of read-once rows there, and
+            // dropping it took 3 ms off the pass at the headline shape (DESIGN.md §3, Roofline)
+            auto ld_alpha = [&](uint32_t row) { return ld_row_once<U>(a_base + row * row_bytes, pol_once); };
+            Vec<U> a_q = (se > sb && lane_act) ? ld_alpha(out_row) : vec_zero<U>();
+            Vec<U> a_q1 = (se > sb + 1 && lane_act) ? ld_alpha(out_row + 1) : vec_zero<U>();
             // own-row terms (den_graph.h DenPlan::own_rows): the next frame's beta-hat rows of the group about to end (this warp
             // wrote them one frame ago) and their coefficients, fetched one group ahead like the alpha rows
             const bool own = P.own != 0;
@@ -1265,8 +1286,8 @@ __global__ void __launch_bounds__(kDenThreads, 1) den_backward_kernel(const __gr
 #pragma unroll
                     for (int u = 0; u < U; ++u) acc1[u] = 0.f;
                 }
-                a_q = ((int)out_row < se && lane_act) ? gather_row<U>(a_base, out_row * row_bytes) : vec_zero<U>();
-                a_q1 = ((int)out_row + 1 < se && lane_act) ? gather_row<U>(a_base, (out_row + 1) * row_bytes) : vec_zero<U>();
+                a_q = ((int)out_row < se && lane_act) ? ld_alpha(out_row) : vec_zero<U>();
+                a_q1 = ((int)out_row + 1 < se && lane_act) ? ld_alpha(out_row + 1) : vec_zero<U>();
                 own_prefetch(out_row);
             };
             if (SMALL) {

@@ -44,3 +44,5 @@ for name, r in out.items():
     cta = work.reshape(steps, n_ctas, -1).max(2)
     print(f"   slowest warp per CTA: mean {cta.mean():.0f} max {cta.max():.0f} min {cta.min():.0f}; start skew across CTAs (ns) p50 {np.median(g0.max(1)-g0.min(1)):.0f}")
     print("   work/frame ratio mean %.2f ; (max work)/frame %.2f" % ((work/total).mean(), (work.max(1)/total.mean(1)).mean()))
+    wait = total - work
+    print(f"   barrier wait cycles mean {wait.mean():.0f} p50 {np.median(wait):.0f}; walk of the slowest warp per frame mean {work.max(1).mean():.0f}")
