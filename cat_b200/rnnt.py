@@ -217,8 +217,9 @@ class _GatherSum(Function):
 def gather_sum(a: torch.Tensor, b: torch.Tensor, la: torch.Tensor, lb: torch.Tensor) -> torch.Tensor:
     """``gather.sum``: the compact broadcast sum of CAT's joiner, out[off_n + t lb_n + u] = a[ta_n + t] + b[ub_n + u] with
     a (sum la, H), b (sum lb, H) and out (sum la lb, H), where ta_n, ub_n and off_n are the running sums over the earlier
-    utterances.  fp32, bf16 or fp16 (a and b alike); la, lb integer lengths on the CPU or the GPU.  Sizing the output costs
-    one host synchronisation when the lengths are on the GPU.  The backward sums in fp32 without atomics."""
+    utterances.  fp32, bf16 or fp16 (a and b alike); la, lb integer lengths on the CPU or the GPU.  With both on the CPU the
+    sizes are taken on the host and the lengths uploaded asynchronously, so the call does not synchronise; sizing the output
+    costs one host synchronisation when the lengths are on the GPU.  The backward sums in fp32 without atomics."""
     if a.dtype not in _DTYPES or b.dtype != a.dtype:
         raise ValueError(f"gather_sum: a and b must share one of fp32, bf16, fp16, not {a.dtype} and {b.dtype}")
     if a.dim() != 2 or b.dim() != 2 or a.shape[1] != b.shape[1] or a.shape[1] == 0:
@@ -228,11 +229,13 @@ def gather_sum(a: torch.Tensor, b: torch.Tensor, la: torch.Tensor, lb: torch.Ten
     if not a.is_cuda or b.device != a.device:
         raise ValueError("gather_sum: a and b must be on one CUDA device")
     dev = a.device
+    host = not la.is_cuda and not lb.is_cuda
     with torch.cuda.device(dev):
-        la64, lb64 = la.to(dev, torch.int64), lb.to(dev, torch.int64)
+        la64, lb64 = (la.long(), lb.long()) if host else (la.to(dev, torch.int64), lb.to(dev, torch.int64))
         rows_out, sa, sb, lo = (int(v) for v in torch.stack([(la64 * lb64).sum(), la64.sum(), lb64.sum(),
                                                               torch.minimum(la64.min(), lb64.min())]).tolist())
         if lo < 0 or sa != a.shape[0] or sb != b.shape[0]:
             raise ValueError(f"gather_sum: the lengths (sums {sa}, {sb}, min {lo}) do not match a {tuple(a.shape)} and "
                              f"b {tuple(b.shape)}")
-        return _GatherSum.apply(a.contiguous(), b.contiguous(), la64.to(torch.int32), lb64.to(torch.int32), rows_out)
+        la32, lb32 = _on_device(dev, la64.to(torch.int32), lb64.to(torch.int32))
+        return _GatherSum.apply(a.contiguous(), b.contiguous(), la32, lb32, rows_out)

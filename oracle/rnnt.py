@@ -13,8 +13,8 @@ from __future__ import annotations
 import numpy as np
 
 
-def lattice(lpb: np.ndarray, lpl: np.ndarray):
-    """lpb (T, U+1), lpl (T, U) in fp64.  Returns (log P, log P from beta, pb (T, U+1), pl (T, U))."""
+def cells(lpb: np.ndarray, lpl: np.ndarray):
+    """lpb (T, U+1), lpl (T, U) in fp64.  Returns the lattice cells (alpha, beta), each (T, U+1)."""
     lpb = np.asarray(lpb, np.float64)
     lpl = np.asarray(lpl, np.float64).reshape(lpb.shape[0], lpb.shape[1] - 1)
     T, U1 = lpb.shape
@@ -38,6 +38,17 @@ def lattice(lpb: np.ndarray, lpl: np.ndarray):
             b1 = np.where(t < T - 1, beta[np.minimum(t + 1, T - 1), u] + lpb[t, u], -np.inf)
             b2 = np.where(u < U, beta[t, np.minimum(u + 1, U)] + lplp[t, u], -np.inf)
             beta[t, u] = np.logaddexp(b1, b2)
+    return alpha, beta
+
+
+def lattice(lpb: np.ndarray, lpl: np.ndarray):
+    """lpb (T, U+1), lpl (T, U) in fp64.  Returns (log P, log P from beta, pb (T, U+1), pl (T, U))."""
+    lpb = np.asarray(lpb, np.float64)
+    lpl = np.asarray(lpl, np.float64).reshape(lpb.shape[0], lpb.shape[1] - 1)
+    T, U1 = lpb.shape
+    U = U1 - 1
+    alpha, beta = cells(lpb, lpl)
+    with np.errstate(invalid="ignore"):
         logp = alpha[T - 1, U] + lpb[T - 1, U]
         nxt = np.full((T, U1), -np.inf)
         nxt[:-1] = beta[1:]
