@@ -33,7 +33,7 @@ SYMBOLS = [
     "ccb_ngram_create", "ccb_ngram_destroy", "ccb_ngram_info", "ccb_ngram_copy", "ccb_ctc_beam_search_lm",
     "ccb_wfst_create", "ccb_wfst_destroy", "ccb_wfst_info", "ccb_wfst_copy", "ccb_wfst_decode_ws_bytes", "ccb_wfst_decode",
     "ccb_rnnt_workspace_bytes", "ccb_rnnt_forward", "ccb_rnnt_backward", "ccb_gather_ws_bytes", "ccb_gather_sum",
-    "ccb_gather_sum_backward",
+    "ccb_gather_sum_backward", "ccb_rnnt_simple_workspace_bytes", "ccb_rnnt_simple_forward", "ccb_rnnt_simple_backward",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -147,6 +147,11 @@ def lib() -> C.CDLL:
     L.ccb_rnnt_forward.restype = C.c_int
     L.ccb_rnnt_backward.argtypes = [vp, i, i, i, l, i, vp, i, vp, vp, vp, vp]
     L.ccb_rnnt_backward.restype = C.c_int
+    L.ccb_rnnt_simple_workspace_bytes.argtypes = [i, i, i]; L.ccb_rnnt_simple_workspace_bytes.restype = C.c_size_t
+    L.ccb_rnnt_simple_forward.argtypes = [vp, vp, i, i, i, i, i, vp, vp, vp, i, i, vp, vp, vp]
+    L.ccb_rnnt_simple_forward.restype = C.c_int
+    L.ccb_rnnt_simple_backward.argtypes = [vp, vp, i, i, i, i, i, vp, i, vp, vp, vp, vp, vp]
+    L.ccb_rnnt_simple_backward.restype = C.c_int
     L.ccb_gather_ws_bytes.argtypes = [i]; L.ccb_gather_ws_bytes.restype = C.c_size_t
     L.ccb_gather_sum.argtypes = [vp, vp, i, i, l, i, vp, vp, vp, vp, vp]; L.ccb_gather_sum.restype = C.c_int
     L.ccb_gather_sum_backward.argtypes = [vp, i, i, l, l, i, vp, vp, vp, vp, vp, vp]

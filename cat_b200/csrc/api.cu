@@ -1321,6 +1321,43 @@ int ccb_rnnt_backward(const void *x, int dtype, int from_logits, int N, long row
     return 0;
 }
 
+size_t ccb_rnnt_simple_workspace_bytes(int N, int Tmax, int Umax) {
+    return N > 0 && Tmax > 0 && Umax >= 0 ? RnntSimpleWsBytes(N, Tmax, Umax) : 0;
+}
+
+int ccb_rnnt_simple_forward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
+                            const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
+                            void *stream) {
+    g_err.clear();
+    if (N <= 0 || Tmax <= 0 || Umax < 0 || V <= 0)
+        return Fail("rnnt_simple_forward: N, Tmax and V must be positive, Umax >= 0");
+    if (N > 65535) return Fail("rnnt_simple_forward: at most 65535 utterances per call");
+    if (!KnownDtype(dtype)) return FailDtype("rnnt_simple_forward", dtype);
+    if (blank < 0 || blank >= V) return Fail("rnnt_simple_forward: blank must lie in [0, V)");
+    if (!f || !g || (Umax && !labels_dev) || !lx_dev || !ly_dev || !workspace || !costs)
+        return Fail("rnnt_simple_forward: missing buffer");
+    const int rc = LaunchRnntSimpleForward(f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev, ly_dev, blank, want_beta,
+                                           workspace, costs, (cudaStream_t)stream);
+    if (rc) return FailCuda("rnnt_simple_forward", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_rnnt_simple_backward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
+                             int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream) {
+    g_err.clear();
+    if (N <= 0 || Tmax <= 0 || Umax < 0 || V <= 0)
+        return Fail("rnnt_simple_backward: N, Tmax and V must be positive, Umax >= 0");
+    if (N > 65535) return Fail("rnnt_simple_backward: at most 65535 utterances per call");
+    if (!KnownDtype(dtype)) return FailDtype("rnnt_simple_backward", dtype);
+    if (blank < 0 || blank >= V) return Fail("rnnt_simple_backward: blank must lie in [0, V)");
+    if (!f || !g || (Umax && !labels_dev) || !workspace || !w || !grad_f || !grad_g)
+        return Fail("rnnt_simple_backward: missing buffer");
+    const int rc = LaunchRnntSimpleBackward(f, g, dtype, N, Tmax, Umax, V, labels_dev, blank, workspace, w, grad_f, grad_g,
+                                            (cudaStream_t)stream);
+    if (rc) return FailCuda("rnnt_simple_backward", (cudaError_t)rc);
+    return 0;
+}
+
 size_t ccb_gather_ws_bytes(int N) { return N > 0 ? GatherWsBytes(N) : 0; }
 
 int ccb_gather_sum(const void *a, const void *b, int dtype, int N, long rows_out, int H, const int *la_dev, const int *lb_dev,

@@ -276,6 +276,14 @@ int LaunchRnntForward(const void *x, int dtype, int from_logits, int compact, in
                       float *costs, float *costs_beta, cudaStream_t s);
 int LaunchRnntBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
                        void *ws, const float *w, void *grad, cudaStream_t s);
+// RNN-T loss of the LogAdd joiner from f (N, Tmax, V) and g (N, Umax+1, V) (rnnt_kernels.cu): the forward runs the prep,
+// row maxima, normaliser GEMM, underflow fix-up and alpha (|| beta) passes; the backward the cell weights and the two
+// gradient GEMMs over the same workspace of RnntSimpleWsBytes(N, Tmax, Umax) bytes.
+size_t RnntSimpleWsBytes(int N, int Tmax, int Umax);
+int LaunchRnntSimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                            const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s);
+int LaunchRnntSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                             int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s);
 // gather.sum of the joiner and its backward; ws: GatherWsBytes(N) bytes of per-utterance offsets
 size_t GatherWsBytes(int N);
 int LaunchGatherSum(const void *a, const void *b, int dtype, int N, long long rows_out, int H, const int *la, const int *lb,

@@ -306,6 +306,19 @@ __global__ void __launch_bounds__(kAbThreads) rnnt_alpha_beta_kernel(const RnntM
     }
 }
 
+// The weighted posteriors of the blank and label transitions out of live cell (t, u) at workspace row `row` (formulas below);
+// shared by the gradient pass and the LogAdd joiner's cell weights.
+__device__ __forceinline__ void CellPosteriors(const RnntMeta &m, long long row, long long t, int u, const double *alpha,
+                                               const double *beta, const float *lpb, const float *lpl, double lP, float wn,
+                                               float &pb, float &pl) {
+    const double a = alpha[row];
+    pb = 0.f; pl = 0.f;
+    if (t < m.T - 1) pb = (float)exp(a + (double)lpb[row] + beta[row + m.ts] - lP);
+    else if (u == m.U) pb = (float)exp(a + (double)lpb[row] - lP);
+    if (u < m.U) pl = (float)exp(a + (double)lpl[row] + beta[row + 1] - lP);
+    pb *= wn; pl *= wn;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Gradient pass: one warp per row, every row of the tensor written once.  Grid (row chunk, N + 1): CTA (x, n < N) walks
 // utterance n's span (rows outside t < T_n, u <= U_n, and every row of a bad utterance, get zeros and are not read);
@@ -341,11 +354,8 @@ __global__ void __launch_bounds__(kRowThreads) rnnt_grad_kernel(const void *x, l
             const int u = (int)(r - t * m.ts);
             if (t < m.T && u <= m.U) {
                 live = true;
-                const double a = alpha[row];
-                if (t < m.T - 1) pb = (float)exp(a + (double)lpb[row] + beta[row + m.ts] - lP);
-                else if (u == m.U) pb = (float)exp(a + (double)lpb[row] - lP);
-                if (u < m.U) { pl = (float)exp(a + (double)lpl[row] + beta[row + 1] - lP); y = labels[m.loff + u]; }
-                pb *= wn; pl *= wn;
+                CellPosteriors(m, row, t, u, alpha, beta, lpb, lpl, lP, wn, pb, pl);
+                if (u < m.U) y = labels[m.loff + u];
                 if constexpr (RAW) l = lse[row];
             }
         }
@@ -426,6 +436,355 @@ __global__ void __launch_bounds__(kRowThreads) gather_sum_bwd_kernel(const void 
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// RNN-T loss of CAT's LogAdd joiner (DESIGN.md §7 "RNN-T loss, LogAdd joiner") from f (N, Tmax, V) and g (N, Umax+1, V),
+// without the joint: z(t,u,k) = f[t,k] + g[u,k], Z(t,u) = logsumexp_k z = mf_t + mg_u + log S(t,u) with the row maxima mf, mg
+// and S = sum_k Ef[t,k] Eg[u,k], Ef = exp(f - mf), Eg = exp(g - mg): one fp32 GEMM per utterance.  The lattice cells are the
+// padded layout's (rnnt_prep_kernel with compact = 0, rnnt_alpha_beta_kernel as they are).  A cell with S < 2^-64 (the
+// peaks of f[t] and g[u] on different tokens) is flagged and gets its Z from an exact logsumexp over f[t] + g[u] instead:
+// the terms the GEMM flushes to zero are each below 2^-126, so for S >= 2^-64 they are below 2^-46 S for V <= 2^16.
+// ------------------------------------------------------------------------------------------------
+constexpr float kSimpleTiny = 0x1p-64f;
+__device__ __forceinline__ bool SimpleFlagged(float s) { return !(s >= kSimpleTiny); }
+// a row maximum as the exponent's offset: a row of -inf exponentiates to zeros, not NaN
+__device__ __forceinline__ float SimpleOffset(float m) { return m == -INFINITY ? 0.f : m; }
+
+struct SimpleLayout {
+    RnntLayout r;                                  // meta .. lse over the N Tmax (Umax+1) cells; lse holds Z
+    size_t mf, mg, ff, fg, S, W, PB, PL, total;    // row maxima and "row has a flagged cell" of f and g; per cell S, W, pb, pl
+};
+
+SimpleLayout MakeSimpleLayout(int N, int Tmax, int Umax) {
+    const size_t nf = (size_t)N * Tmax, ng = (size_t)N * (Umax + 1), cells = nf * (Umax + 1);
+    SimpleLayout L;
+    L.r = MakeRnntLayout(N, (long long)cells);
+    size_t o = L.r.total;
+    L.mf = o; o += Align256(sizeof(float) * nf);
+    L.mg = o; o += Align256(sizeof(float) * ng);
+    L.ff = o; o += Align256(sizeof(int) * nf);
+    L.fg = o; o += Align256(sizeof(int) * ng);
+    L.S = o;  o += Align256(sizeof(float) * cells);
+    L.W = o;  o += Align256(sizeof(float) * cells);
+    L.PB = o; o += Align256(sizeof(float) * cells);
+    L.PL = o; o += Align256(sizeof(float) * cells);
+    L.total = o;
+    return L;
+}
+
+// Row maxima: one warp per live row, of f (blockIdx.z = 0, t < T_n) or of g (z = 1, u <= U_n); also clears the row's flag.
+template <int DT, bool VEC>
+__global__ void __launch_bounds__(kRowThreads) simple_rowmax_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                                    const RnntMeta *meta, float *mf, float *mg, int *ff, int *fg) {
+    constexpr int K = ChunkElems<DT, VEC>();
+    const int n = blockIdx.y;
+    const RnntMeta m = meta[n];
+    if (m.bad) return;
+    const bool is_g = blockIdx.z == 1;
+    const int live = is_g ? m.U + 1 : m.T;
+    const long long first = is_g ? (long long)n * (Umax + 1) : (long long)n * Tmax, chunks = V / K;
+    const void *x = is_g ? g : f;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    for (int r = blockIdx.x * W + warp; r < live; r += gridDim.x * W) {
+        const long long base = (first + r) * V;
+        float mx = -INFINITY;
+        for (long long c = lane; c < chunks; c += 32) {
+            float v[K];
+            LoadChunk<DT, VEC>(x, base, c, v);
+#pragma unroll
+            for (int i = 0; i < K; ++i) mx = fmaxf(mx, v[i]);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        if (lane == 0) {
+            (is_g ? mg : mf)[first + r] = mx;
+            (is_g ? fg : ff)[first + r] = 0;
+        }
+    }
+}
+
+// Normaliser GEMM: CTA (t tile, u tile, n) sums S(t,u) = sum_k Ef[t,k] Eg[u,k] over kSK-wide slabs of k, in increasing k, each
+// thread a 4 x 2 block of cells in fp32 FFMA.  Tiles wholly past T_n or U_n + 1 return at once.  Epilogue per live cell: S;
+// the label check (a label outside [0, V) or equal to blank marks the utterance bad, as the row pass does); then for an
+// unflagged cell Z (in lse), lpb = z(blank) - Z and lpl = z(y_{u+1}) - Z, and for a flagged one the flags of rows t and u.
+constexpr int kST = 64, kSU = 32, kSK = 32;
+template <int DT>
+__global__ void __launch_bounds__(256) simple_norm_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                          const int *labels, int blank, RnntMeta *meta, const float *mf,
+                                                          const float *mg, int *ff, int *fg, float *S, float *lpb, float *lpl,
+                                                          float *lse) {
+    const int n = blockIdx.z;
+    const RnntMeta m = meta[n];
+    const int t0 = blockIdx.x * kST, u0 = blockIdx.y * kSU;
+    if (m.bad || t0 >= m.T || u0 > m.U) return;
+    __shared__ float As[kSK][kST + 1], Bs[kSK][kSU + 1];
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4, lk = tid & 31, lr = tid >> 5;
+    const long long fr0 = (long long)n * Tmax, gr0 = (long long)n * (Umax + 1);
+    float oa[kST / 8], ob[kSU / 8];      // the loader's rows lr + 8 i: their offsets (row maxima)
+#pragma unroll
+    for (int i = 0; i < kST / 8; ++i) { const int t = t0 + lr + 8 * i; oa[i] = t < m.T ? SimpleOffset(mf[fr0 + t]) : 0.f; }
+#pragma unroll
+    for (int i = 0; i < kSU / 8; ++i) { const int u = u0 + lr + 8 * i; ob[i] = u <= m.U ? SimpleOffset(mg[gr0 + u]) : 0.f; }
+    float acc[4][2] = {};
+    for (long long k0 = 0; k0 < V; k0 += kSK) {
+        const long long k = k0 + lk;
+#pragma unroll
+        for (int i = 0; i < kST / 8; ++i) {
+            const int r = lr + 8 * i, t = t0 + r;
+            As[lk][r] = t < m.T && k < V ? expf(load_y(f, DT, (fr0 + t) * V + k) - oa[i]) : 0.f;
+        }
+#pragma unroll
+        for (int i = 0; i < kSU / 8; ++i) {
+            const int r = lr + 8 * i, u = u0 + r;
+            Bs[lk][r] = u <= m.U && k < V ? expf(load_y(g, DT, (gr0 + u) * V + k) - ob[i]) : 0.f;
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int kk = 0; kk < kSK; ++kk) {
+            float a[4], b[2];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) a[i] = As[kk][ty + 16 * i];
+#pragma unroll
+            for (int j = 0; j < 2; ++j) b[j] = Bs[kk][tx + 16 * j];
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 2; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int t = t0 + ty + 16 * i;
+        if (t >= m.T) continue;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+            const int u = u0 + tx + 16 * j;
+            if (u > m.U) continue;
+            const long long row = m.roff + (long long)t * m.ts + u, fb = (fr0 + t) * V, gb = (gr0 + u) * V;
+            const float s = acc[i][j];
+            S[row] = s;
+            int y = -1;
+            if (u < m.U) {
+                y = labels[m.loff + u];
+                if (y < 0 || y >= V || y == blank) { meta[n].bad = 1; lpl[row] = NAN; continue; }
+            }
+            if (SimpleFlagged(s)) { ff[fr0 + t] = 1; fg[gr0 + u] = 1; continue; }
+            const float Z = mf[fr0 + t] + mg[gr0 + u] + logf(s);
+            lse[row] = Z;
+            lpb[row] = (load_y(f, DT, fb + blank) + load_y(g, DT, gb + blank)) - Z;
+            if (y >= 0) lpl[row] = (load_y(f, DT, fb + y) + load_y(g, DT, gb + y)) - Z;
+        }
+    }
+}
+
+// Underflow fix-up: one warp per flagged cell (rows t without a flagged cell are skipped by their flag) takes the exact
+// logsumexp of f[t] + g[u] by an online max / sum, and rewrites Z, lpb and lpl.
+template <int DT, bool VEC>
+__global__ void __launch_bounds__(kRowThreads) simple_fixup_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                                   const int *labels, int blank, const RnntMeta *meta,
+                                                                   const int *ff, const float *S, float *lpb, float *lpl,
+                                                                   float *lse) {
+    constexpr int K = ChunkElems<DT, VEC>();
+    const int n = blockIdx.y;
+    const RnntMeta m = meta[n];
+    if (m.bad) return;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const long long live = (long long)m.T * m.ts, chunks = V / K, fr0 = (long long)n * Tmax, gr0 = (long long)n * (Umax + 1);
+    for (long long r = (long long)blockIdx.x * W + warp; r < live; r += (long long)gridDim.x * W) {
+        const long long t = r / m.ts;
+        const int u = (int)(r - t * m.ts);
+        const long long row = m.roff + r;
+        if (u > m.U || !ff[fr0 + t] || !SimpleFlagged(S[row])) continue;
+        const long long fb = (fr0 + t) * V, gb = (gr0 + u) * V;
+        float mx = -INFINITY, s = 0.f;
+        for (long long c = lane; c < chunks; c += 32) {
+            float v[K], w[K];
+            LoadChunk<DT, VEC>(f, fb, c, v);
+            LoadChunk<DT, VEC>(g, gb, c, w);
+            float cm = -INFINITY;
+#pragma unroll
+            for (int i = 0; i < K; ++i) { v[i] += w[i]; cm = fmaxf(cm, v[i]); }
+            if (cm == -INFINITY) continue;
+            if (cm > mx) { s *= expf(mx - cm); mx = cm; }
+#pragma unroll
+            for (int i = 0; i < K; ++i) s += expf(v[i] - mx);
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float mo = __shfl_xor_sync(0xffffffffu, mx, o), so = __shfl_xor_sync(0xffffffffu, s, o);
+            const float mm = fmaxf(mx, mo);
+            if (mm != -INFINITY) { s = s * expf(mx - mm) + so * expf(mo - mm); mx = mm; }
+        }
+        if (lane == 0) {
+            const float Z = mx == -INFINITY ? -INFINITY : mx + logf(s);
+            lse[row] = Z;
+            lpb[row] = (load_y(f, DT, fb + blank) + load_y(g, DT, gb + blank)) - Z;
+            if (u < m.U) {
+                const int y = labels[m.loff + u];
+                lpl[row] = (load_y(f, DT, fb + y) + load_y(g, DT, gb + y)) - Z;
+            }
+        }
+    }
+}
+
+// Cell weights: per live cell pb, pl (weighted posteriors, as the gradient pass) and W = (pb + pl) / S, 0 for a flagged cell.
+__global__ void __launch_bounds__(kRowThreads) simple_weights_kernel(const RnntMeta *meta, const double *alpha, const double *beta,
+                                                                     const double *logp, const float *lpb, const float *lpl,
+                                                                     const float *S, const float *w, float *W, float *PB,
+                                                                     float *PL) {
+    const int n = blockIdx.y;
+    const RnntMeta m = meta[n];
+    if (m.bad) return;
+    const float wn = w[n];
+    const double lP = logp[n];
+    const long long live = (long long)m.T * m.ts;
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < live; r += (long long)gridDim.x * blockDim.x) {
+        const long long t = r / m.ts;
+        const int u = (int)(r - t * m.ts);
+        if (u > m.U) continue;
+        const long long row = m.roff + r;
+        float pb, pl;
+        CellPosteriors(m, row, t, u, alpha, beta, lpb, lpl, lP, wn, pb, pl);
+        const float s = S[row];
+        PB[row] = pb;
+        PL[row] = pl;
+        W[row] = SimpleFlagged(s) ? 0.f : (pb + pl) / s;
+    }
+}
+
+// Gradient GEMM.  GF: grad_f, output rows r = t and reduction q = u; else grad_g, r = u and q = t.  With "own" the input
+// whose gradient is written and "other" the one summed over,
+//   grad[r,k] = E_own[r,k] sum_q W(r,q) E_other[q,k]  +  sum_{q flagged} (pb + pl) exp(z - Z)
+//               - [k = blank] sum_q pb  -  sum_q pl [k = y_{u+1}],
+// each sum over increasing q in fp32.  CTA (k tile, r tile, n) writes its whole kGR x kGC block: rows past the utterance (and
+// every row of a bad utterance) get zeros and are not read.
+constexpr int kGR = 64, kGC = 64, kGQ = 16;
+template <int DT, bool GF>
+__global__ void __launch_bounds__(256) simple_grad_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                          const int *labels, int blank, const RnntMeta *meta, const float *mf,
+                                                          const float *mg, const int *ff, const int *fg, const float *S,
+                                                          const float *lse, const float *W, const float *PB, const float *PL,
+                                                          void *grad) {
+    const int n = blockIdx.z;
+    const RnntMeta m = meta[n];
+    const int U1 = Umax + 1, Rmax = GF ? Tmax : U1;
+    const int r0 = blockIdx.y * kGR;
+    const long long c0 = (long long)blockIdx.x * kGC;
+    const void *own = GF ? f : g, *oth = GF ? g : f;
+    const float *m_own = GF ? mf : mg, *m_oth = GF ? mg : mf;
+    const int *flag_own = GF ? ff : fg;
+    const long long own0 = GF ? (long long)n * Tmax : (long long)n * U1, oth0 = GF ? (long long)n * U1 : (long long)n * Tmax;
+    const long long fr0 = (long long)n * Tmax, gr0 = (long long)n * U1;
+    const int Rn = m.bad ? 0 : (GF ? m.T : m.U + 1), Qn = m.bad ? 0 : (GF ? m.U + 1 : m.T);
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    // workspace row of cell (r, q)
+    auto cell = [&](int r, int q) { return m.roff + (GF ? (long long)r * m.ts + q : (long long)q * m.ts + r); };
+    float acc[4][4] = {};
+    if (r0 < Rn) {
+        __shared__ float As[kGQ][kGR + 1], Bs[kGQ][kGC];
+        for (int q0 = 0; q0 < Qn; q0 += kGQ) {
+#pragma unroll
+            for (int i = 0; i < kGR * kGQ / 256; ++i) {
+                const int e = tid + 256 * i, qq = e / kGR, rr = e % kGR, r = r0 + rr, q = q0 + qq;
+                As[qq][rr] = r < Rn && q < Qn ? W[cell(r, q)] : 0.f;
+            }
+#pragma unroll
+            for (int i = 0; i < kGC * kGQ / 256; ++i) {
+                const int e = tid + 256 * i, qq = e / kGC, cc = e % kGC, q = q0 + qq;
+                const long long k = c0 + cc;
+                Bs[qq][cc] = q < Qn && k < V ? expf(load_y(oth, DT, (oth0 + q) * V + k) - SimpleOffset(m_oth[oth0 + q])) : 0.f;
+            }
+            __syncthreads();
+#pragma unroll
+            for (int qq = 0; qq < kGQ; ++qq) {
+                float a[4], b[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) a[i] = As[qq][ty + 16 * i];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) b[j] = Bs[qq][tx + 16 * j];
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+            }
+            __syncthreads();
+        }
+    }
+    // epilogue: acc becomes the gradient block
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int r = r0 + ty + 16 * i;
+        if (r >= Rn) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+            continue;
+        }
+        const float mo = SimpleOffset(m_own[own0 + r]);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const long long k = c0 + tx + 16 * j;
+            acc[i][j] = k < V ? expf(load_y(own, DT, (own0 + r) * V + k) - mo) * acc[i][j] : 0.f;
+        }
+        if (flag_own[own0 + r]) {
+            for (int q = 0; q < Qn; ++q) {
+                const long long c = cell(r, q);
+                if (!SimpleFlagged(S[c])) continue;
+                const float occ = PB[c] + PL[c], Z = lse[c];
+                const int t = GF ? r : q, u = GF ? q : r;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const long long k = c0 + tx + 16 * j;
+                    if (k < V)
+                        acc[i][j] += occ * expf(load_y(f, DT, (fr0 + t) * V + k) + load_y(g, DT, (gr0 + u) * V + k) - Z);
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (c0 + tx + 16 * j != blank) continue;
+            float sb = 0.f;
+            for (int q = 0; q < Qn; ++q) sb += PB[cell(r, q)];
+            acc[i][j] -= sb;
+        }
+        if (!GF && r < m.U) {      // grad_g: row u carries label y_{u+1}
+            const int y = labels[m.loff + r];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                if (c0 + tx + 16 * j != y) continue;
+                float sl = 0.f;
+                for (int q = 0; q < Qn; ++q) sl += PL[cell(r, q)];
+                acc[i][j] -= sl;
+            }
+        }
+    }
+    if (GF && r0 < Rn) {           // grad_f: label y_{u+1} of every u < U_n, in increasing u
+        for (int q = 0; q < m.U; ++q) {
+            const int y = labels[m.loff + q];
+            const long long j = y - c0 - tx;
+            if (j < 0 || j >= 16 * 4 || j % 16) continue;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int r = r0 + ty + 16 * i;
+                if (r < Rn) {
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj)
+                        if (jj == j / 16) acc[i][jj] -= PL[cell(r, q)];
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int r = r0 + ty + 16 * i;
+        if (r >= Rmax) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const long long k = c0 + tx + 16 * j;
+            if (k < V) store_y(grad, DT, (own0 + r) * V + k, acc[i][j]);
+        }
+    }
+}
+
 int GridX(long long rows_per_utt, int per_cta) {
     long long g = (rows_per_utt + per_cta - 1) / per_cta;
     return (int)std::max(1LL, std::min(g, 65535LL));
@@ -490,6 +849,61 @@ int LaunchRnntBackward(const void *x, int dtype, int from_logits, int N, long lo
                                                   At<float>(ws, L.lse), w, grad);
     });
     CountLaunch(1);
+    return (int)cudaGetLastError();
+}
+
+size_t RnntSimpleWsBytes(int N, int Tmax, int Umax) { return MakeSimpleLayout(N, Tmax, Umax).total; }
+
+int LaunchRnntSimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                            const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s) {
+    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax);
+    const int U1 = Umax + 1;
+    const long long cells = (long long)N * Tmax * U1;
+    RnntMeta *meta = At<RnntMeta>(ws, L.r.meta);
+    float *mf = At<float>(ws, L.mf), *mg = At<float>(ws, L.mg), *S = At<float>(ws, L.S);
+    float *lpb = At<float>(ws, L.r.lpb), *lpl = At<float>(ws, L.r.lpl), *lse = At<float>(ws, L.r.lse);
+    int *ff = At<int>(ws, L.ff), *fg = At<int>(ws, L.fg);
+    rnnt_prep_kernel<<<1, kPrepThreads, 0, s>>>(lx, ly, N, cells, (long long)N * Umax, 0, Tmax, Umax, meta,
+                                                At<long long>(ws, L.r.tail));
+    const bool vec = RowsVectorisable(f, V, dtype) && RowsVectorisable(g, V, dtype);
+    DispatchDtype(dtype, [&](auto dt) {
+        constexpr int DT = decltype(dt)::value;
+        auto rowmax = vec ? simple_rowmax_kernel<DT, true> : simple_rowmax_kernel<DT, false>;
+        rowmax<<<dim3(GridX(std::max(Tmax, U1), kRowThreads / 32 * 4), N, 2), kRowThreads, 0, s>>>(f, g, V, Tmax, Umax, meta,
+                                                                                                    mf, mg, ff, fg);
+        simple_norm_kernel<DT><<<dim3((Tmax + kST - 1) / kST, (U1 + kSU - 1) / kSU, N), 256, 0, s>>>(
+            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, lse);
+        auto fixup = vec ? simple_fixup_kernel<DT, true> : simple_fixup_kernel<DT, false>;
+        fixup<<<dim3(GridX((long long)Tmax * U1, kRowThreads / 32 * 16), N), kRowThreads, 0, s>>>(
+            f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, lse);
+    });
+    rnnt_alpha_beta_kernel<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(meta, lpb, lpl, At<double>(ws, L.r.alpha),
+                                                                             At<double>(ws, L.r.beta),
+                                                                             At<double>(ws, L.r.logp), N, costs, nullptr);
+    CountLaunch(5);
+    return (int)cudaGetLastError();
+}
+
+int LaunchRnntSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                             int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s) {
+    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax);
+    const int U1 = Umax + 1;
+    const RnntMeta *meta = At<RnntMeta>(ws, L.r.meta);
+    const float *mf = At<float>(ws, L.mf), *mg = At<float>(ws, L.mg), *S = At<float>(ws, L.S), *lse = At<float>(ws, L.r.lse);
+    const int *ff = At<int>(ws, L.ff), *fg = At<int>(ws, L.fg);
+    float *W = At<float>(ws, L.W), *PB = At<float>(ws, L.PB), *PL = At<float>(ws, L.PL);
+    simple_weights_kernel<<<dim3(GridX((long long)Tmax * U1, kRowThreads * 4), N), kRowThreads, 0, s>>>(
+        meta, At<double>(ws, L.r.alpha), At<double>(ws, L.r.beta), At<double>(ws, L.r.logp), At<float>(ws, L.r.lpb),
+        At<float>(ws, L.r.lpl), S, w, W, PB, PL);
+    const int gx = (int)((V + kGC - 1) / kGC);
+    DispatchDtype(dtype, [&](auto dt) {
+        constexpr int DT = decltype(dt)::value;
+        simple_grad_kernel<DT, true><<<dim3(gx, (Tmax + kGR - 1) / kGR, N), 256, 0, s>>>(
+            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, grad_f);
+        simple_grad_kernel<DT, false><<<dim3(gx, (U1 + kGR - 1) / kGR, N), 256, 0, s>>>(
+            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, grad_g);
+    });
+    CountLaunch(3);
     return (int)cudaGetLastError();
 }
 

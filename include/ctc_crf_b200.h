@@ -421,6 +421,29 @@ int ccb_rnnt_forward(const void *x, int dtype, int from_logits, int compact, int
 int ccb_rnnt_backward(const void *x, int dtype, int from_logits, int N, long rows, int V, const int *labels_dev, int blank,
                       void *workspace, const float *w, void *grad, void *stream);
 
+/* RNN-T loss of CAT's LogAdd joiner, from the encoder output f (N, Tmax, V) and the predictor output g (N, Umax+1, V)
+ * without the joint tensor: with z(t,u,k) = f[n,t,k] + g[n,u,k] (fp32 sum of the values as given) and
+ * Z(t,u) = logsumexp_k z(t,u,k), the lattice of ccb_rnnt_forward has lp(t,u,k) = z(t,u,k) - Z(t,u).  f and g share the
+ * CCB_DTYPE_* code dtype and are read in place; labels (N, Umax), lx, ly (N,) int32 device.  Rows t >= T_n of f and u > U_n of
+ * g are never read.  An utterance with T_n < 1, U_n < 0, T_n > Tmax, U_n > Umax, or a label outside [0, V) or equal to
+ * blank, gets cost NaN and zero gradient rows.  Z is mf_t + mg_u + log S(t,u) with the row maxima mf, mg and
+ * S = sum_k exp(f[t,k] - mf_t) exp(g[u,k] - mg_u) from an fp32 GEMM; a cell with S < 2^-64 takes Z from an exact logsumexp
+ * over f[t] + g[u] instead.  No atomics: two identical calls give identical bits.  N <= 65535.
+ *   ccb_rnnt_simple_workspace_bytes: the workspace of a call, sized from the shapes alone: 44 bytes per cell of the padded
+ *     lattice, N Tmax (Umax+1) cells (lp of blank and label, Z, alpha and beta in fp64 as ccb_rnnt_forward; S, the cell
+ *     weight and the weighted blank and label posteriors in fp32), 8 bytes per row of f and of g (row maximum, flag) and
+ *     56 bytes per utterance, each block aligned to 256 bytes.  Nothing needs to be initialised.
+ *   ccb_rnnt_simple_forward: costs (N,) fp32 out.  want_beta != 0 also runs beta, which ccb_rnnt_simple_backward needs.
+ *   ccb_rnnt_simple_backward: after a want_beta forward on the same workspace (untouched since) and the same f, g, labels
+ *     and lengths: grad_f (the shape of f) and grad_g (the shape of g), in dtype, = w[n] d cost[n] / d f and d g, with
+ *     zeros in every row outside the utterances (not read).  The workspace may serve several backward calls. */
+size_t ccb_rnnt_simple_workspace_bytes(int N, int Tmax, int Umax);
+int ccb_rnnt_simple_forward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
+                            const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
+                            void *stream);
+int ccb_rnnt_simple_backward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
+                             int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream);
+
 /* The compact joiner's broadcast sum (CAT's gather.sum): for N utterances with la[n] rows of a and lb[n] rows of b, laid out
  * one utterance after the other in each (offsets ta_n, ub_n and off_n = sum_{m<n} la_m lb_m computed on the device),
  *   out[off_n + t lb_n + u][h] = a[ta_n + t][h] + b[ub_n + u][h]   (fp32 sum, rounded to dtype),
