@@ -34,6 +34,8 @@ SYMBOLS = [
     "ccb_wfst_create", "ccb_wfst_destroy", "ccb_wfst_info", "ccb_wfst_copy", "ccb_wfst_decode_ws_bytes", "ccb_wfst_decode",
     "ccb_rnnt_workspace_bytes", "ccb_rnnt_forward", "ccb_rnnt_backward", "ccb_gather_ws_bytes", "ccb_gather_sum",
     "ccb_gather_sum_backward", "ccb_rnnt_simple_workspace_bytes", "ccb_rnnt_simple_forward", "ccb_rnnt_simple_backward",
+    "ccb_ctct_workspace_bytes", "ccb_ctct_forward", "ccb_ctct_backward", "ccb_ctct_simple_workspace_bytes",
+    "ccb_ctct_simple_forward", "ccb_ctct_simple_backward",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -152,6 +154,10 @@ def lib() -> C.CDLL:
     L.ccb_rnnt_simple_forward.restype = C.c_int
     L.ccb_rnnt_simple_backward.argtypes = [vp, vp, i, i, i, i, i, vp, i, vp, vp, vp, vp, vp]
     L.ccb_rnnt_simple_backward.restype = C.c_int
+    for e in ("workspace_bytes", "forward", "backward", "simple_workspace_bytes", "simple_forward", "simple_backward"):
+        # the CTC-T entries take the RNN-T entries' arguments
+        getattr(L, f"ccb_ctct_{e}").argtypes = getattr(L, f"ccb_rnnt_{e}").argtypes
+        getattr(L, f"ccb_ctct_{e}").restype = getattr(L, f"ccb_rnnt_{e}").restype
     L.ccb_gather_ws_bytes.argtypes = [i]; L.ccb_gather_ws_bytes.restype = C.c_size_t
     L.ccb_gather_sum.argtypes = [vp, vp, i, i, l, i, vp, vp, vp, vp, vp]; L.ccb_gather_sum.restype = C.c_int
     L.ccb_gather_sum_backward.argtypes = [vp, i, i, l, l, i, vp, vp, vp, vp, vp, vp]

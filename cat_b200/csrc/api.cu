@@ -373,6 +373,76 @@ int EnsureLegacy(int dev, const DeviceGraph &g, int N, int T, float *caller_alph
     return 0;
 }
 
+// The RNN-T and CTC-T entries share their checks and launch through `launch` (the two families take the same arguments).
+using RnntFwdLauncher = int (*)(const void *, int, int, int, int, long long, int, int, int, const int *, long long,
+                                const int *, const int *, int, int, void *, float *, float *, cudaStream_t);
+using RnntBwdLauncher = int (*)(const void *, int, int, int, long long, int, const int *, int, void *, const float *, void *,
+                                cudaStream_t);
+using SimpleFwdLauncher = int (*)(const void *, const void *, int, int, int, int, int, const int *, const int *, const int *,
+                                  int, int, void *, float *, cudaStream_t);
+using SimpleBwdLauncher = int (*)(const void *, const void *, int, int, int, int, int, const int *, int, void *, const float *,
+                                  void *, void *, cudaStream_t);
+
+int TransducerForward(const std::string &what, RnntFwdLauncher launch, const void *x, int dtype, int from_logits,
+                             int compact, int N, long rows, int V, int Tmax, int Umax, const int *labels_dev, long n_labels,
+                             const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
+                             float *costs_beta, void *stream) {
+    g_err.clear();
+    if (N <= 0 || rows < 0 || V <= 0 || n_labels < 0) return Fail(what + ": N and V must be positive, rows and n_labels >= 0");
+    if (!KnownDtype(dtype)) return FailDtype(what.c_str(), dtype);
+    if (blank < 0 || blank >= V) return Fail(what + ": blank must lie in [0, V)");
+    if (!compact && (Tmax < 1 || Umax < 0 || rows != (long)N * Tmax * (Umax + 1) || n_labels != (long)N * Umax))
+        return Fail(what + ": the padded layout needs rows = N Tmax (Umax+1) and n_labels = N Umax");
+    if (!x || (n_labels && !labels_dev) || !lx_dev || !ly_dev || !workspace || !costs)
+        return Fail(what + ": missing buffer");
+    const int rc = launch(x, dtype, from_logits, compact, N, rows, V, Tmax, Umax, labels_dev, n_labels, lx_dev, ly_dev, blank,
+                          want_beta, workspace, costs, costs_beta, (cudaStream_t)stream);
+    if (rc) return FailCuda(what.c_str(), (cudaError_t)rc);
+    return 0;
+}
+
+int TransducerBackward(const std::string &what, RnntBwdLauncher launch, const void *x, int dtype, int from_logits, int N,
+                              long rows, int V, const int *labels_dev, int blank, void *workspace, const float *w, void *grad,
+                              void *stream) {
+    g_err.clear();
+    if (N <= 0 || rows < 0 || V <= 0) return Fail(what + ": N and V must be positive, rows >= 0");
+    if (!KnownDtype(dtype)) return FailDtype(what.c_str(), dtype);
+    if (blank < 0 || blank >= V) return Fail(what + ": blank must lie in [0, V)");
+    if ((from_logits && !x) || !workspace || !w || !grad) return Fail(what + ": missing buffer");
+    const int rc = launch(x, dtype, from_logits, N, rows, V, labels_dev, blank, workspace, w, grad, (cudaStream_t)stream);
+    if (rc) return FailCuda(what.c_str(), (cudaError_t)rc);
+    return 0;
+}
+
+int SimpleForward(const std::string &what, SimpleFwdLauncher launch, const void *f, const void *g, int dtype, int N,
+                         int Tmax, int Umax, int V, const int *labels_dev, const int *lx_dev, const int *ly_dev, int blank,
+                         int want_beta, void *workspace, float *costs, void *stream) {
+    g_err.clear();
+    if (N <= 0 || Tmax <= 0 || Umax < 0 || V <= 0) return Fail(what + ": N, Tmax and V must be positive, Umax >= 0");
+    if (N > 65535) return Fail(what + ": at most 65535 utterances per call");
+    if (!KnownDtype(dtype)) return FailDtype(what.c_str(), dtype);
+    if (blank < 0 || blank >= V) return Fail(what + ": blank must lie in [0, V)");
+    if (!f || !g || (Umax && !labels_dev) || !lx_dev || !ly_dev || !workspace || !costs) return Fail(what + ": missing buffer");
+    const int rc = launch(f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev, ly_dev, blank, want_beta, workspace, costs,
+                          (cudaStream_t)stream);
+    if (rc) return FailCuda(what.c_str(), (cudaError_t)rc);
+    return 0;
+}
+
+int SimpleBackward(const std::string &what, SimpleBwdLauncher launch, const void *f, const void *g, int dtype, int N,
+                          int Tmax, int Umax, int V, const int *labels_dev, int blank, void *workspace, const float *w,
+                          void *grad_f, void *grad_g, void *stream) {
+    g_err.clear();
+    if (N <= 0 || Tmax <= 0 || Umax < 0 || V <= 0) return Fail(what + ": N, Tmax and V must be positive, Umax >= 0");
+    if (N > 65535) return Fail(what + ": at most 65535 utterances per call");
+    if (!KnownDtype(dtype)) return FailDtype(what.c_str(), dtype);
+    if (blank < 0 || blank >= V) return Fail(what + ": blank must lie in [0, V)");
+    if (!f || !g || (Umax && !labels_dev) || !workspace || !w || !grad_f || !grad_g) return Fail(what + ": missing buffer");
+    const int rc = launch(f, g, dtype, N, Tmax, Umax, V, labels_dev, blank, workspace, w, grad_f, grad_g, (cudaStream_t)stream);
+    if (rc) return FailCuda(what.c_str(), (cudaError_t)rc);
+    return 0;
+}
+
 }  // namespace
 
 namespace ccb {
@@ -1294,31 +1364,14 @@ size_t ccb_rnnt_workspace_bytes(int N, long rows) { return N > 0 && rows >= 0 ? 
 int ccb_rnnt_forward(const void *x, int dtype, int from_logits, int compact, int N, long rows, int V, int Tmax, int Umax,
                      const int *labels_dev, long n_labels, const int *lx_dev, const int *ly_dev, int blank, int want_beta,
                      void *workspace, float *costs, float *costs_beta, void *stream) {
-    g_err.clear();
-    if (N <= 0 || rows < 0 || V <= 0 || n_labels < 0) return Fail("rnnt_forward: N and V must be positive, rows and n_labels >= 0");
-    if (!KnownDtype(dtype)) return FailDtype("rnnt_forward", dtype);
-    if (blank < 0 || blank >= V) return Fail("rnnt_forward: blank must lie in [0, V)");
-    if (!compact && (Tmax < 1 || Umax < 0 || rows != (long)N * Tmax * (Umax + 1) || n_labels != (long)N * Umax))
-        return Fail("rnnt_forward: the padded layout needs rows = N Tmax (Umax+1) and n_labels = N Umax");
-    if (!x || (n_labels && !labels_dev) || !lx_dev || !ly_dev || !workspace || !costs)
-        return Fail("rnnt_forward: missing buffer");
-    const int rc = LaunchRnntForward(x, dtype, from_logits, compact, N, rows, V, Tmax, Umax, labels_dev, n_labels, lx_dev,
-                                     ly_dev, blank, want_beta, workspace, costs, costs_beta, (cudaStream_t)stream);
-    if (rc) return FailCuda("rnnt_forward", (cudaError_t)rc);
-    return 0;
+    return TransducerForward("rnnt_forward", LaunchRnntForward, x, dtype, from_logits, compact, N, rows, V, Tmax, Umax,
+                             labels_dev, n_labels, lx_dev, ly_dev, blank, want_beta, workspace, costs, costs_beta, stream);
 }
 
 int ccb_rnnt_backward(const void *x, int dtype, int from_logits, int N, long rows, int V, const int *labels_dev, int blank,
                       void *workspace, const float *w, void *grad, void *stream) {
-    g_err.clear();
-    if (N <= 0 || rows < 0 || V <= 0) return Fail("rnnt_backward: N and V must be positive, rows >= 0");
-    if (!KnownDtype(dtype)) return FailDtype("rnnt_backward", dtype);
-    if (blank < 0 || blank >= V) return Fail("rnnt_backward: blank must lie in [0, V)");
-    if ((from_logits && !x) || !workspace || !w || !grad) return Fail("rnnt_backward: missing buffer");
-    const int rc = LaunchRnntBackward(x, dtype, from_logits, N, rows, V, labels_dev, blank, workspace, w, grad,
-                                      (cudaStream_t)stream);
-    if (rc) return FailCuda("rnnt_backward", (cudaError_t)rc);
-    return 0;
+    return TransducerBackward("rnnt_backward", LaunchRnntBackward, x, dtype, from_logits, N, rows, V, labels_dev, blank,
+                              workspace, w, grad, stream);
 }
 
 size_t ccb_rnnt_simple_workspace_bytes(int N, int Tmax, int Umax) {
@@ -1328,34 +1381,46 @@ size_t ccb_rnnt_simple_workspace_bytes(int N, int Tmax, int Umax) {
 int ccb_rnnt_simple_forward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
                             const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
                             void *stream) {
-    g_err.clear();
-    if (N <= 0 || Tmax <= 0 || Umax < 0 || V <= 0)
-        return Fail("rnnt_simple_forward: N, Tmax and V must be positive, Umax >= 0");
-    if (N > 65535) return Fail("rnnt_simple_forward: at most 65535 utterances per call");
-    if (!KnownDtype(dtype)) return FailDtype("rnnt_simple_forward", dtype);
-    if (blank < 0 || blank >= V) return Fail("rnnt_simple_forward: blank must lie in [0, V)");
-    if (!f || !g || (Umax && !labels_dev) || !lx_dev || !ly_dev || !workspace || !costs)
-        return Fail("rnnt_simple_forward: missing buffer");
-    const int rc = LaunchRnntSimpleForward(f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev, ly_dev, blank, want_beta,
-                                           workspace, costs, (cudaStream_t)stream);
-    if (rc) return FailCuda("rnnt_simple_forward", (cudaError_t)rc);
-    return 0;
+    return SimpleForward("rnnt_simple_forward", LaunchRnntSimpleForward, f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev,
+                         ly_dev, blank, want_beta, workspace, costs, stream);
 }
 
 int ccb_rnnt_simple_backward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
                              int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream) {
-    g_err.clear();
-    if (N <= 0 || Tmax <= 0 || Umax < 0 || V <= 0)
-        return Fail("rnnt_simple_backward: N, Tmax and V must be positive, Umax >= 0");
-    if (N > 65535) return Fail("rnnt_simple_backward: at most 65535 utterances per call");
-    if (!KnownDtype(dtype)) return FailDtype("rnnt_simple_backward", dtype);
-    if (blank < 0 || blank >= V) return Fail("rnnt_simple_backward: blank must lie in [0, V)");
-    if (!f || !g || (Umax && !labels_dev) || !workspace || !w || !grad_f || !grad_g)
-        return Fail("rnnt_simple_backward: missing buffer");
-    const int rc = LaunchRnntSimpleBackward(f, g, dtype, N, Tmax, Umax, V, labels_dev, blank, workspace, w, grad_f, grad_g,
-                                            (cudaStream_t)stream);
-    if (rc) return FailCuda("rnnt_simple_backward", (cudaError_t)rc);
-    return 0;
+    return SimpleBackward("rnnt_simple_backward", LaunchRnntSimpleBackward, f, g, dtype, N, Tmax, Umax, V, labels_dev, blank,
+                          workspace, w, grad_f, grad_g, stream);
+}
+
+size_t ccb_ctct_workspace_bytes(int N, long rows) { return N > 0 && rows >= 0 ? CtctWsBytes(N, rows) : 0; }
+
+int ccb_ctct_forward(const void *x, int dtype, int from_logits, int compact, int N, long rows, int V, int Tmax, int Umax,
+                     const int *labels_dev, long n_labels, const int *lx_dev, const int *ly_dev, int blank, int want_beta,
+                     void *workspace, float *costs, float *costs_beta, void *stream) {
+    return TransducerForward("ctct_forward", LaunchCtctForward, x, dtype, from_logits, compact, N, rows, V, Tmax, Umax,
+                             labels_dev, n_labels, lx_dev, ly_dev, blank, want_beta, workspace, costs, costs_beta, stream);
+}
+
+int ccb_ctct_backward(const void *x, int dtype, int from_logits, int N, long rows, int V, const int *labels_dev, int blank,
+                      void *workspace, const float *w, void *grad, void *stream) {
+    return TransducerBackward("ctct_backward", LaunchCtctBackward, x, dtype, from_logits, N, rows, V, labels_dev, blank,
+                              workspace, w, grad, stream);
+}
+
+size_t ccb_ctct_simple_workspace_bytes(int N, int Tmax, int Umax) {
+    return N > 0 && Tmax > 0 && Umax >= 0 ? CtctSimpleWsBytes(N, Tmax, Umax) : 0;
+}
+
+int ccb_ctct_simple_forward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
+                            const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
+                            void *stream) {
+    return SimpleForward("ctct_simple_forward", LaunchCtctSimpleForward, f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev,
+                         ly_dev, blank, want_beta, workspace, costs, stream);
+}
+
+int ccb_ctct_simple_backward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
+                             int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream) {
+    return SimpleBackward("ctct_simple_backward", LaunchCtctSimpleBackward, f, g, dtype, N, Tmax, Umax, V, labels_dev, blank,
+                          workspace, w, grad_f, grad_g, stream);
 }
 
 size_t ccb_gather_ws_bytes(int N) { return N > 0 ? GatherWsBytes(N) : 0; }

@@ -284,6 +284,20 @@ int LaunchRnntSimpleForward(const void *f, const void *g, int dtype, int N, int 
                             const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s);
 int LaunchRnntSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
                              int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s);
+// CTC-T loss (rnnt_kernels.cu), with the arguments of the RNN-T entries above: the forward runs the prep, row (with lpr) and
+// the frame-synchronous alpha (|| beta) passes, the backward the gradient pass, over CtctWsBytes(N, rows) bytes; the LogAdd
+// joiner's CTC-T loss runs the simple loss's passes with the CTC-T lattice over CtctSimpleWsBytes(N, Tmax, Umax) bytes.
+size_t CtctWsBytes(int N, long long rows);
+int LaunchCtctForward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
+                      const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
+                      float *costs, float *costs_beta, cudaStream_t s);
+int LaunchCtctBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
+                       void *ws, const float *w, void *grad, cudaStream_t s);
+size_t CtctSimpleWsBytes(int N, int Tmax, int Umax);
+int LaunchCtctSimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                            const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s);
+int LaunchCtctSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                             int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s);
 // gather.sum of the joiner and its backward; ws: GatherWsBytes(N) bytes of per-utterance offsets
 size_t GatherWsBytes(int N);
 int LaunchGatherSum(const void *a, const void *b, int dtype, int N, long long rows_out, int H, const int *la, const int *lb,

@@ -26,19 +26,23 @@ struct RnntMeta {
 };
 
 struct RnntLayout {
-    size_t meta, tail, logp, alpha, beta, lpb, lpl, lse, total;
+    size_t meta, tail, logp, alpha, beta, lpb, lpl, lpr, lse, total;
 };
 
-RnntLayout MakeRnntLayout(int N, long long rows) {
+// ctct: the CTC-T loss's workspace, with two cells per row in each direction and the lpr block (lpr = 0 otherwise)
+RnntLayout MakeRnntLayout(int N, long long rows, bool ctct = false) {
+    const size_t states = ctct ? 2 : 1;
     RnntLayout L;
     size_t o = 0;
     L.meta = o;  o += Align256(sizeof(RnntMeta) * (size_t)N);
     L.tail = o;  o += 256;
     L.logp = o;  o += Align256(2 * sizeof(double) * (size_t)N);   // from alpha, then from beta
-    L.alpha = o; o += Align256(sizeof(double) * (size_t)rows);
-    L.beta = o;  o += Align256(sizeof(double) * (size_t)rows);
+    L.alpha = o; o += Align256(states * sizeof(double) * (size_t)rows);
+    L.beta = o;  o += Align256(states * sizeof(double) * (size_t)rows);
     L.lpb = o;   o += Align256(sizeof(float) * (size_t)rows);
     L.lpl = o;   o += Align256(sizeof(float) * (size_t)rows);
+    L.lpr = 0;
+    if (ctct) { L.lpr = o; o += Align256(sizeof(float) * (size_t)rows); }
     L.lse = o;   o += Align256(sizeof(float) * (size_t)rows);
     L.total = o;
     return L;
@@ -178,9 +182,18 @@ __global__ void __launch_bounds__(kPrepThreads) rnnt_prep_kernel(const int *lx, 
 // Row pass.  Grid (row chunk, utterance): CTA (x, n) walks the rows t < T_n, u <= U_n of utterance n with stride gridDim.x.
 // lpb = log p(blank), lpl = log p(y_{u+1}) (u < U_n); raw logits: minus the row's logsumexp, which is kept in lse.
 // A label outside [0, V) or equal to blank marks the utterance bad (every writer writes 1; no atomics needed).
+// CTCT (the CTC-T loss) also writes lpr = log p(y_u) (u >= 1), the repeat of the last label, read at the same row.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kRowThreads) rnnt_lp_rows_kernel(const void *x, int dtype, long long V, const int *labels,
-                                                                   int blank, RnntMeta *meta, float *lpb, float *lpl) {
+// lp(row, y) - l for a label y of the utterance, or NaN (and the utterance marked bad) for an invalid one
+__device__ __forceinline__ float LabelLp(const void *x, int dtype, long long V, long long row, int y, int blank, float l,
+                                         RnntMeta *meta, int n) {
+    if (y < 0 || y >= V || y == blank) { meta[n].bad = 1; return NAN; }
+    return load_y(x, dtype, row * V + y) - l;
+}
+
+template <bool CTCT>
+__device__ __forceinline__ void LpRows(const void *x, int dtype, long long V, const int *labels, int blank, RnntMeta *meta,
+                                       float *lpb, float *lpl, float *lpr) {
     const int n = blockIdx.y;
     const RnntMeta m = meta[n];
     if (m.bad) return;
@@ -196,12 +209,26 @@ __global__ void __launch_bounds__(kRowThreads) rnnt_lp_rows_kernel(const void *x
             if (y < 0 || y >= V || y == blank) { meta[n].bad = 1; lpl[row] = NAN; }
             else lpl[row] = load_y(x, dtype, row * V + y);
         }
+        if constexpr (CTCT) {
+            if (u > 0) lpr[row] = LabelLp(x, dtype, V, row, labels[m.loff + u - 1], blank, 0.f, meta, n);
+        }
     }
 }
 
-template <int DT, bool VEC>
-__global__ void __launch_bounds__(kRowThreads) rnnt_logit_rows_kernel(const void *x, long long V, const int *labels, int blank,
-                                                                      RnntMeta *meta, float *lpb, float *lpl, float *lse) {
+__global__ void __launch_bounds__(kRowThreads) rnnt_lp_rows_kernel(const void *x, int dtype, long long V, const int *labels,
+                                                                   int blank, RnntMeta *meta, float *lpb, float *lpl) {
+    LpRows<false>(x, dtype, V, labels, blank, meta, lpb, lpl, nullptr);
+}
+
+__global__ void __launch_bounds__(kRowThreads) ctct_lp_rows_kernel(const void *x, int dtype, long long V, const int *labels,
+                                                                   int blank, RnntMeta *meta, float *lpb, float *lpl,
+                                                                   float *lpr) {
+    LpRows<true>(x, dtype, V, labels, blank, meta, lpb, lpl, lpr);
+}
+
+template <int DT, bool VEC, bool CTCT>
+__device__ __forceinline__ void LogitRows(const void *x, long long V, const int *labels, int blank, RnntMeta *meta, float *lpb,
+                                          float *lpl, float *lpr, float *lse) {
     constexpr int K = ChunkElems<DT, VEC>();
     const int n = blockIdx.y;
     const RnntMeta m = meta[n];
@@ -239,8 +266,24 @@ __global__ void __launch_bounds__(kRowThreads) rnnt_logit_rows_kernel(const void
                 if (y < 0 || y >= V || y == blank) { meta[n].bad = 1; lpl[row] = NAN; }
                 else lpl[row] = load_y(x, DT, base + y) - l;
             }
+            if constexpr (CTCT) {
+                if (u > 0) lpr[row] = LabelLp(x, DT, V, row, labels[m.loff + u - 1], blank, l, meta, n);
+            }
         }
     }
+}
+
+template <int DT, bool VEC>
+__global__ void __launch_bounds__(kRowThreads) rnnt_logit_rows_kernel(const void *x, long long V, const int *labels, int blank,
+                                                                      RnntMeta *meta, float *lpb, float *lpl, float *lse) {
+    LogitRows<DT, VEC, false>(x, V, labels, blank, meta, lpb, lpl, nullptr, lse);
+}
+
+template <int DT, bool VEC>
+__global__ void __launch_bounds__(kRowThreads) ctct_logit_rows_kernel(const void *x, long long V, const int *labels, int blank,
+                                                                      RnntMeta *meta, float *lpb, float *lpl, float *lpr,
+                                                                      float *lse) {
+    LogitRows<DT, VEC, true>(x, V, labels, blank, meta, lpb, lpl, lpr, lse);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -320,6 +363,115 @@ __device__ __forceinline__ void CellPosteriors(const RnntMeta &m, long long row,
 }
 
 // ------------------------------------------------------------------------------------------------
+// CTC-T alpha / beta pass (DESIGN.md §7 "CTC-T loss"): CTA (n, 0) runs alpha, CTA (n, 1) beta, frame by frame, threads over
+// u, each thread both states of its u; one CTA barrier per frame.  Two fp64 cells per row and direction: state b (u labels,
+// the last emission blank or nothing) at cell[2 row], state l (the last emission y_u) at cell[2 row + 1].  Row (t, u) keeps
+// alpha_t(u, .), the states before frame t, and beta_{t+1}(u, .), the states after it:
+//   alpha_{t+1}(u,b) = [alpha_t(u,b) + alpha_t(u,l)] lpb(t,u)
+//   alpha_{t+1}(u,l) = alpha_t(u,l) lpr(t,u) + [alpha_t(u-1,b) + alpha_t(u-1,l) if u = 1 or y_u != y_{u-1}] lpl(t,u-1)
+//   beta_t(u,b) = beta_{t+1}(u,b) lpb(t,u) + beta_{t+1}(u+1,l) lpl(t,u)
+//   beta_t(u,l) = beta_{t+1}(u,b) lpb(t,u) + beta_{t+1}(u,l) lpr(t,u) + [beta_{t+1}(u+1,l) lpl(t,u) if y_{u+1} != y_u]
+// (+ is logaddexp, juxtaposition a product of probabilities), alpha_0(0,b) = 0, beta_T(U,.) = 0, every other boundary cell
+// -inf, and log P = alpha_T(U,b) + alpha_T(U,l) = beta_0(0,b).  An infeasible utterance gets log P = -inf, cost +inf.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kAbThreads) ctct_alpha_beta_kernel(const RnntMeta *meta, const int *labels, const float *lpb,
+                                                                     const float *lpl, const float *lpr, double *alpha,
+                                                                     double *beta, double *logp, int N, float *costs,
+                                                                     float *costs_beta) {
+    const int n = blockIdx.x;
+    const bool bwd = blockIdx.y == 1;
+    const RnntMeta m = meta[n];
+    if (m.bad) {
+        if (threadIdx.x == 0) {
+            logp[bwd ? N + n : n] = NAN;
+            if (bwd) { if (costs_beta) costs_beta[n] = NAN; }
+            else costs[n] = NAN;
+        }
+        return;
+    }
+    const int T = m.T, U = m.U;
+    const long long ts = m.ts, off = m.roff;
+    const int *y = labels + m.loff;     // y[u - 1] = y_u
+    double *cell = bwd ? beta : alpha;
+    double eb = -INFINITY, el = -INFINITY;   // the end state the thread owning u = U (alpha) or u = 0 (beta) returns
+    if (!bwd) {
+        for (int u = threadIdx.x; u <= U; u += blockDim.x) {
+            cell[2 * (off + u)] = u == 0 ? 0.0 : -INFINITY;
+            cell[2 * (off + u) + 1] = -INFINITY;
+        }
+        __syncthreads();
+        for (int t = 0; t < T; ++t) {
+            for (int u = threadIdx.x; u <= U; u += blockDim.x) {
+                const long long r = off + t * ts + u;
+                const double ab = cell[2 * r], al = cell[2 * r + 1];
+                const double nb = LogAddD(ab, al) + (double)lpb[r];
+                double nl = -INFINITY;
+                if (u > 0) {
+                    const double pb = cell[2 * (r - 1)], pl = cell[2 * (r - 1) + 1];
+                    const double src = u == 1 || y[u - 1] != y[u - 2] ? LogAddD(pb, pl) : pb;
+                    nl = LogAddD(al + (double)lpr[r], src + (double)lpl[r - 1]);
+                }
+                if (t + 1 < T) { cell[2 * (r + ts)] = nb; cell[2 * (r + ts) + 1] = nl; }
+                else if (u == U) { eb = nb; el = nl; }
+            }
+            __syncthreads();
+        }
+        if (threadIdx.x == U % blockDim.x) {
+            const double lp = LogAddD(eb, el);
+            logp[n] = lp;
+            costs[n] = (float)-lp;
+        }
+    } else {
+        for (int u = threadIdx.x; u <= U; u += blockDim.x) {
+            const long long r = off + (T - 1) * ts + u;
+            cell[2 * r] = u == U ? 0.0 : -INFINITY;
+            cell[2 * r + 1] = u == U && U > 0 ? 0.0 : -INFINITY;
+        }
+        __syncthreads();
+        for (int t = T - 1; t >= 0; --t) {
+            for (int u = threadIdx.x; u <= U; u += blockDim.x) {
+                const long long r = off + t * ts + u;
+                const double xb = cell[2 * r] + (double)lpb[r];
+                const double xn = u < U ? cell[2 * (r + 1) + 1] + (double)lpl[r] : -INFINITY;
+                const double nb = LogAddD(xb, xn);
+                double nl = -INFINITY;
+                if (u > 0) {
+                    nl = LogAddD(xb, cell[2 * r + 1] + (double)lpr[r]);
+                    if (u < U && y[u] != y[u - 1]) nl = LogAddD(nl, xn);
+                }
+                if (t > 0) { cell[2 * (r - ts)] = nb; cell[2 * (r - ts) + 1] = nl; }
+                else if (u == 0) eb = nb;
+            }
+            __syncthreads();
+        }
+        if (threadIdx.x == 0) {
+            logp[N + n] = eb;
+            if (costs_beta) costs_beta[n] = (float)-eb;
+        }
+    }
+}
+
+// The weighted posteriors of the three CTC-T transitions that read live row (t, u) at workspace row `row`: pb (blank, into
+// (u,b)), pr (the repeat of y_u, into (u,l), u >= 1) and pl (y_{u+1}, into (u+1,l), u < U; from (u,l) too unless
+// y_{u+1} = y_u).  All zero when log P = -inf (no path).  Shared by the gradient pass and the LogAdd joiner's cell weights.
+__device__ __forceinline__ void CtctPosteriors(const RnntMeta &m, const int *labels, long long row, int u, const double *alpha,
+                                               const double *beta, const float *lpb, const float *lpl, const float *lpr,
+                                               double lP, float wn, float &pb, float &pr, float &pl) {
+    pb = 0.f; pr = 0.f; pl = 0.f;
+    if (lP == -INFINITY) return;
+    const double ab = alpha[2 * row], al = alpha[2 * row + 1];   // the two source states, summed as probabilities
+    const double cb = (double)lpb[row] + beta[2 * row] - lP;
+    pb = (float)(exp(ab + cb) + exp(al + cb));
+    if (u > 0) pr = (float)exp(al + (double)lpr[row] + beta[2 * row + 1] - lP);
+    if (u < m.U) {
+        const bool rep = u > 0 && labels[m.loff + u] == labels[m.loff + u - 1];
+        const double cl = (double)lpl[row] + beta[2 * (row + 1) + 1] - lP;
+        pl = (float)(exp(ab + cl) + (rep ? 0.0 : exp(al + cl)));
+    }
+    pb *= wn; pr *= wn; pl *= wn;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Gradient pass: one warp per row, every row of the tensor written once.  Grid (row chunk, N + 1): CTA (x, n < N) walks
 // utterance n's span (rows outside t < T_n, u <= U_n, and every row of a bad utterance, get zeros and are not read);
 // CTA (x, N) zeroes the compact tail behind the last utterance.  With w = w_n,
@@ -375,6 +527,73 @@ __global__ void __launch_bounds__(kRowThreads) rnnt_grad_kernel(const void *x, l
                 for (int i = 0; i < K; ++i) {
                     const long long k = c * K + i;
                     if (k == blank) v[i] -= pb;
+                    if (k == y) v[i] -= pl;
+                }
+            }
+            StoreChunk<DT, VEC>(grad, base, c, v);
+        }
+    }
+}
+
+// CTC-T gradient pass: the RNN-T gradient pass with pb, pr and pl from CtctPosteriors,
+//   grad[k] = [raw: exp(z_k - lse) (pb + pr + pl)] - pb [k == blank] - pr [k == y_u] - pl [k == y_{u+1}],
+// where y_u = y_{u+1} puts both label terms on one element, in that order.
+template <int DT, bool VEC, bool RAW>
+__global__ void __launch_bounds__(kRowThreads) ctct_grad_kernel(const void *x, long long V, const int *labels, int blank, int N,
+                                                                const RnntMeta *meta, const long long *tail, long long rows,
+                                                                const double *alpha, const double *beta, const double *logp,
+                                                                const float *lpb, const float *lpl, const float *lpr,
+                                                                const float *lse, const float *w, void *grad) {
+    constexpr int K = ChunkElems<DT, VEC>();
+    const int n = blockIdx.y;
+    const bool utt = n < N;
+    RnntMeta m{};
+    long long first, count;
+    if (utt) { m = meta[n]; first = m.roff; count = m.span; }
+    else { first = *tail; count = rows - first; }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;
+    const long long chunks = V / K;
+    const float wn = utt && !m.bad ? w[n] : 0.f;
+    const double lP = utt && !m.bad ? logp[n] : 0.0;
+    // (t, u) of row r stepped along with r in 32-bit arithmetic: a 64-bit division here is a subroutine call, and the call
+    // costs this kernel its registers (spills)
+    const unsigned ts = utt ? (unsigned)m.ts : 1u, r0 = blockIdx.x * W + warp, step = gridDim.x * W;
+    const unsigned dt = step / ts, du = step % ts;
+    long long t = r0 / ts;
+    unsigned uq = r0 % ts;
+    for (long long r = r0; r < count; r += step, t += dt, uq += du) {
+        if (uq >= ts) { uq -= ts; ++t; }
+        const long long row = first + r, base = row * V;
+        float pb = 0.f, pr = 0.f, pl = 0.f, l = 0.f;
+        int y = -1, yr = -1;
+        bool live = false;
+        if (utt && !m.bad) {
+            const int u = (int)uq;
+            if (t < m.T && u <= m.U) {
+                live = true;
+                CtctPosteriors(m, labels, row, u, alpha, beta, lpb, lpl, lpr, lP, wn, pb, pr, pl);
+                if (u > 0) yr = labels[m.loff + u - 1];
+                if (u < m.U) y = labels[m.loff + u];
+                if constexpr (RAW) l = lse[row];
+            }
+        }
+        const float occ = pb + pr + pl;
+        for (long long c = lane; c < chunks; c += 32) {
+            float v[K];
+            if (RAW && live) {
+                LoadChunk<DT, VEC>(x, base, c, v);
+#pragma unroll
+                for (int i = 0; i < K; ++i) v[i] = __expf(v[i] - l) * occ;
+            } else {
+#pragma unroll
+                for (int i = 0; i < K; ++i) v[i] = 0.f;
+            }
+            if (live) {
+#pragma unroll
+                for (int i = 0; i < K; ++i) {
+                    const long long k = c * K + i;
+                    if (k == blank) v[i] -= pb;
+                    if (k == yr) v[i] -= pr;
                     if (k == y) v[i] -= pl;
                 }
             }
@@ -450,14 +669,14 @@ __device__ __forceinline__ bool SimpleFlagged(float s) { return !(s >= kSimpleTi
 __device__ __forceinline__ float SimpleOffset(float m) { return m == -INFINITY ? 0.f : m; }
 
 struct SimpleLayout {
-    RnntLayout r;                                  // meta .. lse over the N Tmax (Umax+1) cells; lse holds Z
-    size_t mf, mg, ff, fg, S, W, PB, PL, total;    // row maxima and "row has a flagged cell" of f and g; per cell S, W, pb, pl
-};
+    RnntLayout r;                                     // meta .. lse over the N Tmax (Umax+1) cells; lse holds Z
+    size_t mf, mg, ff, fg, S, W, PB, PL, PR, total;   // row maxima and "row has a flagged cell" of f and g; per cell S, W,
+};                                                    // pb, pl (and pr for the CTC-T loss; PR = 0 otherwise)
 
-SimpleLayout MakeSimpleLayout(int N, int Tmax, int Umax) {
+SimpleLayout MakeSimpleLayout(int N, int Tmax, int Umax, bool ctct = false) {
     const size_t nf = (size_t)N * Tmax, ng = (size_t)N * (Umax + 1), cells = nf * (Umax + 1);
     SimpleLayout L;
-    L.r = MakeRnntLayout(N, (long long)cells);
+    L.r = MakeRnntLayout(N, (long long)cells, ctct);
     size_t o = L.r.total;
     L.mf = o; o += Align256(sizeof(float) * nf);
     L.mg = o; o += Align256(sizeof(float) * ng);
@@ -467,6 +686,8 @@ SimpleLayout MakeSimpleLayout(int N, int Tmax, int Umax) {
     L.W = o;  o += Align256(sizeof(float) * cells);
     L.PB = o; o += Align256(sizeof(float) * cells);
     L.PL = o; o += Align256(sizeof(float) * cells);
+    L.PR = 0;
+    if (ctct) { L.PR = o; o += Align256(sizeof(float) * cells); }
     L.total = o;
     return L;
 }
@@ -506,12 +727,13 @@ __global__ void __launch_bounds__(kRowThreads) simple_rowmax_kernel(const void *
 // thread a 4 x 2 block of cells in fp32 FFMA.  Tiles wholly past T_n or U_n + 1 return at once.  Epilogue per live cell: S;
 // the label check (a label outside [0, V) or equal to blank marks the utterance bad, as the row pass does); then for an
 // unflagged cell Z (in lse), lpb = z(blank) - Z and lpl = z(y_{u+1}) - Z, and for a flagged one the flags of rows t and u.
+// CTCT also writes lpr = z(y_u) - Z (u >= 1) for an unflagged cell; an invalid y_u is skipped here (the cell of u - 1
+// marks the utterance bad).
 constexpr int kST = 64, kSU = 32, kSK = 32;
-template <int DT>
-__global__ void __launch_bounds__(256) simple_norm_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
-                                                          const int *labels, int blank, RnntMeta *meta, const float *mf,
-                                                          const float *mg, int *ff, int *fg, float *S, float *lpb, float *lpl,
-                                                          float *lse) {
+template <int DT, bool CTCT>
+__device__ __forceinline__ void SimpleNorm(const void *f, const void *g, long long V, int Tmax, int Umax, const int *labels,
+                                           int blank, RnntMeta *meta, const float *mf, const float *mg, int *ff, int *fg,
+                                           float *S, float *lpb, float *lpl, float *lpr, float *lse) {
     const int n = blockIdx.z;
     const RnntMeta m = meta[n];
     const int t0 = blockIdx.x * kST, u0 = blockIdx.y * kSU;
@@ -573,17 +795,38 @@ __global__ void __launch_bounds__(256) simple_norm_kernel(const void *f, const v
             lse[row] = Z;
             lpb[row] = (load_y(f, DT, fb + blank) + load_y(g, DT, gb + blank)) - Z;
             if (y >= 0) lpl[row] = (load_y(f, DT, fb + y) + load_y(g, DT, gb + y)) - Z;
+            if constexpr (CTCT) {
+                if (u > 0) {
+                    const int yr = labels[m.loff + u - 1];
+                    if (yr >= 0 && yr < V && yr != blank) lpr[row] = (load_y(f, DT, fb + yr) + load_y(g, DT, gb + yr)) - Z;
+                }
+            }
         }
     }
 }
 
+template <int DT>
+__global__ void __launch_bounds__(256) simple_norm_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                          const int *labels, int blank, RnntMeta *meta, const float *mf,
+                                                          const float *mg, int *ff, int *fg, float *S, float *lpb, float *lpl,
+                                                          float *lse) {
+    SimpleNorm<DT, false>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, nullptr, lse);
+}
+
+template <int DT>
+__global__ void __launch_bounds__(256) ctct_simple_norm_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                               const int *labels, int blank, RnntMeta *meta, const float *mf,
+                                                               const float *mg, int *ff, int *fg, float *S, float *lpb,
+                                                               float *lpl, float *lpr, float *lse) {
+    SimpleNorm<DT, true>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, lpr, lse);
+}
+
 // Underflow fix-up: one warp per flagged cell (rows t without a flagged cell are skipped by their flag) takes the exact
-// logsumexp of f[t] + g[u] by an online max / sum, and rewrites Z, lpb and lpl.
-template <int DT, bool VEC>
-__global__ void __launch_bounds__(kRowThreads) simple_fixup_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
-                                                                   const int *labels, int blank, const RnntMeta *meta,
-                                                                   const int *ff, const float *S, float *lpb, float *lpl,
-                                                                   float *lse) {
+// logsumexp of f[t] + g[u] by an online max / sum, and rewrites Z, lpb and lpl (and lpr when CTCT).
+template <int DT, bool VEC, bool CTCT>
+__device__ __forceinline__ void SimpleFixup(const void *f, const void *g, long long V, int Tmax, int Umax, const int *labels,
+                                            int blank, const RnntMeta *meta, const int *ff, const float *S, float *lpb,
+                                            float *lpl, float *lpr, float *lse) {
     constexpr int K = ChunkElems<DT, VEC>();
     const int n = blockIdx.y;
     const RnntMeta m = meta[n];
@@ -623,8 +866,30 @@ __global__ void __launch_bounds__(kRowThreads) simple_fixup_kernel(const void *f
                 const int y = labels[m.loff + u];
                 lpl[row] = (load_y(f, DT, fb + y) + load_y(g, DT, gb + y)) - Z;
             }
+            if constexpr (CTCT) {
+                if (u > 0) {
+                    const int y = labels[m.loff + u - 1];
+                    lpr[row] = (load_y(f, DT, fb + y) + load_y(g, DT, gb + y)) - Z;
+                }
+            }
         }
     }
+}
+
+template <int DT, bool VEC>
+__global__ void __launch_bounds__(kRowThreads) simple_fixup_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                                   const int *labels, int blank, const RnntMeta *meta,
+                                                                   const int *ff, const float *S, float *lpb, float *lpl,
+                                                                   float *lse) {
+    SimpleFixup<DT, VEC, false>(f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, nullptr, lse);
+}
+
+template <int DT, bool VEC>
+__global__ void __launch_bounds__(kRowThreads) ctct_simple_fixup_kernel(const void *f, const void *g, long long V, int Tmax,
+                                                                        int Umax, const int *labels, int blank,
+                                                                        const RnntMeta *meta, const int *ff, const float *S,
+                                                                        float *lpb, float *lpl, float *lpr, float *lse) {
+    SimpleFixup<DT, VEC, true>(f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, lpr, lse);
 }
 
 // Cell weights: per live cell pb, pl (weighted posteriors, as the gradient pass) and W = (pb + pl) / S, 0 for a flagged cell.
@@ -652,19 +917,47 @@ __global__ void __launch_bounds__(kRowThreads) simple_weights_kernel(const RnntM
     }
 }
 
+// CTC-T cell weights: per live cell pb, pr, pl (CtctPosteriors) and W = (pb + pr + pl) / S, 0 for a flagged cell.
+__global__ void __launch_bounds__(kRowThreads) ctct_simple_weights_kernel(const RnntMeta *meta, const int *labels,
+                                                                          const double *alpha, const double *beta,
+                                                                          const double *logp, const float *lpb,
+                                                                          const float *lpl, const float *lpr, const float *S,
+                                                                          const float *w, float *W, float *PB, float *PL,
+                                                                          float *PR) {
+    const int n = blockIdx.y;
+    const RnntMeta m = meta[n];
+    if (m.bad) return;
+    const float wn = w[n];
+    const double lP = logp[n];
+    const long long live = (long long)m.T * m.ts;
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < live; r += (long long)gridDim.x * blockDim.x) {
+        const long long t = r / m.ts;
+        const int u = (int)(r - t * m.ts);
+        if (u > m.U) continue;
+        const long long row = m.roff + r;
+        float pb, pr, pl;
+        CtctPosteriors(m, labels, row, u, alpha, beta, lpb, lpl, lpr, lP, wn, pb, pr, pl);
+        const float s = S[row];
+        PB[row] = pb;
+        PR[row] = pr;
+        PL[row] = pl;
+        W[row] = SimpleFlagged(s) ? 0.f : (pb + pr + pl) / s;
+    }
+}
+
 // Gradient GEMM.  GF: grad_f, output rows r = t and reduction q = u; else grad_g, r = u and q = t.  With "own" the input
 // whose gradient is written and "other" the one summed over,
 //   grad[r,k] = E_own[r,k] sum_q W(r,q) E_other[q,k]  +  sum_{q flagged} (pb + pl) exp(z - Z)
 //               - [k = blank] sum_q pb  -  sum_q pl [k = y_{u+1}],
 // each sum over increasing q in fp32.  CTA (k tile, r tile, n) writes its whole kGR x kGC block: rows past the utterance (and
-// every row of a bad utterance) get zeros and are not read.
+// every row of a bad utterance) get zeros and are not read.  CTCT: the flagged cells' occupancy is pb + pl + pr, and after
+// the label terms above come - sum_q pr [k = y_u] (u >= 1), in increasing q.
 constexpr int kGR = 64, kGC = 64, kGQ = 16;
-template <int DT, bool GF>
-__global__ void __launch_bounds__(256) simple_grad_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
-                                                          const int *labels, int blank, const RnntMeta *meta, const float *mf,
-                                                          const float *mg, const int *ff, const int *fg, const float *S,
-                                                          const float *lse, const float *W, const float *PB, const float *PL,
-                                                          void *grad) {
+template <int DT, bool GF, bool CTCT>
+__device__ __forceinline__ void SimpleGrad(const void *f, const void *g, long long V, int Tmax, int Umax, const int *labels,
+                                           int blank, const RnntMeta *meta, const float *mf, const float *mg, const int *ff,
+                                           const int *fg, const float *S, const float *lse, const float *W, const float *PB,
+                                           const float *PL, const float *PR, void *grad) {
     const int n = blockIdx.z;
     const RnntMeta m = meta[n];
     const int U1 = Umax + 1, Rmax = GF ? Tmax : U1;
@@ -729,7 +1022,7 @@ __global__ void __launch_bounds__(256) simple_grad_kernel(const void *f, const v
             for (int q = 0; q < Qn; ++q) {
                 const long long c = cell(r, q);
                 if (!SimpleFlagged(S[c])) continue;
-                const float occ = PB[c] + PL[c], Z = lse[c];
+                const float occ = CTCT ? PB[c] + PL[c] + PR[c] : PB[c] + PL[c], Z = lse[c];
                 const int t = GF ? r : q, u = GF ? q : r;
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
@@ -756,6 +1049,18 @@ __global__ void __launch_bounds__(256) simple_grad_kernel(const void *f, const v
                 acc[i][j] -= sl;
             }
         }
+        if constexpr (CTCT) {
+            if (!GF && r > 0) {    // grad_g: row u also carries the repeat of y_u
+                const int y = labels[m.loff + r - 1];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    if (c0 + tx + 16 * j != y) continue;
+                    float sr = 0.f;
+                    for (int q = 0; q < Qn; ++q) sr += PR[cell(r, q)];
+                    acc[i][j] -= sr;
+                }
+            }
+        }
     }
     if (GF && r0 < Rn) {           // grad_f: label y_{u+1} of every u < U_n, in increasing u
         for (int q = 0; q < m.U; ++q) {
@@ -772,6 +1077,22 @@ __global__ void __launch_bounds__(256) simple_grad_kernel(const void *f, const v
                 }
             }
         }
+        if constexpr (CTCT) {      // then the repeat of y_u of every u >= 1, in increasing u
+            for (int q = 1; q <= m.U; ++q) {
+                const int y = labels[m.loff + q - 1];
+                const long long j = y - c0 - tx;
+                if (j < 0 || j >= 16 * 4 || j % 16) continue;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int r = r0 + ty + 16 * i;
+                    if (r < Rn) {
+#pragma unroll
+                        for (int jj = 0; jj < 4; ++jj)
+                            if (jj == j / 16) acc[i][jj] -= PR[cell(r, q)];
+                    }
+                }
+            }
+        }
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -783,6 +1104,24 @@ __global__ void __launch_bounds__(256) simple_grad_kernel(const void *f, const v
             if (k < V) store_y(grad, DT, (own0 + r) * V + k, acc[i][j]);
         }
     }
+}
+
+template <int DT, bool GF>
+__global__ void __launch_bounds__(256) simple_grad_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                          const int *labels, int blank, const RnntMeta *meta, const float *mf,
+                                                          const float *mg, const int *ff, const int *fg, const float *S,
+                                                          const float *lse, const float *W, const float *PB, const float *PL,
+                                                          void *grad) {
+    SimpleGrad<DT, GF, false>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, nullptr, grad);
+}
+
+template <int DT, bool GF>
+__global__ void __launch_bounds__(256) ctct_simple_grad_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
+                                                               const int *labels, int blank, const RnntMeta *meta,
+                                                               const float *mf, const float *mg, const int *ff, const int *fg,
+                                                               const float *S, const float *lse, const float *W,
+                                                               const float *PB, const float *PL, const float *PR, void *grad) {
+    SimpleGrad<DT, GF, true>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, PR, grad);
 }
 
 int GridX(long long rows_per_utt, int per_cta) {
@@ -902,6 +1241,111 @@ int LaunchRnntSimpleBackward(const void *f, const void *g, int dtype, int N, int
             f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, grad_f);
         simple_grad_kernel<DT, false><<<dim3(gx, (U1 + kGR - 1) / kGR, N), 256, 0, s>>>(
             f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, grad_g);
+    });
+    CountLaunch(3);
+    return (int)cudaGetLastError();
+}
+
+size_t CtctWsBytes(int N, long long rows) { return MakeRnntLayout(N, rows, true).total; }
+
+int LaunchCtctForward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
+                      const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
+                      float *costs, float *costs_beta, cudaStream_t s) {
+    const RnntLayout L = MakeRnntLayout(N, rows, true);
+    RnntMeta *meta = At<RnntMeta>(ws, L.meta);
+    float *lpb = At<float>(ws, L.lpb), *lpl = At<float>(ws, L.lpl), *lpr = At<float>(ws, L.lpr);
+    rnnt_prep_kernel<<<1, kPrepThreads, 0, s>>>(lx, ly, N, rows, n_labels, compact, Tmax, Umax, meta, At<long long>(ws, L.tail));
+    const long long per_utt = (rows + N - 1) / N;
+    if (from_logits) {
+        const int gx = GridX(per_utt, kRowThreads / 32 * 4);
+        const bool vec = RowsVectorisable(x, V, dtype);
+        DispatchDtype(dtype, [&](auto dt) {
+            constexpr int DT = decltype(dt)::value;
+            auto k = vec ? ctct_logit_rows_kernel<DT, true> : ctct_logit_rows_kernel<DT, false>;
+            k<<<dim3(gx, N), kRowThreads, 0, s>>>(x, V, labels, blank, meta, lpb, lpl, lpr, At<float>(ws, L.lse));
+        });
+    } else {
+        ctct_lp_rows_kernel<<<dim3(GridX(per_utt, kRowThreads * 4), N), kRowThreads, 0, s>>>(x, dtype, V, labels, blank, meta,
+                                                                                            lpb, lpl, lpr);
+    }
+    ctct_alpha_beta_kernel<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(
+        meta, labels, lpb, lpl, lpr, At<double>(ws, L.alpha), At<double>(ws, L.beta), At<double>(ws, L.logp), N, costs,
+        want_beta ? costs_beta : nullptr);
+    CountLaunch(3);
+    return (int)cudaGetLastError();
+}
+
+int LaunchCtctBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
+                       void *ws, const float *w, void *grad, cudaStream_t s) {
+    const RnntLayout L = MakeRnntLayout(N, rows, true);
+    const long long per_utt = (rows + N - 1) / N;
+    const int gx = GridX(per_utt, kRowThreads / 32 * 4);
+    const bool vec = RowsVectorisable(grad, V, dtype) && (!from_logits || RowsVectorisable(x, V, dtype));
+    DispatchDtype(dtype, [&](auto dt) {
+        constexpr int DT = decltype(dt)::value;
+        auto k = from_logits ? (vec ? ctct_grad_kernel<DT, true, true> : ctct_grad_kernel<DT, false, true>)
+                             : (vec ? ctct_grad_kernel<DT, true, false> : ctct_grad_kernel<DT, false, false>);
+        k<<<dim3(gx, N + 1), kRowThreads, 0, s>>>(x, V, labels, blank, N, At<RnntMeta>(ws, L.meta), At<long long>(ws, L.tail),
+                                                  rows, At<double>(ws, L.alpha), At<double>(ws, L.beta),
+                                                  At<double>(ws, L.logp), At<float>(ws, L.lpb), At<float>(ws, L.lpl),
+                                                  At<float>(ws, L.lpr), At<float>(ws, L.lse), w, grad);
+    });
+    CountLaunch(1);
+    return (int)cudaGetLastError();
+}
+
+size_t CtctSimpleWsBytes(int N, int Tmax, int Umax) { return MakeSimpleLayout(N, Tmax, Umax, true).total; }
+
+int LaunchCtctSimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                            const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s) {
+    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax, true);
+    const int U1 = Umax + 1;
+    const long long cells = (long long)N * Tmax * U1;
+    RnntMeta *meta = At<RnntMeta>(ws, L.r.meta);
+    float *mf = At<float>(ws, L.mf), *mg = At<float>(ws, L.mg), *S = At<float>(ws, L.S);
+    float *lpb = At<float>(ws, L.r.lpb), *lpl = At<float>(ws, L.r.lpl), *lpr = At<float>(ws, L.r.lpr);
+    float *lse = At<float>(ws, L.r.lse);
+    int *ff = At<int>(ws, L.ff), *fg = At<int>(ws, L.fg);
+    rnnt_prep_kernel<<<1, kPrepThreads, 0, s>>>(lx, ly, N, cells, (long long)N * Umax, 0, Tmax, Umax, meta,
+                                                At<long long>(ws, L.r.tail));
+    const bool vec = RowsVectorisable(f, V, dtype) && RowsVectorisable(g, V, dtype);
+    DispatchDtype(dtype, [&](auto dt) {
+        constexpr int DT = decltype(dt)::value;
+        auto rowmax = vec ? simple_rowmax_kernel<DT, true> : simple_rowmax_kernel<DT, false>;
+        rowmax<<<dim3(GridX(std::max(Tmax, U1), kRowThreads / 32 * 4), N, 2), kRowThreads, 0, s>>>(f, g, V, Tmax, Umax, meta,
+                                                                                                    mf, mg, ff, fg);
+        ctct_simple_norm_kernel<DT><<<dim3((Tmax + kST - 1) / kST, (U1 + kSU - 1) / kSU, N), 256, 0, s>>>(
+            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, lpr, lse);
+        auto fixup = vec ? ctct_simple_fixup_kernel<DT, true> : ctct_simple_fixup_kernel<DT, false>;
+        fixup<<<dim3(GridX((long long)Tmax * U1, kRowThreads / 32 * 16), N), kRowThreads, 0, s>>>(
+            f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, lpr, lse);
+    });
+    ctct_alpha_beta_kernel<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(meta, labels, lpb, lpl, lpr,
+                                                                             At<double>(ws, L.r.alpha),
+                                                                             At<double>(ws, L.r.beta),
+                                                                             At<double>(ws, L.r.logp), N, costs, nullptr);
+    CountLaunch(5);
+    return (int)cudaGetLastError();
+}
+
+int LaunchCtctSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                             int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s) {
+    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax, true);
+    const int U1 = Umax + 1;
+    const RnntMeta *meta = At<RnntMeta>(ws, L.r.meta);
+    const float *mf = At<float>(ws, L.mf), *mg = At<float>(ws, L.mg), *S = At<float>(ws, L.S), *lse = At<float>(ws, L.r.lse);
+    const int *ff = At<int>(ws, L.ff), *fg = At<int>(ws, L.fg);
+    float *W = At<float>(ws, L.W), *PB = At<float>(ws, L.PB), *PL = At<float>(ws, L.PL), *PR = At<float>(ws, L.PR);
+    ctct_simple_weights_kernel<<<dim3(GridX((long long)Tmax * U1, kRowThreads * 4), N), kRowThreads, 0, s>>>(
+        meta, labels, At<double>(ws, L.r.alpha), At<double>(ws, L.r.beta), At<double>(ws, L.r.logp), At<float>(ws, L.r.lpb),
+        At<float>(ws, L.r.lpl), At<float>(ws, L.r.lpr), S, w, W, PB, PL, PR);
+    const int gx = (int)((V + kGC - 1) / kGC);
+    DispatchDtype(dtype, [&](auto dt) {
+        constexpr int DT = decltype(dt)::value;
+        ctct_simple_grad_kernel<DT, true><<<dim3(gx, (Tmax + kGR - 1) / kGR, N), 256, 0, s>>>(
+            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, PR, grad_f);
+        ctct_simple_grad_kernel<DT, false><<<dim3(gx, (U1 + kGR - 1) / kGR, N), 256, 0, s>>>(
+            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, PR, grad_g);
     });
     CountLaunch(3);
     return (int)cudaGetLastError();

@@ -15,51 +15,53 @@ from ._C import _DTYPES, _PinnedRing, _check, _rings, _stream
 REDUCTIONS = ("mean", "sum", "none")
 
 
-def check_rnnt_args(log_probs, labels, frames_lengths, labels_lengths, reduction, blank, compact) -> Tuple[int, int, int, int, int]:
-    """The arguments of ``rnnt_loss``, checked before anything touches a device: dtypes (AssertionError, as the CTC entries
-    assert theirs), then reduction, blank, shapes and -- for lengths on the CPU -- the row and label counts they imply
-    (ValueError).  Returns (N, rows, V, Tmax, Umax); Tmax and Umax are 0 for the compact layout."""
+def check_rnnt_args(log_probs, labels, frames_lengths, labels_lengths, reduction, blank, compact,
+                    name="rnnt_loss") -> Tuple[int, int, int, int, int]:
+    """The arguments of ``rnnt_loss`` (or of the loss called `name` that shares them), checked before anything touches a
+    device: dtypes (AssertionError, as the CTC entries assert theirs), then reduction, blank, shapes and -- for lengths on
+    the CPU -- the row and label counts they imply (ValueError).  Returns (N, rows, V, Tmax, Umax); Tmax and Umax are 0 for
+    the compact layout."""
     assert log_probs.dtype in _DTYPES, f"log_probs must be fp32, bf16 or fp16, not {log_probs.dtype}"
-    for name, t in (("labels", labels), ("frames_lengths", frames_lengths), ("labels_lengths", labels_lengths)):
-        assert t.dtype == torch.int32, f"{name} must be int32, not {t.dtype}"
+    for arg, t in (("labels", labels), ("frames_lengths", frames_lengths), ("labels_lengths", labels_lengths)):
+        assert t.dtype == torch.int32, f"{arg} must be int32, not {t.dtype}"
     if reduction not in REDUCTIONS:
-        raise ValueError(f"rnnt_loss: reduction must be one of {REDUCTIONS}, not {reduction!r}")
+        raise ValueError(f"{name}: reduction must be one of {REDUCTIONS}, not {reduction!r}")
     V = int(log_probs.shape[-1]) if log_probs.dim() else 0
     if isinstance(blank, bool) or not isinstance(blank, int) or not 0 <= blank < max(V, 1) or V == 0:
-        raise ValueError(f"rnnt_loss: blank must be an int in [0, V) with V = {V}, not {blank!r}")
+        raise ValueError(f"{name}: blank must be an int in [0, V) with V = {V}, not {blank!r}")
     if frames_lengths.dim() != 1 or labels_lengths.shape != frames_lengths.shape or frames_lengths.numel() == 0:
-        raise ValueError(f"rnnt_loss: frames_lengths and labels_lengths must both be (N,) with N >= 1, not "
+        raise ValueError(f"{name}: frames_lengths and labels_lengths must both be (N,) with N >= 1, not "
                          f"{tuple(frames_lengths.shape)} and {tuple(labels_lengths.shape)}")
     N = int(frames_lengths.numel())
     if compact:
         if log_probs.dim() != 2 or labels.dim() != 1:
-            raise ValueError(f"rnnt_loss(compact=True): log_probs must be (sum T(U+1), V) and labels (sum U,), not "
+            raise ValueError(f"{name}(compact=True): log_probs must be (sum T(U+1), V) and labels (sum U,), not "
                              f"{tuple(log_probs.shape)} and {tuple(labels.shape)}")
         rows, Tmax, Umax = int(log_probs.shape[0]), 0, 0
     else:
         if log_probs.dim() != 4 or log_probs.shape[0] != N or log_probs.shape[2] < 1:
-            raise ValueError(f"rnnt_loss: log_probs must be (N, Tmax, Umax+1, V) with N = {N}, not {tuple(log_probs.shape)}")
+            raise ValueError(f"{name}: log_probs must be (N, Tmax, Umax+1, V) with N = {N}, not {tuple(log_probs.shape)}")
         Tmax, Umax = int(log_probs.shape[1]), int(log_probs.shape[2]) - 1
         if tuple(labels.shape) != (N, Umax):
-            raise ValueError(f"rnnt_loss: labels must be (N, Umax) = {(N, Umax)}, not {tuple(labels.shape)}")
+            raise ValueError(f"{name}: labels must be (N, Umax) = {(N, Umax)}, not {tuple(labels.shape)}")
         rows = N * Tmax * (Umax + 1)
     if not frames_lengths.is_cuda and not labels_lengths.is_cuda:
         T, U = frames_lengths.long(), labels_lengths.long()
         if int(T.min()) < 1 or int(U.min()) < 0:
-            raise ValueError("rnnt_loss: every frames_length must be >= 1 and every labels_length >= 0")
+            raise ValueError(f"{name}: every frames_length must be >= 1 and every labels_length >= 0")
         if compact:
             need, n_lab = int((T * (U + 1)).sum()), int(U.sum())
             if need != rows:
-                raise ValueError(f"rnnt_loss(compact=True): the lengths give sum T(U+1) = {need} rows, log_probs has {rows}")
+                raise ValueError(f"{name}(compact=True): the lengths give sum T(U+1) = {need} rows, log_probs has {rows}")
             if n_lab != labels.numel():
-                raise ValueError(f"rnnt_loss(compact=True): the label lengths sum to {n_lab}, labels has {labels.numel()}")
+                raise ValueError(f"{name}(compact=True): the label lengths sum to {n_lab}, labels has {labels.numel()}")
         elif int(T.max()) > Tmax or int(U.max()) > Umax:
-            raise ValueError(f"rnnt_loss: lengths up to T = {int(T.max())}, U = {int(U.max())} overrun log_probs "
+            raise ValueError(f"{name}: lengths up to T = {int(T.max())}, U = {int(U.max())} overrun log_probs "
                              f"(Tmax = {Tmax}, Umax = {Umax})")
         if not labels.is_cuda:
             used = labels if compact else labels[torch.arange(Umax)[None, :] < U[:, None]]
             if used.numel() and (int(used.min()) < 0 or int(used.max()) >= V or bool((used == blank).any())):
-                raise ValueError(f"rnnt_loss: labels must lie in [0, {V}) and differ from blank = {blank}")
+                raise ValueError(f"{name}: labels must lie in [0, {V}) and differ from blank = {blank}")
     return N, rows, V, Tmax, Umax
 
 
@@ -82,20 +84,21 @@ def _on_device(dev, *ts) -> list:
     return out
 
 
-def _forward(x, labels, lx, ly, blank, compact, from_logits, want_beta, shape):
-    """One native forward.  Returns (costs (N,) fp32, costs from beta or None, workspace, device labels)."""
+def _forward(x, labels, lx, ly, blank, compact, from_logits, want_beta, shape, family="rnnt"):
+    """One native forward of the ccb_<family>_* entries ("rnnt", or "ctct" for the CTC-T loss, which takes the same
+    arguments).  Returns (costs (N,) fp32, costs from beta or None, workspace, device labels)."""
     N, rows, V, Tmax, Umax = shape
     L = _lib.lib()
     dev = x.device
     labels_d, lx_d, ly_d = _on_device(dev, labels, lx, ly)
-    ws = torch.empty(int(L.ccb_rnnt_workspace_bytes(N, rows)), dtype=torch.uint8, device=dev)
+    ws = torch.empty(int(getattr(L, f"ccb_{family}_workspace_bytes")(N, rows)), dtype=torch.uint8, device=dev)
     costs = torch.empty(N, dtype=torch.float32, device=dev)
     costs_b = torch.empty(N, dtype=torch.float32, device=dev) if want_beta else None
-    rc = L.ccb_rnnt_forward(x.data_ptr(), _DTYPES[x.dtype], int(from_logits), int(compact), N, rows, V, Tmax, Umax,
-                            labels_d.data_ptr(), int(labels_d.numel()), lx_d.data_ptr(), ly_d.data_ptr(), int(blank),
-                            int(want_beta), ws.data_ptr(), costs.data_ptr(),
-                            None if costs_b is None else costs_b.data_ptr(), _stream(dev))
-    _check(rc, "rnnt_loss")
+    rc = getattr(L, f"ccb_{family}_forward")(x.data_ptr(), _DTYPES[x.dtype], int(from_logits), int(compact), N, rows, V,
+                                             Tmax, Umax, labels_d.data_ptr(), int(labels_d.numel()), lx_d.data_ptr(),
+                                             ly_d.data_ptr(), int(blank), int(want_beta), ws.data_ptr(), costs.data_ptr(),
+                                             None if costs_b is None else costs_b.data_ptr(), _stream(dev))
+    _check(rc, f"{family}_loss")
     return costs, costs_b, ws, labels_d
 
 

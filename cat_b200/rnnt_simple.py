@@ -16,45 +16,46 @@ from .rnnt import REDUCTIONS, _on_device, _reduce
 _INT32_MAX = 2 ** 31 - 1
 
 
-def check_rnnt_simple_args(f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank) -> Tuple[int, int, int, int]:
-    """The arguments of ``rnnt_loss_simple``, checked before anything touches a device: dtypes (AssertionError), then
-    reduction, blank, shapes and -- for lengths on the CPU -- the lengths and the labels they select (ValueError).
-    Returns (N, Tmax, Umax, V)."""
+def check_rnnt_simple_args(f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank,
+                           name="rnnt_loss_simple") -> Tuple[int, int, int, int]:
+    """The arguments of ``rnnt_loss_simple`` (or of the loss called `name` that shares them), checked before anything
+    touches a device: dtypes (AssertionError), then reduction, blank, shapes and -- for lengths on the CPU -- the lengths and
+    the labels they select (ValueError).  Returns (N, Tmax, Umax, V)."""
     assert f_enc.dtype in _DTYPES, f"f_enc must be fp32, bf16 or fp16, not {f_enc.dtype}"
     assert g_pred.dtype == f_enc.dtype, f"g_pred must have f_enc's dtype {f_enc.dtype}, not {g_pred.dtype}"
-    for name, t in (("labels", labels), ("frames_lengths", frames_lengths), ("labels_lengths", labels_lengths)):
-        assert t.dtype in (torch.int32, torch.int64), f"{name} must be int32 or int64, not {t.dtype}"
+    for arg, t in (("labels", labels), ("frames_lengths", frames_lengths), ("labels_lengths", labels_lengths)):
+        assert t.dtype in (torch.int32, torch.int64), f"{arg} must be int32 or int64, not {t.dtype}"
     if reduction not in REDUCTIONS:
-        raise ValueError(f"rnnt_loss_simple: reduction must be one of {REDUCTIONS}, not {reduction!r}")
+        raise ValueError(f"{name}: reduction must be one of {REDUCTIONS}, not {reduction!r}")
     if f_enc.dim() != 3 or g_pred.dim() != 3:
-        raise ValueError(f"rnnt_loss_simple: f_enc must be (N, Tmax, V) and g_pred (N, Umax+1, V), not "
+        raise ValueError(f"{name}: f_enc must be (N, Tmax, V) and g_pred (N, Umax+1, V), not "
                          f"{tuple(f_enc.shape)} and {tuple(g_pred.shape)}")
     N, Tmax, V = (int(s) for s in f_enc.shape)
     if g_pred.shape[0] != N or g_pred.shape[2] != V or g_pred.shape[1] < 1 or Tmax < 1 or N < 1 or V < 1:
-        raise ValueError(f"rnnt_loss_simple: f_enc (N, Tmax, V) and g_pred (N, Umax+1, V) must share N >= 1 and V >= 1, with "
+        raise ValueError(f"{name}: f_enc (N, Tmax, V) and g_pred (N, Umax+1, V) must share N >= 1 and V >= 1, with "
                          f"Tmax >= 1, not {tuple(f_enc.shape)} and {tuple(g_pred.shape)}")
     Umax = int(g_pred.shape[1]) - 1
     if isinstance(blank, bool) or not isinstance(blank, int) or not 0 <= blank < V:
-        raise ValueError(f"rnnt_loss_simple: blank must be an int in [0, V) with V = {V}, not {blank!r}")
+        raise ValueError(f"{name}: blank must be an int in [0, V) with V = {V}, not {blank!r}")
     if frames_lengths.dim() != 1 or labels_lengths.shape != frames_lengths.shape or frames_lengths.numel() != N:
-        raise ValueError(f"rnnt_loss_simple: frames_lengths and labels_lengths must both be (N,) with N = {N}, not "
+        raise ValueError(f"{name}: frames_lengths and labels_lengths must both be (N,) with N = {N}, not "
                          f"{tuple(frames_lengths.shape)} and {tuple(labels_lengths.shape)}")
     if tuple(labels.shape) != (N, Umax):
-        raise ValueError(f"rnnt_loss_simple: labels must be (N, Umax) = {(N, Umax)} with g_pred (N, Umax+1, V), not "
+        raise ValueError(f"{name}: labels must be (N, Umax) = {(N, Umax)} with g_pred (N, Umax+1, V), not "
                          f"{tuple(labels.shape)}")
     if not frames_lengths.is_cuda and not labels_lengths.is_cuda:
         T, U = frames_lengths.long(), labels_lengths.long()
         if int(T.max()) > _INT32_MAX or int(U.max()) > _INT32_MAX:
-            raise ValueError("rnnt_loss_simple: lengths beyond the int32 range")
+            raise ValueError(f"{name}: lengths beyond the int32 range")
         if int(T.min()) < 1 or int(U.min()) < 0:
-            raise ValueError("rnnt_loss_simple: every frames_length must be >= 1 and every labels_length >= 0")
+            raise ValueError(f"{name}: every frames_length must be >= 1 and every labels_length >= 0")
         if int(T.max()) > Tmax or int(U.max()) > Umax:
-            raise ValueError(f"rnnt_loss_simple: lengths up to T = {int(T.max())}, U = {int(U.max())} overrun f_enc and "
+            raise ValueError(f"{name}: lengths up to T = {int(T.max())}, U = {int(U.max())} overrun f_enc and "
                              f"g_pred (Tmax = {Tmax}, Umax = {Umax})")
         if not labels.is_cuda:
             used = labels[torch.arange(Umax)[None, :] < U[:, None]]
             if used.numel() and (int(used.min()) < 0 or int(used.max()) >= V or bool((used == blank).any())):
-                raise ValueError(f"rnnt_loss_simple: labels must lie in [0, {V}) and differ from blank = {blank}")
+                raise ValueError(f"{name}: labels must lie in [0, {V}) and differ from blank = {blank}")
     return N, Tmax, Umax, V
 
 
@@ -66,18 +67,19 @@ def _int32(t: torch.Tensor) -> torch.Tensor:
     return t.clamp(-1, _INT32_MAX).to(torch.int32)
 
 
-def _forward(f, g, labels, lx, ly, blank, want_beta, shape):
-    """One native forward.  Returns (costs (N,) fp32, workspace, device labels)."""
+def _forward(f, g, labels, lx, ly, blank, want_beta, shape, family="rnnt"):
+    """One native forward of the ccb_<family>_simple_* entries ("rnnt", or "ctct" for the CTC-T loss, which takes the same
+    arguments).  Returns (costs (N,) fp32, workspace, device labels)."""
     N, Tmax, Umax, V = shape
     L = _lib.lib()
     dev = f.device
     labels_d, lx_d, ly_d = _on_device(dev, _int32(labels), _int32(lx), _int32(ly))
-    ws = torch.empty(int(L.ccb_rnnt_simple_workspace_bytes(N, Tmax, Umax)), dtype=torch.uint8, device=dev)
+    ws = torch.empty(int(getattr(L, f"ccb_{family}_simple_workspace_bytes")(N, Tmax, Umax)), dtype=torch.uint8, device=dev)
     costs = torch.empty(N, dtype=torch.float32, device=dev)
-    rc = L.ccb_rnnt_simple_forward(f.data_ptr(), g.data_ptr(), _DTYPES[f.dtype], N, Tmax, Umax, V, labels_d.data_ptr(),
-                                   lx_d.data_ptr(), ly_d.data_ptr(), int(blank), int(want_beta), ws.data_ptr(),
-                                   costs.data_ptr(), _stream(dev))
-    _check(rc, "rnnt_loss_simple")
+    rc = getattr(L, f"ccb_{family}_simple_forward")(f.data_ptr(), g.data_ptr(), _DTYPES[f.dtype], N, Tmax, Umax, V,
+                                                    labels_d.data_ptr(), lx_d.data_ptr(), ly_d.data_ptr(), int(blank),
+                                                    int(want_beta), ws.data_ptr(), costs.data_ptr(), _stream(dev))
+    _check(rc, "rnnt_loss_simple" if family == "rnnt" else f"{family}_simple_loss")
     return costs, ws, labels_d
 
 

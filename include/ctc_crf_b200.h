@@ -444,6 +444,42 @@ int ccb_rnnt_simple_forward(const void *f, const void *g, int dtype, int N, int 
 int ccb_rnnt_simple_backward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
                              int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream);
 
+/* CTC-T loss (DESIGN.md §7 "CTC-T loss"), the loss of CAT's `topo: ctct` transducers: every frame emits exactly one symbol,
+ * as in CTC, and reads the row of the labels emitted so far, as in RNN-T.  Over the states (u, b) (u labels emitted, the
+ * last emission blank or none yet) and (u, l) (u >= 1, the last emission y_u), with lp(t,u,k) the log-prob of token k at row
+ * (t,u), alpha_0(0,b) = 0 and every other alpha_0 = -inf, and logaddexp written (+):
+ *   alpha_{t+1}(u,b) = [alpha_t(u,b) (+) alpha_t(u,l)] + lp(t,u,blank)
+ *   alpha_{t+1}(u,l) = [alpha_t(u,l) + lp(t,u,y_u)] (+) [alpha_t(u-1,b) + lp(t,u-1,y_u)]
+ *                      (+) [alpha_t(u-1,l) + lp(t,u-1,y_u)]   (only if u = 1 or y_u != y_{u-1})
+ *   cost[n] = -(alpha_T(U,b) (+) alpha_T(U,l)).
+ * Each entry takes the arguments of its RNN-T counterpart and keeps its conventions: layouts, fp64 cells, NaN cost and zero
+ * gradient rows for a bad utterance, no atomics, no host synchronisation.  An infeasible utterance (T_n < U_n + the number of
+ * adjacent repeats in its labels) gets cost +inf and zero gradient, never NaN.
+ *   ccb_ctct_workspace_bytes: about 48 bytes per row (alpha and beta as two fp64 cells each; lp of blank, of y_{u+1} and of
+ *     y_u and the row's logsumexp in fp32) plus 56 bytes per utterance.  Nothing needs to be initialised.
+ *   ccb_ctct_forward: as ccb_rnnt_forward; costs_beta gets -beta_0(0,b).
+ *   ccb_ctct_backward: as ccb_rnnt_backward, with pb, pr and pl the posteriors of the blank, the repeat of y_u and the new
+ *     label y_{u+1} read at row (t,u): log-prob input: -pb at blank, -pr at y_u, -pl at y_{u+1} (added where y_u = y_{u+1});
+ *     raw logits: softmax(x) (pb + pr + pl) minus the same terms. */
+size_t ccb_ctct_workspace_bytes(int N, long rows);
+int ccb_ctct_forward(const void *x, int dtype, int from_logits, int compact, int N, long rows, int V, int Tmax, int Umax,
+                     const int *labels_dev, long n_labels, const int *lx_dev, const int *ly_dev, int blank, int want_beta,
+                     void *workspace, float *costs, float *costs_beta, void *stream);
+int ccb_ctct_backward(const void *x, int dtype, int from_logits, int N, long rows, int V, const int *labels_dev, int blank,
+                      void *workspace, const float *w, void *grad, void *stream);
+
+/* CTC-T loss of CAT's LogAdd joiner, lp(t,u,k) = f[n,t,k] + g[n,u,k] - Z(t,u) as for ccb_rnnt_simple_forward, with the
+ * lattice of ccb_ctct_forward.  Arguments and conventions as the ccb_rnnt_simple_* entries.
+ *   ccb_ctct_simple_workspace_bytes: the layout of ccb_rnnt_simple_workspace_bytes with the CTC-T lattice (two fp64 cells
+ *     per direction and lp of y_u per cell) and one more fp32 per cell (the repeat posterior): 68 bytes per cell of the padded
+ *     lattice, 8 bytes per row of f and of g and 56 bytes per utterance, each block aligned to 256 bytes. */
+size_t ccb_ctct_simple_workspace_bytes(int N, int Tmax, int Umax);
+int ccb_ctct_simple_forward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
+                            const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
+                            void *stream);
+int ccb_ctct_simple_backward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
+                             int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream);
+
 /* The compact joiner's broadcast sum (CAT's gather.sum): for N utterances with la[n] rows of a and lb[n] rows of b, laid out
  * one utterance after the other in each (offsets ta_n, ub_n and off_n = sum_{m<n} la_m lb_m computed on the device),
  *   out[off_n + t lb_n + u][h] = a[ta_n + t][h] + b[ub_n + u][h]   (fp32 sum, rounded to dtype),
