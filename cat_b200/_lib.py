@@ -35,7 +35,8 @@ SYMBOLS = [
     "ccb_rnnt_workspace_bytes", "ccb_rnnt_forward", "ccb_rnnt_backward", "ccb_gather_ws_bytes", "ccb_gather_sum",
     "ccb_gather_sum_backward", "ccb_rnnt_simple_workspace_bytes", "ccb_rnnt_simple_forward", "ccb_rnnt_simple_backward",
     "ccb_ctct_workspace_bytes", "ccb_ctct_forward", "ccb_ctct_backward", "ccb_ctct_simple_workspace_bytes",
-    "ccb_ctct_simple_forward", "ccb_ctct_simple_backward",
+    "ccb_ctct_simple_forward", "ccb_ctct_simple_backward", "ccb_rnnt_beam_ws_bytes", "ccb_rnnt_beam_init",
+    "ccb_rnnt_beam_step", "ccb_rnnt_beam_finish",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -158,6 +159,11 @@ def lib() -> C.CDLL:
         # the CTC-T entries take the RNN-T entries' arguments
         getattr(L, f"ccb_ctct_{e}").argtypes = getattr(L, f"ccb_rnnt_{e}").argtypes
         getattr(L, f"ccb_ctct_{e}").restype = getattr(L, f"ccb_rnnt_{e}").restype
+    L.ccb_rnnt_beam_ws_bytes.argtypes = [i, i, i]; L.ccb_rnnt_beam_ws_bytes.restype = C.c_size_t
+    L.ccb_rnnt_beam_init.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp]; L.ccb_rnnt_beam_init.restype = C.c_int
+    L.ccb_rnnt_beam_step.argtypes = [vp, vp, i, i, i, i, i, i, i, vp, i, vp, vp, vp, vp, vp, vp]
+    L.ccb_rnnt_beam_step.restype = C.c_int
+    L.ccb_rnnt_beam_finish.argtypes = [i, i, i, i, vp, vp, vp, vp, vp, vp, vp]; L.ccb_rnnt_beam_finish.restype = C.c_int
     L.ccb_gather_ws_bytes.argtypes = [i]; L.ccb_gather_ws_bytes.restype = C.c_size_t
     L.ccb_gather_sum.argtypes = [vp, vp, i, i, l, i, vp, vp, vp, vp, vp]; L.ccb_gather_sum.restype = C.c_int
     L.ccb_gather_sum_backward.argtypes = [vp, i, i, l, l, i, vp, vp, vp, vp, vp, vp]

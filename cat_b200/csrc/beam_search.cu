@@ -20,6 +20,7 @@
 // final score adds alpha ln P(</s> | state).
 #include <cmath>
 
+#include "beam_common.cuh"
 #include "common.cuh"
 
 namespace ccb {
@@ -29,32 +30,10 @@ namespace {
 constexpr int kThreads = 512;
 constexpr int kChunkSort = 2048;    // candidates + running best per bitonic sort (at least; a larger vocabulary widens it)
 constexpr int kMapSlots = 256;      // (parent rank, token) -> child map, at most kBeamMax keys
-constexpr double kNegInf = -INFINITY;
 
-__host__ __device__ __forceinline__ int Pow2Ceil(int x) {
-    int p = 1;
-    while (p < x) p <<= 1;
-    return p;
-}
-
-__host__ __device__ __forceinline__ size_t Up256(size_t x) { return (x + 255) & ~(size_t)255; }
-
-__host__ __device__ __forceinline__ size_t NodeCap(int T, int B) { return (size_t)B * (size_t)T + 1; }
-__host__ __device__ __forceinline__ size_t HashSlots(int T, int B) {
-    size_t h = 1;
-    while (h < 2 * NodeCap(T, B)) h <<= 1;
-    return h;
-}
 // per utterance: parent, token, first frame and beam rank of every node, then the hash table (node ids, -1 = empty)
 __host__ __device__ __forceinline__ size_t UttBytes(int T, int B) {
     return Up256((4 * NodeCap(T, B) + HashSlots(T, B)) * sizeof(int));
-}
-
-// log(exp(a) + exp(b)) in fp64: the larger plus log1p(exp(smaller - larger)); exact when one side is -inf
-__device__ __forceinline__ double lse(double a, double b) {
-    const double m = fmax(a, b), o = fmin(a, b);
-    if (o == kNegInf) return m;
-    return m + log1p(exp(o - m));
 }
 
 struct Graph {   // crf mode: the split den graph's out-arc CSR (DenPlan::out_*), labels and finals
@@ -129,32 +108,7 @@ __device__ __forceinline__ Slots Stay(bool crf, const Graph &g, const Beam &o, i
     return s;
 }
 
-// a ranks before b: larger mass, then smaller key
-__device__ __forceinline__ bool Before(double ma, int ka, double mb, int kb) { return ma > mb || (ma == mb && ka < kb); }
-
-// bitonic sort of m/k[0, P) into Before order (P a power of two), by the whole CTA
-__device__ void BitonicSort(double *m, int *k, int P) {
-    for (int size = 2; size <= P; size <<= 1)
-        for (int j = size >> 1; j > 0; j >>= 1) {
-            for (int i = threadIdx.x; i < P; i += blockDim.x) {
-                const int x = i ^ j;
-                if (x > i) {
-                    const bool up = (i & size) == 0;
-                    const bool sw = up ? Before(m[x], k[x], m[i], k[i]) : Before(m[i], k[i], m[x], k[x]);
-                    if (sw) {
-                        const double tm = m[i]; m[i] = m[x]; m[x] = tm;
-                        const int tk = k[i]; k[i] = k[x]; k[x] = tk;
-                    }
-                }
-            }
-            __syncthreads();
-        }
-}
-
 __device__ __forceinline__ unsigned MapHash(int key) { return ((unsigned)key * 0x9E3779B1u) >> 24; }   // kMapSlots = 256
-__device__ __forceinline__ unsigned TrieHash(int parent, int tok, size_t slots) {
-    return (unsigned)((((unsigned)parent * 0x9E3779B1u) ^ ((unsigned)tok * 0x85EBCA77u)) & (unsigned)(slots - 1));
-}
 
 struct Params {
     Graph g;

@@ -298,6 +298,14 @@ int LaunchCtctSimpleForward(const void *f, const void *g, int dtype, int N, int 
                             const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s);
 int LaunchCtctSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
                              int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s);
+// Transducer beam search (rnnt_decode.cu): init, one step per frame, finish; one CTA per utterance each
+constexpr int kRnntBeamMaxV = 1 << 24;
+size_t RnntBeamWsBytes(int N, int T, int B);
+int LaunchRnntBeamInit(int N, int T, int B, void *ws, int *parent, int *token, int *node, double *score, cudaStream_t s);
+int LaunchRnntBeamStep(const void *rows, const void *enc, int dtype, int mode, int N, int T, int B, int V, int t,
+                       const int *len, int blank, void *ws, int *parent, int *token, int *node, double *score, cudaStream_t s);
+int LaunchRnntBeamFinish(int N, int T, int B, int nbest, const void *ws, const int *node, const double *score, int *tokens,
+                         int *lengths, float *scores, cudaStream_t s);
 // gather.sum of the joiner and its backward; ws: GatherWsBytes(N) bytes of per-utterance offsets
 size_t GatherWsBytes(int N);
 int LaunchGatherSum(const void *a, const void *b, int dtype, int N, long long rows_out, int H, const int *la, const int *lb,

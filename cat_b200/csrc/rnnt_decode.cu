@@ -1,0 +1,302 @@
+// Transducer (RNN-T, monotonic) beam search: one launch per frame, one CTA per utterance (DESIGN.md §7 "Transducer beam
+// search").  The caller runs the predictor and joiner networks between launches; each step reads the (N*B, V) row block of
+// the current beam slots and
+//   1. selects the B best candidates (r, k), value s_r + lp_r[k] in fp64, by (value desc, flat index r*V + k asc), exactly:
+//      the flat index range is scanned in windows, a candidate is kept only when it ranks before the B-th best so far, and
+//      the kept ones are bitonic-sorted together with the best B when the buffer fills (or at the end);
+//   2. finds the target prefix of each: the slot's own trie node for blank, else the child (node, k), looked up in the
+//      utterance's open-addressing hash and created (ids in visiting order) if missing;
+//   3. merges candidates with the same target in increasing flat index, logaddexp in fp64, in that order -- no atomics;
+//   4. writes each slot of the next beam (order of first appearance): parent slot, token (-1: stay), trie node, score.
+// The finish launch ranks the beam by score (stable), walks the trie back and writes the N-best.
+#include "beam_common.cuh"
+#include "common.cuh"
+
+namespace ccb {
+
+namespace {
+
+constexpr int kThreads = 512;
+constexpr int kSort = 2048;                  // sort buffer: the best B, then the candidates waiting to be sorted
+constexpr int kWindow = 2 * kThreads;        // flat indices scanned between two looks at the buffer
+constexpr int kNoKey = 0x7fffffff;
+
+// per utterance: parent and token of every node, the hash table (node ids, -1 = empty), the next free node id
+__host__ __device__ __forceinline__ size_t UttBytes(int T, int B) {
+    return Up256((2 * NodeCap(T, B) + HashSlots(T, B) + 1) * sizeof(int));
+}
+
+struct Trie {
+    int *parent, *tok, *hash, *next;
+    size_t hslots;
+};
+
+__device__ __forceinline__ Trie UttTrie(char *ws, int n, int T, int B) {
+    Trie tr;
+    const size_t cap = NodeCap(T, B);
+    tr.parent = reinterpret_cast<int *>(ws + (size_t)n * UttBytes(T, B));
+    tr.tok = tr.parent + cap;
+    tr.hash = tr.tok + cap;
+    tr.hslots = HashSlots(T, B);
+    tr.next = tr.hash + tr.hslots;
+    return tr;
+}
+
+struct StepParams {
+    const void *rows;    // (N*B, V): log-probs (mode 0), raw logits (1) or the LogAdd g rows (2)
+    const void *enc;     // mode 2: f (N, T, V)
+    int dtype, mode;
+    int N, T, B, V, t, blank;
+    const int *len;
+    char *ws;
+    int *parent, *token, *node;
+    double *score;
+};
+
+// the step's fp32 row value before normalisation: the input (modes 0, 1) or f[n, t] + g_slot (mode 2)
+__device__ __forceinline__ float RowZ(const StepParams &P, long row, long frow, int k) {
+    const float z = load_y(P.rows, P.dtype, row + k);
+    return P.mode == 2 ? load_y(P.enc, P.dtype, frow + k) + z : z;
+}
+
+__global__ void __launch_bounds__(kThreads) rnnt_beam_init_kernel(int T, int B, char *ws, int *parent, int *token, int *node,
+                                                                  double *score) {
+    const int n = blockIdx.x;
+    const Trie tr = UttTrie(ws, n, T, B);
+    for (size_t i = threadIdx.x; i < tr.hslots; i += blockDim.x) tr.hash[i] = -1;
+    for (int q = threadIdx.x; q < B; q += blockDim.x) {
+        const size_t s = (size_t)n * B + q;
+        parent[s] = q; token[s] = -1;
+        node[s] = q == 0 ? 0 : -1;
+        score[s] = q == 0 ? 0.0 : kNegInf;
+    }
+    if (threadIdx.x == 0) { tr.parent[0] = -1; tr.tok[0] = -1; *tr.next = 1; }
+}
+
+__global__ void __launch_bounds__(kThreads) rnnt_beam_step_kernel(const StepParams P) {
+    __shared__ double sort_m[kSort];
+    __shared__ int sort_k[kSort];
+    __shared__ double s_score[kBeamMax], o_m[kBeamMax];
+    __shared__ int s_node[kBeamMax], o_f[kBeamMax], o_tgt[kBeamMax], o_first[kBeamMax];
+    __shared__ float s_lse[kBeamMax];
+    __shared__ int s_nb, s_cnt, s_kept;
+    const int n = blockIdx.x, tid = threadIdx.x;
+    const int B = P.B, V = P.V, T = P.T, t = P.t;
+    const size_t slot0 = (size_t)n * B;
+    if (t >= P.len[n]) {   // the utterance has ended: every slot stays itself
+        for (int q = tid; q < B; q += blockDim.x) { P.parent[slot0 + q] = q; P.token[slot0 + q] = -1; }
+        return;
+    }
+    for (int q = tid; q < B; q += blockDim.x) { s_score[q] = P.score[slot0 + q]; s_node[q] = P.node[slot0 + q]; }
+    for (int i = tid; i < B; i += blockDim.x) { sort_m[i] = kNegInf; sort_k[i] = kNoKey; }
+    if (tid == 0) s_cnt = 0;
+    __syncthreads();
+    if (tid == 0) {   // the live slots are a prefix of the beam
+        int nb = 0;
+        while (nb < B && s_score[nb] > kNegInf) ++nb;
+        s_nb = nb;
+    }
+    __syncthreads();
+    const int nb = s_nb;
+    const long frow = ((long)n * T + t) * V;
+    // row normalisers (modes 1, 2): one warp per row, an online (max, sum of exp) in fp32, merged in a fixed tree
+    if (P.mode != 0) {
+        const int lane = tid & 31, warp = tid >> 5;
+        for (int r = warp; r < nb; r += blockDim.x >> 5) {
+            const long row = (long)(slot0 + r) * V;
+            float m = -INFINITY, s = 0.f;
+            for (int k = lane; k < V; k += 32) {
+                const float z = RowZ(P, row, frow, k);
+                if (z == -INFINITY) continue;
+                if (z > m) { s = s * expf(m - z) + 1.f; m = z; } else { s += expf(z - m); }
+            }
+            for (int o = 16; o > 0; o >>= 1) {
+                const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+                const float mm = fmaxf(m, m2);
+                if (mm > -INFINITY) s = (m > -INFINITY ? s * expf(m - mm) : 0.f) + (m2 > -INFINITY ? s2 * expf(m2 - mm) : 0.f);
+                m = mm;
+            }
+            if (lane == 0) s_lse[r] = m > -INFINITY ? m + logf(s) : -INFINITY;
+        }
+        __syncthreads();
+    }
+    // 1. exact top-B over the nb * V candidates
+    const int total = nb * V;
+    const int cap = kSort - B;
+    for (int w0 = 0; w0 < total; w0 += kWindow) {
+        const double thr_m = sort_m[B - 1];
+        const int thr_k = sort_k[B - 1];
+        for (int f = w0 + tid; f < min(total, w0 + kWindow); f += blockDim.x) {
+            const int r = f / V, k = f - r * V;
+            const long row = (long)(slot0 + r) * V;
+            float v = RowZ(P, row, frow, k);
+            if (P.mode != 0) v = v - s_lse[r];
+            const double m = s_score[r] + (double)v;
+            if (m > kNegInf && Before(m, f, thr_m, thr_k)) {
+                const int pos = atomicAdd(&s_cnt, 1);
+                sort_m[B + pos] = m;
+                sort_k[B + pos] = f;
+            }
+        }
+        __syncthreads();
+        const int cnt = s_cnt;
+        if (cnt > 0 && (cnt > cap - kWindow || w0 + kWindow >= total)) {
+            const int ps = Pow2Ceil(B + cnt);
+            for (int i = B + cnt + tid; i < ps; i += blockDim.x) { sort_m[i] = kNegInf; sort_k[i] = kNoKey; }
+            __syncthreads();
+            BitonicSort(sort_m, sort_k, ps);
+            if (tid == 0) s_cnt = 0;
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        int k = 0;
+        while (k < B && sort_m[k] > kNegInf) ++k;
+        s_kept = k;
+    }
+    __syncthreads();
+    const int kept = s_kept;
+    // 2. the kept candidates in visiting order (increasing flat index) and their target trie nodes
+    for (int j = tid; j < kept; j += blockDim.x) {
+        int pos = 0;
+        for (int i = 0; i < kept; ++i) pos += sort_k[i] < sort_k[j];
+        o_f[pos] = sort_k[j];
+        o_m[pos] = sort_m[j];
+    }
+    __syncthreads();
+    const Trie tr = UttTrie(P.ws, n, T, B);
+    for (int j = tid; j < kept; j += blockDim.x) {
+        const int r = o_f[j] / V, k = o_f[j] - r * V, parent = s_node[r];
+        int found = -1;
+        if (k == P.blank) {
+            found = parent;
+        } else {
+            for (unsigned h = TrieHash(parent, k, tr.hslots);; h = (h + 1) & (unsigned)(tr.hslots - 1)) {
+                const int x = tr.hash[h];
+                if (x < 0) break;
+                if (tr.parent[x] == parent && tr.tok[x] == k) { found = x; break; }
+            }
+        }
+        o_tgt[j] = found;
+    }
+    __syncthreads();
+    if (tid == 0) {   // missing children created in visiting order (distinct: the beam's prefixes are distinct)
+        int next = *tr.next;
+        for (int j = 0; j < kept; ++j) {
+            if (o_tgt[j] >= 0) continue;
+            const int r = o_f[j] / V, k = o_f[j] - r * V, x = next++;
+            tr.parent[x] = s_node[r]; tr.tok[x] = k;
+            unsigned h = TrieHash(s_node[r], k, tr.hslots);
+            while (tr.hash[h] >= 0) h = (h + 1) & (unsigned)(tr.hslots - 1);
+            tr.hash[h] = x;
+            o_tgt[j] = x;
+        }
+        *tr.next = next;
+    }
+    __syncthreads();
+    // 3. the first candidate of each target and its position in the next beam
+    for (int j = tid; j < kept; j += blockDim.x) {
+        int first = j;
+        for (int i = 0; i < j; ++i)
+            if (o_tgt[i] == o_tgt[j]) { first = i; break; }
+        o_first[j] = first;
+    }
+    __syncthreads();
+    // 4. the next beam: slot q from its first candidate j, the later ones with the same target folded in visiting order
+    for (int j = tid; j < kept; j += blockDim.x) {
+        if (o_first[j] != j) continue;
+        int q = 0;
+        for (int i = 0; i < j; ++i) q += o_first[i] == i;
+        double s = o_m[j];
+        for (int i = j + 1; i < kept; ++i)
+            if (o_tgt[i] == o_tgt[j]) s = lse(s, o_m[i]);
+        const int r = o_f[j] / V, k = o_f[j] - r * V;
+        P.parent[slot0 + q] = r;
+        P.token[slot0 + q] = k == P.blank ? -1 : k;
+        P.node[slot0 + q] = o_tgt[j];
+        P.score[slot0 + q] = s;
+    }
+    if (tid == 0) {
+        int nb2 = 0;
+        for (int j = 0; j < kept; ++j) nb2 += o_first[j] == j;
+        s_cnt = nb2;
+    }
+    __syncthreads();
+    for (int q = s_cnt + tid; q < B; q += blockDim.x) {
+        P.parent[slot0 + q] = q; P.token[slot0 + q] = -1; P.node[slot0 + q] = -1; P.score[slot0 + q] = kNegInf;
+    }
+}
+
+// ranks the beam by score (desc; ties: beam order) and writes the first nbest rows: tokens -1 padded, lengths (-1 past the
+// hypotheses found), scores (-inf there)
+__global__ void __launch_bounds__(kThreads) rnnt_beam_finish_kernel(int T, int B, int nbest, const char *ws, const int *node,
+                                                                    const double *score, int *tokens, int *lengths,
+                                                                    float *scores) {
+    __shared__ double s_score[kBeamMax];
+    __shared__ int s_nb;
+    const int n = blockIdx.x, tid = threadIdx.x;
+    const size_t slot0 = (size_t)n * B;
+    for (int q = tid; q < B; q += blockDim.x) s_score[q] = score[slot0 + q];
+    __syncthreads();
+    if (tid == 0) {
+        int nb = 0;
+        while (nb < B && s_score[nb] > kNegInf) ++nb;
+        s_nb = nb;
+    }
+    __syncthreads();
+    const int nb = s_nb;
+    const Trie tr = UttTrie(const_cast<char *>(ws), n, T, B);
+    const size_t row0 = (size_t)n * nbest;
+    for (int q = tid; q < B; q += blockDim.x) {
+        int pos = q, x = -1;
+        if (q < nb) {
+            pos = 0;
+            for (int j = 0; j < nb; ++j) pos += Before(s_score[j], j, s_score[q], q);
+            x = node[slot0 + q];
+        }
+        if (pos >= nbest) continue;
+        int *tk = tokens + (row0 + pos) * T;
+        int L = -1;
+        if (x >= 0) {
+            L = 0;
+            for (int y = x; y > 0; y = tr.parent[y]) ++L;
+            int i = L;
+            for (int y = x; y > 0; y = tr.parent[y]) tk[--i] = tr.tok[y];
+        }
+        for (int i = max(L, 0); i < T; ++i) tk[i] = -1;
+        lengths[row0 + pos] = L;
+        scores[row0 + pos] = x >= 0 ? (float)s_score[q] : -INFINITY;
+    }
+}
+
+}  // namespace
+
+size_t RnntBeamWsBytes(int N, int T, int B) { return (size_t)N * UttBytes(T, B); }
+
+int LaunchRnntBeamInit(int N, int T, int B, void *ws, int *parent, int *token, int *node, double *score, cudaStream_t s) {
+    rnnt_beam_init_kernel<<<N, kThreads, 0, s>>>(T, B, reinterpret_cast<char *>(ws), parent, token, node, score);
+    CountLaunch();
+    return (int)cudaGetLastError();
+}
+
+int LaunchRnntBeamStep(const void *rows, const void *enc, int dtype, int mode, int N, int T, int B, int V, int t,
+                       const int *len, int blank, void *ws, int *parent, int *token, int *node, double *score, cudaStream_t s) {
+    StepParams p;
+    p.rows = rows; p.enc = enc; p.dtype = dtype; p.mode = mode;
+    p.N = N; p.T = T; p.B = B; p.V = V; p.t = t; p.blank = blank;
+    p.len = len; p.ws = reinterpret_cast<char *>(ws);
+    p.parent = parent; p.token = token; p.node = node; p.score = score;
+    rnnt_beam_step_kernel<<<N, kThreads, 0, s>>>(p);
+    CountLaunch();
+    return (int)cudaGetLastError();
+}
+
+int LaunchRnntBeamFinish(int N, int T, int B, int nbest, const void *ws, const int *node, const double *score, int *tokens,
+                         int *lengths, float *scores, cudaStream_t s) {
+    rnnt_beam_finish_kernel<<<N, kThreads, 0, s>>>(T, B, nbest, reinterpret_cast<const char *>(ws), node, score, tokens,
+                                                   lengths, scores);
+    CountLaunch();
+    return (int)cudaGetLastError();
+}
+
+}  // namespace ccb

@@ -493,6 +493,31 @@ int ccb_gather_sum(const void *a, const void *b, int dtype, int N, long rows_out
 int ccb_gather_sum_backward(const void *grad_out, int dtype, int N, long rows_a, long rows_b, int H, const int *la_dev,
                             const int *lb_dev, void *workspace, void *grad_a, void *grad_b, void *stream);
 
+/* Transducer (RNN-T, monotonic) beam search, one launch per frame; the caller runs the networks between launches.  Each
+ * utterance keeps a beam of `beam` slots (1 .. 128): per slot, parent / token / node int32 and score fp64, all (N, beam)
+ * device arrays.  Live slots are a prefix of the beam (score > -inf); the empty prefix is trie node 0.
+ *   ccb_rnnt_beam_init: the beam [empty prefix, score 0] and an empty trie.
+ *   ccb_rnnt_beam_step (frame t; utterances with t >= len_dev[n] keep their beam, each slot its own parent, token -1):
+ *     rows (N*beam, V) in the CCB_DTYPE_* code dtype, row n*beam + q for slot q of utterance n (rows of dead slots are not
+ *     read).  mode 0: log-probs; 1: raw joiner logits, normalised by the row's logsumexp; 2: the LogAdd joiner's g rows,
+ *     z = f[n, t] + g in fp32 with enc = f (N, Tmax, V) of the same dtype, normalised likewise.  Candidate (r, k) has
+ *     value score_r + lp_r[k] (fp64); the min(beam, live * V) best, by value desc then r * V + k asc, -inf dropped, are
+ *     merged in increasing r * V + k by target prefix (blank: the slot's own prefix, else prefix + k), logaddexp in fp64.
+ *     Each slot of the new beam (order of first appearance) gets its parent slot, token (-1 for blank), trie node and
+ *     score; dead slots parent = itself, token -1, node -1, score -inf.  V <= 2^24, blank in [0, V).
+ *   ccb_rnnt_beam_finish: the beam ranked by score (stable), the first nbest (1 .. beam) rows written: tokens
+ *     (N, nbest, Tmax) int32 -1 padded, lengths (N, nbest) int32 (-1 past the hypotheses found), scores (N, nbest) fp32.
+ * workspace: ccb_rnnt_beam_ws_bytes(N, Tmax, beam) bytes (0 for beam outside [1, 128]): per utterance the trie (at most
+ * 1 + beam * Tmax nodes) and its hash table; ccb_rnnt_beam_init initialises it. */
+size_t ccb_rnnt_beam_ws_bytes(int N, int Tmax, int beam);
+int ccb_rnnt_beam_init(int N, int Tmax, int beam, void *workspace, int *parent, int *token, int *node, double *score,
+                       void *stream);
+int ccb_rnnt_beam_step(const void *rows, const void *enc, int dtype, int mode, int N, int Tmax, int beam, int V, int t,
+                       const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node, double *score,
+                       void *stream);
+int ccb_rnnt_beam_finish(int N, int Tmax, int beam, int nbest, const void *workspace, const int *node, const double *score,
+                         int *tokens, int *lengths, float *scores, void *stream);
+
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 long ccb_launch_count(void);
 
