@@ -36,7 +36,7 @@ SYMBOLS = [
     "ccb_gather_sum_backward", "ccb_rnnt_simple_workspace_bytes", "ccb_rnnt_simple_forward", "ccb_rnnt_simple_backward",
     "ccb_ctct_workspace_bytes", "ccb_ctct_forward", "ccb_ctct_backward", "ccb_ctct_simple_workspace_bytes",
     "ccb_ctct_simple_forward", "ccb_ctct_simple_backward", "ccb_rnnt_beam_ws_bytes", "ccb_rnnt_beam_init",
-    "ccb_rnnt_beam_step", "ccb_rnnt_beam_finish",
+    "ccb_rnnt_beam_step", "ccb_rnnt_beam_finish", "ccb_ctct_beam_ws_bytes", "ccb_ctct_beam_init", "ccb_ctct_beam_step",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -164,6 +164,10 @@ def lib() -> C.CDLL:
     L.ccb_rnnt_beam_step.argtypes = [vp, vp, i, i, i, i, i, i, i, vp, i, vp, vp, vp, vp, vp, vp]
     L.ccb_rnnt_beam_step.restype = C.c_int
     L.ccb_rnnt_beam_finish.argtypes = [i, i, i, i, vp, vp, vp, vp, vp, vp, vp]; L.ccb_rnnt_beam_finish.restype = C.c_int
+    L.ccb_ctct_beam_ws_bytes.argtypes = [i, i, i]; L.ccb_ctct_beam_ws_bytes.restype = C.c_size_t
+    L.ccb_ctct_beam_init.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp]; L.ccb_ctct_beam_init.restype = C.c_int
+    L.ccb_ctct_beam_step.argtypes = [vp, vp, i, i, i, i, i, i, i, vp, i, vp, vp, vp, vp, vp, vp]
+    L.ccb_ctct_beam_step.restype = C.c_int
     L.ccb_gather_ws_bytes.argtypes = [i]; L.ccb_gather_ws_bytes.restype = C.c_size_t
     L.ccb_gather_sum.argtypes = [vp, vp, i, i, l, i, vp, vp, vp, vp, vp]; L.ccb_gather_sum.restype = C.c_int
     L.ccb_gather_sum_backward.argtypes = [vp, i, i, l, l, i, vp, vp, vp, vp, vp, vp]

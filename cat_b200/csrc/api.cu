@@ -1475,6 +1475,39 @@ int ccb_rnnt_beam_finish(int N, int Tmax, int beam, int nbest, const void *works
     return 0;
 }
 
+/* ---- CTC-T beam search (finished by ccb_rnnt_beam_finish) ------------------------------------- */
+size_t ccb_ctct_beam_ws_bytes(int N, int Tmax, int beam) {
+    return N > 0 && Tmax >= 0 && beam >= 1 && beam <= kBeamMax ? CtctBeamWsBytes(N, Tmax, beam) : 0;
+}
+
+int ccb_ctct_beam_init(int N, int Tmax, int beam, void *workspace, int *parent, int *token, int *node, double *score,
+                       void *stream) {
+    g_err.clear();
+    if (CheckRnntBeam("ctct_beam_init", N, Tmax, beam)) return 1;
+    if (!workspace || !parent || !token || !node || !score) return Fail("ctct_beam_init: missing buffer");
+    const int rc = LaunchCtctBeamInit(N, Tmax, beam, workspace, parent, token, node, score, (cudaStream_t)stream);
+    if (rc) return FailCuda("ctct_beam_init", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_ctct_beam_step(const void *rows, const void *enc, int dtype, int mode, int N, int Tmax, int beam, int V, int t,
+                       const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node, double *score,
+                       void *stream) {
+    g_err.clear();
+    if (CheckRnntBeam("ctct_beam_step", N, Tmax, beam)) return 1;
+    if (!KnownDtype(dtype)) return FailDtype("ctct_beam_step", dtype);
+    if (mode < 0 || mode > 2) return Fail("ctct_beam_step: mode must be 0 (log-probs), 1 (logits) or 2 (LogAdd)");
+    if (V <= 0 || V > kRnntBeamMaxV) return Fail("ctct_beam_step: V must lie in [1, 2^24], not " + std::to_string(V));
+    if (t < 0 || t >= Tmax) return Fail("ctct_beam_step: frame t must lie in [0, Tmax)");
+    if (blank < 0 || blank >= V) return Fail("ctct_beam_step: blank must lie in [0, V)");
+    if (!rows || (mode == 2 && !enc) || !len_dev || !workspace || !parent || !token || !node || !score)
+        return Fail("ctct_beam_step: missing buffer");
+    const int rc = LaunchCtctBeamStep(rows, enc, dtype, mode, N, Tmax, beam, V, t, len_dev, blank, workspace, parent, token,
+                                      node, score, (cudaStream_t)stream);
+    if (rc) return FailCuda("ctct_beam_step", (cudaError_t)rc);
+    return 0;
+}
+
 size_t ccb_gather_ws_bytes(int N) { return N > 0 ? GatherWsBytes(N) : 0; }
 
 int ccb_gather_sum(const void *a, const void *b, int dtype, int N, long rows_out, int H, const int *la_dev, const int *lb_dev,

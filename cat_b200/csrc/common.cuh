@@ -306,6 +306,12 @@ int LaunchRnntBeamStep(const void *rows, const void *enc, int dtype, int mode, i
                        const int *len, int blank, void *ws, int *parent, int *token, int *node, double *score, cudaStream_t s);
 int LaunchRnntBeamFinish(int N, int T, int B, int nbest, const void *ws, const int *node, const double *score, int *tokens,
                          int *lengths, float *scores, cudaStream_t s);
+// CTC-T beam search (ctct_decode.cu): init and one step per frame over a workspace that starts with the transducer beam
+// search's tries (same stride), so that LaunchRnntBeamFinish finishes it
+size_t CtctBeamWsBytes(int N, int T, int B);
+int LaunchCtctBeamInit(int N, int T, int B, void *ws, int *parent, int *token, int *node, double *score, cudaStream_t s);
+int LaunchCtctBeamStep(const void *rows, const void *enc, int dtype, int mode, int N, int T, int B, int V, int t,
+                       const int *len, int blank, void *ws, int *parent, int *token, int *node, double *score, cudaStream_t s);
 // gather.sum of the joiner and its backward; ws: GatherWsBytes(N) bytes of per-utterance offsets
 size_t GatherWsBytes(int N);
 int LaunchGatherSum(const void *a, const void *b, int dtype, int N, long long rows_out, int H, const int *la, const int *lb,

@@ -9,8 +9,7 @@
 //   3. merges candidates with the same target in increasing flat index, logaddexp in fp64, in that order -- no atomics;
 //   4. writes each slot of the next beam (order of first appearance): parent slot, token (-1: stay), trie node, score.
 // The finish launch ranks the beam by score (stable), walks the trie back and writes the N-best.
-#include "beam_common.cuh"
-#include "common.cuh"
+#include "transducer_beam.cuh"
 
 namespace ccb {
 
@@ -20,44 +19,6 @@ constexpr int kThreads = 512;
 constexpr int kSort = 2048;                  // sort buffer: the best B, then the candidates waiting to be sorted
 constexpr int kWindow = 2 * kThreads;        // flat indices scanned between two looks at the buffer
 constexpr int kNoKey = 0x7fffffff;
-
-// per utterance: parent and token of every node, the hash table (node ids, -1 = empty), the next free node id
-__host__ __device__ __forceinline__ size_t UttBytes(int T, int B) {
-    return Up256((2 * NodeCap(T, B) + HashSlots(T, B) + 1) * sizeof(int));
-}
-
-struct Trie {
-    int *parent, *tok, *hash, *next;
-    size_t hslots;
-};
-
-__device__ __forceinline__ Trie UttTrie(char *ws, int n, int T, int B) {
-    Trie tr;
-    const size_t cap = NodeCap(T, B);
-    tr.parent = reinterpret_cast<int *>(ws + (size_t)n * UttBytes(T, B));
-    tr.tok = tr.parent + cap;
-    tr.hash = tr.tok + cap;
-    tr.hslots = HashSlots(T, B);
-    tr.next = tr.hash + tr.hslots;
-    return tr;
-}
-
-struct StepParams {
-    const void *rows;    // (N*B, V): log-probs (mode 0), raw logits (1) or the LogAdd g rows (2)
-    const void *enc;     // mode 2: f (N, T, V)
-    int dtype, mode;
-    int N, T, B, V, t, blank;
-    const int *len;
-    char *ws;
-    int *parent, *token, *node;
-    double *score;
-};
-
-// the step's fp32 row value before normalisation: the input (modes 0, 1) or f[n, t] + g_slot (mode 2)
-__device__ __forceinline__ float RowZ(const StepParams &P, long row, long frow, int k) {
-    const float z = load_y(P.rows, P.dtype, row + k);
-    return P.mode == 2 ? load_y(P.enc, P.dtype, frow + k) + z : z;
-}
 
 __global__ void __launch_bounds__(kThreads) rnnt_beam_init_kernel(int T, int B, char *ws, int *parent, int *token, int *node,
                                                                   double *score) {

@@ -18,38 +18,38 @@ MAX_BEAM = 128
 _MODE_LOGPROBS, _MODE_LOGITS, _MODE_LOGADD = 0, 1, 2
 
 
-def _check_args(enc_out, frame_lens, beam_size, nbest, blank) -> Tuple[int, int, int]:
-    """The arguments of ``rnnt_beam_search`` (ValueError), checked before anything runs.  Returns (N, Tmax, nbest)."""
+def _check_args(enc_out, frame_lens, beam_size, nbest, blank, name) -> Tuple[int, int, int]:
+    """The arguments of the search ``name`` (ValueError), checked before anything runs.  Returns (N, Tmax, nbest)."""
     if not isinstance(enc_out, torch.Tensor) or enc_out.dim() != 3 or not enc_out.is_cuda:
-        raise ValueError("rnnt_beam_search: enc_out must be an (N, T, H) CUDA tensor")
+        raise ValueError(f"{name}: enc_out must be an (N, T, H) CUDA tensor")
     N, Tmax = int(enc_out.shape[0]), int(enc_out.shape[1])
     if N < 1:
-        raise ValueError("rnnt_beam_search: enc_out holds no utterance")
+        raise ValueError(f"{name}: enc_out holds no utterance")
     if isinstance(beam_size, bool) or not isinstance(beam_size, int) or not 1 <= beam_size <= MAX_BEAM:
-        raise ValueError(f"rnnt_beam_search: beam_size must be an int in [1, {MAX_BEAM}], not {beam_size!r}")
+        raise ValueError(f"{name}: beam_size must be an int in [1, {MAX_BEAM}], not {beam_size!r}")
     nbest = beam_size if nbest is None else nbest
     if isinstance(nbest, bool) or not isinstance(nbest, int) or not 1 <= nbest <= beam_size:
-        raise ValueError(f"rnnt_beam_search: nbest must be an int in [1, beam_size = {beam_size}], not {nbest!r}")
+        raise ValueError(f"{name}: nbest must be an int in [1, beam_size = {beam_size}], not {nbest!r}")
     if isinstance(blank, bool) or not isinstance(blank, int) or blank < 0:
-        raise ValueError(f"rnnt_beam_search: blank must be an int >= 0, not {blank!r}")
+        raise ValueError(f"{name}: blank must be an int >= 0, not {blank!r}")
     if not isinstance(frame_lens, torch.Tensor) or frame_lens.dtype not in (torch.int32, torch.int64) \
             or tuple(frame_lens.shape) != (N,):
-        raise ValueError(f"rnnt_beam_search: frame_lens must be an int32 or int64 (N,) tensor with N = {N}")
+        raise ValueError(f"{name}: frame_lens must be an int32 or int64 (N,) tensor with N = {N}")
     if frame_lens.is_cuda:
         if frame_lens.device != enc_out.device:
-            raise ValueError(f"rnnt_beam_search: frame_lens is on {frame_lens.device}, enc_out on {enc_out.device}")
+            raise ValueError(f"{name}: frame_lens is on {frame_lens.device}, enc_out on {enc_out.device}")
     elif N and (int(frame_lens.min()) < 0 or int(frame_lens.max()) > Tmax):
-        raise ValueError(f"rnnt_beam_search: frame_lens must lie in [0, T = {Tmax}]")
+        raise ValueError(f"{name}: frame_lens must lie in [0, T = {Tmax}]")
     return N, Tmax, nbest
 
 
-def _check_state(predictor, state, R: int):
+def _check_state(predictor, state, R: int, name):
     """The predictor states the search can carry per slot: None, or a tuple of 3-D tensors with the batch on dim 1."""
     if state is None:
         return
     if isinstance(state, tuple) and all(isinstance(s, torch.Tensor) and s.dim() == 3 and s.shape[1] == R for s in state):
         return
-    raise NotImplementedError(f"rnnt_beam_search: the state of predictor {type(predictor).__name__} is neither None nor a "
+    raise NotImplementedError(f"{name}: the state of predictor {type(predictor).__name__} is neither None nor a "
                               "tuple of 3-D tensors with the batch on dim 1 (an LSTM's); it cannot be carried per beam slot")
 
 
@@ -57,9 +57,10 @@ class _Joiner:
     """How the joiner's rows for a frame reach the kernel: LogAdd (f and g rows), JointNet in "add" mode (raw logits from
     fc(fc_enc(enc) + fc_dec(pn)), fc_enc applied once per call) or any other joiner (log-probs of joiner(enc, pn))."""
 
-    def __init__(self, joiner, enc_out):
+    def __init__(self, joiner, enc_out, caller):
         name = type(joiner).__name__
         self.joiner = joiner
+        self.caller = caller
         if name == "LogAdd":
             self.mode = _MODE_LOGADD
             self.f = enc_out.contiguous()
@@ -76,7 +77,7 @@ class _Joiner:
         if self.mode == _MODE_LOGADD:
             g = pn_out.reshape(R, -1)
             if g.shape[1] != self.f.shape[2]:
-                raise ValueError(f"rnnt_beam_search: the LogAdd joiner's f (N, T, {self.f.shape[2]}) and g (R, "
+                raise ValueError(f"{self.caller}: the LogAdd joiner's f (N, T, {self.f.shape[2]}) and g (R, "
                                  f"{g.shape[1]}) rows differ in V")
             dt = torch.promote_types(self.f.dtype, g.dtype)
             if self.f.dtype != dt:
@@ -87,6 +88,75 @@ class _Joiner:
             return self.joiner.fc(h).reshape(R, -1).contiguous(), None
         enc = self.enc[:, t, None, None, :].expand(N, B, 1, -1).reshape(R, 1, -1)
         return self.joiner(enc, pn_out).reshape(R, -1).contiguous(), None
+
+
+def _beam_search(name: str, family: str, enc_out, frame_lens, predictor, joiner, beam_size, nbest, blank):
+    """The frame loop of the transducer searches: ``family`` "rnnt" or "ctct" picks the native ws-bytes, init and step entries
+    (``ccb_<family>_beam_*``); both are finished by ``ccb_rnnt_beam_finish``.  ``name`` is the calling function's, for its
+    errors.  Each frame runs the predictor once over all N*B slots, every slot keeping its parent's output and state or
+    advancing them by the token it emitted; nothing synchronises the host."""
+    N, Tmax, nbest = _check_args(enc_out, frame_lens, beam_size, nbest, blank, name)
+    B, R = beam_size, N * beam_size
+    dev = enc_out.device
+    L = _lib.lib()
+
+    def entry(e):   # the native entry, looked up where it is called: the argument checks run before any native access
+        return getattr(L, f"ccb_{family}_beam_{e}")
+
+    with torch.no_grad(), torch.cuda.device(dev):
+        lens = _on_device(dev, _int32(frame_lens))[0]
+        if Tmax:
+            pn_out, state = predictor(torch.full((R, 1), blank, dtype=torch.long, device=dev), None)
+            _check_state(predictor, state, R, name)
+            join = _Joiner(joiner, enc_out, name)
+        parent = torch.empty((N, B), dtype=torch.int32, device=dev)
+        token = torch.empty((N, B), dtype=torch.int32, device=dev)
+        node = torch.empty((N, B), dtype=torch.int32, device=dev)
+        score = torch.empty((N, B), dtype=torch.float64, device=dev)
+        tokens = torch.empty((N, nbest, Tmax), dtype=torch.int32, device=dev)
+        lengths = torch.empty((N, nbest), dtype=torch.int32, device=dev)
+        scores = torch.empty((N, nbest), dtype=torch.float32, device=dev)
+        slot_base = (torch.arange(N, device=dev, dtype=torch.long) * B)[:, None]
+        ws = None
+
+        def init():   # (after the first frame's rows: every argument error is raised before a native call)
+            nonlocal ws
+            ws = torch.empty(int(entry("ws_bytes")(N, Tmax, B)), dtype=torch.uint8, device=dev)
+            _check(entry("init")(N, Tmax, B, ws.data_ptr(), parent.data_ptr(), token.data_ptr(), node.data_ptr(),
+                                 score.data_ptr(), _stream(dev)), name)
+
+        if Tmax == 0:
+            init()
+        for t in range(Tmax):
+            rows, f = join.rows(t, pn_out, N, B)
+            if rows.dtype not in _DTYPES:
+                rows = rows.float()
+                f = f.float() if f is not None else None
+            V = int(rows.shape[1])
+            if blank >= V:
+                raise ValueError(f"{name}: blank = {blank} is not a label of the joiner's V = {V}")
+            if t == 0:
+                init()
+            _check(entry("step")(rows.data_ptr(), f.data_ptr() if f is not None else None, _DTYPES[rows.dtype], join.mode,
+                                 N, Tmax, B, V, t, lens.data_ptr(), blank, ws.data_ptr(), parent.data_ptr(),
+                                 token.data_ptr(), node.data_ptr(), score.data_ptr(), _stream(dev)), name)
+            if t + 1 == Tmax:
+                break
+            # each slot's predictor output and state: its parent's, advanced by the token it emitted (if any)
+            src = (slot_base + parent.long()).reshape(R)
+            tok = token.reshape(R)
+            ext = tok >= 0
+            pn_par = pn_out.index_select(0, src)
+            st_par = None if state is None else tuple(s.index_select(1, src) for s in state)
+            out_new, st_new = predictor(torch.where(ext, tok, blank).long().reshape(R, 1), st_par)
+            _check_state(predictor, st_new, R, name)
+            pn_out = torch.where(ext.view(R, *([1] * (out_new.dim() - 1))), out_new, pn_par.to(out_new.dtype))
+            state = None if st_new is None else tuple(
+                torch.where(ext.view(1, R, 1), sn, sp.to(sn.dtype)) for sn, sp in zip(st_new, st_par))
+        _check(L.ccb_rnnt_beam_finish(N, Tmax, B, nbest, ws.data_ptr(), node.data_ptr(), score.data_ptr(),
+                                      tokens.data_ptr(), lengths.data_ptr(), scores.data_ptr(), _stream(dev)), name)
+        lens.record_stream(torch.cuda.current_stream(dev))
+    return tokens, lengths, scores
 
 
 def rnnt_beam_search(enc_out: torch.Tensor, frame_lens: torch.Tensor, predictor, joiner, beam_size: int = 5,
@@ -100,66 +170,7 @@ def rnnt_beam_search(enc_out: torch.Tensor, frame_lens: torch.Tensor, predictor,
     JointNet or any module called as joiner(enc (R, 1, H), pn (R, 1, H')) returning log-probs.  Returns device tensors
     tokens (N, nbest, T) int32 -1 padded, lengths (N, nbest) int32 (-1 past the hypotheses found) and scores (N, nbest)
     fp32, best first.  The frame loop runs to T; nothing synchronises the host."""
-    N, Tmax, nbest = _check_args(enc_out, frame_lens, beam_size, nbest, blank)
-    B, R = beam_size, N * beam_size
-    dev = enc_out.device
-    L = _lib.lib()
-    with torch.no_grad(), torch.cuda.device(dev):
-        lens = _on_device(dev, _int32(frame_lens))[0]
-        if Tmax:
-            pn_out, state = predictor(torch.full((R, 1), blank, dtype=torch.long, device=dev), None)
-            _check_state(predictor, state, R)
-            join = _Joiner(joiner, enc_out)
-        parent = torch.empty((N, B), dtype=torch.int32, device=dev)
-        token = torch.empty((N, B), dtype=torch.int32, device=dev)
-        node = torch.empty((N, B), dtype=torch.int32, device=dev)
-        score = torch.empty((N, B), dtype=torch.float64, device=dev)
-        tokens = torch.empty((N, nbest, Tmax), dtype=torch.int32, device=dev)
-        lengths = torch.empty((N, nbest), dtype=torch.int32, device=dev)
-        scores = torch.empty((N, nbest), dtype=torch.float32, device=dev)
-        slot_base = (torch.arange(N, device=dev, dtype=torch.long) * B)[:, None]
-        ws = None
-
-        def init():   # (after the first frame's rows: every argument error is raised before a native call)
-            nonlocal ws
-            ws = torch.empty(int(L.ccb_rnnt_beam_ws_bytes(N, Tmax, B)), dtype=torch.uint8, device=dev)
-            _check(L.ccb_rnnt_beam_init(N, Tmax, B, ws.data_ptr(), parent.data_ptr(), token.data_ptr(), node.data_ptr(),
-                                        score.data_ptr(), _stream(dev)), "rnnt_beam_search")
-
-        if Tmax == 0:
-            init()
-        for t in range(Tmax):
-            rows, f = join.rows(t, pn_out, N, B)
-            if rows.dtype not in _DTYPES:
-                rows = rows.float()
-                f = f.float() if f is not None else None
-            V = int(rows.shape[1])
-            if blank >= V:
-                raise ValueError(f"rnnt_beam_search: blank = {blank} is not a label of the joiner's V = {V}")
-            if t == 0:
-                init()
-            _check(L.ccb_rnnt_beam_step(rows.data_ptr(), f.data_ptr() if f is not None else None, _DTYPES[rows.dtype],
-                                        join.mode, N, Tmax, B, V, t, lens.data_ptr(), blank, ws.data_ptr(),
-                                        parent.data_ptr(), token.data_ptr(), node.data_ptr(), score.data_ptr(),
-                                        _stream(dev)), "rnnt_beam_search")
-            if t + 1 == Tmax:
-                break
-            # each slot's predictor output and state: its parent's, advanced by the token it emitted (if any)
-            src = (slot_base + parent.long()).reshape(R)
-            tok = token.reshape(R)
-            ext = tok >= 0
-            pn_par = pn_out.index_select(0, src)
-            st_par = None if state is None else tuple(s.index_select(1, src) for s in state)
-            out_new, st_new = predictor(torch.where(ext, tok, blank).long().reshape(R, 1), st_par)
-            _check_state(predictor, st_new, R)
-            pn_out = torch.where(ext.view(R, *([1] * (out_new.dim() - 1))), out_new, pn_par.to(out_new.dtype))
-            state = None if st_new is None else tuple(
-                torch.where(ext.view(1, R, 1), sn, sp.to(sn.dtype)) for sn, sp in zip(st_new, st_par))
-        _check(L.ccb_rnnt_beam_finish(N, Tmax, B, nbest, ws.data_ptr(), node.data_ptr(), score.data_ptr(),
-                                      tokens.data_ptr(), lengths.data_ptr(), scores.data_ptr(), _stream(dev)),
-               "rnnt_beam_search")
-        lens.record_stream(torch.cuda.current_stream(dev))
-    return tokens, lengths, scores
+    return _beam_search("rnnt_beam_search", "rnnt", enc_out, frame_lens, predictor, joiner, beam_size, nbest, blank)
 
 
 class RNNTDecoder:
@@ -197,17 +208,27 @@ class RNNTDecoder:
     def __call__(self, enc_out: torch.Tensor, frame_lens: Optional[torch.Tensor] = None
                  ) -> List[Tuple[List[List[int]], List[float]]]:
         """[(token lists without bos, scores), ...] per utterance, best first: CAT's return value.  One host copy."""
-        if frame_lens is None:
-            frame_lens = torch.full((enc_out.size(0),), enc_out.size(1), dtype=torch.int32)
-        tokens, lengths, scores = rnnt_beam_search(enc_out, frame_lens, self.predictor, self.joiner, self.beam_size,
-                                                   self.nbest, self.blank_id)
-        N, K, T = tokens.shape
-        host = torch.cat([tokens.reshape(N, K * T), lengths, scores.view(torch.int32)], dim=1).cpu()
-        out = []
-        for n in range(N):
-            toks = host[n, :K * T].view(K, T)
-            lens = host[n, K * T:K * T + K].tolist()
-            sc = host[n, K * T + K:].contiguous().view(torch.float32).tolist()
-            hyps = [(toks[k, :lens[k]].tolist(), sc[k]) for k in range(K) if lens[k] >= 0]
-            out.append(([h for h, _ in hyps], [s for _, s in hyps]))
-        return out
+        return _to_lists(*rnnt_beam_search(enc_out, _frame_lens(enc_out, frame_lens), self.predictor, self.joiner,
+                                           self.beam_size, self.nbest, self.blank_id))
+
+
+def _frame_lens(enc_out, frame_lens):
+    """CAT's default: every utterance runs to T."""
+    if frame_lens is None:
+        return torch.full((enc_out.size(0),), enc_out.size(1), dtype=torch.int32)
+    return frame_lens
+
+
+def _to_lists(tokens, lengths, scores) -> List[Tuple[List[List[int]], List[float]]]:
+    """[(token lists, scores), ...] per utterance from a search's device tensors, as CAT's decoders return them.  One host
+    copy."""
+    N, K, T = tokens.shape
+    host = torch.cat([tokens.reshape(N, K * T), lengths, scores.view(torch.int32)], dim=1).cpu()
+    out = []
+    for n in range(N):
+        toks = host[n, :K * T].view(K, T)
+        lens = host[n, K * T:K * T + K].tolist()
+        sc = host[n, K * T + K:].contiguous().view(torch.float32).tolist()
+        hyps = [(toks[k, :lens[k]].tolist(), sc[k]) for k in range(K) if lens[k] >= 0]
+        out.append(([h for h, _ in hyps], [s for _, s in hyps]))
+    return out

@@ -518,6 +518,28 @@ int ccb_rnnt_beam_step(const void *rows, const void *enc, int dtype, int mode, i
 int ccb_rnnt_beam_finish(int N, int Tmax, int beam, int nbest, const void *workspace, const int *node, const double *score,
                          int *tokens, int *lengths, float *scores, void *stream);
 
+/* CTC-T (CTC-Transducer) prefix beam search, one launch per frame, with the arguments and slot arrays of the transducer beam
+ * search above; every frame emits one symbol, as in ccb_ctct_forward.  Each live slot holds a prefix with masses b (last
+ * emission blank, or none yet) and n (last emission its last token) in the workspace; its score is s = b (+) n.
+ *   ccb_ctct_beam_init: the beam [empty prefix, b = -inf, n = 0] and an empty trie.
+ *   ccb_ctct_beam_step (frame t; utterances with t >= len_dev[n] keep their beam, each slot its own parent, token -1): rows
+ *     and modes as ccb_rnnt_beam_step.  Row r's candidate tokens C_r are the k = min(beam, V - 1) non-blank tokens with the
+ *     largest lp_r (ties: lower token).  Extension (r, j), c = C_r[j], adds (c == last_r ? b_r : s_r) + lp_r[c] to
+ *     n(prefix_r + c); the stay of r adds s_r + lp_r[blank] to b(prefix_r) and, for a non-empty prefix, n_r + lp_r[last_r]
+ *     to n(prefix_r); logaddexp in fp64.  Keys: r (k + 1) + j for an extension, r (k + 1) + k for a stay; a target's key is
+ *     its smallest.  The min(beam, #targets with s > -inf) best targets by s desc then key asc form the new beam in that
+ *     order: parent slot, token (c for a new extension, -1 for a stay or an extension merged into one), trie node, s.  Dead
+ *     slots as in ccb_rnnt_beam_step.  V <= 2^24, blank in [0, V).
+ *   ccb_rnnt_beam_finish is the finish for a CTC-T workspace: the beam is already ranked, and the trie comes first in it.
+ * workspace: ccb_ctct_beam_ws_bytes(N, Tmax, beam) bytes (0 for beam outside [1, 128]): ccb_rnnt_beam_ws_bytes(N, Tmax,
+ * beam) for the tries, then per utterance b and n of every slot and the beam x beam candidate tokens, masses and merges. */
+size_t ccb_ctct_beam_ws_bytes(int N, int Tmax, int beam);
+int ccb_ctct_beam_init(int N, int Tmax, int beam, void *workspace, int *parent, int *token, int *node, double *score,
+                       void *stream);
+int ccb_ctct_beam_step(const void *rows, const void *enc, int dtype, int mode, int N, int Tmax, int beam, int V, int t,
+                       const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node, double *score,
+                       void *stream);
+
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 long ccb_launch_count(void);
 

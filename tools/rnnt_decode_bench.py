@@ -43,8 +43,8 @@ def timed(fn, reps):
     return a.elapsed_time(b) / reps
 
 
-def split(fn, pred, joiner):
-    """GPU time of the step kernel, the predictor and the joiner in one profiled call (ms)."""
+def split(fn, pred, joiner, kernel="rnnt_beam_step_kernel"):
+    """GPU time of the step kernel (named ``kernel``), the predictor and the joiner in one profiled call (ms)."""
     rf = {}
 
     def pre(name):
@@ -71,7 +71,7 @@ def split(fn, pred, joiner):
             out["predictor"] += t
         elif e.key == "bench::joiner":
             out["joiner"] += t
-        elif "rnnt_beam_step_kernel" in e.key:
+        elif kernel in e.key:
             out["step_kernel"] += t
     for e in p.events():
         if e.device_type == torch.autograd.DeviceType.CUDA:
