@@ -1225,6 +1225,29 @@ int ccb_ngram_copy(void *lm, int which, void *dst, size_t dst_bytes) {
     return 0;
 }
 
+int ccb_ngram_slot_rows(const void *lm, int N, int beam, int V, const int *parent, const int *token, const int *state_in,
+                        int *state_out, float *rows, void *stream) {
+    g_err.clear();
+    if (!lm) return Fail("ngram_slot_rows: missing LM");
+    NGram *m = reinterpret_cast<NGram *>(const_cast<void *>(lm));
+    if (N <= 0 || V <= 0) return Fail("ngram_slot_rows: N and V must be positive");
+    if (beam < 1 || beam > kBeamMax)
+        return Fail("ngram_slot_rows: beam must lie in [1, " + std::to_string(kBeamMax) + "], not " + std::to_string(beam));
+    if (m->host.V != V)
+        return Fail("ngram_slot_rows: the LM was loaded for " + std::to_string(m->host.V) + " labels, V is " + std::to_string(V));
+    if ((parent && (!token || !state_in)) || !state_out || !rows) return Fail("ngram_slot_rows: missing buffer");
+    const size_t smem = NgramSlotRowsSmemBytes(m->host.W);
+    if (smem > 200 * 1024)
+        return Fail("ngram_slot_rows: the LM has " + std::to_string(m->host.W) + " words; its rows are built in shared "
+                    "memory, which holds at most " + std::to_string(200 * 1024 / 8));
+    const NGramDev *lmd = nullptr;
+    if (EnsureNGram(m, &lmd)) return 1;
+    const int rc = LaunchNgramSlotRows(*lmd, m->host.W, N, beam, V, parent, token, state_in, state_out, rows,
+                                       (cudaStream_t)stream);
+    if (rc) return FailCuda("ngram_slot_rows", (cudaError_t)rc);
+    return 0;
+}
+
 /* ---- TLG decoding graph and its Viterbi beam search ------------------------------------------- */
 // A decoding graph handle (ccb_wfst_create): the host tables, and their device copies, uploaded by the first search that
 // uses the graph on a device and freed by ccb_wfst_destroy
@@ -1445,21 +1468,54 @@ int ccb_rnnt_beam_init(int N, int Tmax, int beam, void *workspace, int *parent, 
     return 0;
 }
 
+// the arguments every RNN-T step entry takes
+static int CheckRnntStep(const char *what, const void *rows, const void *enc, int dtype, int mode, int N, int Tmax, int beam,
+                         int V, int t, const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node,
+                         double *score) {
+    const std::string w(what);
+    if (CheckRnntBeam(what, N, Tmax, beam)) return 1;
+    if (!KnownDtype(dtype)) return FailDtype(what, dtype);
+    if (mode < 0 || mode > 2) return Fail(w + ": mode must be 0 (log-probs), 1 (logits) or 2 (LogAdd)");
+    if (V <= 0 || V > kRnntBeamMaxV) return Fail(w + ": V must lie in [1, 2^24], not " + std::to_string(V));
+    if (t < 0 || t >= Tmax) return Fail(w + ": frame t must lie in [0, Tmax)");
+    if (blank < 0 || blank >= V) return Fail(w + ": blank must lie in [0, V)");
+    if (!rows || (mode == 2 && !enc) || !len_dev || !workspace || !parent || !token || !node || !score)
+        return Fail(w + ": missing buffer");
+    return 0;
+}
+
 int ccb_rnnt_beam_step(const void *rows, const void *enc, int dtype, int mode, int N, int Tmax, int beam, int V, int t,
                        const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node, double *score,
                        void *stream) {
     g_err.clear();
-    if (CheckRnntBeam("rnnt_beam_step", N, Tmax, beam)) return 1;
-    if (!KnownDtype(dtype)) return FailDtype("rnnt_beam_step", dtype);
-    if (mode < 0 || mode > 2) return Fail("rnnt_beam_step: mode must be 0 (log-probs), 1 (logits) or 2 (LogAdd)");
-    if (V <= 0 || V > kRnntBeamMaxV) return Fail("rnnt_beam_step: V must lie in [1, 2^24], not " + std::to_string(V));
-    if (t < 0 || t >= Tmax) return Fail("rnnt_beam_step: frame t must lie in [0, Tmax)");
-    if (blank < 0 || blank >= V) return Fail("rnnt_beam_step: blank must lie in [0, V)");
-    if (!rows || (mode == 2 && !enc) || !len_dev || !workspace || !parent || !token || !node || !score)
-        return Fail("rnnt_beam_step: missing buffer");
+    if (CheckRnntStep("rnnt_beam_step", rows, enc, dtype, mode, N, Tmax, beam, V, t, len_dev, blank, workspace, parent, token,
+                      node, score))
+        return 1;
     const int rc = LaunchRnntBeamStep(rows, enc, dtype, mode, N, Tmax, beam, V, t, len_dev, blank, workspace, parent, token,
                                       node, score, (cudaStream_t)stream);
     if (rc) return FailCuda("rnnt_beam_step", (cudaError_t)rc);
+    return 0;
+}
+
+int ccb_rnnt_beam_step_fused(const void *rows, const void *enc, int dtype, int mode, int N, int Tmax, int beam, int V, int t,
+                             const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node,
+                             double *score, const void *lm_rows, int lm_dtype, double alpha, double beta,
+                             const void *ilm_rows, int ilm_dtype, double ilm_weight, double *lm_part, void *stream) {
+    g_err.clear();
+    if (CheckRnntStep("rnnt_beam_step_fused", rows, enc, dtype, mode, N, Tmax, beam, V, t, len_dev, blank, workspace, parent,
+                      token, node, score))
+        return 1;
+    if (!lm_rows && !ilm_rows)
+        return Fail("rnnt_beam_step_fused: neither LM rows nor ILM rows: use rnnt_beam_step for the search without fusion");
+    if (!lm_part) return Fail("rnnt_beam_step_fused: missing buffer");
+    if (lm_rows && !KnownDtype(lm_dtype)) return FailDtype("rnnt_beam_step_fused", lm_dtype);
+    if (ilm_rows && !KnownDtype(ilm_dtype)) return FailDtype("rnnt_beam_step_fused", ilm_dtype);
+    if (!std::isfinite(alpha) || !std::isfinite(beta) || !std::isfinite(ilm_weight))
+        return Fail("rnnt_beam_step_fused: alpha, beta and ilm_weight must be finite");
+    const int rc = LaunchRnntBeamStepFused(rows, enc, dtype, mode, N, Tmax, beam, V, t, len_dev, blank, workspace, parent,
+                                           token, node, score, lm_rows, lm_dtype, alpha, beta, ilm_rows, ilm_dtype,
+                                           ilm_weight, lm_part, (cudaStream_t)stream);
+    if (rc) return FailCuda("rnnt_beam_step_fused", (cudaError_t)rc);
     return 0;
 }
 

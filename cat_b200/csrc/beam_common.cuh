@@ -1,7 +1,10 @@
 // Helpers shared by the prefix searches that keep a per-utterance trie: the CTC prefix beam search (beam_search.cu) and the
-// transducer beam search (rnnt_decode.cu).  One CTA per utterance in both; the trie lives in the caller's workspace.
+// transducer beam search (rnnt_decode.cu).  One CTA per utterance in both; the trie lives in the caller's workspace.  Both
+// score a token n-gram LM by the same back-off walk, LmLog10.
 #pragma once
 #include <cmath>
+
+#include "common.cuh"
 
 namespace ccb {
 
@@ -57,6 +60,38 @@ __device__ void BitonicSort(double *m, int *k, int P) {
 // open-addressing hash of a trie node (parent, token); slots a power of two
 __device__ __forceinline__ unsigned TrieHash(int parent, int tok, size_t slots) {
     return (unsigned)((((unsigned)parent * 0x9E3779B1u) ^ ((unsigned)tok * 0x85EBCA77u)) & (unsigned)(slots - 1));
+}
+
+constexpr double kLn10 = 2.302585092994045684;
+
+// log10 P(word w | LM state s) by the back-off walk (ngram.h); *dst the state after w.  An arc whose probability is NaN
+// was inserted by the loader's prefix closure: it gives the destination, the probability is the back-off value.
+__device__ __forceinline__ double LmLog10(const NGramDev &lm, int s, int w, int *dst) {
+    double acc = 0.0;
+    int d = -1;
+    for (;;) {
+        if (s == 0) {
+            acc += (double)lm.root_p[w];
+            if (d < 0) d = lm.root_dst[w];
+            break;
+        }
+        int lo = lm.arc_off[s];
+        const int end = lm.arc_off[s + 1];
+        int hi = end;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (lm.arc_word[mid] < w) lo = mid + 1; else hi = mid;
+        }
+        if (lo < end && lm.arc_word[lo] == w) {
+            if (d < 0) d = lm.arc_dst[lo];
+            const float p = lm.arc_p[lo];
+            if (p == p) { acc += (double)p; break; }
+        }
+        acc += (double)lm.bow[s];
+        s = lm.back[s];
+    }
+    *dst = d;
+    return acc;
 }
 
 }  // namespace

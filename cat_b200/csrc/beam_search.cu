@@ -125,38 +125,6 @@ struct Params {
     double alpha, beta;
 };
 
-constexpr double kLn10 = 2.302585092994045684;
-
-// log10 P(word w | LM state s) by the back-off walk (ngram.h); *dst the state after w.  An arc whose probability is NaN
-// was inserted by the loader's prefix closure: it gives the destination, the probability is the back-off value.
-__device__ __forceinline__ double LmLog10(const NGramDev &lm, int s, int w, int *dst) {
-    double acc = 0.0;
-    int d = -1;
-    for (;;) {
-        if (s == 0) {
-            acc += (double)lm.root_p[w];
-            if (d < 0) d = lm.root_dst[w];
-            break;
-        }
-        int lo = lm.arc_off[s];
-        const int end = lm.arc_off[s + 1];
-        int hi = end;
-        while (lo < hi) {
-            const int mid = (lo + hi) >> 1;
-            if (lm.arc_word[mid] < w) lo = mid + 1; else hi = mid;
-        }
-        if (lo < end && lm.arc_word[lo] == w) {
-            if (d < 0) d = lm.arc_dst[lo];
-            const float p = lm.arc_p[lo];
-            if (p == p) { acc += (double)p; break; }
-        }
-        acc += (double)lm.bow[s];
-        s = lm.back[s];
-    }
-    *dst = d;
-    return acc;
-}
-
 // What an extension by token c from LM state s adds to a prefix's LM part: alpha ln P(c | s) + beta; *dst the state after
 // c.  alpha = 0 does not consult the LM.
 __device__ __forceinline__ double LmTerm(const Params &P, int s, int c, int *dst) {

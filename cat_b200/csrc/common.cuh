@@ -253,6 +253,11 @@ struct NGramDev {
 int LaunchBeamSearch(const DeviceGraph *g, const void *y, int y_dtype, int N, int T, int V, const int *len, int B, int topn,
                      void *ws, int *tokens, int *lengths, int *timesteps, float *scores, cudaStream_t stream,
                      const NGramDev *lm = nullptr, double alpha = 0.0, double beta = 0.0);
+// The n-gram LM's rows for the fused RNN-T step (rnnt_decode.cu): one CTA per slot of N*B, W the LM's word count; its
+// dynamic shared memory is NgramSlotRowsSmemBytes(W)
+size_t NgramSlotRowsSmemBytes(int W);
+int LaunchNgramSlotRows(const NGramDev &lm, int W, int N, int B, int V, const int *parent, const int *token,
+                        const int *state_in, int *state_out, float *rows, cudaStream_t s);
 // A decoding graph's tables on one device (wfst.h WfstHost), for the TLG Viterbi beam search (wfst_decode.cu)
 struct WfstDev {
     const int *arc_off = nullptr, *eps_off = nullptr, *dst = nullptr, *tok = nullptr, *olabel = nullptr, *fid = nullptr,
@@ -306,6 +311,11 @@ int LaunchRnntBeamStep(const void *rows, const void *enc, int dtype, int mode, i
                        const int *len, int blank, void *ws, int *parent, int *token, int *node, double *score, cudaStream_t s);
 int LaunchRnntBeamFinish(int N, int T, int B, int nbest, const void *ws, const int *node, const double *score, int *tokens,
                          int *lengths, float *scores, cudaStream_t s);
+// the step with LM / ILM fusion (either row block may be null, not both); lm_part (N, B) fp64 read and written
+int LaunchRnntBeamStepFused(const void *rows, const void *enc, int dtype, int mode, int N, int T, int B, int V, int t,
+                            const int *len, int blank, void *ws, int *parent, int *token, int *node, double *score,
+                            const void *lm_rows, int lm_dtype, double alpha, double beta, const void *ilm_rows, int ilm_dtype,
+                            double ilm_weight, double *lm_part, cudaStream_t s);
 // CTC-T beam search (ctct_decode.cu): init and one step per frame over a workspace that starts with the transducer beam
 // search's tries (same stride), so that LaunchRnntBeamFinish finishes it
 size_t CtctBeamWsBytes(int N, int T, int B);

@@ -1,16 +1,20 @@
 """Beam search for CAT's RNN-T transducers (``topo: rnnt``) on the GPU: the drop-in for ``cat/rnnt/rnnt_decoder.py``'s
-``RNNTDecoder`` without an external LM, ILM estimation or ``<eos>`` early stop.  The networks run in torch, under the
-caller's autocast; the search (exact top-B, prefix trie, fixed-order merge) is one native launch per frame
-(``cat_b200/csrc/rnnt_decode.cu``).  Definition and differences from CAT: DESIGN.md §7 "Transducer beam search".
+``RNNTDecoder``, with CAT's external LM fusion (``alpha``, ``beta``) and ILM estimation (``ilm_weight``), without the
+``<eos>`` early stop.  The networks run in torch, under the caller's autocast; the search (exact top-B, prefix trie,
+fixed-order merge, the fusion terms) is one native launch per frame (``cat_b200/csrc/rnnt_decode.cu``), and an n-gram LM's
+rows are one more.  Definition and differences from CAT: DESIGN.md §7 "Transducer beam search" and "RNN-T beam search with
+LM fusion".
 """
 from __future__ import annotations
 
+import math
 from typing import List, Optional, Tuple
 
 import torch
 
 from . import _lib
 from ._C import _DTYPES, _check, _stream
+from .ngram import NGramLM
 from .rnnt import _on_device
 from .rnnt_simple import _int32
 
@@ -43,36 +47,109 @@ def _check_args(enc_out, frame_lens, beam_size, nbest, blank, name) -> Tuple[int
     return N, Tmax, nbest
 
 
-def _check_state(predictor, state, R: int, name):
-    """The predictor states the search can carry per slot: None, or a tuple of 3-D tensors with the batch on dim 1."""
+def _check_state(predictor, state, R: int, name, what="predictor"):
+    """The predictor (or LM) states the search can carry per slot: None, or a tuple of 3-D tensors with the batch on dim 1."""
     if state is None:
         return
     if isinstance(state, tuple) and all(isinstance(s, torch.Tensor) and s.dim() == 3 and s.shape[1] == R for s in state):
         return
-    raise NotImplementedError(f"{name}: the state of predictor {type(predictor).__name__} is neither None nor a "
+    raise NotImplementedError(f"{name}: the state of {what} {type(predictor).__name__} is neither None nor a "
                               "tuple of 3-D tensors with the batch on dim 1 (an LSTM's); it cannot be carried per beam slot")
+
+
+def _carry(step, out, state, src, tok, ext, blank: int, check):
+    """Each slot's network output and state after a frame: its parent's (rows ``src`` of ``out`` and of dim 1 of ``state``),
+    advanced by ``step(tokens (R, 1), state)`` where the slot emitted a token (``ext``).  The predictor and a neural LM are
+    carried alike; ``check`` validates the new state."""
+    R = src.shape[0]
+    out_par = out.index_select(0, src)
+    st_par = None if state is None else tuple(s.index_select(1, src) for s in state)
+    out_new, st_new = step(torch.where(ext, tok, blank).long().reshape(R, 1), st_par)
+    check(st_new)
+    out = torch.where(ext.view(R, *([1] * (out_new.dim() - 1))), out_new, out_par.to(out_new.dtype))
+    state = None if st_new is None else tuple(
+        torch.where(ext.view(1, R, 1), sn, sp.to(sn.dtype)) for sn, sp in zip(st_new, st_par))
+    return out, state
+
+
+# CAT's LMs the search cannot carry per slot, and what to use instead
+_REFUSED_LMS = {
+    "NGram": "load its ARPA file (cat/utils/pipeline/ngram.sh --arpa) as cat_b200.ngram.NGramLM(<ARPA>, labels) instead",
+    "MultiDecoder": "several LMs at once are not supported",
+    "PretrainedTransformer": "a Transformer LM's state grows with the prefix",
+    "CausalTransformer": "a Transformer LM's state grows with the prefix",
+}
+
+
+def _check_lm(lm, caller):
+    """An LM the search can fuse (NotImplementedError otherwise): an ``NGramLM``, or a module with ``get_log_prob``."""
+    name = type(lm).__name__
+    if isinstance(lm, NGramLM):
+        return
+    if name in _REFUSED_LMS:
+        raise NotImplementedError(f"{caller}: LM {name} is not supported: {_REFUSED_LMS[name]}")
+    if not callable(getattr(lm, "get_log_prob", None)):
+        raise NotImplementedError(f"{caller}: LM {name} is not supported: the LM must be a cat_b200.ngram.NGramLM or a "
+                                  "module with get_log_prob(tokens (R, 1), state) -> (log-probs (R, 1, V), state)")
+
+
+def _check_ilm_joiner(joiner, caller):
+    """A joiner the ILM can be estimated from (NotImplementedError otherwise): one with ``impl_forward``, except LogAdd."""
+    name = type(joiner).__name__
+    if name == "LogAdd":
+        raise NotImplementedError(f"{caller}: ILM estimation is not supported for the LogAdd joiner (its impl_forward "
+                                  "raises in CAT)")
+    if not callable(getattr(joiner, "impl_forward", None)):
+        raise NotImplementedError(f"{caller}: ILM estimation needs the joiner's impl_forward; {name} has none")
+
+
+def _weight(x, what, caller) -> float:
+    if isinstance(x, bool) or not isinstance(x, (int, float)) or not math.isfinite(x):
+        raise ValueError(f"{caller}: {what} must be a finite number, not {x!r}")
+    return float(x)
 
 
 class _Joiner:
     """How the joiner's rows for a frame reach the kernel: LogAdd (f and g rows), JointNet in "add" mode (raw logits from
     fc(fc_enc(enc) + fc_dec(pn)), fc_enc applied once per call) or any other joiner (log-probs of joiner(enc, pn))."""
 
-    def __init__(self, joiner, enc_out, caller):
+    def __init__(self, joiner, enc_out, caller, ilm=False):
         name = type(joiner).__name__
         self.joiner = joiner
         self.caller = caller
+        self.ilm = ilm
         if name == "LogAdd":
             self.mode = _MODE_LOGADD
             self.f = enc_out.contiguous()
         elif name == "JointNet" and getattr(joiner, "_mode", None) == "add":
             self.mode = _MODE_LOGITS
             self.fe = joiner.fc_enc(enc_out)
+            if ilm:   # impl_forward(0, pn) = fc(fc_enc(0) + fc_dec(pn)): fc_enc(0) is fc_enc's bias, once per call
+                self.fe0 = joiner.fc_enc(torch.zeros_like(enc_out[:1, :1]))
         else:
             self.mode = _MODE_LOGPROBS
             self.enc = enc_out
 
-    def rows(self, t: int, pn_out: torch.Tensor, N: int, B: int) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
-        """(rows (N*B, V) contiguous, f (N, Tmax, V) of the rows' dtype for LogAdd else None)"""
+    def ilm_rows(self, pn_out: torch.Tensor, R: int) -> torch.Tensor:
+        """The ILM logits (R, V) of every slot, impl_forward(zeros, pn) (mode 0 joiners; JointNet "add" shares rows()'s
+        fc_dec)"""
+        enc = torch.zeros((R, 1, self.enc.shape[2]), dtype=self.enc.dtype, device=self.enc.device)
+        return self.joiner.impl_forward(enc, pn_out).reshape(R, -1).contiguous()
+
+    def rows(self, t: int, pn_out: torch.Tensor, N: int, B: int):
+        """(rows (N*B, V) contiguous, f (N, Tmax, V) of the rows' dtype for LogAdd else None, and with ``ilm`` the ILM
+        logits (N*B, V))"""
+        R = N * B
+        if self.mode == _MODE_LOGITS:
+            fd = self.joiner.fc_dec(pn_out).reshape(N, B, -1)
+            rows = self.joiner.fc(self.fe[:, t, None, :] + fd).reshape(R, -1).contiguous()
+            if not self.ilm:
+                return rows, None
+            return rows, None, self.joiner.fc(self.fe0 + fd).reshape(R, -1).contiguous()
+        out = self._rows(t, pn_out, N, B)
+        return out + (self.ilm_rows(pn_out, R),) if self.ilm else out
+
+    def _rows(self, t: int, pn_out: torch.Tensor, N: int, B: int) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         R = N * B
         if self.mode == _MODE_LOGADD:
             g = pn_out.reshape(R, -1)
@@ -83,18 +160,92 @@ class _Joiner:
             if self.f.dtype != dt:
                 self.f = self.f.to(dt)
             return g.to(dt).contiguous(), self.f
-        if self.mode == _MODE_LOGITS:
-            h = self.fe[:, t, None, :] + self.joiner.fc_dec(pn_out).reshape(N, B, -1)
-            return self.joiner.fc(h).reshape(R, -1).contiguous(), None
         enc = self.enc[:, t, None, None, :].expand(N, B, 1, -1).reshape(R, 1, -1)
         return self.joiner(enc, pn_out).reshape(R, -1).contiguous(), None
 
 
-def _beam_search(name: str, family: str, enc_out, frame_lens, predictor, joiner, beam_size, nbest, blank):
+class _Fusion:
+    """The external LM and ILM terms of the RNN-T search (DESIGN.md §7 "RNN-T beam search with LM fusion"), checked before
+    anything runs.  The LM term is on iff ``lm`` is given and alpha != 0, the ILM term iff ilm_weight != 0.  Per call it
+    carries the LM's per-slot state: an ``NGramLM``'s int32 states (double-buffered) and rows from
+    ``ccb_ngram_slot_rows``, or a neural LM's output and state, carried like the predictor's."""
+
+    def __init__(self, lm, alpha, beta, ilm_weight, joiner, blank, caller):
+        self.alpha = _weight(alpha, "alpha", caller)
+        self.beta = _weight(beta, "beta", caller)
+        self.ilm_weight = _weight(ilm_weight, "ilm_weight", caller)
+        self.lm = lm if lm is not None and self.alpha != 0.0 else None
+        self.ilm = self.ilm_weight != 0.0
+        self.caller = caller
+        if self.lm is not None:
+            _check_lm(self.lm, caller)
+            if isinstance(self.lm, NGramLM) and blank != 0:
+                raise ValueError(f"{caller}: an NGramLM's label 0 is the blank, so blank must be 0, not {blank}")
+        if self.ilm:
+            _check_ilm_joiner(joiner, caller)
+
+    @property
+    def active(self) -> bool:
+        return self.lm is not None or self.ilm
+
+    def start(self, N: int, B: int, blank: int, dev):
+        """The LM at the start of every hypothesis (no native call yet)"""
+        self.N, self.B, self.R, self.blank = N, B, N * B, blank
+        if isinstance(self.lm, NGramLM):
+            self.state = [torch.empty((N, B), dtype=torch.int32, device=dev) for _ in range(2)]
+            self.rows = None
+        elif self.lm is not None:
+            self.out, self.st = self.lm.get_log_prob(torch.full((self.R, 1), blank, dtype=torch.long, device=dev), None)
+            _check_state(self.lm, self.st, self.R, self.caller, "LM")
+
+    def check_v(self, V: int):
+        """The LM's V against the joiner's (ValueError, before the first native call)"""
+        lv = self.lm.V if isinstance(self.lm, NGramLM) else None if self.lm is None else int(self.out.shape[-1])
+        if lv is not None and lv != V:
+            raise ValueError(f"{self.caller}: the LM has V = {lv} labels, the joiner V = {V}")
+        if isinstance(self.lm, NGramLM) and self.rows is None:
+            self.rows = torch.empty((self.R, V), dtype=torch.float32, device=self.state[0].device)
+
+    def _ngram_rows(self, parent=None, token=None):
+        # the next beam's states go to the other buffer; rows are overwritten (stream order keeps the last step's reads)
+        src, dst = self.state
+        _check(_lib.lib().ccb_ngram_slot_rows(
+            self.lm.handle, self.N, self.B, self.rows.shape[1], None if parent is None else parent.data_ptr(),
+            None if token is None else token.data_ptr(), None if parent is None else src.data_ptr(), dst.data_ptr(),
+            self.rows.data_ptr(), _stream(dst.device)), self.caller)
+        self.state.reverse()
+
+    def first(self):
+        """The first frame's LM rows (after the workspace's init)"""
+        if isinstance(self.lm, NGramLM):
+            self._ngram_rows()
+
+    def lm_rows(self) -> Optional[torch.Tensor]:
+        """The current beam's LM log-prob rows (R, V), or None without the LM term"""
+        if self.lm is None:
+            return None
+        if isinstance(self.lm, NGramLM):
+            return self.rows
+        rows = self.out.reshape(self.R, -1)
+        return (rows if rows.dtype in _DTYPES else rows.float()).contiguous()
+
+    def advance(self, src, tok, ext, parent, token):
+        """Every slot's LM after a frame: its parent's, advanced by the token it emitted"""
+        if isinstance(self.lm, NGramLM):
+            self._ngram_rows(parent, token)
+        elif self.lm is not None:
+            self.out, self.st = _carry(self.lm.get_log_prob, self.out, self.st, src, tok, ext, self.blank,
+                                       lambda st: _check_state(self.lm, st, self.R, self.caller, "LM"))
+
+
+def _beam_search(name: str, family: str, enc_out, frame_lens, predictor, joiner, beam_size, nbest, blank,
+                 fusion: Optional[_Fusion] = None):
     """The frame loop of the transducer searches: ``family`` "rnnt" or "ctct" picks the native ws-bytes, init and step entries
     (``ccb_<family>_beam_*``); both are finished by ``ccb_rnnt_beam_finish``.  ``name`` is the calling function's, for its
     errors.  Each frame runs the predictor once over all N*B slots, every slot keeping its parent's output and state or
-    advancing them by the token it emitted; nothing synchronises the host."""
+    advancing them by the token it emitted; nothing synchronises the host.  With an active ``fusion`` (RNN-T only) the step
+    is ``ccb_rnnt_beam_step_fused``, the LM is carried per slot like the predictor, and the returned scores are acoustic
+    plus LM part."""
     N, Tmax, nbest = _check_args(enc_out, frame_lens, beam_size, nbest, blank, name)
     B, R = beam_size, N * beam_size
     dev = enc_out.device
@@ -108,7 +259,9 @@ def _beam_search(name: str, family: str, enc_out, frame_lens, predictor, joiner,
         if Tmax:
             pn_out, state = predictor(torch.full((R, 1), blank, dtype=torch.long, device=dev), None)
             _check_state(predictor, state, R, name)
-            join = _Joiner(joiner, enc_out, name)
+            join = _Joiner(joiner, enc_out, name, ilm=fusion is not None and fusion.ilm)
+            if fusion is not None:
+                fusion.start(N, B, blank, dev)
         parent = torch.empty((N, B), dtype=torch.int32, device=dev)
         token = torch.empty((N, B), dtype=torch.int32, device=dev)
         node = torch.empty((N, B), dtype=torch.int32, device=dev)
@@ -117,6 +270,7 @@ def _beam_search(name: str, family: str, enc_out, frame_lens, predictor, joiner,
         lengths = torch.empty((N, nbest), dtype=torch.int32, device=dev)
         scores = torch.empty((N, nbest), dtype=torch.float32, device=dev)
         slot_base = (torch.arange(N, device=dev, dtype=torch.long) * B)[:, None]
+        lm_part = torch.zeros((N, B), dtype=torch.float64, device=dev) if fusion is not None else None
         ws = None
 
         def init():   # (after the first frame's rows: every argument error is raised before a native call)
@@ -128,31 +282,46 @@ def _beam_search(name: str, family: str, enc_out, frame_lens, predictor, joiner,
         if Tmax == 0:
             init()
         for t in range(Tmax):
-            rows, f = join.rows(t, pn_out, N, B)
+            rows, f, *ilm = join.rows(t, pn_out, N, B)
             if rows.dtype not in _DTYPES:
                 rows = rows.float()
                 f = f.float() if f is not None else None
             V = int(rows.shape[1])
             if blank >= V:
                 raise ValueError(f"{name}: blank = {blank} is not a label of the joiner's V = {V}")
+            if fusion is not None:
+                fusion.check_v(V)
             if t == 0:
                 init()
-            _check(entry("step")(rows.data_ptr(), f.data_ptr() if f is not None else None, _DTYPES[rows.dtype], join.mode,
-                                 N, Tmax, B, V, t, lens.data_ptr(), blank, ws.data_ptr(), parent.data_ptr(),
-                                 token.data_ptr(), node.data_ptr(), score.data_ptr(), _stream(dev)), name)
+                if fusion is not None:
+                    fusion.first()
+            if fusion is None:
+                _check(entry("step")(rows.data_ptr(), f.data_ptr() if f is not None else None, _DTYPES[rows.dtype],
+                                     join.mode, N, Tmax, B, V, t, lens.data_ptr(), blank, ws.data_ptr(), parent.data_ptr(),
+                                     token.data_ptr(), node.data_ptr(), score.data_ptr(), _stream(dev)), name)
+            else:
+                lmr = fusion.lm_rows()
+                ilr = ilm[0] if ilm else None
+                if ilr is not None and ilr.dtype not in _DTYPES:
+                    ilr = ilr.float()
+                _check(L.ccb_rnnt_beam_step_fused(
+                    rows.data_ptr(), f.data_ptr() if f is not None else None, _DTYPES[rows.dtype], join.mode, N, Tmax, B, V,
+                    t, lens.data_ptr(), blank, ws.data_ptr(), parent.data_ptr(), token.data_ptr(), node.data_ptr(),
+                    score.data_ptr(), None if lmr is None else lmr.data_ptr(), _DTYPES[lmr.dtype] if lmr is not None else 0,
+                    fusion.alpha, fusion.beta, None if ilr is None else ilr.data_ptr(),
+                    _DTYPES[ilr.dtype] if ilr is not None else 0, fusion.ilm_weight, lm_part.data_ptr(), _stream(dev)), name)
             if t + 1 == Tmax:
                 break
-            # each slot's predictor output and state: its parent's, advanced by the token it emitted (if any)
+            # each slot's predictor output and state (and LM): its parent's, advanced by the token it emitted (if any)
             src = (slot_base + parent.long()).reshape(R)
             tok = token.reshape(R)
             ext = tok >= 0
-            pn_par = pn_out.index_select(0, src)
-            st_par = None if state is None else tuple(s.index_select(1, src) for s in state)
-            out_new, st_new = predictor(torch.where(ext, tok, blank).long().reshape(R, 1), st_par)
-            _check_state(predictor, st_new, R, name)
-            pn_out = torch.where(ext.view(R, *([1] * (out_new.dim() - 1))), out_new, pn_par.to(out_new.dtype))
-            state = None if st_new is None else tuple(
-                torch.where(ext.view(1, R, 1), sn, sp.to(sn.dtype)) for sn, sp in zip(st_new, st_par))
+            pn_out, state = _carry(predictor, pn_out, state, src, tok, ext, blank,
+                                   lambda st: _check_state(predictor, st, R, name))
+            if fusion is not None:
+                fusion.advance(src, tok, ext, parent, token)
+        if fusion is not None:
+            score.add_(lm_part)   # the hypothesis score: acoustic plus LM part
         _check(L.ccb_rnnt_beam_finish(N, Tmax, B, nbest, ws.data_ptr(), node.data_ptr(), score.data_ptr(),
                                       tokens.data_ptr(), lengths.data_ptr(), scores.data_ptr(), _stream(dev)), name)
         lens.record_stream(torch.cuda.current_stream(dev))
@@ -160,35 +329,47 @@ def _beam_search(name: str, family: str, enc_out, frame_lens, predictor, joiner,
 
 
 def rnnt_beam_search(enc_out: torch.Tensor, frame_lens: torch.Tensor, predictor, joiner, beam_size: int = 5,
-                     nbest: Optional[int] = None, blank: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                     nbest: Optional[int] = None, blank: int = 0, lm=None, alpha: float = 0.0, beta: float = 0.0,
+                     ilm_weight: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """The nbest (default beam_size) best label sequences of every utterance by CAT's RNA beam search (DESIGN.md §7
-    "Transducer beam search"), blank = bos = ``blank``.
+    "Transducer beam search"), blank = bos = ``blank``, with CAT's LM fusion and ILM estimation (§7 "RNN-T beam search with
+    LM fusion").
 
     enc_out (N, T, H) on a CUDA device; frame_lens (N,) int32 or int64 on the CPU or that device (T_n in [0, T]; an
     utterance with T_n = 0 gets the empty hypothesis, score 0).  ``predictor(tokens (R, 1), state)`` returns (out (R, 1, H'),
     state) with a state that is None or a tuple of 3-D tensors with the batch on dim 1; ``joiner`` is CAT's LogAdd, a
     JointNet or any module called as joiner(enc (R, 1, H), pn (R, 1, H')) returning log-probs.  Returns device tensors
     tokens (N, nbest, T) int32 -1 padded, lengths (N, nbest) int32 (-1 past the hypotheses found) and scores (N, nbest)
-    fp32, best first.  The frame loop runs to T; nothing synchronises the host."""
-    return _beam_search("rnnt_beam_search", "rnnt", enc_out, frame_lens, predictor, joiner, beam_size, nbest, blank)
+    fp32, best first.  The frame loop runs to T; nothing synchronises the host.
+
+    LM fusion (on iff ``lm`` is given and alpha != 0): every extension by token k != blank adds beta + alpha ln P_LM(k |
+    prefix) to the hypothesis's LM part.  ``lm`` is a ``cat_b200.ngram.NGramLM`` loaded for the joiner's V labels (label 0
+    the blank, so blank must be 0), or a module whose ``get_log_prob(tokens (R, 1), state)`` returns (log-probs (R, 1, V),
+    state) with a state like the predictor's (CAT's LSTM LM); any other LM raises NotImplementedError.  ILM estimation (on
+    iff ilm_weight != 0): every extension adds ilm_weight (I[k] - logsumexp over the non-blank I), I the joiner's
+    impl_forward(zeros, pn) logits (JointNet "add": fc(fc_enc's bias + fc_dec(pn))); LogAdd and joiners without
+    impl_forward raise NotImplementedError.  Candidates rank by acoustic score plus LM part; merged hypotheses add only
+    their acoustic scores and keep the LM part of the first; the returned scores are acoustic plus LM part.  alpha, beta
+    and ilm_weight may have any sign."""
+    fusion = _Fusion(lm, alpha, beta, ilm_weight, joiner, blank, "rnnt_beam_search")
+    return _beam_search("rnnt_beam_search", "rnnt", enc_out, frame_lens, predictor, joiner, beam_size, nbest, blank,
+                        fusion if fusion.active else None)
 
 
 class RNNTDecoder:
     """CAT's ``cat.rnnt.rnnt_decoder.RNNTDecoder`` with its constructor, decoding on the GPU through ``rnnt_beam_search``.
-    Not supported (NotImplementedError): an LM with alpha != 0, ILM estimation with ilm_weight != 0, an ``<eos>`` early stop
-    and bos_id != blank_id.  alpha == 0 drops the LM, as in CAT."""
+    CAT's rules: alpha == 0 drops the LM whatever beta is, and ILM estimation is on iff est_ilm and ilm_weight != 0.
+    ``lm_module`` is a ``cat_b200.ngram.NGramLM`` (in place of CAT's KenLM ``NGram``) or a neural LM with CAT's
+    ``get_log_prob`` and an LSTM-like state.  Returned scores are CAT's ``Hypothesis.score``: acoustic plus LM part.  Not
+    supported (NotImplementedError, raised here): other LMs (KenLM ``NGram``, ``MultiDecoder``, Transformers), ILM
+    estimation with LogAdd or a joiner without ``impl_forward``, an ``<eos>`` early stop and bos_id != blank_id."""
 
     def __init__(self, predictor, joiner, blank_id: int = 0, bos_id: int = 0, eos_id: int = -1, beam_size: int = 5,
                  nbest: int = -1, lm_module=None, alpha: float = 0.0, beta: float = 0.0, est_ilm: bool = False,
                  ilm_weight: float = 0.0):
         if bos_id != blank_id:
             raise NotImplementedError(f"RNNTDecoder: bos_id ({bos_id}) must equal blank_id ({blank_id}), as in CAT")
-        if alpha == 0.0:
-            lm_module = None
-        if lm_module is not None:
-            raise NotImplementedError("RNNTDecoder: external LM fusion (lm_module with alpha != 0) is not supported")
-        if est_ilm and ilm_weight != 0.0:
-            raise NotImplementedError("RNNTDecoder: ILM estimation (est_ilm with ilm_weight != 0) is not supported")
+        fusion = _Fusion(lm_module, alpha, beta, ilm_weight if est_ilm else 0.0, joiner, blank_id, "RNNTDecoder")
         if eos_id not in (-1, blank_id):
             raise NotImplementedError(f"RNNTDecoder: the <eos> early stop (eos_id = {eos_id}) is not supported")
         if isinstance(beam_size, bool) or not isinstance(beam_size, int) or not 1 <= beam_size <= MAX_BEAM:
@@ -204,12 +385,15 @@ class RNNTDecoder:
         self.eos_id = -1
         self.beam_size = beam_size
         self.nbest = min(nbest, beam_size)
+        self.lm, self.alpha, self.beta = fusion.lm, fusion.alpha, fusion.beta
+        self.ilm_weight = fusion.ilm_weight
 
     def __call__(self, enc_out: torch.Tensor, frame_lens: Optional[torch.Tensor] = None
                  ) -> List[Tuple[List[List[int]], List[float]]]:
         """[(token lists without bos, scores), ...] per utterance, best first: CAT's return value.  One host copy."""
         return _to_lists(*rnnt_beam_search(enc_out, _frame_lens(enc_out, frame_lens), self.predictor, self.joiner,
-                                           self.beam_size, self.nbest, self.blank_id))
+                                           self.beam_size, self.nbest, self.blank_id, self.lm, self.alpha, self.beta,
+                                           self.ilm_weight))
 
 
 def _frame_lens(enc_out, frame_lens):

@@ -518,6 +518,31 @@ int ccb_rnnt_beam_step(const void *rows, const void *enc, int dtype, int mode, i
 int ccb_rnnt_beam_finish(int N, int Tmax, int beam, int nbest, const void *workspace, const int *node, const double *score,
                          int *tokens, int *lengths, float *scores, void *stream);
 
+/* The transducer beam search step with an external LM and / or an internal-LM (ILM) estimate fused in, as CAT's RNNTDecoder
+ * does with --alpha / --beta / --ilm-weight (DESIGN.md §7 "RNN-T beam search with LM fusion").  Arguments and slot arrays as
+ * ccb_rnnt_beam_step, plus lm_part (N, beam) fp64: each slot's LM part, read for the current beam and written for the next
+ * (ccb_rnnt_beam_init does not touch it: zero it for the first frame).  lm_rows (N*beam, V) are the slots' external-LM
+ * log-probs, ilm_rows (N*beam, V) their ILM logits, each in its own CCB_DTYPE_* code dtype; a null block turns its term off,
+ * and both null is an error.  alpha, beta, ilm_weight: finite, any sign.  Candidate (r, k) ranks by
+ *   ((score_r + lp_r[k]) + lm_part_r) + [k != blank] term_r[k],
+ *   term_r[k] = (beta + alpha LM_r[k]) + ilm_weight (I_r[k] - logsumexp_{j != blank} I_r[j])   (the absent term dropped),
+ * fp64, I_r[k] - lse in fp32; a -inf LM or ILM entry makes the candidate -inf.  Selection and merge as ccb_rnnt_beam_step,
+ * except that a new slot's score is the logaddexp of its candidates' acoustic parts score_r + lp_r[k] alone and its LM part
+ * is its first candidate's: lm_part_r for blank, lm_part_r + term_r[k] for an extension.  The hypothesis score is
+ * score + lm_part: add it into score before ccb_rnnt_beam_finish.  Dead slots get lm_part 0. */
+int ccb_rnnt_beam_step_fused(const void *rows, const void *enc, int dtype, int mode, int N, int Tmax, int beam, int V, int t,
+                             const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node,
+                             double *score, const void *lm_rows, int lm_dtype, double alpha, double beta,
+                             const void *ilm_rows, int ilm_dtype, double ilm_weight, double *lm_part, void *stream);
+/* A token n-gram LM's (ccb_ngram_create) rows for ccb_rnnt_beam_step_fused.  For every slot q of N*beam: its LM state is
+ * state_in[n*beam + parent[q]] advanced by token[q] when token[q] >= 0 (the back-off walk's destination rule), or, with
+ * parent null (token and state_in then unused), the state after </s> from the root: the start of every hypothesis.  It is
+ * written to state_out[q] (int32, a different array from state_in), and rows[q] (V fp32) gets ln P(label k | state) for
+ * every k, the fp64 log10 value times ln 10 rounded once; a label without an LM word (label 0) gets 0.  The LM must have
+ * been loaded for V labels and have at most 25600 words. */
+int ccb_ngram_slot_rows(const void *lm, int N, int beam, int V, const int *parent, const int *token, const int *state_in,
+                        int *state_out, float *rows, void *stream);
+
 /* CTC-T (CTC-Transducer) prefix beam search, one launch per frame, with the arguments and slot arrays of the transducer beam
  * search above; every frame emits one symbol, as in ccb_ctct_forward.  Each live slot holds a prefix with masses b (last
  * emission blank, or none yet) and n (last emission its last token) in the workspace; its score is s = b (+) n.
