@@ -1248,6 +1248,67 @@ int ccb_ngram_slot_rows(const void *lm, int N, int beam, int V, const int *paren
     return 0;
 }
 
+int ccb_lm_mix_slot_rows(int n_ngram, const void *const *ngrams, const double *ngram_w, const int *const *state_in,
+                         int *const *state_out, int n_neural, const void *const *neural_rows, const int *neural_dtype,
+                         const double *neural_w, const int *order, int N, int beam, int V, const int *parent,
+                         const int *token, float *rows, void *stream) {
+    g_err.clear();
+    const int K = n_ngram + n_neural;
+    if (n_ngram < 0 || n_neural < 0 || K < 1 || K > kLmMixMax)
+        return Fail("lm_mix_slot_rows: a mix has 1 to " + std::to_string(kLmMixMax) + " members, not " + std::to_string(K));
+    if (N <= 0 || V <= 0) return Fail("lm_mix_slot_rows: N and V must be positive");
+    if (beam < 1 || beam > kBeamMax)
+        return Fail("lm_mix_slot_rows: beam must lie in [1, " + std::to_string(kBeamMax) + "], not " + std::to_string(beam));
+    if (!order || (parent && !token) || !rows || (n_ngram && (!ngrams || !ngram_w || !state_out || (parent && !state_in))) ||
+        (n_neural && (!neural_rows || !neural_dtype || !neural_w)))
+        return Fail("lm_mix_slot_rows: missing buffer");
+    LmMixDev mix;
+    mix.K = K;
+    bool seen[kLmMixMax] = {};
+    int W = 0;
+    for (int i = 0; i < K; ++i) {
+        const int j = order[i];
+        if (j < 0 || j >= K || seen[j])
+            return Fail("lm_mix_slot_rows: order must be a permutation of the members 0 .. " + std::to_string(K - 1));
+        seen[j] = true;
+        LmMixMember &m = mix.m[i];
+        if (j < n_ngram) {
+            if (!ngrams[j]) return Fail("lm_mix_slot_rows: missing LM");
+            if (!state_out[j] || (parent && !state_in[j])) return Fail("lm_mix_slot_rows: missing buffer");
+            NGram *g = reinterpret_cast<NGram *>(const_cast<void *>(ngrams[j]));
+            if (g->host.V != V)
+                return Fail("lm_mix_slot_rows: an LM was loaded for " + std::to_string(g->host.V) + " labels, V is " +
+                            std::to_string(V));
+            m.w = ngram_w[j];
+            m.W = g->host.W;
+            m.state_in = parent ? state_in[j] : nullptr;
+            m.state_out = state_out[j];
+            W = std::max(W, m.W);
+        } else {
+            const int k = j - n_ngram;
+            if (!neural_rows[k]) return Fail("lm_mix_slot_rows: missing buffer");
+            if (!KnownDtype(neural_dtype[k])) return FailDtype("lm_mix_slot_rows", neural_dtype[k]);
+            m.rows = neural_rows[k];
+            m.dtype = neural_dtype[k];
+            m.w = neural_w[k];
+        }
+        if (!std::isfinite(m.w) || m.w == 0.0) return Fail("lm_mix_slot_rows: the weights must be finite and non-zero");
+    }
+    if (LmMixSlotRowsSmemBytes(W, V) > 200 * 1024)
+        return Fail("lm_mix_slot_rows: the largest LM has " + std::to_string(W) + " words and V is " + std::to_string(V) +
+                    "; the rows are built in shared memory, which holds at most " + std::to_string(200 * 1024 / 8) +
+                    " words plus labels");
+    for (int i = 0; i < K; ++i) {   // the n-gram tables on the device (uploaded once per LM and device)
+        if (mix.m[i].rows) continue;
+        const NGramDev *lmd = nullptr;
+        if (EnsureNGram(reinterpret_cast<NGram *>(const_cast<void *>(ngrams[order[i]])), &lmd)) return 1;
+        mix.m[i].lm = *lmd;
+    }
+    const int rc = LaunchLmMixSlotRows(mix, W, N, beam, V, parent, token, rows, (cudaStream_t)stream);
+    if (rc) return FailCuda("lm_mix_slot_rows", (cudaError_t)rc);
+    return 0;
+}
+
 /* ---- TLG decoding graph and its Viterbi beam search ------------------------------------------- */
 // A decoding graph handle (ccb_wfst_create): the host tables, and their device copies, uploaded by the first search that
 // uses the graph on a device and freed by ccb_wfst_destroy

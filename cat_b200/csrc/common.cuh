@@ -258,6 +258,26 @@ int LaunchBeamSearch(const DeviceGraph *g, const void *y, int y_dtype, int N, in
 size_t NgramSlotRowsSmemBytes(int W);
 int LaunchNgramSlotRows(const NGramDev &lm, int W, int N, int B, int V, const int *parent, const int *token,
                         const int *state_in, int *state_out, float *rows, cudaStream_t s);
+// The rows of a weighted LM mix for the fused RNN-T step (rnnt_decode.cu): one CTA per slot of N*B.  Member i is an n-gram
+// LM (rows null: its tables, word count W and (N, B) int32 state arrays) or a neural LM (its (N*B, V) row block in the
+// CCB_DTYPE_* code dtype); w is its weight.  W: the largest n-gram word count (0 without one); the dynamic shared memory is
+// LmMixSlotRowsSmemBytes(W, V)
+constexpr int kLmMixMax = 8;
+struct LmMixMember {
+    NGramDev lm;
+    const int *state_in = nullptr;
+    int *state_out = nullptr;
+    const void *rows = nullptr;
+    int dtype = 0, W = 0;
+    double w = 0.0;
+};
+struct LmMixDev {
+    int K = 0;
+    LmMixMember m[kLmMixMax];
+};
+size_t LmMixSlotRowsSmemBytes(int W, int V);
+int LaunchLmMixSlotRows(const LmMixDev &mix, int W, int N, int B, int V, const int *parent, const int *token, float *rows,
+                        cudaStream_t s);
 // A decoding graph's tables on one device (wfst.h WfstHost), for the TLG Viterbi beam search (wfst_decode.cu)
 struct WfstDev {
     const int *arc_off = nullptr, *eps_off = nullptr, *dst = nullptr, *tok = nullptr, *olabel = nullptr, *fid = nullptr,

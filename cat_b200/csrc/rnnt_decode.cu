@@ -12,7 +12,8 @@
 // The FUSE instantiation adds an external LM and/or an ILM estimate (DESIGN.md §7 "RNN-T beam search with LM fusion"):
 // each slot also carries an LM part lm_r (fp64, caller-owned), a candidate ranks by ((s_r + v) + lm_r) + term, and a new
 // slot keeps the LM part of its first candidate while only the acoustic parts s_r + v are merged.  The instantiation
-// without it is the plain search.  ngram_slot_rows_kernel produces the n-gram LM's rows for the fused step.
+// without it is the plain search.  ngram_slot_rows_kernel produces the n-gram LM's rows for the fused step, and
+// lm_mix_slot_rows_kernel the rows of a weighted mix of n-gram and neural LMs.
 #include "ngram.h"
 #include "transducer_beam.cuh"
 
@@ -337,6 +338,78 @@ __global__ void __launch_bounds__(kRowThreads) ngram_slot_rows_kernel(const NGra
     }
 }
 
+// acc after a member's value v of weight w: the product rounded on its own, then the sum (the first product starts it);
+// a -inf value, and a -inf sum, stay -inf
+__device__ __forceinline__ void MixAdd(double &acc, bool first, double w, float v) {
+    if (v == -INFINITY || (!first && acc == kNegInf)) { acc = kNegInf; return; }
+    const double x = __dmul_rn(w, (double)v);
+    acc = first ? x : __dadd_rn(acc, x);
+}
+
+// One CTA per slot q of the next beam: the mix row MIX[k] = sum_i w_i LM_i[k] of an LM mix (DESIGN.md §7 "RNN-T beam search
+// with an LM mix"), fp32.  Members are visited in the mix's order.  An n-gram member advances its state and builds its word
+// row exactly as ngram_slot_rows_kernel does (the shared word row is rebuilt per member), and contributes the fp32 value
+// that kernel writes; a neural member contributes its row block's entry, widened exactly.  Each product w_i LM_i[k] and
+// each sum is rounded in fp64 on its own, the first product starting the sum; a -inf in any member makes the entry -inf.
+// Each thread owns the labels k = tid (mod blockDim) of the fp64 accumulator for the whole launch.
+__global__ void __launch_bounds__(kRowThreads) lm_mix_slot_rows_kernel(const LmMixDev mix, int V, int B, const int *parent,
+                                                                       const int *token, float *rows) {
+    extern __shared__ double smem[];   // [V] label accumulator, then [W] word row
+    double *acc = smem, *wrow = smem + V;
+    __shared__ int s_chain[kChainMax];
+    __shared__ double s_c[kChainMax];
+    __shared__ int s_len;
+    const int q = blockIdx.x, tid = threadIdx.x;
+    const size_t row = (size_t)q * V;
+    for (int i = 0; i < mix.K; ++i) {
+        const LmMixMember &m = mix.m[i];
+        if (m.rows) {   // a neural member's row block
+            for (int k = tid; k < V; k += blockDim.x) MixAdd(acc[k], i == 0, m.w, load_y(m.rows, m.dtype, (long)(row + k)));
+            continue;
+        }
+        const NGramDev &lm = m.lm;
+        if (tid == 0) {
+            int s = lm.root_dst[lm.eos];
+            if (parent) {
+                s = m.state_in[(size_t)(q / B) * B + parent[q]];
+                const int w = token[q] >= 0 ? lm.tok2word[token[q]] : -1;
+                if (w >= 0) { int d; LmLog10(lm, s, w, &d); s = d; }
+            }
+            m.state_out[q] = s;
+            int L = 0;
+            double c = 0.0;
+            for (;;) {
+                s_chain[L] = s; s_c[L] = c;
+                if (s == 0) break;
+                c += (double)lm.bow[s];
+                s = lm.back[s];
+                ++L;
+            }
+            s_len = L;
+        }
+        __syncthreads();   // (also: the previous n-gram member's word row has been read)
+        const int L = s_len;
+        const double croot = s_c[L];
+        for (int w = tid; w < m.W; w += blockDim.x) wrow[w] = croot + (double)lm.root_p[w];
+        __syncthreads();
+        for (int j = L - 1; j >= 0; --j) {
+            const int s = s_chain[j];
+            const double c = s_c[j];
+            for (int a = lm.arc_off[s] + tid; a < lm.arc_off[s + 1]; a += blockDim.x) {
+                const float p = lm.arc_p[a];
+                if (p == p) wrow[lm.arc_word[a]] = c + (double)p;
+            }
+            __syncthreads();
+        }
+        for (int k = tid; k < V; k += blockDim.x) {
+            const int w = lm.tok2word[k];
+            MixAdd(acc[k], i == 0, m.w, w < 0 ? 0.f : (float)__dmul_rn(wrow[w], kLn10));
+        }
+        __syncthreads();   // s_len and the word row are rewritten by the next n-gram member
+    }
+    for (int k = tid; k < V; k += blockDim.x) rows[row + k] = (float)acc[k];
+}
+
 // ranks the beam by score (desc; ties: beam order) and writes the first nbest rows: tokens -1 padded, lengths (-1 past the
 // hypotheses found), scores (-inf there)
 __global__ void __launch_bounds__(kThreads) rnnt_beam_finish_kernel(int T, int B, int nbest, const char *ws, const int *node,
@@ -429,6 +502,21 @@ int LaunchNgramSlotRows(const NGramDev &lm, int W, int N, int B, int V, const in
         if (e != cudaSuccess) return (int)e;
     }
     ngram_slot_rows_kernel<<<N * B, kRowThreads, smem, s>>>(lm, W, V, B, parent, token, state_in, state_out, rows);
+    CountLaunch();
+    return (int)cudaGetLastError();
+}
+
+size_t LmMixSlotRowsSmemBytes(int W, int V) { return ((size_t)W + V) * sizeof(double); }
+
+int LaunchLmMixSlotRows(const LmMixDev &mix, int W, int N, int B, int V, const int *parent, const int *token, float *rows,
+                        cudaStream_t s) {
+    const size_t smem = LmMixSlotRowsSmemBytes(W, V);
+    if (smem > 48 * 1024) {
+        const cudaError_t e = cudaFuncSetAttribute(lm_mix_slot_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   (int)smem);
+        if (e != cudaSuccess) return (int)e;
+    }
+    lm_mix_slot_rows_kernel<<<N * B, kRowThreads, smem, s>>>(mix, V, B, parent, token, rows);
     CountLaunch();
     return (int)cudaGetLastError();
 }

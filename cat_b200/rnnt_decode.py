@@ -2,11 +2,13 @@
 ``RNNTDecoder``, with CAT's external LM fusion (``alpha``, ``beta``) and ILM estimation (``ilm_weight``), without the
 ``<eos>`` early stop.  The networks run in torch, under the caller's autocast; the search (exact top-B, prefix trie,
 fixed-order merge, the fusion terms) is one native launch per frame (``cat_b200/csrc/rnnt_decode.cu``), and an n-gram LM's
-rows are one more.  Definition and differences from CAT: DESIGN.md §7 "Transducer beam search" and "RNN-T beam search with
-LM fusion".
+rows, or the rows of a weighted LM mix (``MultiLM``, CAT's ``MultiDecoder``, as LODR decoding uses), are one more.
+Definition and differences from CAT: DESIGN.md §7 "Transducer beam search", "RNN-T beam search with LM fusion" and
+"RNN-T beam search with an LM mix".
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 from typing import List, Optional, Tuple
 
@@ -19,6 +21,8 @@ from .rnnt import _on_device
 from .rnnt_simple import _int32
 
 MAX_BEAM = 128
+MAX_MIX = 8                  # members of a MultiLM (rnnt_decode.cu kLmMixMax)
+_MIX_SMEM = 200 * 1024       # the mix rows kernel's shared memory: 8 (largest n-gram word count + V) bytes at most
 _MODE_LOGPROBS, _MODE_LOGITS, _MODE_LOGADD = 0, 1, 2
 
 
@@ -75,22 +79,84 @@ def _carry(step, out, state, src, tok, ext, blank: int, check):
 # CAT's LMs the search cannot carry per slot, and what to use instead
 _REFUSED_LMS = {
     "NGram": "load its ARPA file (cat/utils/pipeline/ngram.sh --arpa) as cat_b200.ngram.NGramLM(<ARPA>, labels) instead",
-    "MultiDecoder": "several LMs at once are not supported",
+    "MultiDecoder": "its members (_weights, _decs) cannot be read; build a cat_b200.rnnt_decode.MultiLM(weights, lms) "
+                    "from the built members instead",
     "PretrainedTransformer": "a Transformer LM's state grows with the prefix",
     "CausalTransformer": "a Transformer LM's state grows with the prefix",
 }
 
 
-def _check_lm(lm, caller):
-    """An LM the search can fuse (NotImplementedError otherwise): an ``NGramLM``, or a module with ``get_log_prob``."""
+def _check_lm(lm, caller, mix_ok=True):
+    """An LM the search can fuse (NotImplementedError otherwise): an ``NGramLM``, a module with ``get_log_prob`` or, with
+    ``mix_ok``, a ``MultiLM``."""
     name = type(lm).__name__
-    if isinstance(lm, NGramLM):
+    if isinstance(lm, NGramLM) or (mix_ok and isinstance(lm, MultiLM)):
         return
+    if isinstance(lm, MultiLM) or name == "MultiDecoder":
+        raise NotImplementedError(f"{caller}: LM {name} is not supported as a member of a mix: mixes do not nest")
     if name in _REFUSED_LMS:
         raise NotImplementedError(f"{caller}: LM {name} is not supported: {_REFUSED_LMS[name]}")
     if not callable(getattr(lm, "get_log_prob", None)):
         raise NotImplementedError(f"{caller}: LM {name} is not supported: the LM must be a cat_b200.ngram.NGramLM or a "
                                   "module with get_log_prob(tokens (R, 1), state) -> (log-probs (R, 1, V), state)")
+
+
+class MultiLM:
+    """A weighted mix of LMs, the GPU stand-in for CAT's ``MultiDecoder`` (``cat/shared/decoder.py``), as LODR decoding uses
+    it: ``MultiLM([0.28125, -0.3125], [NGramLM(<5-gram ARPA>, labels), NGramLM(<LODR bigram ARPA>, labels)])``.  Its row
+    after a prefix is sum_i w_i LM_i, summed in fp64 in member order and rounded to fp32 once (DESIGN.md §7 "RNN-T beam
+    search with an LM mix"); the search fuses it like one LM, with alpha and beta.  Members are ``NGramLM`` objects and
+    neural LMs with CAT's ``get_log_prob`` and an LSTM-like state, built by the caller (CAT builds them from config files).
+    As in CAT, zero-weight members are dropped.  ValueError: weights and lms of different lengths, a weight that is not a
+    finite number, no member left, more than ``MAX_MIX`` members, n-gram members over different label sets, or n-gram
+    members whose word rows do not fit the rows kernel's shared memory; NotImplementedError: a member the search cannot
+    carry (CAT's KenLM ``NGram``, Transformers, nested mixes)."""
+
+    def __init__(self, weights, lms):
+        weights, lms = list(weights), list(lms)
+        if len(weights) != len(lms):
+            raise ValueError(f"MultiLM: {len(weights)} weights for {len(lms)} LMs")
+        weights = [_weight(w, "every weight", "MultiLM") for w in weights]
+        kept = [(w, lm) for w, lm in zip(weights, lms) if w != 0.0]
+        if not kept:
+            raise ValueError("MultiLM: every weight is zero, so nothing is left to fuse")
+        if len(kept) > MAX_MIX:
+            raise ValueError(f"MultiLM: at most {MAX_MIX} members of non-zero weight, not {len(kept)}")
+        for _, lm in kept:
+            _check_lm(lm, "MultiLM", mix_ok=False)
+        self.weights = [w for w, _ in kept]
+        self.lms = [lm for _, lm in kept]
+        vs = {lm.V for lm in self.lms if isinstance(lm, NGramLM)}
+        if len(vs) > 1:
+            raise ValueError(f"MultiLM: the n-gram members are loaded for different numbers of labels {sorted(vs)}")
+        if vs:
+            self.check_smem(vs.pop(), "MultiLM")
+
+    @property
+    def has_ngram(self) -> bool:
+        return any(isinstance(lm, NGramLM) for lm in self.lms)
+
+    def check_smem(self, V: int, caller):
+        """The rows kernel builds each n-gram word row and the V-wide fp64 sum in shared memory (ValueError if too big)"""
+        W = max([lm.num_words for lm in self.lms if isinstance(lm, NGramLM)], default=0)
+        if 8 * (W + V) > _MIX_SMEM:
+            raise ValueError(f"{caller}: the mix's largest n-gram LM has {W} words and V = {V}; the mix rows are built in "
+                             f"shared memory, which holds at most {_MIX_SMEM // 8} words plus labels")
+
+    def __repr__(self):
+        return f"MultiLM({self.weights}, [{', '.join(type(lm).__name__ for lm in self.lms)}])"
+
+
+def _as_lm(lm, caller):
+    """CAT's ``MultiDecoder`` as a ``MultiLM`` when its ``_weights`` and ``_decs`` can be read (every member then checked as
+    a ``MultiLM`` member); any other LM as it is."""
+    if type(lm).__name__ != "MultiDecoder" or isinstance(lm, MultiLM):
+        return lm
+    try:
+        weights, decs = list(lm._weights), list(lm._decs)
+    except (AttributeError, TypeError):
+        raise NotImplementedError(f"{caller}: LM MultiDecoder is not supported: {_REFUSED_LMS['MultiDecoder']}") from None
+    return MultiLM(weights, decs)
 
 
 def _check_ilm_joiner(joiner, caller):
@@ -168,18 +234,20 @@ class _Fusion:
     """The external LM and ILM terms of the RNN-T search (DESIGN.md §7 "RNN-T beam search with LM fusion"), checked before
     anything runs.  The LM term is on iff ``lm`` is given and alpha != 0, the ILM term iff ilm_weight != 0.  Per call it
     carries the LM's per-slot state: an ``NGramLM``'s int32 states (double-buffered) and rows from
-    ``ccb_ngram_slot_rows``, or a neural LM's output and state, carried like the predictor's."""
+    ``ccb_ngram_slot_rows``, or a neural LM's output and state, carried like the predictor's.  A ``MultiLM`` carries
+    each member so (every n-gram member double-buffered, every neural member through ``_carry``), and one
+    ``ccb_lm_mix_slot_rows`` launch per frame makes the mix rows."""
 
     def __init__(self, lm, alpha, beta, ilm_weight, joiner, blank, caller):
         self.alpha = _weight(alpha, "alpha", caller)
         self.beta = _weight(beta, "beta", caller)
         self.ilm_weight = _weight(ilm_weight, "ilm_weight", caller)
-        self.lm = lm if lm is not None and self.alpha != 0.0 else None
+        self.lm = _as_lm(lm, caller) if lm is not None and self.alpha != 0.0 else None
         self.ilm = self.ilm_weight != 0.0
         self.caller = caller
         if self.lm is not None:
             _check_lm(self.lm, caller)
-            if isinstance(self.lm, NGramLM) and blank != 0:
+            if (isinstance(self.lm, NGramLM) or isinstance(self.lm, MultiLM) and self.lm.has_ngram) and blank != 0:
                 raise ValueError(f"{caller}: an NGramLM's label 0 is the blank, so blank must be 0, not {blank}")
         if self.ilm:
             _check_ilm_joiner(joiner, caller)
@@ -194,12 +262,32 @@ class _Fusion:
         if isinstance(self.lm, NGramLM):
             self.state = [torch.empty((N, B), dtype=torch.int32, device=dev) for _ in range(2)]
             self.rows = None
+        elif isinstance(self.lm, MultiLM):
+            # per member: an n-gram's two state buffers, or a neural LM's [output, state]
+            self.members = []
+            for lm in self.lm.lms:
+                if isinstance(lm, NGramLM):
+                    self.members.append([torch.empty((N, B), dtype=torch.int32, device=dev) for _ in range(2)])
+                else:
+                    out, st = lm.get_log_prob(torch.full((self.R, 1), blank, dtype=torch.long, device=dev), None)
+                    _check_state(lm, st, self.R, self.caller, "LM")
+                    self.members.append([out, st])
+            self.rows = None
         elif self.lm is not None:
             self.out, self.st = self.lm.get_log_prob(torch.full((self.R, 1), blank, dtype=torch.long, device=dev), None)
             _check_state(self.lm, self.st, self.R, self.caller, "LM")
 
     def check_v(self, V: int):
         """The LM's V against the joiner's (ValueError, before the first native call)"""
+        if isinstance(self.lm, MultiLM):
+            for i, (lm, m) in enumerate(zip(self.lm.lms, self.members)):
+                lv = lm.V if isinstance(lm, NGramLM) else int(m[0].shape[-1])
+                if lv != V:
+                    raise ValueError(f"{self.caller}: member {i} of the LM mix has V = {lv} labels, the joiner V = {V}")
+            self.lm.check_smem(V, self.caller)
+            if self.rows is None:
+                self.rows = torch.empty((self.R, V), dtype=torch.float32, device=self.members[0][0].device)
+            return
         lv = self.lm.V if isinstance(self.lm, NGramLM) else None if self.lm is None else int(self.out.shape[-1])
         if lv is not None and lv != V:
             raise ValueError(f"{self.caller}: the LM has V = {lv} labels, the joiner V = {V}")
@@ -215,27 +303,62 @@ class _Fusion:
             self.rows.data_ptr(), _stream(dst.device)), self.caller)
         self.state.reverse()
 
+    def _mix_rows(self, parent=None, token=None):
+        # one launch: every n-gram member's next states (into its other buffer) and the mix rows (R, V) fp32.  The entry
+        # takes the n-gram members first, then the neural ones, and the mix's order as a permutation of that list.
+        lms, ws, mem = self.lm.lms, self.lm.weights, self.members
+        ng = [i for i, lm in enumerate(lms) if isinstance(lm, NGramLM)]
+        nn = [i for i, lm in enumerate(lms) if not isinstance(lm, NGramLM)]
+        nrows = [_neural_rows(mem[i][0], self.R) for i in nn]   # (alive until the launch is enqueued)
+
+        def arr(ctype, xs):
+            return (ctype * max(len(xs), 1))(*xs)
+
+        vp = C.c_void_p
+        _check(_lib.lib().ccb_lm_mix_slot_rows(
+            len(ng), arr(vp, [lms[i].handle for i in ng]), arr(C.c_double, [ws[i] for i in ng]),
+            arr(vp, [mem[i][0].data_ptr() for i in ng]), arr(vp, [mem[i][1].data_ptr() for i in ng]),
+            len(nn), arr(vp, [r.data_ptr() for r in nrows]), arr(C.c_int, [_DTYPES[r.dtype] for r in nrows]),
+            arr(C.c_double, [ws[i] for i in nn]), arr(C.c_int, [(ng + nn).index(i) for i in range(len(lms))]),
+            self.N, self.B, self.rows.shape[1], None if parent is None else parent.data_ptr(),
+            None if token is None else token.data_ptr(), self.rows.data_ptr(), _stream(self.rows.device)), self.caller)
+        for i in ng:
+            mem[i].reverse()
+
     def first(self):
         """The first frame's LM rows (after the workspace's init)"""
         if isinstance(self.lm, NGramLM):
             self._ngram_rows()
+        elif isinstance(self.lm, MultiLM):
+            self._mix_rows()
 
     def lm_rows(self) -> Optional[torch.Tensor]:
         """The current beam's LM log-prob rows (R, V), or None without the LM term"""
         if self.lm is None:
             return None
-        if isinstance(self.lm, NGramLM):
+        if isinstance(self.lm, (NGramLM, MultiLM)):
             return self.rows
-        rows = self.out.reshape(self.R, -1)
-        return (rows if rows.dtype in _DTYPES else rows.float()).contiguous()
+        return _neural_rows(self.out, self.R)
 
     def advance(self, src, tok, ext, parent, token):
         """Every slot's LM after a frame: its parent's, advanced by the token it emitted"""
         if isinstance(self.lm, NGramLM):
             self._ngram_rows(parent, token)
+        elif isinstance(self.lm, MultiLM):
+            for lm, m in zip(self.lm.lms, self.members):
+                if not isinstance(lm, NGramLM):
+                    m[0], m[1] = _carry(lm.get_log_prob, m[0], m[1], src, tok, ext, self.blank,
+                                        lambda st, lm=lm: _check_state(lm, st, self.R, self.caller, "LM"))
+            self._mix_rows(parent, token)
         elif self.lm is not None:
             self.out, self.st = _carry(self.lm.get_log_prob, self.out, self.st, src, tok, ext, self.blank,
                                        lambda st: _check_state(self.lm, st, self.R, self.caller, "LM"))
+
+
+def _neural_rows(out, R: int) -> torch.Tensor:
+    """A neural LM's output as the (R, V) row block the kernels read: fp32, bf16 or fp16, contiguous"""
+    rows = out.reshape(R, -1)
+    return (rows if rows.dtype in _DTYPES else rows.float()).contiguous()
 
 
 def _beam_search(name: str, family: str, enc_out, frame_lens, predictor, joiner, beam_size, nbest, blank,
@@ -344,8 +467,10 @@ def rnnt_beam_search(enc_out: torch.Tensor, frame_lens: torch.Tensor, predictor,
 
     LM fusion (on iff ``lm`` is given and alpha != 0): every extension by token k != blank adds beta + alpha ln P_LM(k |
     prefix) to the hypothesis's LM part.  ``lm`` is a ``cat_b200.ngram.NGramLM`` loaded for the joiner's V labels (label 0
-    the blank, so blank must be 0), or a module whose ``get_log_prob(tokens (R, 1), state)`` returns (log-probs (R, 1, V),
-    state) with a state like the predictor's (CAT's LSTM LM); any other LM raises NotImplementedError.  ILM estimation (on
+    the blank, so blank must be 0), a module whose ``get_log_prob(tokens (R, 1), state)`` returns (log-probs (R, 1, V),
+    state) with a state like the predictor's (CAT's LSTM LM), or a ``MultiLM`` of such members (or CAT's ``MultiDecoder``
+    with readable members), whose row sum_i w_i LM_i takes the place of ln P_LM, as in LODR decoding; any other LM raises
+    NotImplementedError.  ILM estimation (on
     iff ilm_weight != 0): every extension adds ilm_weight (I[k] - logsumexp over the non-blank I), I the joiner's
     impl_forward(zeros, pn) logits (JointNet "add": fc(fc_enc's bias + fc_dec(pn))); LogAdd and joiners without
     impl_forward raise NotImplementedError.  Candidates rank by acoustic score plus LM part; merged hypotheses add only
@@ -359,10 +484,12 @@ def rnnt_beam_search(enc_out: torch.Tensor, frame_lens: torch.Tensor, predictor,
 class RNNTDecoder:
     """CAT's ``cat.rnnt.rnnt_decoder.RNNTDecoder`` with its constructor, decoding on the GPU through ``rnnt_beam_search``.
     CAT's rules: alpha == 0 drops the LM whatever beta is, and ILM estimation is on iff est_ilm and ilm_weight != 0.
-    ``lm_module`` is a ``cat_b200.ngram.NGramLM`` (in place of CAT's KenLM ``NGram``) or a neural LM with CAT's
-    ``get_log_prob`` and an LSTM-like state.  Returned scores are CAT's ``Hypothesis.score``: acoustic plus LM part.  Not
-    supported (NotImplementedError, raised here): other LMs (KenLM ``NGram``, ``MultiDecoder``, Transformers), ILM
-    estimation with LogAdd or a joiner without ``impl_forward``, an ``<eos>`` early stop and bos_id != blank_id."""
+    ``lm_module`` is a ``cat_b200.ngram.NGramLM`` (in place of CAT's KenLM ``NGram``), a neural LM with CAT's
+    ``get_log_prob`` and an LSTM-like state, or a weighted mix of those: a ``MultiLM``, or CAT's ``MultiDecoder`` whose
+    ``_weights`` and ``_decs`` are such members (LODR decoding).  Returned scores are CAT's ``Hypothesis.score``: acoustic
+    plus LM part.  Not supported (NotImplementedError, raised here): other LMs (KenLM ``NGram``, a ``MultiDecoder`` without
+    readable members, Transformers), ILM estimation with LogAdd or a joiner without ``impl_forward``, an ``<eos>`` early
+    stop and bos_id != blank_id."""
 
     def __init__(self, predictor, joiner, blank_id: int = 0, bos_id: int = 0, eos_id: int = -1, beam_size: int = 5,
                  nbest: int = -1, lm_module=None, alpha: float = 0.0, beta: float = 0.0, est_ilm: bool = False,

@@ -542,6 +542,21 @@ int ccb_rnnt_beam_step_fused(const void *rows, const void *enc, int dtype, int m
  * been loaded for V labels and have at most 25600 words. */
 int ccb_ngram_slot_rows(const void *lm, int N, int beam, int V, const int *parent, const int *token, const int *state_in,
                         int *state_out, float *rows, void *stream);
+/* The rows of a weighted mix of LMs (LODR and the like: DESIGN.md §7 "RNN-T beam search with an LM mix") for
+ * ccb_rnnt_beam_step_fused: for every slot q of N*beam, rows[q][k] (V fp32) = sum over the members i, in the given order,
+ * of w_i LM_i[q][k], each product and sum rounded in fp64 on its own, the first product starting the sum, rounded to fp32
+ * once; -inf if any member's entry is -inf.  The members are n_ngram token n-gram LMs (ccb_ngram_create; ngrams[j],
+ * weight ngram_w[j], (N, beam) int32 state arrays state_in[j] and state_out[j]) and n_neural row blocks (neural_rows[j],
+ * (N*beam, V) in the CCB_DTYPE_* code neural_dtype[j], weight neural_w[j]); the pointer and weight arrays are host arrays.
+ * order[i] (a permutation of 0 .. K-1, K = n_ngram + n_neural) is the i-th member: n-gram order[i] if it is below n_ngram,
+ * else neural row block order[i] - n_ngram.  An n-gram member's state and row are those of ccb_ngram_slot_rows with the
+ * same parent, token and state arrays (parent null: the start state; token and state_in then unused), and it contributes
+ * the fp32 value that entry writes; a neural member's entry is widened exactly.  1 <= K <= 8, weights finite and non-zero,
+ * every LM loaded for V labels, and 8 (W + V) bytes at most 200 KiB, W the largest n-gram member's word count. */
+int ccb_lm_mix_slot_rows(int n_ngram, const void *const *ngrams, const double *ngram_w, const int *const *state_in,
+                         int *const *state_out, int n_neural, const void *const *neural_rows, const int *neural_dtype,
+                         const double *neural_w, const int *order, int N, int beam, int V, const int *parent,
+                         const int *token, float *rows, void *stream);
 
 /* CTC-T (CTC-Transducer) prefix beam search, one launch per frame, with the arguments and slot arrays of the transducer beam
  * search above; every frame emits one symbol, as in ccb_ctct_forward.  Each live slot holds a prefix with masses b (last
