@@ -373,20 +373,11 @@ int EnsureLegacy(int dev, const DeviceGraph &g, int N, int T, float *caller_alph
     return 0;
 }
 
-// The RNN-T and CTC-T entries share their checks and launch through `launch` (the two families take the same arguments).
-using RnntFwdLauncher = int (*)(const void *, int, int, int, int, long long, int, int, int, const int *, long long,
-                                const int *, const int *, int, int, void *, float *, float *, cudaStream_t);
-using RnntBwdLauncher = int (*)(const void *, int, int, int, long long, int, const int *, int, void *, const float *, void *,
-                                cudaStream_t);
-using SimpleFwdLauncher = int (*)(const void *, const void *, int, int, int, int, int, const int *, const int *, const int *,
-                                  int, int, void *, float *, cudaStream_t);
-using SimpleBwdLauncher = int (*)(const void *, const void *, int, int, int, int, int, const int *, int, void *, const float *,
-                                  void *, void *, cudaStream_t);
-
-int TransducerForward(const std::string &what, RnntFwdLauncher launch, const void *x, int dtype, int from_logits,
-                             int compact, int N, long rows, int V, int Tmax, int Umax, const int *labels_dev, long n_labels,
-                             const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
-                             float *costs_beta, void *stream) {
+// The RNN-T (CTCT = false) and CTC-T (CTCT = true) entries share their checks and launchers.
+template <bool CTCT>
+int TransducerForward(const std::string &what, const void *x, int dtype, int from_logits, int compact, int N, long rows, int V,
+                      int Tmax, int Umax, const int *labels_dev, long n_labels, const int *lx_dev, const int *ly_dev, int blank,
+                      int want_beta, void *workspace, float *costs, float *costs_beta, void *stream) {
     g_err.clear();
     if (N <= 0 || rows < 0 || V <= 0 || n_labels < 0) return Fail(what + ": N and V must be positive, rows and n_labels >= 0");
     if (!KnownDtype(dtype)) return FailDtype(what.c_str(), dtype);
@@ -395,50 +386,54 @@ int TransducerForward(const std::string &what, RnntFwdLauncher launch, const voi
         return Fail(what + ": the padded layout needs rows = N Tmax (Umax+1) and n_labels = N Umax");
     if (!x || (n_labels && !labels_dev) || !lx_dev || !ly_dev || !workspace || !costs)
         return Fail(what + ": missing buffer");
-    const int rc = launch(x, dtype, from_logits, compact, N, rows, V, Tmax, Umax, labels_dev, n_labels, lx_dev, ly_dev, blank,
-                          want_beta, workspace, costs, costs_beta, (cudaStream_t)stream);
+    const int rc = TransducerLoss<CTCT>::Forward(x, dtype, from_logits, compact, N, rows, V, Tmax, Umax, labels_dev, n_labels,
+                                                 lx_dev, ly_dev, blank, want_beta, workspace, costs, costs_beta,
+                                                 (cudaStream_t)stream);
     if (rc) return FailCuda(what.c_str(), (cudaError_t)rc);
     return 0;
 }
 
-int TransducerBackward(const std::string &what, RnntBwdLauncher launch, const void *x, int dtype, int from_logits, int N,
-                              long rows, int V, const int *labels_dev, int blank, void *workspace, const float *w, void *grad,
-                              void *stream) {
+template <bool CTCT>
+int TransducerBackward(const std::string &what, const void *x, int dtype, int from_logits, int N, long rows, int V,
+                       const int *labels_dev, int blank, void *workspace, const float *w, void *grad, void *stream) {
     g_err.clear();
     if (N <= 0 || rows < 0 || V <= 0) return Fail(what + ": N and V must be positive, rows >= 0");
     if (!KnownDtype(dtype)) return FailDtype(what.c_str(), dtype);
     if (blank < 0 || blank >= V) return Fail(what + ": blank must lie in [0, V)");
     if ((from_logits && !x) || !workspace || !w || !grad) return Fail(what + ": missing buffer");
-    const int rc = launch(x, dtype, from_logits, N, rows, V, labels_dev, blank, workspace, w, grad, (cudaStream_t)stream);
+    const int rc = TransducerLoss<CTCT>::Backward(x, dtype, from_logits, N, rows, V, labels_dev, blank, workspace, w, grad,
+                                                  (cudaStream_t)stream);
     if (rc) return FailCuda(what.c_str(), (cudaError_t)rc);
     return 0;
 }
 
-int SimpleForward(const std::string &what, SimpleFwdLauncher launch, const void *f, const void *g, int dtype, int N,
-                         int Tmax, int Umax, int V, const int *labels_dev, const int *lx_dev, const int *ly_dev, int blank,
-                         int want_beta, void *workspace, float *costs, void *stream) {
+template <bool CTCT>
+int SimpleForward(const std::string &what, const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V,
+                  const int *labels_dev, const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace,
+                  float *costs, void *stream) {
     g_err.clear();
     if (N <= 0 || Tmax <= 0 || Umax < 0 || V <= 0) return Fail(what + ": N, Tmax and V must be positive, Umax >= 0");
     if (N > 65535) return Fail(what + ": at most 65535 utterances per call");
     if (!KnownDtype(dtype)) return FailDtype(what.c_str(), dtype);
     if (blank < 0 || blank >= V) return Fail(what + ": blank must lie in [0, V)");
     if (!f || !g || (Umax && !labels_dev) || !lx_dev || !ly_dev || !workspace || !costs) return Fail(what + ": missing buffer");
-    const int rc = launch(f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev, ly_dev, blank, want_beta, workspace, costs,
-                          (cudaStream_t)stream);
+    const int rc = TransducerLoss<CTCT>::SimpleForward(f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev, ly_dev, blank,
+                                                       want_beta, workspace, costs, (cudaStream_t)stream);
     if (rc) return FailCuda(what.c_str(), (cudaError_t)rc);
     return 0;
 }
 
-int SimpleBackward(const std::string &what, SimpleBwdLauncher launch, const void *f, const void *g, int dtype, int N,
-                          int Tmax, int Umax, int V, const int *labels_dev, int blank, void *workspace, const float *w,
-                          void *grad_f, void *grad_g, void *stream) {
+template <bool CTCT>
+int SimpleBackward(const std::string &what, const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V,
+                   const int *labels_dev, int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream) {
     g_err.clear();
     if (N <= 0 || Tmax <= 0 || Umax < 0 || V <= 0) return Fail(what + ": N, Tmax and V must be positive, Umax >= 0");
     if (N > 65535) return Fail(what + ": at most 65535 utterances per call");
     if (!KnownDtype(dtype)) return FailDtype(what.c_str(), dtype);
     if (blank < 0 || blank >= V) return Fail(what + ": blank must lie in [0, V)");
     if (!f || !g || (Umax && !labels_dev) || !workspace || !w || !grad_f || !grad_g) return Fail(what + ": missing buffer");
-    const int rc = launch(f, g, dtype, N, Tmax, Umax, V, labels_dev, blank, workspace, w, grad_f, grad_g, (cudaStream_t)stream);
+    const int rc = TransducerLoss<CTCT>::SimpleBackward(f, g, dtype, N, Tmax, Umax, V, labels_dev, blank, workspace, w, grad_f,
+                                                        grad_g, (cudaStream_t)stream);
     if (rc) return FailCuda(what.c_str(), (cudaError_t)rc);
     return 0;
 }
@@ -1443,68 +1438,68 @@ int ccb_wfst_decode(const void *logits, int dtype, int N, int T, int V, const in
     return 0;
 }
 
-size_t ccb_rnnt_workspace_bytes(int N, long rows) { return N > 0 && rows >= 0 ? RnntWsBytes(N, rows) : 0; }
+size_t ccb_rnnt_workspace_bytes(int N, long rows) { return N > 0 && rows >= 0 ? TransducerLoss<false>::WsBytes(N, rows) : 0; }
 
 int ccb_rnnt_forward(const void *x, int dtype, int from_logits, int compact, int N, long rows, int V, int Tmax, int Umax,
                      const int *labels_dev, long n_labels, const int *lx_dev, const int *ly_dev, int blank, int want_beta,
                      void *workspace, float *costs, float *costs_beta, void *stream) {
-    return TransducerForward("rnnt_forward", LaunchRnntForward, x, dtype, from_logits, compact, N, rows, V, Tmax, Umax,
-                             labels_dev, n_labels, lx_dev, ly_dev, blank, want_beta, workspace, costs, costs_beta, stream);
+    return TransducerForward<false>("rnnt_forward", x, dtype, from_logits, compact, N, rows, V, Tmax, Umax, labels_dev, n_labels,
+                                    lx_dev, ly_dev, blank, want_beta, workspace, costs, costs_beta, stream);
 }
 
 int ccb_rnnt_backward(const void *x, int dtype, int from_logits, int N, long rows, int V, const int *labels_dev, int blank,
                       void *workspace, const float *w, void *grad, void *stream) {
-    return TransducerBackward("rnnt_backward", LaunchRnntBackward, x, dtype, from_logits, N, rows, V, labels_dev, blank,
-                              workspace, w, grad, stream);
+    return TransducerBackward<false>("rnnt_backward", x, dtype, from_logits, N, rows, V, labels_dev, blank, workspace, w, grad,
+                                     stream);
 }
 
 size_t ccb_rnnt_simple_workspace_bytes(int N, int Tmax, int Umax) {
-    return N > 0 && Tmax > 0 && Umax >= 0 ? RnntSimpleWsBytes(N, Tmax, Umax) : 0;
+    return N > 0 && Tmax > 0 && Umax >= 0 ? TransducerLoss<false>::SimpleWsBytes(N, Tmax, Umax) : 0;
 }
 
 int ccb_rnnt_simple_forward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
                             const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
                             void *stream) {
-    return SimpleForward("rnnt_simple_forward", LaunchRnntSimpleForward, f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev,
-                         ly_dev, blank, want_beta, workspace, costs, stream);
+    return SimpleForward<false>("rnnt_simple_forward", f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev, ly_dev, blank,
+                                want_beta, workspace, costs, stream);
 }
 
 int ccb_rnnt_simple_backward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
                              int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream) {
-    return SimpleBackward("rnnt_simple_backward", LaunchRnntSimpleBackward, f, g, dtype, N, Tmax, Umax, V, labels_dev, blank,
-                          workspace, w, grad_f, grad_g, stream);
+    return SimpleBackward<false>("rnnt_simple_backward", f, g, dtype, N, Tmax, Umax, V, labels_dev, blank, workspace, w, grad_f,
+                                 grad_g, stream);
 }
 
-size_t ccb_ctct_workspace_bytes(int N, long rows) { return N > 0 && rows >= 0 ? CtctWsBytes(N, rows) : 0; }
+size_t ccb_ctct_workspace_bytes(int N, long rows) { return N > 0 && rows >= 0 ? TransducerLoss<true>::WsBytes(N, rows) : 0; }
 
 int ccb_ctct_forward(const void *x, int dtype, int from_logits, int compact, int N, long rows, int V, int Tmax, int Umax,
                      const int *labels_dev, long n_labels, const int *lx_dev, const int *ly_dev, int blank, int want_beta,
                      void *workspace, float *costs, float *costs_beta, void *stream) {
-    return TransducerForward("ctct_forward", LaunchCtctForward, x, dtype, from_logits, compact, N, rows, V, Tmax, Umax,
-                             labels_dev, n_labels, lx_dev, ly_dev, blank, want_beta, workspace, costs, costs_beta, stream);
+    return TransducerForward<true>("ctct_forward", x, dtype, from_logits, compact, N, rows, V, Tmax, Umax, labels_dev, n_labels,
+                                   lx_dev, ly_dev, blank, want_beta, workspace, costs, costs_beta, stream);
 }
 
 int ccb_ctct_backward(const void *x, int dtype, int from_logits, int N, long rows, int V, const int *labels_dev, int blank,
                       void *workspace, const float *w, void *grad, void *stream) {
-    return TransducerBackward("ctct_backward", LaunchCtctBackward, x, dtype, from_logits, N, rows, V, labels_dev, blank,
-                              workspace, w, grad, stream);
+    return TransducerBackward<true>("ctct_backward", x, dtype, from_logits, N, rows, V, labels_dev, blank, workspace, w, grad,
+                                    stream);
 }
 
 size_t ccb_ctct_simple_workspace_bytes(int N, int Tmax, int Umax) {
-    return N > 0 && Tmax > 0 && Umax >= 0 ? CtctSimpleWsBytes(N, Tmax, Umax) : 0;
+    return N > 0 && Tmax > 0 && Umax >= 0 ? TransducerLoss<true>::SimpleWsBytes(N, Tmax, Umax) : 0;
 }
 
 int ccb_ctct_simple_forward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
                             const int *lx_dev, const int *ly_dev, int blank, int want_beta, void *workspace, float *costs,
                             void *stream) {
-    return SimpleForward("ctct_simple_forward", LaunchCtctSimpleForward, f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev,
-                         ly_dev, blank, want_beta, workspace, costs, stream);
+    return SimpleForward<true>("ctct_simple_forward", f, g, dtype, N, Tmax, Umax, V, labels_dev, lx_dev, ly_dev, blank,
+                               want_beta, workspace, costs, stream);
 }
 
 int ccb_ctct_simple_backward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels_dev,
                              int blank, void *workspace, const float *w, void *grad_f, void *grad_g, void *stream) {
-    return SimpleBackward("ctct_simple_backward", LaunchCtctSimpleBackward, f, g, dtype, N, Tmax, Umax, V, labels_dev, blank,
-                          workspace, w, grad_f, grad_g, stream);
+    return SimpleBackward<true>("ctct_simple_backward", f, g, dtype, N, Tmax, Umax, V, labels_dev, blank, workspace, w, grad_f,
+                                grad_g, stream);
 }
 
 /* ---- transducer beam search ------------------------------------------------------------------ */
@@ -1529,7 +1524,7 @@ int ccb_rnnt_beam_init(int N, int Tmax, int beam, void *workspace, int *parent, 
     return 0;
 }
 
-// the arguments every RNN-T step entry takes
+// the arguments every transducer step entry takes (RNN-T and CTC-T)
 static int CheckRnntStep(const char *what, const void *rows, const void *enc, int dtype, int mode, int N, int Tmax, int beam,
                          int V, int t, const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node,
                          double *score) {
@@ -1611,14 +1606,9 @@ int ccb_ctct_beam_step(const void *rows, const void *enc, int dtype, int mode, i
                        const int *len_dev, int blank, void *workspace, int *parent, int *token, int *node, double *score,
                        void *stream) {
     g_err.clear();
-    if (CheckRnntBeam("ctct_beam_step", N, Tmax, beam)) return 1;
-    if (!KnownDtype(dtype)) return FailDtype("ctct_beam_step", dtype);
-    if (mode < 0 || mode > 2) return Fail("ctct_beam_step: mode must be 0 (log-probs), 1 (logits) or 2 (LogAdd)");
-    if (V <= 0 || V > kRnntBeamMaxV) return Fail("ctct_beam_step: V must lie in [1, 2^24], not " + std::to_string(V));
-    if (t < 0 || t >= Tmax) return Fail("ctct_beam_step: frame t must lie in [0, Tmax)");
-    if (blank < 0 || blank >= V) return Fail("ctct_beam_step: blank must lie in [0, V)");
-    if (!rows || (mode == 2 && !enc) || !len_dev || !workspace || !parent || !token || !node || !score)
-        return Fail("ctct_beam_step: missing buffer");
+    if (CheckRnntStep("ctct_beam_step", rows, enc, dtype, mode, N, Tmax, beam, V, t, len_dev, blank, workspace, parent, token,
+                      node, score))
+        return 1;
     const int rc = LaunchCtctBeamStep(rows, enc, dtype, mode, N, Tmax, beam, V, t, len_dev, blank, workspace, parent, token,
                                       node, score, (cudaStream_t)stream);
     if (rc) return FailCuda("ctct_beam_step", (cudaError_t)rc);

@@ -293,36 +293,24 @@ size_t WfstWsBytes(const WfstDev &g, int N, int T, int K);
 int LaunchWfstDecode(const WfstDev &g, const void *y, int y_dtype, int N, int T, int V, const int *len, float acwt, float lmwt,
                      float wip, float beam, int K, void *ws, int *words, int *num_words, int *align, float *ac_logp,
                      float *graph_cost, float *cost, int *reached_final, cudaStream_t stream);
-// RNN-T loss (rnnt_kernels.cu): the forward runs the prep, row and alpha (|| beta when want_beta) passes; the backward the
-// gradient pass over the same workspace of RnntWsBytes(N, rows) bytes.  Lengths and labels are device pointers.
-size_t RnntWsBytes(int N, long long rows);
-int LaunchRnntForward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
-                      const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
-                      float *costs, float *costs_beta, cudaStream_t s);
-int LaunchRnntBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
-                       void *ws, const float *w, void *grad, cudaStream_t s);
-// RNN-T loss of the LogAdd joiner from f (N, Tmax, V) and g (N, Umax+1, V) (rnnt_kernels.cu): the forward runs the prep,
-// row maxima, normaliser GEMM, underflow fix-up and alpha (|| beta) passes; the backward the cell weights and the two
-// gradient GEMMs over the same workspace of RnntSimpleWsBytes(N, Tmax, Umax) bytes.
-size_t RnntSimpleWsBytes(int N, int Tmax, int Umax);
-int LaunchRnntSimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
-                            const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s);
-int LaunchRnntSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
-                             int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s);
-// CTC-T loss (rnnt_kernels.cu), with the arguments of the RNN-T entries above: the forward runs the prep, row (with lpr) and
-// the frame-synchronous alpha (|| beta) passes, the backward the gradient pass, over CtctWsBytes(N, rows) bytes; the LogAdd
-// joiner's CTC-T loss runs the simple loss's passes with the CTC-T lattice over CtctSimpleWsBytes(N, Tmax, Umax) bytes.
-size_t CtctWsBytes(int N, long long rows);
-int LaunchCtctForward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
-                      const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
-                      float *costs, float *costs_beta, cudaStream_t s);
-int LaunchCtctBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
-                       void *ws, const float *w, void *grad, cudaStream_t s);
-size_t CtctSimpleWsBytes(int N, int Tmax, int Umax);
-int LaunchCtctSimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
-                            const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s);
-int LaunchCtctSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
-                             int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s);
+// The RNN-T (CTCT = false) and CTC-T (CTCT = true) losses (rnnt_kernels.cu); lengths and labels are device pointers.
+// Over the joint tensor: the forward runs the prep, row and alpha (|| beta when want_beta) passes; the backward the gradient
+// pass over the same workspace of WsBytes(N, rows) bytes.  Of the LogAdd joiner, from f (N, Tmax, V) and g (N, Umax+1, V):
+// the forward runs the prep, row maxima, normaliser GEMM, underflow fix-up and alpha (|| beta) passes; the backward the cell
+// weights and the two gradient GEMMs over the same workspace of SimpleWsBytes(N, Tmax, Umax) bytes.
+template <bool CTCT> struct TransducerLoss {
+    static size_t WsBytes(int N, long long rows);
+    static int Forward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
+                       const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
+                       float *costs, float *costs_beta, cudaStream_t s);
+    static int Backward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
+                        void *ws, const float *w, void *grad, cudaStream_t s);
+    static size_t SimpleWsBytes(int N, int Tmax, int Umax);
+    static int SimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                             const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s);
+    static int SimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
+                              int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s);
+};
 // Transducer beam search (rnnt_decode.cu): init, one step per frame, finish; one CTA per utterance each
 constexpr int kRnntBeamMaxV = 1 << 24;
 size_t RnntBeamWsBytes(int N, int T, int B);

@@ -30,7 +30,7 @@ struct RnntLayout {
 };
 
 // ctct: the CTC-T loss's workspace, with two cells per row in each direction and the lpr block (lpr = 0 otherwise)
-RnntLayout MakeRnntLayout(int N, long long rows, bool ctct = false) {
+RnntLayout MakeRnntLayout(int N, long long rows, bool ctct) {
     const size_t states = ctct ? 2 : 1;
     RnntLayout L;
     size_t o = 0;
@@ -49,6 +49,8 @@ RnntLayout MakeRnntLayout(int N, long long rows, bool ctct = false) {
 }
 
 template <typename T> T *At(void *ws, size_t off) { return reinterpret_cast<T *>(reinterpret_cast<char *>(ws) + off); }
+// a block that only the CTC-T layouts hold (lpr, PR: offset 0 otherwise), or nullptr
+template <typename T> T *AtOpt(void *ws, size_t off) { return off ? At<T>(ws, off) : nullptr; }
 
 // ------------------------------------------------------------------------------------------------
 // 16-byte row chunks in a compile-time dtype (VEC) or single elements through load_y (rows whose byte length or base is not
@@ -215,15 +217,13 @@ __device__ __forceinline__ void LpRows(const void *x, int dtype, long long V, co
     }
 }
 
-__global__ void __launch_bounds__(kRowThreads) rnnt_lp_rows_kernel(const void *x, int dtype, long long V, const int *labels,
-                                                                   int blank, RnntMeta *meta, float *lpb, float *lpl) {
-    LpRows<false>(x, dtype, V, labels, blank, meta, lpb, lpl, nullptr);
-}
-
-__global__ void __launch_bounds__(kRowThreads) ctct_lp_rows_kernel(const void *x, int dtype, long long V, const int *labels,
-                                                                   int blank, RnntMeta *meta, float *lpb, float *lpl,
-                                                                   float *lpr) {
-    LpRows<true>(x, dtype, V, labels, blank, meta, lpb, lpl, lpr);
+// One kernel for both losses, here and for the other bodies shared under CTCT (LogitRows, SimpleNorm, SimpleFixup,
+// SimpleGrad): CTCT is the first template argument, so that a profile tells <false, ...> (RNN-T) from <true, ...> (CTC-T),
+// and the RNN-T loss passes nullptr for lpr and PR.
+template <bool CTCT>
+__global__ void __launch_bounds__(kRowThreads) lp_rows_kernel(const void *x, int dtype, long long V, const int *labels,
+                                                              int blank, RnntMeta *meta, float *lpb, float *lpl, float *lpr) {
+    LpRows<CTCT>(x, dtype, V, labels, blank, meta, lpb, lpl, lpr);
 }
 
 template <int DT, bool VEC, bool CTCT>
@@ -273,17 +273,10 @@ __device__ __forceinline__ void LogitRows(const void *x, long long V, const int 
     }
 }
 
-template <int DT, bool VEC>
-__global__ void __launch_bounds__(kRowThreads) rnnt_logit_rows_kernel(const void *x, long long V, const int *labels, int blank,
-                                                                      RnntMeta *meta, float *lpb, float *lpl, float *lse) {
-    LogitRows<DT, VEC, false>(x, V, labels, blank, meta, lpb, lpl, nullptr, lse);
-}
-
-template <int DT, bool VEC>
-__global__ void __launch_bounds__(kRowThreads) ctct_logit_rows_kernel(const void *x, long long V, const int *labels, int blank,
-                                                                      RnntMeta *meta, float *lpb, float *lpl, float *lpr,
-                                                                      float *lse) {
-    LogitRows<DT, VEC, true>(x, V, labels, blank, meta, lpb, lpl, lpr, lse);
+template <bool CTCT, int DT, bool VEC>
+__global__ void __launch_bounds__(kRowThreads) logit_rows_kernel(const void *x, long long V, const int *labels, int blank,
+                                                                 RnntMeta *meta, float *lpb, float *lpl, float *lpr, float *lse) {
+    LogitRows<DT, VEC, CTCT>(x, V, labels, blank, meta, lpb, lpl, lpr, lse);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -291,10 +284,12 @@ __global__ void __launch_bounds__(kRowThreads) ctct_logit_rows_kernel(const void
 // in the workspace and read back by the next diagonal after the CTA barrier.
 //   alpha(t,u) = logaddexp(alpha(t-1,u) + lpb(t-1,u), alpha(t,u-1) + lpl(t,u-1)),  log P = alpha(T-1,U) + lpb(T-1,U)
 //   beta(t,u)  = logaddexp(beta(t+1,u) + lpb(t,u),   beta(t,u+1) + lpl(t,u)),     beta(T-1,U) = lpb(T-1,U), log P = beta(0,0)
+// The parameters are ctct_alpha_beta_kernel's, so that one launch runs either; labels and lpr are not read.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kAbThreads) rnnt_alpha_beta_kernel(const RnntMeta *meta, const float *lpb, const float *lpl,
-                                                                     double *alpha, double *beta, double *logp, int N,
-                                                                     float *costs, float *costs_beta) {
+__global__ void __launch_bounds__(kAbThreads) rnnt_alpha_beta_kernel(const RnntMeta *meta, const int *labels, const float *lpb,
+                                                                     const float *lpl, const float *lpr, double *alpha,
+                                                                     double *beta, double *logp, int N, float *costs,
+                                                                     float *costs_beta) {
     const int n = blockIdx.x;
     const bool bwd = blockIdx.y == 1;
     const RnntMeta m = meta[n];
@@ -478,13 +473,14 @@ __device__ __forceinline__ void CtctPosteriors(const RnntMeta &m, const int *lab
 //   pb = w exp(alpha + lpb + beta(t+1,u) - log P)   (at t = T-1 only for u = U, as exp(alpha + lpb - log P))
 //   pl = w exp(alpha + lpl + beta(t,u+1) - log P)   (u < U)
 //   grad[k] = [raw: exp(z_k - lse) (pb + pl)] - pb [k == blank] - pl [k == y_{u+1}]
+// The parameters are ctct_grad_kernel's; lpr is not read.
 // ------------------------------------------------------------------------------------------------
 template <int DT, bool VEC, bool RAW>
 __global__ void __launch_bounds__(kRowThreads) rnnt_grad_kernel(const void *x, long long V, const int *labels, int blank, int N,
                                                                 const RnntMeta *meta, const long long *tail, long long rows,
                                                                 const double *alpha, const double *beta, const double *logp,
-                                                                const float *lpb, const float *lpl, const float *lse,
-                                                                const float *w, void *grad) {
+                                                                const float *lpb, const float *lpl, const float *lpr,
+                                                                const float *lse, const float *w, void *grad) {
     constexpr int K = ChunkElems<DT, VEC>();
     const int n = blockIdx.y;
     const bool utt = n < N;
@@ -602,6 +598,11 @@ __global__ void __launch_bounds__(kRowThreads) ctct_grad_kernel(const void *x, l
     }
 }
 
+// the gradient pass of either loss, whose kernels share ctct_grad_kernel's parameters
+template <bool CTCT, int DT, bool VEC, bool RAW> auto GradKernel() {
+    return CTCT ? ctct_grad_kernel<DT, VEC, RAW> : rnnt_grad_kernel<DT, VEC, RAW>;
+}
+
 // ------------------------------------------------------------------------------------------------
 // gather.sum: out[off_n + t lb_n + u][h] = a[ta_n + t][h] + b[ub_n + u][h]; one warp per output row.  Backward: grad_a by a
 // sum over u (contiguous rows), grad_b by a sum over t (rows at stride lb_n), each a fixed-order fp32 sum per (row, h).
@@ -673,7 +674,7 @@ struct SimpleLayout {
     size_t mf, mg, ff, fg, S, W, PB, PL, PR, total;   // row maxima and "row has a flagged cell" of f and g; per cell S, W,
 };                                                    // pb, pl (and pr for the CTC-T loss; PR = 0 otherwise)
 
-SimpleLayout MakeSimpleLayout(int N, int Tmax, int Umax, bool ctct = false) {
+SimpleLayout MakeSimpleLayout(int N, int Tmax, int Umax, bool ctct) {
     const size_t nf = (size_t)N * Tmax, ng = (size_t)N * (Umax + 1), cells = nf * (Umax + 1);
     SimpleLayout L;
     L.r = MakeRnntLayout(N, (long long)cells, ctct);
@@ -805,20 +806,12 @@ __device__ __forceinline__ void SimpleNorm(const void *f, const void *g, long lo
     }
 }
 
-template <int DT>
+template <bool CTCT, int DT>
 __global__ void __launch_bounds__(256) simple_norm_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
                                                           const int *labels, int blank, RnntMeta *meta, const float *mf,
                                                           const float *mg, int *ff, int *fg, float *S, float *lpb, float *lpl,
-                                                          float *lse) {
-    SimpleNorm<DT, false>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, nullptr, lse);
-}
-
-template <int DT>
-__global__ void __launch_bounds__(256) ctct_simple_norm_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
-                                                               const int *labels, int blank, RnntMeta *meta, const float *mf,
-                                                               const float *mg, int *ff, int *fg, float *S, float *lpb,
-                                                               float *lpl, float *lpr, float *lse) {
-    SimpleNorm<DT, true>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, lpr, lse);
+                                                          float *lpr, float *lse) {
+    SimpleNorm<DT, CTCT>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, lpr, lse);
 }
 
 // Underflow fix-up: one warp per flagged cell (rows t without a flagged cell are skipped by their flag) takes the exact
@@ -876,27 +869,21 @@ __device__ __forceinline__ void SimpleFixup(const void *f, const void *g, long l
     }
 }
 
-template <int DT, bool VEC>
+template <bool CTCT, int DT, bool VEC>
 __global__ void __launch_bounds__(kRowThreads) simple_fixup_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
                                                                    const int *labels, int blank, const RnntMeta *meta,
                                                                    const int *ff, const float *S, float *lpb, float *lpl,
-                                                                   float *lse) {
-    SimpleFixup<DT, VEC, false>(f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, nullptr, lse);
-}
-
-template <int DT, bool VEC>
-__global__ void __launch_bounds__(kRowThreads) ctct_simple_fixup_kernel(const void *f, const void *g, long long V, int Tmax,
-                                                                        int Umax, const int *labels, int blank,
-                                                                        const RnntMeta *meta, const int *ff, const float *S,
-                                                                        float *lpb, float *lpl, float *lpr, float *lse) {
-    SimpleFixup<DT, VEC, true>(f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, lpr, lse);
+                                                                   float *lpr, float *lse) {
+    SimpleFixup<DT, VEC, CTCT>(f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, lpr, lse);
 }
 
 // Cell weights: per live cell pb, pl (weighted posteriors, as the gradient pass) and W = (pb + pl) / S, 0 for a flagged cell.
-__global__ void __launch_bounds__(kRowThreads) simple_weights_kernel(const RnntMeta *meta, const double *alpha, const double *beta,
-                                                                     const double *logp, const float *lpb, const float *lpl,
-                                                                     const float *S, const float *w, float *W, float *PB,
-                                                                     float *PL) {
+// The parameters are ctct_simple_weights_kernel's; labels, lpr and PR are not used.
+__global__ void __launch_bounds__(kRowThreads) simple_weights_kernel(const RnntMeta *meta, const int *labels, const double *alpha,
+                                                                     const double *beta, const double *logp, const float *lpb,
+                                                                     const float *lpl, const float *lpr, const float *S,
+                                                                     const float *w, float *W, float *PB, float *PL,
+                                                                     float *PR) {
     const int n = blockIdx.y;
     const RnntMeta m = meta[n];
     if (m.bad) return;
@@ -1106,22 +1093,15 @@ __device__ __forceinline__ void SimpleGrad(const void *f, const void *g, long lo
     }
 }
 
-template <int DT, bool GF>
+// GF before DT: the --profile reports of tools/*_bench.py key kernels by their first 60 characters, which then still
+// tell grad_f from grad_g
+template <bool CTCT, bool GF, int DT>
 __global__ void __launch_bounds__(256) simple_grad_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
                                                           const int *labels, int blank, const RnntMeta *meta, const float *mf,
                                                           const float *mg, const int *ff, const int *fg, const float *S,
                                                           const float *lse, const float *W, const float *PB, const float *PL,
-                                                          void *grad) {
-    SimpleGrad<DT, GF, false>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, nullptr, grad);
-}
-
-template <int DT, bool GF>
-__global__ void __launch_bounds__(256) ctct_simple_grad_kernel(const void *f, const void *g, long long V, int Tmax, int Umax,
-                                                               const int *labels, int blank, const RnntMeta *meta,
-                                                               const float *mf, const float *mg, const int *ff, const int *fg,
-                                                               const float *S, const float *lse, const float *W,
-                                                               const float *PB, const float *PL, const float *PR, void *grad) {
-    SimpleGrad<DT, GF, true>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, PR, grad);
+                                                          const float *PR, void *grad) {
+    SimpleGrad<DT, GF, CTCT>(f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, PR, grad);
 }
 
 int GridX(long long rows_per_utt, int per_cta) {
@@ -1143,13 +1123,17 @@ bool RowsVectorisable(const void *p, long long V, int dtype) {
 
 }  // namespace
 
-size_t RnntWsBytes(int N, long long rows) { return MakeRnntLayout(N, rows).total; }
+template <bool CTCT> size_t TransducerLoss<CTCT>::WsBytes(int N, long long rows) {
+    return MakeRnntLayout(N, rows, CTCT).total;
+}
 
-int LaunchRnntForward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
-                      const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
-                      float *costs, float *costs_beta, cudaStream_t s) {
-    const RnntLayout L = MakeRnntLayout(N, rows);
+template <bool CTCT>
+int TransducerLoss<CTCT>::Forward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax,
+                                  int Umax, const int *labels, long long n_labels, const int *lx, const int *ly, int blank,
+                                  int want_beta, void *ws, float *costs, float *costs_beta, cudaStream_t s) {
+    const RnntLayout L = MakeRnntLayout(N, rows, CTCT);
     RnntMeta *meta = At<RnntMeta>(ws, L.meta);
+    float *lpb = At<float>(ws, L.lpb), *lpl = At<float>(ws, L.lpl), *lpr = AtOpt<float>(ws, L.lpr);
     rnnt_prep_kernel<<<1, kPrepThreads, 0, s>>>(lx, ly, N, rows, n_labels, compact, Tmax, Umax, meta, At<long long>(ws, L.tail));
     const long long per_utt = (rows + N - 1) / N;
     if (from_logits) {
@@ -1157,153 +1141,55 @@ int LaunchRnntForward(const void *x, int dtype, int from_logits, int compact, in
         const bool vec = RowsVectorisable(x, V, dtype);
         DispatchDtype(dtype, [&](auto dt) {
             constexpr int DT = decltype(dt)::value;
-            auto k = vec ? rnnt_logit_rows_kernel<DT, true> : rnnt_logit_rows_kernel<DT, false>;
-            k<<<dim3(gx, N), kRowThreads, 0, s>>>(x, V, labels, blank, meta, At<float>(ws, L.lpb), At<float>(ws, L.lpl),
-                                                  At<float>(ws, L.lse));
-        });
-    } else {
-        rnnt_lp_rows_kernel<<<dim3(GridX(per_utt, kRowThreads * 4), N), kRowThreads, 0, s>>>(
-            x, dtype, V, labels, blank, meta, At<float>(ws, L.lpb), At<float>(ws, L.lpl));
-    }
-    rnnt_alpha_beta_kernel<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(
-        meta, At<float>(ws, L.lpb), At<float>(ws, L.lpl), At<double>(ws, L.alpha), At<double>(ws, L.beta),
-        At<double>(ws, L.logp), N, costs, want_beta ? costs_beta : nullptr);
-    CountLaunch(3);
-    return (int)cudaGetLastError();
-}
-
-int LaunchRnntBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
-                       void *ws, const float *w, void *grad, cudaStream_t s) {
-    const RnntLayout L = MakeRnntLayout(N, rows);
-    const long long per_utt = (rows + N - 1) / N;
-    const int gx = GridX(per_utt, kRowThreads / 32 * 4);
-    const bool vec = RowsVectorisable(grad, V, dtype) && (!from_logits || RowsVectorisable(x, V, dtype));
-    DispatchDtype(dtype, [&](auto dt) {
-        constexpr int DT = decltype(dt)::value;
-        auto k = from_logits ? (vec ? rnnt_grad_kernel<DT, true, true> : rnnt_grad_kernel<DT, false, true>)
-                             : (vec ? rnnt_grad_kernel<DT, true, false> : rnnt_grad_kernel<DT, false, false>);
-        k<<<dim3(gx, N + 1), kRowThreads, 0, s>>>(x, V, labels, blank, N, At<RnntMeta>(ws, L.meta), At<long long>(ws, L.tail),
-                                                  rows, At<double>(ws, L.alpha), At<double>(ws, L.beta),
-                                                  At<double>(ws, L.logp), At<float>(ws, L.lpb), At<float>(ws, L.lpl),
-                                                  At<float>(ws, L.lse), w, grad);
-    });
-    CountLaunch(1);
-    return (int)cudaGetLastError();
-}
-
-size_t RnntSimpleWsBytes(int N, int Tmax, int Umax) { return MakeSimpleLayout(N, Tmax, Umax).total; }
-
-int LaunchRnntSimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
-                            const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s) {
-    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax);
-    const int U1 = Umax + 1;
-    const long long cells = (long long)N * Tmax * U1;
-    RnntMeta *meta = At<RnntMeta>(ws, L.r.meta);
-    float *mf = At<float>(ws, L.mf), *mg = At<float>(ws, L.mg), *S = At<float>(ws, L.S);
-    float *lpb = At<float>(ws, L.r.lpb), *lpl = At<float>(ws, L.r.lpl), *lse = At<float>(ws, L.r.lse);
-    int *ff = At<int>(ws, L.ff), *fg = At<int>(ws, L.fg);
-    rnnt_prep_kernel<<<1, kPrepThreads, 0, s>>>(lx, ly, N, cells, (long long)N * Umax, 0, Tmax, Umax, meta,
-                                                At<long long>(ws, L.r.tail));
-    const bool vec = RowsVectorisable(f, V, dtype) && RowsVectorisable(g, V, dtype);
-    DispatchDtype(dtype, [&](auto dt) {
-        constexpr int DT = decltype(dt)::value;
-        auto rowmax = vec ? simple_rowmax_kernel<DT, true> : simple_rowmax_kernel<DT, false>;
-        rowmax<<<dim3(GridX(std::max(Tmax, U1), kRowThreads / 32 * 4), N, 2), kRowThreads, 0, s>>>(f, g, V, Tmax, Umax, meta,
-                                                                                                    mf, mg, ff, fg);
-        simple_norm_kernel<DT><<<dim3((Tmax + kST - 1) / kST, (U1 + kSU - 1) / kSU, N), 256, 0, s>>>(
-            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, lse);
-        auto fixup = vec ? simple_fixup_kernel<DT, true> : simple_fixup_kernel<DT, false>;
-        fixup<<<dim3(GridX((long long)Tmax * U1, kRowThreads / 32 * 16), N), kRowThreads, 0, s>>>(
-            f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, lse);
-    });
-    rnnt_alpha_beta_kernel<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(meta, lpb, lpl, At<double>(ws, L.r.alpha),
-                                                                             At<double>(ws, L.r.beta),
-                                                                             At<double>(ws, L.r.logp), N, costs, nullptr);
-    CountLaunch(5);
-    return (int)cudaGetLastError();
-}
-
-int LaunchRnntSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
-                             int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s) {
-    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax);
-    const int U1 = Umax + 1;
-    const RnntMeta *meta = At<RnntMeta>(ws, L.r.meta);
-    const float *mf = At<float>(ws, L.mf), *mg = At<float>(ws, L.mg), *S = At<float>(ws, L.S), *lse = At<float>(ws, L.r.lse);
-    const int *ff = At<int>(ws, L.ff), *fg = At<int>(ws, L.fg);
-    float *W = At<float>(ws, L.W), *PB = At<float>(ws, L.PB), *PL = At<float>(ws, L.PL);
-    simple_weights_kernel<<<dim3(GridX((long long)Tmax * U1, kRowThreads * 4), N), kRowThreads, 0, s>>>(
-        meta, At<double>(ws, L.r.alpha), At<double>(ws, L.r.beta), At<double>(ws, L.r.logp), At<float>(ws, L.r.lpb),
-        At<float>(ws, L.r.lpl), S, w, W, PB, PL);
-    const int gx = (int)((V + kGC - 1) / kGC);
-    DispatchDtype(dtype, [&](auto dt) {
-        constexpr int DT = decltype(dt)::value;
-        simple_grad_kernel<DT, true><<<dim3(gx, (Tmax + kGR - 1) / kGR, N), 256, 0, s>>>(
-            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, grad_f);
-        simple_grad_kernel<DT, false><<<dim3(gx, (U1 + kGR - 1) / kGR, N), 256, 0, s>>>(
-            f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, grad_g);
-    });
-    CountLaunch(3);
-    return (int)cudaGetLastError();
-}
-
-size_t CtctWsBytes(int N, long long rows) { return MakeRnntLayout(N, rows, true).total; }
-
-int LaunchCtctForward(const void *x, int dtype, int from_logits, int compact, int N, long long rows, int V, int Tmax, int Umax,
-                      const int *labels, long long n_labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
-                      float *costs, float *costs_beta, cudaStream_t s) {
-    const RnntLayout L = MakeRnntLayout(N, rows, true);
-    RnntMeta *meta = At<RnntMeta>(ws, L.meta);
-    float *lpb = At<float>(ws, L.lpb), *lpl = At<float>(ws, L.lpl), *lpr = At<float>(ws, L.lpr);
-    rnnt_prep_kernel<<<1, kPrepThreads, 0, s>>>(lx, ly, N, rows, n_labels, compact, Tmax, Umax, meta, At<long long>(ws, L.tail));
-    const long long per_utt = (rows + N - 1) / N;
-    if (from_logits) {
-        const int gx = GridX(per_utt, kRowThreads / 32 * 4);
-        const bool vec = RowsVectorisable(x, V, dtype);
-        DispatchDtype(dtype, [&](auto dt) {
-            constexpr int DT = decltype(dt)::value;
-            auto k = vec ? ctct_logit_rows_kernel<DT, true> : ctct_logit_rows_kernel<DT, false>;
+            auto k = vec ? logit_rows_kernel<CTCT, DT, true> : logit_rows_kernel<CTCT, DT, false>;
             k<<<dim3(gx, N), kRowThreads, 0, s>>>(x, V, labels, blank, meta, lpb, lpl, lpr, At<float>(ws, L.lse));
         });
     } else {
-        ctct_lp_rows_kernel<<<dim3(GridX(per_utt, kRowThreads * 4), N), kRowThreads, 0, s>>>(x, dtype, V, labels, blank, meta,
+        lp_rows_kernel<CTCT><<<dim3(GridX(per_utt, kRowThreads * 4), N), kRowThreads, 0, s>>>(x, dtype, V, labels, blank, meta,
                                                                                             lpb, lpl, lpr);
     }
-    ctct_alpha_beta_kernel<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(
-        meta, labels, lpb, lpl, lpr, At<double>(ws, L.alpha), At<double>(ws, L.beta), At<double>(ws, L.logp), N, costs,
-        want_beta ? costs_beta : nullptr);
+    const auto alpha_beta = CTCT ? ctct_alpha_beta_kernel : rnnt_alpha_beta_kernel;
+    alpha_beta<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(meta, labels, lpb, lpl, lpr, At<double>(ws, L.alpha),
+                                                                 At<double>(ws, L.beta), At<double>(ws, L.logp), N, costs,
+                                                                 want_beta ? costs_beta : nullptr);
     CountLaunch(3);
     return (int)cudaGetLastError();
 }
 
-int LaunchCtctBackward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels, int blank,
-                       void *ws, const float *w, void *grad, cudaStream_t s) {
-    const RnntLayout L = MakeRnntLayout(N, rows, true);
+template <bool CTCT>
+int TransducerLoss<CTCT>::Backward(const void *x, int dtype, int from_logits, int N, long long rows, int V, const int *labels,
+                                   int blank, void *ws, const float *w, void *grad, cudaStream_t s) {
+    const RnntLayout L = MakeRnntLayout(N, rows, CTCT);
     const long long per_utt = (rows + N - 1) / N;
     const int gx = GridX(per_utt, kRowThreads / 32 * 4);
     const bool vec = RowsVectorisable(grad, V, dtype) && (!from_logits || RowsVectorisable(x, V, dtype));
     DispatchDtype(dtype, [&](auto dt) {
         constexpr int DT = decltype(dt)::value;
-        auto k = from_logits ? (vec ? ctct_grad_kernel<DT, true, true> : ctct_grad_kernel<DT, false, true>)
-                             : (vec ? ctct_grad_kernel<DT, true, false> : ctct_grad_kernel<DT, false, false>);
+        auto k = from_logits ? (vec ? GradKernel<CTCT, DT, true, true>() : GradKernel<CTCT, DT, false, true>())
+                             : (vec ? GradKernel<CTCT, DT, true, false>() : GradKernel<CTCT, DT, false, false>());
         k<<<dim3(gx, N + 1), kRowThreads, 0, s>>>(x, V, labels, blank, N, At<RnntMeta>(ws, L.meta), At<long long>(ws, L.tail),
                                                   rows, At<double>(ws, L.alpha), At<double>(ws, L.beta),
                                                   At<double>(ws, L.logp), At<float>(ws, L.lpb), At<float>(ws, L.lpl),
-                                                  At<float>(ws, L.lpr), At<float>(ws, L.lse), w, grad);
+                                                  AtOpt<float>(ws, L.lpr), At<float>(ws, L.lse), w, grad);
     });
     CountLaunch(1);
     return (int)cudaGetLastError();
 }
 
-size_t CtctSimpleWsBytes(int N, int Tmax, int Umax) { return MakeSimpleLayout(N, Tmax, Umax, true).total; }
+template <bool CTCT> size_t TransducerLoss<CTCT>::SimpleWsBytes(int N, int Tmax, int Umax) {
+    return MakeSimpleLayout(N, Tmax, Umax, CTCT).total;
+}
 
-int LaunchCtctSimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
-                            const int *lx, const int *ly, int blank, int want_beta, void *ws, float *costs, cudaStream_t s) {
-    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax, true);
+template <bool CTCT>
+int TransducerLoss<CTCT>::SimpleForward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V,
+                                        const int *labels, const int *lx, const int *ly, int blank, int want_beta, void *ws,
+                                        float *costs, cudaStream_t s) {
+    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax, CTCT);
     const int U1 = Umax + 1;
     const long long cells = (long long)N * Tmax * U1;
     RnntMeta *meta = At<RnntMeta>(ws, L.r.meta);
     float *mf = At<float>(ws, L.mf), *mg = At<float>(ws, L.mg), *S = At<float>(ws, L.S);
-    float *lpb = At<float>(ws, L.r.lpb), *lpl = At<float>(ws, L.r.lpl), *lpr = At<float>(ws, L.r.lpr);
+    float *lpb = At<float>(ws, L.r.lpb), *lpl = At<float>(ws, L.r.lpl), *lpr = AtOpt<float>(ws, L.r.lpr);
     float *lse = At<float>(ws, L.r.lse);
     int *ff = At<int>(ws, L.ff), *fg = At<int>(ws, L.fg);
     rnnt_prep_kernel<<<1, kPrepThreads, 0, s>>>(lx, ly, N, cells, (long long)N * Umax, 0, Tmax, Umax, meta,
@@ -1314,42 +1200,48 @@ int LaunchCtctSimpleForward(const void *f, const void *g, int dtype, int N, int 
         auto rowmax = vec ? simple_rowmax_kernel<DT, true> : simple_rowmax_kernel<DT, false>;
         rowmax<<<dim3(GridX(std::max(Tmax, U1), kRowThreads / 32 * 4), N, 2), kRowThreads, 0, s>>>(f, g, V, Tmax, Umax, meta,
                                                                                                     mf, mg, ff, fg);
-        ctct_simple_norm_kernel<DT><<<dim3((Tmax + kST - 1) / kST, (U1 + kSU - 1) / kSU, N), 256, 0, s>>>(
+        simple_norm_kernel<CTCT, DT><<<dim3((Tmax + kST - 1) / kST, (U1 + kSU - 1) / kSU, N), 256, 0, s>>>(
             f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lpb, lpl, lpr, lse);
-        auto fixup = vec ? ctct_simple_fixup_kernel<DT, true> : ctct_simple_fixup_kernel<DT, false>;
+        auto fixup = vec ? simple_fixup_kernel<CTCT, DT, true> : simple_fixup_kernel<CTCT, DT, false>;
         fixup<<<dim3(GridX((long long)Tmax * U1, kRowThreads / 32 * 16), N), kRowThreads, 0, s>>>(
             f, g, V, Tmax, Umax, labels, blank, meta, ff, S, lpb, lpl, lpr, lse);
     });
-    ctct_alpha_beta_kernel<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(meta, labels, lpb, lpl, lpr,
-                                                                             At<double>(ws, L.r.alpha),
-                                                                             At<double>(ws, L.r.beta),
-                                                                             At<double>(ws, L.r.logp), N, costs, nullptr);
+    const auto alpha_beta = CTCT ? ctct_alpha_beta_kernel : rnnt_alpha_beta_kernel;
+    alpha_beta<<<dim3(N, want_beta ? 2 : 1), kAbThreads, 0, s>>>(meta, labels, lpb, lpl, lpr, At<double>(ws, L.r.alpha),
+                                                                 At<double>(ws, L.r.beta), At<double>(ws, L.r.logp), N, costs,
+                                                                 nullptr);
     CountLaunch(5);
     return (int)cudaGetLastError();
 }
 
-int LaunchCtctSimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V, const int *labels,
-                             int blank, void *ws, const float *w, void *grad_f, void *grad_g, cudaStream_t s) {
-    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax, true);
+template <bool CTCT>
+int TransducerLoss<CTCT>::SimpleBackward(const void *f, const void *g, int dtype, int N, int Tmax, int Umax, int V,
+                                         const int *labels, int blank, void *ws, const float *w, void *grad_f, void *grad_g,
+                                         cudaStream_t s) {
+    const SimpleLayout L = MakeSimpleLayout(N, Tmax, Umax, CTCT);
     const int U1 = Umax + 1;
     const RnntMeta *meta = At<RnntMeta>(ws, L.r.meta);
     const float *mf = At<float>(ws, L.mf), *mg = At<float>(ws, L.mg), *S = At<float>(ws, L.S), *lse = At<float>(ws, L.r.lse);
     const int *ff = At<int>(ws, L.ff), *fg = At<int>(ws, L.fg);
-    float *W = At<float>(ws, L.W), *PB = At<float>(ws, L.PB), *PL = At<float>(ws, L.PL), *PR = At<float>(ws, L.PR);
-    ctct_simple_weights_kernel<<<dim3(GridX((long long)Tmax * U1, kRowThreads * 4), N), kRowThreads, 0, s>>>(
+    float *W = At<float>(ws, L.W), *PB = At<float>(ws, L.PB), *PL = At<float>(ws, L.PL), *PR = AtOpt<float>(ws, L.PR);
+    const auto weights = CTCT ? ctct_simple_weights_kernel : simple_weights_kernel;
+    weights<<<dim3(GridX((long long)Tmax * U1, kRowThreads * 4), N), kRowThreads, 0, s>>>(
         meta, labels, At<double>(ws, L.r.alpha), At<double>(ws, L.r.beta), At<double>(ws, L.r.logp), At<float>(ws, L.r.lpb),
-        At<float>(ws, L.r.lpl), At<float>(ws, L.r.lpr), S, w, W, PB, PL, PR);
+        At<float>(ws, L.r.lpl), AtOpt<float>(ws, L.r.lpr), S, w, W, PB, PL, PR);
     const int gx = (int)((V + kGC - 1) / kGC);
     DispatchDtype(dtype, [&](auto dt) {
         constexpr int DT = decltype(dt)::value;
-        ctct_simple_grad_kernel<DT, true><<<dim3(gx, (Tmax + kGR - 1) / kGR, N), 256, 0, s>>>(
+        simple_grad_kernel<CTCT, true, DT><<<dim3(gx, (Tmax + kGR - 1) / kGR, N), 256, 0, s>>>(
             f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, PR, grad_f);
-        ctct_simple_grad_kernel<DT, false><<<dim3(gx, (U1 + kGR - 1) / kGR, N), 256, 0, s>>>(
+        simple_grad_kernel<CTCT, false, DT><<<dim3(gx, (U1 + kGR - 1) / kGR, N), 256, 0, s>>>(
             f, g, V, Tmax, Umax, labels, blank, meta, mf, mg, ff, fg, S, lse, W, PB, PL, PR, grad_g);
     });
     CountLaunch(3);
     return (int)cudaGetLastError();
 }
+
+template struct TransducerLoss<false>;
+template struct TransducerLoss<true>;
 
 size_t GatherWsBytes(int N) { return Align256(sizeof(GatherMeta) * (size_t)N); }
 

@@ -13,6 +13,7 @@ from . import _lib
 from ._C import _DTYPES, _PinnedRing, _check, _rings, _stream
 
 REDUCTIONS = ("mean", "sum", "none")
+_INT32_MAX = 2 ** 31 - 1
 
 
 def check_rnnt_args(log_probs, labels, frames_lengths, labels_lengths, reduction, blank, compact,
@@ -84,6 +85,14 @@ def _on_device(dev, *ts) -> list:
     return out
 
 
+def _int32(t: torch.Tensor) -> torch.Tensor:
+    """int32 labels or lengths, on t's device and without a synchronisation.  int64 values outside the int32 range are
+    clamped to -1 or the int32 maximum first, so that the kernels see them as invalid instead of wrapped round."""
+    if t.dtype == torch.int32:
+        return t
+    return t.clamp(-1, _INT32_MAX).to(torch.int32)
+
+
 def _forward(x, labels, lx, ly, blank, compact, from_logits, want_beta, shape, family="rnnt"):
     """One native forward of the ccb_<family>_* entries ("rnnt", or "ctct" for the CTC-T loss, which takes the same
     arguments).  Returns (costs (N,) fp32, costs from beta or None, workspace, device labels)."""
@@ -108,15 +117,23 @@ def _reduce(costs, reduction):
     return costs.sum() if reduction == "sum" else costs
 
 
-class _RNNT(Function):
-    """The RNN-T loss with its gradient.  The forward runs the row pass and alpha || beta, keeping only the O(rows)
-    workspace; the backward writes w_n d cost_n / d x in one pass, in x's dtype (w_n = grad_output, / N for 'mean')."""
+def _weights(grad_output, N, reduction, dev):
+    """The per-utterance weights w_n of the backward: grad_output, / N for 'mean', expanded to (N,) fp32."""
+    g = grad_output.to(device=dev, dtype=torch.float32)
+    w = (g / N).expand(N) if reduction == "mean" else g.expand(N) if reduction == "sum" else g
+    return w.contiguous()
+
+
+class _Loss(Function):
+    """The RNN-T or CTC-T loss (family "rnnt" or "ctct") with its gradient.  The forward runs the row pass and alpha ||
+    beta, keeping only the O(rows) workspace; the backward writes w_n d cost_n / d x in one pass, in x's dtype."""
 
     @staticmethod
-    def forward(ctx, x, labels, lx, ly, reduction, blank, compact, from_logits, shape):
+    def forward(ctx, x, labels, lx, ly, reduction, blank, compact, from_logits, shape, family, name):
         x = x.contiguous()
-        costs, _, ws, labels_d = _forward(x, labels, lx, ly, blank, compact, from_logits, True, shape)
+        costs, _, ws, labels_d = _forward(x, labels, lx, ly, blank, compact, from_logits, True, shape, family)
         ctx.ws, ctx.labels, ctx.shape, ctx.reduction, ctx.blank, ctx.from_logits = ws, labels_d, shape, reduction, blank, from_logits
+        ctx.family, ctx.name = family, name
         ctx.x = x if from_logits else None
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         return _reduce(costs, reduction)
@@ -125,19 +142,41 @@ class _RNNT(Function):
     def backward(ctx, grad_output):
         N, rows, V = ctx.shape[:3]
         dev = ctx.ws.device
-        g = grad_output.to(device=dev, dtype=torch.float32)
-        w = (g / N).expand(N) if ctx.reduction == "mean" else g.expand(N) if ctx.reduction == "sum" else g
-        w = w.contiguous()
+        w = _weights(grad_output, N, ctx.reduction, dev)
         grad = torch.empty(ctx.x_shape, dtype=ctx.x_dtype, device=dev)
         x = ctx.x
         L = _lib.lib()
         with torch.cuda.device(dev):
-            rc = L.ccb_rnnt_backward(None if x is None else x.data_ptr(), _DTYPES[ctx.x_dtype], int(ctx.from_logits), N, rows, V,
-                                     ctx.labels.data_ptr(), int(ctx.blank), ctx.ws.data_ptr(), w.data_ptr(), grad.data_ptr(),
-                                     _stream(dev))
-        _check(rc, "rnnt_loss backward")
+            rc = getattr(L, f"ccb_{ctx.family}_backward")(None if x is None else x.data_ptr(), _DTYPES[ctx.x_dtype],
+                                                          int(ctx.from_logits), N, rows, V, ctx.labels.data_ptr(),
+                                                          int(ctx.blank), ctx.ws.data_ptr(), w.data_ptr(), grad.data_ptr(),
+                                                          _stream(dev))
+        _check(rc, f"{ctx.name} backward")
         ctx.ws = ctx.x = ctx.labels = None
-        return (grad,) + (None,) * 8
+        return (grad,) + (None,) * 10
+
+
+def _loss(family, name, log_probs, labels, frames_lengths, labels_lengths, reduction, blank, compact, from_logits):
+    """The loss `name` of the ccb_<family>_* entries over the joint tensor: the argument checks, the forward alone under
+    ``torch.no_grad`` (or for an input that does not require grad), else the autograd Function."""
+    shape = check_rnnt_args(log_probs, labels, frames_lengths, labels_lengths, reduction, blank, compact, name)
+    if not log_probs.is_cuda:
+        raise ValueError(f"{name}: log_probs must be on a CUDA device")
+    with torch.cuda.device(log_probs.device):
+        if torch.is_grad_enabled() and log_probs.requires_grad:
+            return _Loss.apply(log_probs, labels, frames_lengths, labels_lengths, reduction, blank, bool(compact),
+                               bool(from_logits), shape, family, name)
+        costs = _forward(log_probs.detach().contiguous(), labels, frames_lengths, labels_lengths, blank, compact, from_logits,
+                         False, shape, family)[0]
+        return _reduce(costs, reduction)
+
+
+def _costs_both_ways(family, name, log_probs, labels, frames_lengths, labels_lengths, blank, compact, from_logits):
+    shape = check_rnnt_args(log_probs, labels, frames_lengths, labels_lengths, "none", blank, compact, name)
+    with torch.no_grad(), torch.cuda.device(log_probs.device):
+        costs, costs_b, _, _ = _forward(log_probs.contiguous(), labels, frames_lengths, labels_lengths, blank, compact,
+                                        from_logits, True, shape, family)
+    return costs, costs_b
 
 
 def rnnt_loss(log_probs: torch.Tensor, labels: torch.Tensor, frames_lengths: torch.Tensor, labels_lengths: torch.Tensor,
@@ -155,25 +194,13 @@ def rnnt_loss(log_probs: torch.Tensor, labels: torch.Tensor, frames_lengths: tor
     [0, V) or equal to blank, gets cost NaN and zero gradient instead.  reduction: 'mean' (default) of the N costs, 'sum' or
     'none' (the (N,) fp32 costs).  The gradient comes back in log_probs' dtype.  Under ``torch.no_grad`` (or for an input
     that does not require grad) only the forward recursion runs."""
-    shape = check_rnnt_args(log_probs, labels, frames_lengths, labels_lengths, reduction, blank, compact)
-    if not log_probs.is_cuda:
-        raise ValueError("rnnt_loss: log_probs must be on a CUDA device")
-    with torch.cuda.device(log_probs.device):
-        if torch.is_grad_enabled() and log_probs.requires_grad:
-            return _RNNT.apply(log_probs, labels, frames_lengths, labels_lengths, reduction, blank, bool(compact),
-                               bool(from_logits), shape)
-        costs = _forward(log_probs.detach().contiguous(), labels, frames_lengths, labels_lengths, blank, compact, from_logits,
-                         False, shape)[0]
-        return _reduce(costs, reduction)
+    return _loss("rnnt", "rnnt_loss", log_probs, labels, frames_lengths, labels_lengths, reduction, blank, compact, from_logits)
 
 
 def rnnt_costs_both_ways(log_probs, labels, frames_lengths, labels_lengths, blank=0, compact=False, from_logits=False):
     """The (N,) costs from alpha and from beta, which agree up to rounding (a check of the two recursions)."""
-    shape = check_rnnt_args(log_probs, labels, frames_lengths, labels_lengths, "none", blank, compact)
-    with torch.no_grad(), torch.cuda.device(log_probs.device):
-        costs, costs_b, _, _ = _forward(log_probs.contiguous(), labels, frames_lengths, labels_lengths, blank, compact,
-                                        from_logits, True, shape)
-    return costs, costs_b
+    return _costs_both_ways("rnnt", "rnnt_loss", log_probs, labels, frames_lengths, labels_lengths, blank, compact,
+                            from_logits)
 
 
 # ---------------------------------------------------------------------------------------------------

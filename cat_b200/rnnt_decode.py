@@ -17,8 +17,7 @@ import torch
 from . import _lib
 from ._C import _DTYPES, _check, _stream
 from .ngram import NGramLM
-from .rnnt import _on_device
-from .rnnt_simple import _int32
+from .rnnt import _int32, _on_device
 
 MAX_BEAM = 128
 MAX_MIX = 8                  # members of a MultiLM (rnnt_decode.cu kLmMixMax)

@@ -11,9 +11,7 @@ from torch.autograd import Function
 
 from . import _lib
 from ._C import _DTYPES, _check, _stream
-from .rnnt import REDUCTIONS, _on_device, _reduce
-
-_INT32_MAX = 2 ** 31 - 1
+from .rnnt import _INT32_MAX, REDUCTIONS, _int32, _on_device, _reduce, _weights
 
 
 def check_rnnt_simple_args(f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank,
@@ -59,14 +57,6 @@ def check_rnnt_simple_args(f_enc, g_pred, labels, frames_lengths, labels_lengths
     return N, Tmax, Umax, V
 
 
-def _int32(t: torch.Tensor) -> torch.Tensor:
-    """int32 labels or lengths, on t's device and without a synchronisation.  int64 values outside the int32 range are
-    clamped to -1 or the int32 maximum first, so that the kernels see them as invalid instead of wrapped round."""
-    if t.dtype == torch.int32:
-        return t
-    return t.clamp(-1, _INT32_MAX).to(torch.int32)
-
-
 def _forward(f, g, labels, lx, ly, blank, want_beta, shape, family="rnnt"):
     """One native forward of the ccb_<family>_simple_* entries ("rnnt", or "ctct" for the CTC-T loss, which takes the same
     arguments).  Returns (costs (N,) fp32, workspace, device labels)."""
@@ -83,15 +73,16 @@ def _forward(f, g, labels, lx, ly, blank, want_beta, shape, family="rnnt"):
     return costs, ws, labels_d
 
 
-class _RNNTSimple(Function):
-    """The LogAdd joiner's RNN-T loss with its gradients on f and g.  The forward keeps only the O(cells + rows) workspace;
-    the backward writes w_n d cost_n / d f and d g (w_n = grad_output, / N for 'mean') in f's dtype."""
+class _SimpleLoss(Function):
+    """The LogAdd joiner's RNN-T or CTC-T loss (family "rnnt" or "ctct") with its gradients on f and g.  The forward keeps
+    only the O(cells + rows) workspace; the backward writes w_n d cost_n / d f and d g in f's dtype."""
 
     @staticmethod
-    def forward(ctx, f, g, labels, lx, ly, reduction, blank, shape):
+    def forward(ctx, f, g, labels, lx, ly, reduction, blank, shape, family, name):
         f, g = f.contiguous(), g.contiguous()
-        costs, ws, labels_d = _forward(f, g, labels, lx, ly, blank, True, shape)
+        costs, ws, labels_d = _forward(f, g, labels, lx, ly, blank, True, shape, family)
         ctx.f, ctx.g, ctx.ws, ctx.labels, ctx.shape, ctx.reduction, ctx.blank = f, g, ws, labels_d, shape, reduction, blank
+        ctx.family, ctx.name = family, name
         return _reduce(costs, reduction)
 
     @staticmethod
@@ -99,19 +90,33 @@ class _RNNTSimple(Function):
         N, Tmax, Umax, V = ctx.shape
         f, g = ctx.f, ctx.g
         dev = f.device
-        go = grad_output.to(device=dev, dtype=torch.float32)
-        w = (go / N).expand(N) if ctx.reduction == "mean" else go.expand(N) if ctx.reduction == "sum" else go
-        w = w.contiguous()
+        w = _weights(grad_output, N, ctx.reduction, dev)
         grad_f = torch.empty(f.shape, dtype=f.dtype, device=dev)
         grad_g = torch.empty(g.shape, dtype=g.dtype, device=dev)
         L = _lib.lib()
         with torch.cuda.device(dev):
-            rc = L.ccb_rnnt_simple_backward(f.data_ptr(), g.data_ptr(), _DTYPES[f.dtype], N, Tmax, Umax, V,
-                                            ctx.labels.data_ptr(), int(ctx.blank), ctx.ws.data_ptr(), w.data_ptr(),
-                                            grad_f.data_ptr(), grad_g.data_ptr(), _stream(dev))
-        _check(rc, "rnnt_loss_simple backward")
+            rc = getattr(L, f"ccb_{ctx.family}_simple_backward")(f.data_ptr(), g.data_ptr(), _DTYPES[f.dtype], N, Tmax, Umax,
+                                                                 V, ctx.labels.data_ptr(), int(ctx.blank), ctx.ws.data_ptr(),
+                                                                 w.data_ptr(), grad_f.data_ptr(), grad_g.data_ptr(),
+                                                                 _stream(dev))
+        _check(rc, f"{ctx.name} backward")
         ctx.f = ctx.g = ctx.ws = ctx.labels = None
-        return (grad_f if ctx.needs_input_grad[0] else None, grad_g if ctx.needs_input_grad[1] else None) + (None,) * 6
+        return (grad_f if ctx.needs_input_grad[0] else None, grad_g if ctx.needs_input_grad[1] else None) + (None,) * 8
+
+
+def _simple_loss(family, name, f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank):
+    """The loss `name` of the ccb_<family>_simple_* entries: the argument checks, the forward alone under
+    ``torch.no_grad`` (or for inputs that do not require grad), else the autograd Function."""
+    shape = check_rnnt_simple_args(f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank, name)
+    if not f_enc.is_cuda or g_pred.device != f_enc.device:
+        raise ValueError(f"{name}: f_enc and g_pred must be on one CUDA device")
+    with torch.cuda.device(f_enc.device):
+        if torch.is_grad_enabled() and (f_enc.requires_grad or g_pred.requires_grad):
+            return _SimpleLoss.apply(f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank, shape, family,
+                                     name)
+        costs = _forward(f_enc.detach().contiguous(), g_pred.detach().contiguous(), labels, frames_lengths, labels_lengths,
+                         blank, False, shape, family)[0]
+        return _reduce(costs, reduction)
 
 
 def rnnt_loss_simple(f_enc: torch.Tensor, g_pred: torch.Tensor, labels: torch.Tensor, frames_lengths: torch.Tensor,
@@ -126,12 +131,4 @@ def rnnt_loss_simple(f_enc: torch.Tensor, g_pred: torch.Tensor, labels: torch.Te
     overruns the tensors, or a label outside [0, V) or equal to blank, gets cost NaN and zero gradient instead.
     reduction: 'mean' (default) of the N costs, 'sum' or 'none' (the (N,) fp32 costs).  No host synchronisation; the
     gradients come back in the inputs' dtype; under ``torch.no_grad`` only the forward recursion runs."""
-    shape = check_rnnt_simple_args(f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank)
-    if not f_enc.is_cuda or g_pred.device != f_enc.device:
-        raise ValueError("rnnt_loss_simple: f_enc and g_pred must be on one CUDA device")
-    with torch.cuda.device(f_enc.device):
-        if torch.is_grad_enabled() and (f_enc.requires_grad or g_pred.requires_grad):
-            return _RNNTSimple.apply(f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank, shape)
-        costs = _forward(f_enc.detach().contiguous(), g_pred.detach().contiguous(), labels, frames_lengths, labels_lengths,
-                         blank, False, shape)[0]
-        return _reduce(costs, reduction)
+    return _simple_loss("rnnt", "rnnt_loss_simple", f_enc, g_pred, labels, frames_lengths, labels_lengths, reduction, blank)

@@ -296,13 +296,13 @@ def _bits(t):
 @pytest.mark.parametrize("compact", [False, True], ids=["padded", "compact"])
 @pytest.mark.parametrize("fl", [False, True], ids=["logprobs", "logits"])
 def test_poisoned_allocator(monkeypatch, compact, fl):
-    """Every buffer the loss allocates filled with 0x00, 0xFF and 0x7F: the same bits out, including an infeasible
-    utterance, a bad one (device lengths) and, compact, tail rows behind the last utterance, which get exact zeros."""
-    import cat_b200.ctct as C
+    """Every buffer the loss allocates (in cat_b200.rnnt, which runs both losses) filled with 0x00, 0xFF and 0x7F: the
+    same bits out, including an infeasible utterance, a bad one (device lengths) and, compact, tail rows behind the last
+    utterance, which get exact zeros."""
     import cat_b200.rnnt as R
+    from cat_b200 import _lib
     proxy = ScratchProxy(0)
     monkeypatch.setattr(R, "torch", proxy)
-    monkeypatch.setattr(C, "torch", proxy)
     V, blank = 24, 5
     z, y, lx, ly = _batch([6, 4, 7, 3, 5], [3, 2, 4, 1, 2], V, blank, seed=9, Tmax=8, Umax=5)
     y[2] = torch.tensor([7, 7, 7, 7, 1], dtype=torch.int32)           # needs 7 frames: feasible; utterance 3: U = 1
@@ -330,6 +330,9 @@ def test_poisoned_allocator(monkeypatch, compact, fl):
         return dict(c=c, g=g, ce=ce)
 
     clean = {k: _bits(v) for k, v in run().items()}
+    rows = x.shape[0] if compact else x[..., 0].numel()
+    seen = {nb for nb, _, d in proxy.record if d.type == "cuda"}
+    assert int(_lib.lib().ccb_ctct_workspace_bytes(len(lx), rows)) in seen, sorted(seen)
     c = clean["c"].view(torch.float32)
     assert torch.isnan(c[1]) and c[4] == float("inf") and torch.isfinite(c[[0, 2, 3]]).all()
     assert torch.equal(clean["c"], clean["ce"])
