@@ -37,7 +37,7 @@ SYMBOLS = [
     "ccb_ctct_workspace_bytes", "ccb_ctct_forward", "ccb_ctct_backward", "ccb_ctct_simple_workspace_bytes",
     "ccb_ctct_simple_forward", "ccb_ctct_simple_backward", "ccb_rnnt_beam_ws_bytes", "ccb_rnnt_beam_init",
     "ccb_rnnt_beam_step", "ccb_rnnt_beam_finish", "ccb_ctct_beam_ws_bytes", "ccb_ctct_beam_init", "ccb_ctct_beam_step",
-    "ccb_rnnt_beam_step_fused", "ccb_ngram_slot_rows", "ccb_lm_mix_slot_rows",
+    "ccb_rnnt_beam_step_fused", "ccb_ngram_slot_rows", "ccb_lm_mix_slot_rows", "ccb_ngram_score",
 ]
 GLOBALS = ["DEN_NUM_ARCS", "DEN_NUM_STATES"]
 
@@ -171,6 +171,7 @@ def lib() -> C.CDLL:
     L.ccb_ngram_slot_rows.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp]; L.ccb_ngram_slot_rows.restype = C.c_int
     L.ccb_lm_mix_slot_rows.argtypes = [i, vp, vp, vp, vp, i, vp, vp, vp, vp, i, i, i, vp, vp, vp, vp]
     L.ccb_lm_mix_slot_rows.restype = C.c_int
+    L.ccb_ngram_score.argtypes = [vp, i, i, vp, l, i, vp, l, i, vp, i, vp, vp]; L.ccb_ngram_score.restype = C.c_int
     L.ccb_ctct_beam_ws_bytes.argtypes = [i, i, i]; L.ccb_ctct_beam_ws_bytes.restype = C.c_size_t
     L.ccb_ctct_beam_init.argtypes = [i, i, i, vp, vp, vp, vp, vp, vp]; L.ccb_ctct_beam_init.restype = C.c_int
     L.ccb_ctct_beam_step.argtypes = [vp, vp, i, i, i, i, i, i, i, vp, i, vp, vp, vp, vp, vp, vp]

@@ -13,7 +13,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libctc_crf_b200.so")
-SOURCES = ["api.cu", "den_kernels.cu", "den_sample.cu", "beam_search.cu", "ctc_kernels.cu", "den_graph.cc", "ngram.cc", "wfst_decode.cu", "wfst.cc", "rnnt_kernels.cu", "rnnt_decode.cu", "ctct_decode.cu"]
+SOURCES = ["api.cu", "den_kernels.cu", "den_sample.cu", "beam_search.cu", "ctc_kernels.cu", "den_graph.cc", "ngram.cc", "wfst_decode.cu", "wfst.cc", "rnnt_kernels.cu", "rnnt_decode.cu", "ctct_decode.cu", "ngram_score.cu"]
 HEADERS = ["common.cuh", "beam_common.cuh", "transducer_beam.cuh", "den_graph.h", "den_launch.h", "ngram.h", "wfst.h", os.path.join("..", "..", "include", "ctc_crf_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]

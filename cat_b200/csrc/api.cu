@@ -1243,6 +1243,31 @@ int ccb_ngram_slot_rows(const void *lm, int N, int beam, int V, const int *paren
     return 0;
 }
 
+int ccb_ngram_score(const void *lm, int R, int U, const void *ids, long ids_stride, int ids_i64, const void *last,
+                    long last_stride, int last_i64, const void *lens, int lens_i64, float *out, void *stream) {
+    g_err.clear();
+    if (!lm) return Fail("ngram_score: missing LM");
+    NGram *m = reinterpret_cast<NGram *>(const_cast<void *>(lm));
+    if (R <= 0 || U <= 0) return Fail("ngram_score: R and U must be positive");
+    if (ids_stride < U || last_stride < 0) return Fail("ngram_score: ids_stride must be >= U and last_stride >= 0");
+    if ((ids_i64 | last_i64 | lens_i64) & ~1) return Fail("ngram_score: the *_i64 flags are 0 (int32) or 1 (int64)");
+    if (!ids || !last || !out) return Fail("ngram_score: missing buffer");
+    if (m->host.bos_word < 0 || !m->host.eos_listed)
+        return Fail(std::string("ngram_score: the LM lists no ") + (m->host.bos_word < 0 ? "<s>" : "</s>") +
+                    "; a sentence score starts with <s> and ends with </s>");
+    const NGramDev *lmd = nullptr;
+    if (EnsureNGram(m, &lmd)) return 1;
+    NGramScoreArgs a;
+    a.lm = *lmd;
+    a.V = m->host.V; a.order = m->host.order; a.bos_word = m->host.bos_word; a.R = R; a.U = U;
+    a.ids = ids; a.ids_stride = ids_stride; a.ids_i64 = ids_i64;
+    a.last = last; a.last_stride = last_stride; a.last_i64 = last_i64;
+    a.lens = lens; a.lens_i64 = lens_i64; a.out = out;
+    const int rc = LaunchNgramScore(a, (cudaStream_t)stream);
+    if (rc) return FailCuda("ngram_score", (cudaError_t)rc);
+    return 0;
+}
+
 int ccb_lm_mix_slot_rows(int n_ngram, const void *const *ngrams, const double *ngram_w, const int *const *state_in,
                          int *const *state_out, int n_neural, const void *const *neural_rows, const int *neural_dtype,
                          const double *neural_w, const int *order, int N, int beam, int V, const int *parent,

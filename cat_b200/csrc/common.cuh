@@ -278,6 +278,18 @@ struct LmMixDev {
 size_t LmMixSlotRowsSmemBytes(int W, int V);
 int LaunchLmMixSlotRows(const LmMixDev &mix, int W, int N, int B, int V, const int *parent, const int *token, float *rows,
                         cudaStream_t s);
+// Sentence scores under an n-gram LM (ngram_score.cu), one launch: R rows of token ids (row stride ids_stride, U columns
+// read up to each row's length), each row's last target (row stride last_stride), lengths (null: U); *_i64 selects int64
+// over int32.  bos_word: the word id of <s>; order: the LM's order.  out: (R,) fp32, NaN for a row with a bad token or length.
+struct NGramScoreArgs {
+    NGramDev lm;
+    int V = 0, order = 0, bos_word = 0, R = 0, U = 0;
+    const void *ids = nullptr, *last = nullptr, *lens = nullptr;
+    long ids_stride = 0, last_stride = 0;
+    int ids_i64 = 0, last_i64 = 0, lens_i64 = 0;
+    float *out = nullptr;
+};
+int LaunchNgramScore(const NGramScoreArgs &a, cudaStream_t s);
 // A decoding graph's tables on one device (wfst.h WfstHost), for the TLG Viterbi beam search (wfst_decode.cu)
 struct WfstDev {
     const int *arc_off = nullptr, *eps_off = nullptr, *dst = nullptr, *tok = nullptr, *olabel = nullptr, *fid = nullptr,

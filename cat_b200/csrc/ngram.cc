@@ -291,8 +291,10 @@ bool LoadArpa(const char *path, const char *const *labels, int V, NGramHost *out
         }
     auto bos = vocab.find("<s>");
     m.bos = bos != vocab.end() && order >= 2 ? base[1] + bos->second : 0;
+    m.bos_word = bos != vocab.end() ? bos->second : -1;
     auto eos = vocab.find("</s>");
     m.eos = eos != vocab.end() ? eos->second : unk;
+    m.eos_listed = eos != vocab.end();
     return true;
 }
 

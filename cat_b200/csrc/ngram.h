@@ -24,6 +24,8 @@ struct NGramHost {
     bool unk_substituted = false;
     int bos = 0;                        // state after <s> (the root when the file lists no <s>)
     int eos = 0;                        // word id of </s> (<unk> when the file lists none)
+    int bos_word = -1;                  // word id of <s>, -1 when the file lists none
+    bool eos_listed = false;            // the file lists </s>
     std::vector<int> tok2word;          // [V]: -1 for the blank (token 0), <unk> for a label the LM does not list
     std::vector<float> root_p;          // [W]
     std::vector<int> root_dst;          // [W]

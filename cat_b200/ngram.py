@@ -9,6 +9,7 @@ import ctypes as C
 from typing import Sequence, Union
 
 import numpy as np
+import torch
 
 from . import _lib
 
@@ -66,6 +67,69 @@ class NGramLM:
             out[name] = a
         out["bos"], out["eos"] = self.bos, self.eos
         return out
+
+    def score(self, input_ids, targets, input_lengths=None):
+        """CAT's ``NGram.score`` (``AbsDecoder.score``): the (N,) fp32 natural-log score of each row's word string
+        w_0 .. w_L, L = input_lengths[b] (the width U when None): w_i is the word of input_ids[b, i] for i < L, and w_L the
+        word of ``targets[b, -1]``, the last column whatever L is (both CAT callers put token 0 there).  Token 0 is </s>,
+        or <s> at position 0; every term is ARPA back-off from the empty history, as KenLM's score(bos=False, eos=False),
+        summed in fp64 and rounded once (DESIGN.md §7 "N-gram sentence scoring").  One kernel launch.
+        input_ids (N, U) and targets (N, U') are int32 or int64 on one device; input_lengths (N,) int32 or int64 on any.
+        CUDA inputs: the result is on that device and nothing synchronises the host; a device token outside [0, V) or
+        length outside [1, U] gives that row NaN.  CPU inputs: computed on the current CUDA device, returned on the CPU.
+        ValueError: bad ranks, dtypes or shapes, host tokens or lengths out of range, or an LM whose file lists no <s> or
+        no </s>."""
+        ids, tgt = input_ids, targets
+        ints = (torch.int32, torch.int64)
+        if not isinstance(ids, torch.Tensor) or ids.dim() != 2 or ids.dtype not in ints or ids.shape[1] < 1:
+            raise ValueError("NGramLM.score: input_ids must be an int32 or int64 (N, U) tensor with U >= 1")
+        N, U = int(ids.shape[0]), int(ids.shape[1])
+        if not isinstance(tgt, torch.Tensor) or tgt.dim() != 2 or tgt.dtype not in ints or tgt.shape[0] != N \
+                or tgt.shape[1] < 1:
+            raise ValueError(f"NGramLM.score: targets must be an int32 or int64 (N, U') tensor with N = {N}, U' >= 1")
+        if tgt.device != ids.device:
+            raise ValueError(f"NGramLM.score: targets is on {tgt.device}, input_ids on {ids.device}")
+        lens = input_lengths
+        if lens is not None and (not isinstance(lens, torch.Tensor) or lens.dtype not in ints or tuple(lens.shape) != (N,)):
+            raise ValueError(f"NGramLM.score: input_lengths must be None or an int32 or int64 (N,) tensor with N = {N}")
+        if lens is not None and lens.is_cuda and ids.is_cuda and lens.device != ids.device:
+            raise ValueError(f"NGramLM.score: input_lengths is on {lens.device}, input_ids on {ids.device}")
+        on_host = not ids.is_cuda
+        if lens is not None and (on_host or not lens.is_cuda):     # host lengths are checked here
+            lens = lens.cpu()
+            if N and (int(lens.min()) < 1 or int(lens.max()) > U):
+                raise ValueError(f"NGramLM.score: input_lengths must lie in [1, U = {U}]")
+        last = tgt[:, -1]
+        if on_host and N:
+            used = ids if lens is None else ids[torch.arange(U)[None, :] < lens[:, None]]
+            lo, hi = min(int(used.min()), int(last.min())), max(int(used.max()), int(last.max()))
+            if lo < 0 or hi >= self.V:
+                raise ValueError(f"NGramLM.score: tokens must lie in [0, V = {self.V})")
+        if N == 0:
+            return torch.empty(0, dtype=torch.float32, device=ids.device)
+        entry = _lib.lib().ccb_ngram_score
+        from .rnnt import _int32, _on_device
+        dev = ids.device if not on_host else torch.device("cuda", torch.cuda.current_device())
+        if on_host:
+            ids, last = ids.to(dev), last.to(dev)
+        if ids.stride(1) != 1 or ids.stride(0) < U:
+            ids = ids.contiguous()
+        if lens is not None:
+            if lens.is_cuda:
+                lens = lens.contiguous()
+            else:
+                lens = lens.to(dev) if on_host else _on_device(dev, _int32(lens))[0]
+        out = torch.empty(N, dtype=torch.float32, device=dev)
+        i64 = lambda t: int(t.dtype == torch.int64)
+        with torch.cuda.device(dev):
+            rc = entry(self._h, N, U, ids.data_ptr(), ids.stride(0), i64(ids), last.data_ptr(),
+                                   last.stride(0), i64(last), lens.data_ptr() if lens is not None else None,
+                                   i64(lens) if lens is not None else 0, out.data_ptr(),
+                                   torch.cuda.current_stream(dev).cuda_stream)
+        if rc:
+            msg = _lib.last_error()
+            raise (ValueError if "lists no" in msg else RuntimeError)(f"NGramLM.score: {msg}")
+        return out.cpu() if on_host else out
 
     def __del__(self):
         h = getattr(self, "_h", None)

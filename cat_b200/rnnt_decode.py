@@ -142,6 +142,16 @@ class MultiLM:
             raise ValueError(f"{caller}: the mix's largest n-gram LM has {W} words and V = {V}; the mix rows are built in "
                              f"shared memory, which holds at most {_MIX_SMEM // 8} words plus labels")
 
+    def score(self, input_ids, targets, input_lengths=None) -> torch.Tensor:
+        """CAT's ``MultiDecoder.score``: sum_i w_i member_i.score(input_ids, targets, input_lengths), in member order,
+        each product and sum in fp64, rounded to fp32 once.  ``NGramLM`` members score on the GPU (``NGramLM.score``); a
+        neural member uses its own CAT ``score``.  The result is on input_ids' device."""
+        out = None
+        for w, lm in zip(self.weights, self.lms):
+            x = w * lm.score(input_ids, targets, input_lengths).to(input_ids.device, torch.float64)
+            out = x if out is None else out + x
+        return out.float()
+
     def __repr__(self):
         return f"MultiLM({self.weights}, [{', '.join(type(lm).__name__ for lm in self.lms)}])"
 

@@ -542,6 +542,17 @@ int ccb_rnnt_beam_step_fused(const void *rows, const void *enc, int dtype, int m
  * been loaded for V labels and have at most 25600 words. */
 int ccb_ngram_slot_rows(const void *lm, int N, int beam, int V, const int *parent, const int *token, const int *state_in,
                         int *state_out, float *rows, void *stream);
+/* Sentence scores under a token n-gram LM (ccb_ngram_create), as CAT's NGram.score computes them (DESIGN.md §7 "N-gram
+ * sentence scoring"), one launch.  Row b of R: ids + b*ids_stride holds its tokens (U columns, contiguous), last +
+ * b*last_stride its last target (CAT's targets[b, -1]), lens[b] its length L (lens null: every L = U); each array is int32,
+ * or int64 where its *_i64 flag is 1, on the device, read in place, and only ids[b][0 .. L) is read.  out[b] (fp32) =
+ * ln 10 * sum_{i=0..L} log10 P(w_i | w_max(0,i-n+1) .. w_i-1) by ARPA back-off from the empty history (KenLM's score with
+ * bos = eos = False), summed in fp64 in a fixed order that depends on the row alone and rounded once; w_i is the word of
+ * ids[b][i] for i < L and w_L that of the last target, token 0 being </s>, or <s> at position 0.  A token outside [0, V)
+ * or a length outside [1, U] makes that row's out NaN; device values are not checked on the host.  The LM must list <s>
+ * and </s> ("ngram_score: the LM lists no ..." before any launch otherwise). */
+int ccb_ngram_score(const void *lm, int R, int U, const void *ids, long ids_stride, int ids_i64, const void *last,
+                    long last_stride, int last_i64, const void *lens, int lens_i64, float *out, void *stream);
 /* The rows of a weighted mix of LMs (LODR and the like: DESIGN.md §7 "RNN-T beam search with an LM mix") for
  * ccb_rnnt_beam_step_fused: for every slot q of N*beam, rows[q][k] (V fp32) = sum over the members i, in the given order,
  * of w_i LM_i[q][k], each product and sum rounded in fp64 on its own, the first product starting the sum, rounded to fp32
